@@ -1,11 +1,12 @@
 #!/usr/bin/env python
-"""bench.py -- ROIs/s of the GDRNPP per-ROI pose path (BASELINE.json metric) on N B200s of one node.
+"""bench.py -- ROIs/s of the GDRNPP per-ROI pose path (BASELINE.json metric) on N H100s of one node.
 
   python bench.py --gpus 1 --steps 20 --warmup 5
   python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 --master-port P \
          bench.py --gpus N --steps K --warmup W
   python bench.py --impl reference ...      (the CPU path on the host cores; oracle port, see DESIGN.md)
   python bench.py --workload fps|voting|nnd|flow|raster|upnp|refine|ycbv5|native   (one JSON line per record)
+  python bench.py ... --dump-outputs DIR    (after the timed steps: DIR/rot.npy, DIR/trans.npy of the last timed step)
 
 A step = one forward of the whole hot path (ConvNeXt-base + geometry head + Patch-PnP + pose lift) over one batch of 64
 synthetic 256x256 ROIs per GPU (BASELINE.json configs[1]); ROIs are sharded across ranks with no data-path collective
@@ -43,13 +44,13 @@ def workload_config(world, precision):
                         "the end (configs[3])",
             "global_batch": BATCH * world,
             "l2": "inputs rotate over 4 distinct batches; per-step working set (~2 GB activations + 0.4 GB weights in "
-                  "bf16x3) >> 126 MB L2",
+                  "bf16x3) >> 50 MB L2",
             "parallelism": "roi-shard x%d" % world, "precision": precision}
 
 
 def load_peaks(timed_region_s=None):
-    """bf16 roofline denominator: the BURST figure for a timed region under ~1 s (the GPU has not hit its power-capped
-    steady state yet), the sustained one for seconds-long regions (B200_PROFILING.md)."""
+    """bf16 roofline denominator: MEASURED_PEAKS.json when present (the BURST figure for a timed region under ~1 s, the
+    sustained one for seconds-long regions), else the H100 SXM data sheet (dense BF16, HBM3, max SM clock)."""
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         with open(p) as f:
@@ -58,7 +59,7 @@ def load_peaks(timed_region_s=None):
         tf = d.get("bf16_tflops") if burst else d.get("bf16_tflops_sustained", d.get("bf16_tflops"))
         return {"bf16_tflops": tf, "hbm_gbs": d.get("hbm_gbs"), "sm_max_mhz": d.get("sm_max_mhz"),
                 "source": "measured (MEASURED_PEAKS.json, %s; timed region %.2f s)" % ("burst" if burst else "sustained", timed_region_s or 0.0)}
-    return {"bf16_tflops": 1590.0, "hbm_gbs": 6650.0, "sm_max_mhz": 1965.0, "source": "fallback (B200_PROFILING.md)"}
+    return {"bf16_tflops": 989.0, "hbm_gbs": 3350.0, "sm_max_mhz": 1980.0, "source": "H100 SXM data sheet (700 W card)"}
 
 
 class ClockSampler:
@@ -219,6 +220,10 @@ def main():
                     help="bf16x3 (default, the mode of record): split-bf16 GEMMs, fp32 parity; bf16: throughput mode")
     ap.add_argument("--workload", default="pose64",
                     help="pose64 (default) | native | fps | voting | nnd | flow | raster | upnp | refine | ycbv5")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the poses of the last timed step as DIR/rot.npy, DIR/trans.npy "
+                         "(float32) so that two builds can be compared output for output; with several ranks, rank 0's "
+                         "shard only")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3)
     rank = int(os.environ.get("RANK", "0"))
@@ -258,7 +263,7 @@ def main():
     model = GDRN_DoubleMask(default_cfg(), max_batch=BATCH, precision=args.precision)
     model.load_state_dict(make_state_dict())
     model.to(dev)
-    NB = 4  # distinct input batches: 4 x 50 MB of images + ~2 GB of activations per step >> 126 MB L2
+    NB = 4  # distinct input batches: 4 x 50 MB of images + ~2 GB of activations per step >> 50 MB L2
     keys = ("roi_img", "roi_classes", "roi_coord_2d", "roi_cams", "roi_centers", "roi_whs", "resize_ratios",
             "roi_extents")
     host = []
@@ -348,6 +353,13 @@ def main():
         launches = (L.gdrn_launch_count() - c0_) * args.steps
     ms_total = max_over_ranks(e0.elapsed_time(e1))
     value = world * BATCH * args.steps / (ms_total / 1e3)
+    if args.dump_outputs and rank == 0:
+        import numpy as np
+
+        # the inputs are the seeded make_batch() batches, so the same arguments give the same inputs on every run
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        np.save(os.path.join(args.dump_outputs, "rot.npy"), rots[-1].float().cpu().numpy())
+        np.save(os.path.join(args.dump_outputs, "trans.npy"), transes[-1].float().cpu().numpy())
 
     # ---------------- end-to-end through the public API with host buffers ----------------
     # Every step: H2D of that step's inputs from pinned host memory, forward, D2H of that step's poses.
@@ -406,7 +418,7 @@ def main():
     ms_e2e = max_over_ranks(e0.elapsed_time(e1))
     e2e_value = world * BATCH * args.steps / (ms_e2e / 1e3)
 
-    # ---------------- roofline of the dominant kernel family (tcgen05 GEMMs), measured live with CUDA events ----------------
+    # ---------------- roofline of the dominant kernel family (wgmma GEMMs), measured live with CUDA events ----------------
     import ctypes
     peaks = load_peaks(ms_total / 1e3)
     L.gdrn_model_set_profiling(model._handle, 1)
@@ -424,56 +436,24 @@ def main():
     L.gdrn_model_set_profiling(model._handle, 0)
     x3 = args.precision == "bf16x3"
     gemm_tflops = BATCH * GEMM_GFLOP_PER_ROI_EXECUTED / gemm_ms if gemm_ms > 0 else 0.0  # GFLOP / ms = TFLOP/s (algorithmic)
-    # DRAM bytes per GEMM launch from the committed ncu capture of this same command (profiles/, tools/make_traffic.py)
-    traffic, traffic_src = None, None
-    for tname in (("r02_traffic_x3.json" if x3 else "r02_traffic_bf16.json"), "r01_traffic.json"):
-        tpath = os.path.join(ROOT, "profiles", tname)
-        if not os.path.exists(tpath) or (x3 and tname == "r01_traffic.json"):
-            continue
-        try:
-            tj = json.load(open(tpath))
-            fam = [v for k, v in tj["families"].items() if k.startswith("gemm")]
-            if fam:
-                traffic = fam[0]["dram_bytes_per_launch"]
-                traffic_src = "profiles/%s (ncu dram__bytes_read.sum + dram__bytes_write.sum, mean over the %d tcgen05 GEMM " \
-                              "launches of one step; build %s)" % (tname, fam[0]["launches"], tj.get("build", "see file"))
-                break
-        except Exception:  # noqa: BLE001
-            traffic = None
-    # tensor-pipe activity of the whole forward (BASELINE.json metric: "backbone tensor-pipe %") from the committed ncu
-    # launch list of this same workload (profiles/r02_step_tensor.json, tools/r02b_ncu_step.sh + step_tensor_share.py)
-    tensor_pipe = None
-    tp_path = os.path.join(ROOT, "profiles", "r02_step_tensor.json")
-    if x3 and os.path.exists(tp_path):
-        try:
-            tj = json.load(open(tp_path))
-            tensor_pipe = {"forward_pct_of_elapsed": tj["tensor_pipe_pct_of_elapsed_forward"],
-                           "tcgen05_kernels_pct_of_elapsed": tj["tensor_pipe_pct_of_elapsed_tcgen05_kernels"],
-                           "tcgen05_kernels_pct_of_active": tj["tensor_pipe_pct_of_active_tcgen05_kernels"],
-                           "tcgen05_time_share": tj["tcgen05_time_share"],
-                           "source": "profiles/r02_step_tensor.json (ncu sm__pipe_tensor_cycles_active, time-weighted over the %d "
-                                     "launches of one forward; build %s)" % (tj["launches"], tj.get("build"))}
-        except Exception:  # noqa: BLE001
-            tensor_pipe = None
     step_ms = ms_total / args.steps
     roofline = {
         "bound": "tensor",
-        "kernel": ("gemm_pair_x3_kernel + gemm_tc_kernel (split-bf16 tcgen05/TMA implicit GEMM, all %d launches of a step)" if x3
-                   else "gemm_tc_kernel + gemm_pair_kernel + mlp_fused_kernel (tcgen05/TMA implicit GEMM, all %d launches of a step)") % gemm_n,
+        "kernel": ("gemm_tc_kernel (split-bf16 wgmma/TMA implicit GEMM, all %d launches of a step)" if x3
+                   else "gemm_tc_kernel (wgmma/TMA implicit GEMM, all %d launches of a step)") % gemm_n,
         "achieved": gemm_tflops, "peak": peaks["bf16_tflops"], "unit": "TFLOP/s",
-        "frac": gemm_tflops / peaks["bf16_tflops"], "traffic": traffic, "traffic_source": traffic_src,
+        "frac": gemm_tflops / peaks["bf16_tflops"],
         "algorithmic_flop_per_launch": BATCH * GEMM_GFLOP_PER_ROI_EXECUTED * 1e9 / max(gemm_n, 1),
         "avg_launch_us": gemm_ms * 1e3 / max(gemm_n, 1), "peak_source": peaks["source"],
         "gemm_ms_per_step": gemm_ms, "dwconv_ms_per_step": dw_ms, "other_ms_per_step": other_ms,
         "whole_step_tflops_reference_flops": BATCH * GFLOP_PER_ROI_REFERENCE / step_ms,
         "whole_step_frac_reference_flops": BATCH * GFLOP_PER_ROI_REFERENCE / step_ms / peaks["bf16_tflops"],
         "whole_step_tflops_executed_flops": BATCH * GFLOP_PER_ROI_EXECUTED / step_ms,
-        "tensor_pipe": tensor_pipe,
     }
     if x3:
         # `achieved` / `frac` count every multiply-add of the reference's fp32 GEMMs ONCE (algorithmic work).  The
         # tensor pipe issues three bf16 products per algorithmic MAC to reach fp32-class accuracy, so frac tops out at
-        # 1/3; tensor_executed_* is what ncu's sm__pipe_tensor_cycles_active corresponds to.
+        # 1/3; tensor_executed_* counts every product the tensor cores execute.
         roofline.update({"products_per_mac": 3, "x3_ceiling_frac": 1.0 / 3.0,
                          "tensor_executed_tflops": 3 * gemm_tflops,
                          "tensor_executed_frac": 3 * gemm_tflops / peaks["bf16_tflops"]})

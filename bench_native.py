@@ -4,10 +4,10 @@ rasteriser, fast depth refine, uncertainty-PnP) at the SURVEY.md §8(d) shapes, 
 Used by bench.py (`native_ops` record of the default line, or `--workload <op>` for a single op).  Every record:
 achieved HBM GB/s (or FP32 GFLOP/s for chamfer) from the ALGORITHMIC bytes/flops of SURVEY.md §8(d) over the
 CUDA-event time, against MEASURED_PEAKS.json; the reference's own CUDA build (oracle/_ref/<mod>.so, built unmodified for
-sm_100a) timed beside ours for voting / nnd / flow; the reference's CPU path for FPS (its .cpp, single thread) and the
+sm_90a) timed beside ours for voting / nnd / flow; the reference's CPU path for FPS (its .cpp, single thread) and the
 CPU port for uncertainty-PnP, with the core count.  The oracle / _ref modules are baselines here, never the thing measured.
 
-Timing: CUDA events around every call on the launching stream; a 256 MB memset evicts the 126 MB L2 before each timed
+Timing: CUDA events around every call on the launching stream; a 256 MB memset evicts the 50 MB L2 before each timed
 call ("l2": "flushed"); 3 warm-up calls.
 """
 import ctypes
@@ -19,6 +19,8 @@ import numpy as np
 import torch
 
 ROOT = os.path.dirname(os.path.abspath(__file__))
+# oracle/build_ref.py builds the reference arm only when GDRN_REFERENCE_SRC names a reference checkout at build() time
+REF_NOT_BUILT = "not built (oracle/_ref absent: set GDRN_REFERENCE_SRC for build())"
 
 
 def _load_ref_ext(name):
@@ -89,6 +91,8 @@ def bench_fps(dev, T, peaks):
             extra["cpu_reference_ms_per_cloud"] = (time.perf_counter() - t0) * 1e3
             extra["cpu_cores"] = 1
             extra["cpu_kind"] = "reference (farthest_point_sampling.cpp compiled into oracle/_ref/libfps_ref.so)"
+        else:
+            extra["cpu_kind"] = REF_NOT_BUILT
         out.append(_rec(name, {"batch": b, "pn": pn, "sn": sn}, ms, alg_bytes=b * (12 * pn + 4 * sn), peaks=peaks, **extra))
     return out
 
@@ -118,11 +122,14 @@ def bench_voting(dev, T, peaks):
     if ref is not None:
         rinl = torch.zeros_like(inl)
         recs[0]["reference_cuda_ms"] = T.time(lambda: ref.voting_for_hypothesis(direct, coords, hyp, rinl, 0.999))
-        recs[0]["reference_cuda_kind"] = "reference ransac_voting_kernel.cu built unmodified for sm_100a (oracle/_ref)"
+        recs[0]["reference_cuda_kind"] = "reference ransac_voting_kernel.cu built unmodified for sm_90a (oracle/_ref)"
         # the reference round = mask vote + torch.sum over tn (ransac_voting_gpu.py:56-60)
         recs[1]["reference_cuda_ms"] = T.time(lambda: (ref.voting_for_hypothesis(direct, coords, hyp, rinl, 0.999), torch.sum(rinl, 2)))
         recs[1]["reference_cuda_kind"] = "reference vote kernel + torch.sum(inlier, 2), what one reference RANSAC round costs"
         recs[2]["reference_cuda_ms"] = T.time(lambda: ref.generate_hypothesis(direct, coords, idxs))
+    else:
+        for r in recs[:3]:
+            r["reference_cuda_kind"] = REF_NOT_BUILT
     return recs
 
 
@@ -140,7 +147,9 @@ def bench_nnd(dev, T, peaks):
     ref = _load_ref_ext("torch_nndistance_aten")
     if ref is not None:
         rec["reference_cuda_ms"] = T.time(lambda: ref.nnd_forward_cuda(a, bb, d1, d2, i1, i2))
-        rec["reference_cuda_kind"] = "reference nnd_cuda_kernel.cu built unmodified for sm_100a (oracle/_ref)"
+        rec["reference_cuda_kind"] = "reference nnd_cuda_kernel.cu built unmodified for sm_90a (oracle/_ref)"
+    else:
+        rec["reference_cuda_kind"] = REF_NOT_BUILT
     return [rec]
 
 
@@ -162,7 +171,9 @@ def bench_flow(dev, T, peaks):
     ref = _load_ref_ext("flow_cuda")
     if ref is not None:
         rec["reference_cuda_ms"] = T.time(lambda: ref.forward(ds, dt, KT, Kinv))
-        rec["reference_cuda_kind"] = "reference flow_cuda_kernel.cu built unmodified for sm_100a (oracle/_ref)"
+        rec["reference_cuda_kind"] = "reference flow_cuda_kernel.cu built unmodified for sm_90a (oracle/_ref)"
+    else:
+        rec["reference_cuda_kind"] = REF_NOT_BUILT
     return [rec]
 
 
@@ -337,8 +348,8 @@ WORKLOADS = {"fps": bench_fps, "voting": bench_voting, "nnd": bench_nnd, "flow":
 
 def peaks_with_fp32(peaks):
     p = dict(peaks)
-    mhz = p.get("sm_max_mhz") or 1965.0
-    p["fp32_gflops"] = 148 * 128 * 2 * mhz * 1e6 / 1e9   # 148 SMs x 128 FMA lanes x 2 FLOP x clock
+    mhz = p.get("sm_max_mhz") or 1980.0
+    p["fp32_gflops"] = 132 * 128 * 2 * mhz * 1e6 / 1e9   # H100 SXM: 132 SMs x 128 FMA lanes x 2 FLOP x clock
     return p
 
 

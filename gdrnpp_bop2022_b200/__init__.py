@@ -1,1 +1,1 @@
-"""B200-native GDRNPP per-ROI pose inference hot path."""
+"""H100-native GDRNPP per-ROI pose inference hot path."""

@@ -1,4 +1,4 @@
-"""Build libgdrn_b200.so in-tree with nvcc for sm_100a (no torch dependency in the library)."""
+"""Build libgdrn_b200.so in-tree with nvcc for sm_90a (no torch dependency in the library)."""
 import os
 import subprocess
 import sys
@@ -9,7 +9,7 @@ CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libgdrn_b200.so")
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
     "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr",
 ]
 
@@ -51,7 +51,7 @@ def build(verbose=False, force=False):
         list(ex.map(compile_one, jobs))
     objs = [os.path.join(objdir, f[:-3] + ".o") for f in sources()]
     if jobs or not os.path.exists(LIB):
-        cmd = [NVCC, "-shared", "-gencode", "arch=compute_100a,code=sm_100a", "-o", LIB] + objs + ["-lcudart"]
+        cmd = [NVCC, "-shared", "-gencode", "arch=compute_90a,code=sm_90a", "-o", LIB] + objs + ["-lcudart"]
         r = subprocess.run(cmd, capture_output=True, text=True)
         if r.returncode != 0:
             raise RuntimeError(f"link failed:\n{r.stdout}\n{r.stderr}")

@@ -73,34 +73,28 @@ extern "C" int gdrn_gemm_bf16(const void* A, const void* W, const float* bias, c
   GDRN_CHECK_CUDA(cudaMemcpyAsync(h, d_trace, sizeof(h), cudaMemcpyDeviceToHost, (cudaStream_t)stream));
   GDRN_CHECK_CUDA(cudaStreamSynchronize((cudaStream_t)stream));
   fprintf(stderr, "[gemm trace] M=%lld N=%d K=%d epi=%d bn=%d: cta0 cycles=%lld tiles=%lld | producer empty-wait=%lld | "
-                  "mma full-wait=%lld acc-wait=%lld | epi0 acc-wait=%lld busy=%lld (tmem-ld=%lld compute=%lld flush=%lld)\n",
-          (long long)M, N, K, epi, block_n, h[6], h[7], h[0], h[1], h[2], h[3], h[4], h[8], h[9], h[10]);
+                  "consumer full-wait=%lld acc hand-over=%lld | epi0 acc-ld=%lld compute=%lld flush=%lld\n",
+          (long long)M, N, K, epi, block_n, h[6], h[7], h[0], h[1], h[3], h[8], h[9], h[10]);
   return GDRN_OK;
 }
 
 extern "C" int gdrn_mlp_fused_x3(const void* A, const void* W1, const float* b1, const void* W2, const float* b2,
                                  const float* gamma, float* x, long long M, int C, void* stream) {
   GDRN_REQUIRE(A && W1 && b1 && W2 && b2 && gamma && x, "mlp_fused_x3: null argument");
-  GDRN_REQUIRE(mlp_fused_x3_supported(C, M), "mlp_fused_x3: needs C == 128 and M a multiple of 128, M >= 128 * 148");
   return mlp_fused_x3_launch(A, W1, b1, W2, b2, gamma, x, M, C, (cudaStream_t)stream);
 }
 
-static int gemm_x3_impl(const void* A, const void* W, const float* bias, const float* gamma, const float* resid, void* out,
-                       int M, int N, int K, int epi, int block_n, unsigned* sk_flags, int sk_flag_words, void* stream);
-
 extern "C" int gdrn_gemm_x3(const void* A, const void* W, const float* bias, const float* gamma, const float* resid,
-                            void* out, int M, int N, int K, int epi, int block_n, void* stream) {
-  return gemm_x3_impl(A, W, bias, gamma, resid, out, M, N, K, epi, block_n, nullptr, 0, stream);
-}
+                            void* out, int M, int N, int K, int epi, int block_n, void* stream);
 
 extern "C" int gdrn_gemm_x3_ksplit(const void* A, const void* W, const float* bias, const float* gamma, float* x, int M, int N,
                                    int K, int block_n, unsigned* flags, int flag_words, void* stream) {
   GDRN_REQUIRE(flags != nullptr && flag_words > 0, "gemm_x3_ksplit: flags must be a zeroed device buffer");
-  return gemm_x3_impl(A, W, bias, gamma, x, x, M, N, K, EPI_RESID, block_n, flags, flag_words, stream);
+  return gdrn_gemm_x3(A, W, bias, gamma, x, x, M, N, K, EPI_RESID, block_n, stream);
 }
 
-static int gemm_x3_impl(const void* A, const void* W, const float* bias, const float* gamma, const float* resid, void* out,
-                       int M, int N, int K, int epi, int block_n, unsigned* sk_flags, int sk_flag_words, void* stream) {
+extern "C" int gdrn_gemm_x3(const void* A, const void* W, const float* bias, const float* gamma, const float* resid,
+                            void* out, int M, int N, int K, int epi, int block_n, void* stream) {
   GDRN_REQUIRE(M > 0 && N > 0 && K > 0, "gemm_x3: empty problem");
   GDRN_REQUIRE(K % 64 == 0, "gemm_x3: K must be a multiple of 64 (the lo half starts at a k-chunk boundary)");
   GDRN_REQUIRE(epi >= 0 && epi <= 2, "gemm_x3: epi must be 0 (store fp32), 1 (gelu -> split bf16) or 2 (resid)");
@@ -137,7 +131,6 @@ static int gemm_x3_impl(const void* A, const void* W, const float* bias, const f
   p.bias = bias;
   p.gamma = gamma;
   p.resid = resid;
-  p.sk_flags = sk_flags; p.sk_flag_words = sk_flag_words;
   static int trace_on = -1;
   if (trace_on < 0) trace_on = getenv("GDRN_GEMM_TRACE") ? 1 : 0;
   if (trace_on) {
@@ -150,9 +143,9 @@ static int gemm_x3_impl(const void* A, const void* W, const float* bias, const f
     long long h[16];
     GDRN_CHECK_CUDA(cudaMemcpyAsync(h, d_trace, sizeof(h), cudaMemcpyDeviceToHost, (cudaStream_t)stream));
     GDRN_CHECK_CUDA(cudaStreamSynchronize((cudaStream_t)stream));
-    fprintf(stderr, "[gemm x3 trace] M=%d N=%d K=%d epi=%d bn=%d: pair0 cycles=%lld tiles=%lld | producer empty-wait=%lld | "
-                    "mma full-wait=%lld acc-wait=%lld | epi0 acc-wait=%lld busy=%lld (tmem-ld=%lld compute=%lld wait+sts+store=%lld)\n",
-            M, N, K, epi, block_n, h[6], h[7], h[0], h[1], h[2], h[3], h[4], h[8], h[9], h[10]);
+    fprintf(stderr, "[gemm x3 trace] M=%d N=%d K=%d epi=%d bn=%d: cta0 cycles=%lld tiles=%lld | producer empty-wait=%lld | "
+                    "consumer full-wait=%lld acc hand-over=%lld | epi0 acc-ld=%lld compute=%lld flush=%lld\n",
+            M, N, K, epi, block_n, h[6], h[7], h[0], h[1], h[3], h[8], h[9], h[10]);
     return GDRN_OK;
   }
   return gemm_tc_launch(p, block_n, (cudaStream_t)stream);

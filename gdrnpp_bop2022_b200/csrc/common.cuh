@@ -1,4 +1,4 @@
-// Shared device/host helpers for libgdrn_b200.so (sm_100a only).
+// Shared device/host helpers for libgdrn_b200.so (sm_90a).
 #pragma once
 #include <cuda.h>
 #include <cuda_bf16.h>
@@ -44,7 +44,7 @@ static inline int gdrn_num_sms() {
   const int dev = gdrn_cur_device();
   if (n[dev] == 0) {
     cudaDeviceGetAttribute(&n[dev], cudaDevAttrMultiProcessorCount, dev);
-    if (n[dev] <= 0) n[dev] = 148;
+    if (n[dev] <= 0) n[dev] = 132;
   }
   return n[dev];
 }
@@ -62,7 +62,7 @@ static inline int gdrn_num_sms() {
 
 // ---- programmatic dependent launch (PDL) ----
 // Every kernel of the per-ROI step is launched with cudaLaunchAttributeProgrammaticStreamSerialization: the next kernel's
-// CTAs are placed on SMs as the previous kernel's CTAs retire and run their prologue (barrier init, TMEM allocation,
+// CTAs are placed on SMs as the previous kernel's CTAs retire and run their prologue (barrier init,
 // tensor-map prefetch, filter-tap loads) under the previous kernel's tail; ptx::griddep_wait() then holds them until the
 // previous grid has completed and flushed.  CONTRACT: a kernel launched through gdrn_launch_dep() executes
 // ptx::griddep_launch() first and ptx::griddep_wait() in EVERY thread before its first access to global memory that another
@@ -148,6 +148,26 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
   }
 }
 
+// The same bound without the printf, for kernels that issue wgmma: any function call in such a kernel makes ptxas
+// serialize the wgmma pipeline (C7510).  A protocol bug still traps.
+__device__ __forceinline__ void mbar_wait_nocall(uint32_t bar, uint32_t parity) {
+  uint32_t done = 0;
+  long long t0 = 0;
+  int spins = 0;
+  while (true) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\t"
+        "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
+        "selp.u32 %0, 1, 0, p;\n\t}\n"
+        : "=r"(done)
+        : "r"(bar), "r"(parity)
+        : "memory");
+    if (done) break;
+    if (++spins == 64) t0 = clock64();
+    if (spins > 64 && (clock64() - t0) > 4000000000LL) asm volatile("trap;");
+  }
+}
+
 // Bounded cluster-scope acquire wait on a barrier of THIS CTA that peers complete with st.async transaction bytes.
 __device__ __forceinline__ void mbar_wait_cluster(uint32_t bar, uint32_t parity) {
   uint32_t done = 0;
@@ -229,32 +249,7 @@ __device__ __forceinline__ void tma_load_5d(uint32_t dst, const void* tmap, uint
       : "memory");
 }
 
-// ---- tcgen05 / TMEM -------------------------------------------------------------------------
-__device__ __forceinline__ void tmem_alloc(uint32_t dst_smem, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(dst_smem), "r"(ncols)
-               : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-// D[tmem] (+)= A[smem] * B[smem], bf16 inputs, fp32 accumulate.
-__device__ __forceinline__ void tc_mma_bf16(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc,
-                                            uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}\n" ::"r"(d_tmem),
-      "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// ---- cta_group::2 (CTA pair) variants -----------------------------------------------------------
+// ---- thread-block clusters ----------------------------------------------------------------
 __device__ __forceinline__ uint32_t cluster_ctarank() {
   uint32_t r;
   asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
@@ -269,117 +264,25 @@ __device__ __forceinline__ uint32_t mapa_shared(uint32_t local_addr, uint32_t ct
   asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(local_addr), "r"(cta_rank));
   return r;
 }
-// default semantics (release at CTA scope), like cutlass::arch::ClusterBarrier::arrive(cta_id): the signal only says
-// "this warp's tcgen05.ld of the accumulator stage have completed" (ordered by tcgen05.fence::before_thread_sync).
-// The .release.cluster form compiles to MEMBAR.ALL.GPU + ERRBAR per arrive -- 25 % of the epilogue warps' stall
-// samples in the first ncu capture of the pair kernel.
-__device__ __forceinline__ void mbar_arrive_cluster(uint32_t cluster_addr) {
-  asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(cluster_addr) : "memory");
-}
-// TMA load issued by either CTA of a pair: data lands in the issuing CTA's shared memory, the transaction bytes are
-// signalled on `bar` which may live in the peer (leader) CTA (shared::cluster address)
-__device__ __forceinline__ void tma_load_2d_pair(uint32_t dst, const void* tmap, uint32_t bar_cluster, int c0, int c1) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-      ::"r"(dst), "l"(tmap), "r"(bar_cluster), "r"(c0), "r"(c1)
-      : "memory");
-}
-__device__ __forceinline__ void tma_load_4d_pair(uint32_t dst, const void* tmap, uint32_t bar_cluster, int c0, int c1, int c2,
-                                                 int c3) {
-  asm volatile(
-      "cp.async.bulk.tensor.4d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], "
-      "[%2];" ::"r"(dst), "l"(tmap), "r"(bar_cluster), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
-      : "memory");
-}
-__device__ __forceinline__ void tma_load_5d_pair(uint32_t dst, const void* tmap, uint32_t bar_cluster, int c0, int c1, int c2,
-                                                 int c3, int c4) {
-  asm volatile(
-      "cp.async.bulk.tensor.5d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6, "
-      "%7}], [%2];" ::"r"(dst), "l"(tmap), "r"(bar_cluster), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(c4)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_alloc_pair(uint32_t smem_dst, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_dst), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish_pair() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc_pair(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-// arrive (once the pair's prior MMAs retire) on the barrier at the same offset in every CTA of `cta_mask`
-__device__ __forceinline__ void tc_commit_pair(uint32_t bar, uint16_t cta_mask) {
-  asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-               ::"r"(bar), "h"(cta_mask)
-               : "memory");
-}
-// D[tmem of both CTAs] (+)= [A_cta0; A_cta1] (256 x 16) * [B_cta0 | B_cta1] (16 x N): issued by the leader CTA only
-__device__ __forceinline__ void tc_mma_bf16_pair(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc,
-                                                 uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}\n" ::"r"(d_tmem),
-      "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// the same with the A-operand collector: KEEP = collector::a::fill (A stays in the collector buffer after this MMA),
-// REUSE = collector::a::lastuse (A is taken from the collector instead of shared memory).  SASS: UTCHMMA ... .A_KEEP / .A_REUSE
-__device__ __forceinline__ void tc_mma_bf16_pair_a_keep(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc,
-                                                        uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16.collector::a::fill [%0], %1, %2, %3, p;\n\t}\n" ::"r"(d_tmem),
-      "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-__device__ __forceinline__ void tc_mma_bf16_pair_a_reuse(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc,
-                                                         uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16.collector::a::lastuse [%0], %1, %2, %3, p;\n\t}\n" ::"r"(d_tmem),
-      "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-
-// 32 lanes x 32 consecutive fp32 columns: thread t of the warp gets row (lane base + t), cols [c, c+32).
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-        "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-        "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
+// ---- wgmma (sm_90a warpgroup MMA) ------------------------------------------------------------
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+__device__ __forceinline__ void named_bar_sync(int id, int count) {
+  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory");
 }
 
-// K-major, 128-byte-swizzled operand tile (rows of 64 bf16 = 128 B, 8-row atoms of 1024 B):
-// start address >> 4 | LBO(ignored for swizzled K-major)=1 | SBO = 1024 B | version 1 (sm_100) | SWIZZLE_128B.
-// Field layout follows cute::UMMA::SmemDescriptor (cute/arch/mma_sm100_desc.hpp).
+// K-major, 128-byte-swizzled operand tile (rows of 64 bf16 = 128 B, 8-row atoms of 1024 B), as the TMA writes it with
+// CU_TENSOR_MAP_SWIZZLE_128B: start address >> 4 | LBO (unused for swizzled K-major) = 1 | SBO = 1024 B | SWIZZLE_128B.
+// Field layout of the sm_90 matrix descriptor (PTX ISA, "Matrix Descriptor Format" of wgmma).
 __device__ __forceinline__ uint64_t make_sw128_kmajor_desc(uint32_t smem_addr) {
   uint64_t d = 0;
   d |= (uint64_t)((smem_addr & 0x3FFFF) >> 4);        // [0,14)  start address
   d |= (uint64_t)1 << 16;                             // [16,30) leading byte offset (>>4)
   d |= (uint64_t)(1024 >> 4) << 32;                   // [32,46) stride byte offset (>>4)
-  d |= (uint64_t)1 << 46;                             // [46,48) descriptor version = 1
-  d |= (uint64_t)2 << 61;                             // [61,64) layout type SWIZZLE_128B
+  d |= (uint64_t)1 << 62;                             // [62,64) layout type SWIZZLE_128B
   return d;
-}
-// kind::f16 instruction descriptor: D fp32, A/B bf16, both K-major (cute::UMMA::InstrDescriptor).
-__host__ __device__ constexpr uint32_t make_idesc_bf16(uint32_t M, uint32_t N) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | ((N >> 3) << 17) | ((M >> 4) << 24);
 }
 
 }  // namespace ptx
@@ -407,44 +310,22 @@ __device__ __forceinline__ float gelu_erf(float x) {
   return x * (x >= 0.0f ? 1.0f - h : h);
 }
 
-// ---- packed fp32 (sm_100: FFMA2 / FMUL2 / FADD2, two lanes per instruction on the FMA pipe) ----
-// A three-register scalar FFMA issues every second cycle per scheduler; the packed forms carry two results per issue, so
-// FMA-pipe-bound epilogues and the depthwise convolution evaluate element PAIRS.
-typedef unsigned long long f32x2_t;
-__device__ __forceinline__ f32x2_t f2_pack(float lo, float hi) {
-  f32x2_t r;
-  asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(lo), "f"(hi));
-  return r;
-}
-__device__ __forceinline__ f32x2_t f2_dup(float v) { return f2_pack(v, v); }
-__device__ __forceinline__ float2 f2_unpack(f32x2_t v) {
-  float2 r;
-  asm("mov.b64 {%0, %1}, %2;" : "=f"(r.x), "=f"(r.y) : "l"(v));
-  return r;
-}
+// ---- fp32 element pairs ----
+// The FMA-pipe-bound epilogues and the depthwise convolution evaluate element PAIRS.  Each helper performs the same IEEE
+// operation per lane (round-to-nearest, never contracted), so results do not depend on how the pair is issued.
+typedef float2 f32x2_t;
+__device__ __forceinline__ f32x2_t f2_pack(float lo, float hi) { return make_float2(lo, hi); }
+__device__ __forceinline__ f32x2_t f2_dup(float v) { return make_float2(v, v); }
+__device__ __forceinline__ float2 f2_unpack(f32x2_t v) { return v; }
 __device__ __forceinline__ f32x2_t f2_fma(f32x2_t a, f32x2_t b, f32x2_t c) {
-  f32x2_t d;
-  asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(d) : "l"(a), "l"(b), "l"(c));
-  return d;
+  return make_float2(__fmaf_rn(a.x, b.x, c.x), __fmaf_rn(a.y, b.y, c.y));
 }
-__device__ __forceinline__ f32x2_t f2_mul(f32x2_t a, f32x2_t b) {
-  f32x2_t d;
-  asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b));
-  return d;
-}
-__device__ __forceinline__ f32x2_t f2_add(f32x2_t a, f32x2_t b) {
-  f32x2_t d;
-  asm("add.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b));
-  return d;
-}
-__device__ __forceinline__ f32x2_t f2_sub(f32x2_t a, f32x2_t b) {
-  f32x2_t d;
-  asm("sub.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b));
-  return d;
-}
+__device__ __forceinline__ f32x2_t f2_mul(f32x2_t a, f32x2_t b) { return make_float2(__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y)); }
+__device__ __forceinline__ f32x2_t f2_add(f32x2_t a, f32x2_t b) { return make_float2(__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y)); }
+__device__ __forceinline__ f32x2_t f2_sub(f32x2_t a, f32x2_t b) { return make_float2(__fsub_rn(a.x, b.x), __fsub_rn(a.y, b.y)); }
 
-// gelu_erf for an element pair: the same A&S 7.1.26 evaluation, 16 packed FMA-pipe instructions per PAIR (incl. none of
-// the selects: Phi = 0.5 + copysign(0.5 - h, x), the sign moved with one LOP3 per element on the ALU pipe) + 4 MUFU.
+// gelu_erf for an element pair: the same A&S 7.1.26 evaluation without the selects (Phi = 0.5 + copysign(0.5 - h, x),
+// the sign moved with one LOP3 per element on the ALU pipe) + 4 MUFU.
 __device__ __forceinline__ f32x2_t gelu_erf2(f32x2_t x) {
   const float2 xf = f2_unpack(x);
   const f32x2_t z = f2_mul(x, f2_dup(0.70710678118654752440f));                 // signed; only z^2 and |z| are used

@@ -1,4 +1,4 @@
-// CUDA-core kernels around the tcgen05 GEMMs of the dense path: weight repacking, stem patchify,
+// CUDA-core kernels around the wgmma GEMMs of the dense path: weight repacking, stem patchify,
 // ConvNeXt depthwise-7x7 + LayerNorm, LayerNorm + 2x2 patchify, GroupNorm/GELU/bilinear, pose lift.
 // Reference semantics: timm 0.6.7 ConvNeXtBlock (third-party), heads/top_down_doublemask_xyz_region_head.py,
 // heads/conv_pnp_net.py, core/utils/rot_reps.py:34-55, models/pose_from_pred_centroid_z.py:56-154,
@@ -220,7 +220,7 @@ dwconv_ln_kernel(const float* __restrict__ x, const float* __restrict__ w49c, co
 //          load overlaps the other's arithmetic; 8x8 x 128 ch for 8x8 images).  The zero-padded (TW+6)x(TH+6) x CPC
 //          fp32 input tile is fetched by ONE TMA box load (halo = out-of-bounds zero fill).
 //   thread = a PAIR of adjacent channels x one output row (TW pixels).  All arithmetic is fma.rn.f32x2
-//          (SASS FFMA2: two FMAs per issued instruction, the Blackwell packed-FP32 path); the input pairs
+//          (f2_* element pairs, the same IEEE operation per lane); the input pairs
 //          and the filter pairs are 8-byte shared-memory loads, conflict-free with lanes = channel pairs.
 //   cluster = the C/CPC CTAs (2/4/8) that together hold all channels of the tile: the LayerNorm statistics are
 //          combined across them through distributed shared memory with ONE cluster barrier (see below).

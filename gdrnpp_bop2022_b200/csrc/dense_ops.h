@@ -1,4 +1,4 @@
-// Internal launchers of the CUDA-core kernels around the tcgen05 GEMMs (dense_ops.cu).
+// Internal launchers of the CUDA-core kernels around the wgmma GEMMs (dense_ops.cu).
 #pragma once
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>

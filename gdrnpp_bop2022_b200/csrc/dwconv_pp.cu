@@ -52,7 +52,7 @@ constexpr size_t PP_SMEM = (size_t)(2 * PP_SLOT_FLOATS + 49 * PP_CPC) * 4 + (siz
 // R2 = the convolution's thread tile: false = one output row x 16 pixels per thread (warp = output row: 22 halo + 7 tap
 // LDS.64 per filter row, 203 per tile), true = TWO output rows x 8 pixels (warp = row pair x half of the tile width): an
 // input row is loaded once for both output rows and a filter row's taps are kept for the second one, 161 LDS.64 per tile for
-// the same 784 FFMA2, same per-output accumulation order (bit-identical results).
+// the same 784 FMA pairs, same per-output accumulation order (bit-identical results).
 template <int NR, bool SPLIT, bool TRACE, bool R2 = false>
 __global__ void __launch_bounds__(2 * PP_WG_THREADS, 1)
 dwconv_ln_pp_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_constant__ CUtensorMap tmap_w,

@@ -2,7 +2,7 @@
 // (float instantiation; launch surface src/flow_cuda.cpp:30-42).
 //
 // HBM-bound elementwise op: 4 B depth read + 4 B gathered target depth + 12 B written per pixel = 20 B/pixel.
-// Arithmetic is spelled out with explicit intrinsics in the contraction ptxas 12.9 / sm_100a applies to
+// Arithmetic is spelled out with explicit intrinsics in the contraction ptxas 12.9 / sm_90a applies to
 // the reference source (a*K0 + b*K1 + c  ->  fma(a,K0, b*K1) + c), double-literal comparisons included,
 // so flow/valid are bit-identical to the reference build.
 #include "common.cuh"

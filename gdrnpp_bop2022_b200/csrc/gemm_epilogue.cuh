@@ -1,16 +1,19 @@
-// Internal header shared by the tcgen05 GEMM translation units (gemm_tc.cu, gemm_pair.cu, mlp_fused.cu): tile constants,
-// output-row mapping and the epilogues (TMEM -> registers -> fused math -> global / shared memory).
+// Internal header of the wgmma GEMM kernel (gemm_tc.cu): tile constants, output-row mapping and the epilogues
+// (shared-memory accumulator tile -> registers -> fused math -> global / shared memory).
 #pragma once
 #include "common.cuh"
 #include "gemm_tc.h"
+
+// dynamic shared memory of the GEMM kernel (gemm_tc.cu): accumulator tile, operand ring, epilogue staging, barriers
+extern __shared__ uint8_t gemm_smem[];
 
 namespace {
 
 constexpr int BLOCK_M = 128;
 constexpr int BLOCK_K = 64;  // 64 bf16 = 128 B = one swizzle row
-constexpr int UMMA_K = 16;
+constexpr int MMA_K = 16;
 constexpr int A_STAGE_BYTES = BLOCK_M * BLOCK_K * 2;  // 16 KB
-constexpr int NUM_THREADS = 384;              // 4 control warps + 8 epilogue warps
+constexpr int NUM_THREADS = 384;              // producer warpgroup + 2 MMA / epilogue warpgroups (8 warps)
 constexpr int NUM_EPI_WARPS = 8;
 constexpr int EPI_STAGE_PITCH = 80;           // 64-byte row segment + 16 B pad (conflict-free 16-byte accesses)
 // per epilogue warp: either the TMA-store staging tile (32 rows x 128 B, 128B-swizzled, 1024-aligned) or, for the
@@ -104,25 +107,36 @@ __device__ __forceinline__ void load_vec(const float* __restrict__ src, int col,
   }
 }
 
-template <int CH>
-__device__ __forceinline__ void tmem_load_chunk(uint32_t taddr, float (&v)[CH]) {
-  if constexpr (CH == 32) {
-    uint32_t r[32];
-    ptx::tmem_ld32(taddr, r);
-    ptx::tmem_ld_wait();
+// The accumulator tile lives in shared memory, [BLOCK_M][acc_pitch] fp32 at the 1024-aligned start of the GEMM kernel's
+// dynamic shared memory (gemm_tc.cu writes it from the wgmma register fragments).  Epilogues address it as
+// (row << 16) | column (the tmem_* names below); lane l of a warp reads row `row + l`, CH consecutive columns.
+// Widths that are multiples of 32 keep dense rows and XOR-swizzle the 16-byte column groups by (row & 7), the others
+// pad each row by 16 bytes: either way the 16-byte row reads of 8 consecutive lanes hit distinct banks.
+template <int BLOCK_N>
+constexpr int acc_pitch() { return BLOCK_N % 32 == 0 ? BLOCK_N : BLOCK_N + 4; }  // floats
+template <int BLOCK_N>
+constexpr int acc_bytes() { return (BLOCK_M * acc_pitch<BLOCK_N>() * 4 + 1023) / 1024 * 1024; }
+template <int BLOCK_N>
+__device__ __forceinline__ int acc_index(int row, int col) {  // col: even; a float2 / float4 never straddles groups
+  return row * acc_pitch<BLOCK_N>() + (BLOCK_N % 32 == 0 ? col ^ ((row & 7) << 2) : col);
+}
+__device__ __forceinline__ float* acc_tile() {
+  const uint32_t a = ptx::smem_u32(gemm_smem);
+  return reinterpret_cast<float*>(gemm_smem + (((a + 1023u) & ~1023u) - a));
+}
+template <int BLOCK_N, int CH>
+__device__ __forceinline__ void acc_load_chunk(uint32_t aaddr, float (&v)[CH]) {
+  const float* acc = acc_tile();
+  const int row = (aaddr >> 16) + (threadIdx.x & 31), col = aaddr & 0xffff;
 #pragma unroll
-    for (int j = 0; j < 32; ++j) v[j] = __uint_as_float(r[j]);
-  } else {
-    uint32_t r[16];
-    ptx::tmem_ld16(taddr, r);
-    ptx::tmem_ld_wait();
-#pragma unroll
-    for (int j = 0; j < 16; ++j) v[j] = __uint_as_float(r[j]);
+  for (int j = 0; j < CH; j += 4) {
+    const float4 t = *reinterpret_cast<const float4*>(acc + acc_index<BLOCK_N>(row, col + j));
+    v[j] = t.x; v[j + 1] = t.y; v[j + 2] = t.z; v[j + 3] = t.w;
   }
 }
 
 // ------------------------------------------------------------------------------------------------
-// Epilogues.  Each of the 128 epilogue threads owns one accumulator row (TMEM lane).
+// Epilogues.  Each of the 128 epilogue threads owns one accumulator row.
 // ------------------------------------------------------------------------------------------------
 template <int BLOCK_N, int EPI>
 __device__ __forceinline__ void epilogue_tile(const GemmPlan& p, int m_tile, int n_tile, uint32_t tmem_row, int lane,
@@ -136,7 +150,7 @@ __device__ __forceinline__ void epilogue_tile(const GemmPlan& p, int m_tile, int
 #pragma unroll 1
     for (int c = 0; c < BLOCK_N; c += CH) {
       float v[CH];
-      tmem_load_chunk<CH>(tmem_row + c, v);
+      acc_load_chunk<BLOCK_N, CH>(tmem_row + c, v);
       const int col = n0 + c;
       if (!ri.valid || col >= p.N) continue;
       float bias[CH];
@@ -168,7 +182,7 @@ __device__ __forceinline__ void epilogue_tile(const GemmPlan& p, int m_tile, int
 #pragma unroll 1
     for (int c = 0; c < BLOCK_N; c += CH) {
       float v[CH];
-      tmem_load_chunk<CH>(tmem_row + c, v);
+      acc_load_chunk<BLOCK_N, CH>(tmem_row + c, v);
       const int col = n0 + c;
       if (col >= p.N) continue;
       if (ri.valid) store_row_chunk<CH>(p, ri, col, v, p.out_f32 != 0);
@@ -210,12 +224,12 @@ __device__ __forceinline__ void epilogue_tile(const GemmPlan& p, int m_tile, int
       }
     }
   } else if constexpr (EPI == EPI_BIAS_LN) {
-    // N <= BLOCK_N (N % 32 == 0): the thread sees the whole channel vector of its pixel. Three TMEM passes.
+    // N <= BLOCK_N (N % 32 == 0): the thread sees the whole channel vector of its pixel. Three passes over the accumulator row.
     float sum = 0.f;
 #pragma unroll 1
     for (int c = 0; c < p.N; c += CH) {
       float v[CH], bias[CH];
-      tmem_load_chunk<CH>(tmem_row + c, v);
+      acc_load_chunk<BLOCK_N, CH>(tmem_row + c, v);
       load_vec<CH>(p.bias, c, p.N, bias);
 #pragma unroll
       for (int j = 0; j < CH; ++j) sum += v[j] + bias[j];
@@ -226,7 +240,7 @@ __device__ __forceinline__ void epilogue_tile(const GemmPlan& p, int m_tile, int
 #pragma unroll 1
     for (int c = 0; c < p.N; c += CH) {
       float v[CH], bias[CH];
-      tmem_load_chunk<CH>(tmem_row + c, v);
+      acc_load_chunk<BLOCK_N, CH>(tmem_row + c, v);
       load_vec<CH>(p.bias, c, p.N, bias);
 #pragma unroll
       for (int j = 0; j < CH; ++j) { float d = v[j] + bias[j] - mean; sq = fmaf(d, d, sq); }
@@ -236,7 +250,7 @@ __device__ __forceinline__ void epilogue_tile(const GemmPlan& p, int m_tile, int
 #pragma unroll 1
     for (int c = 0; c < p.N; c += CH) {
       float v[CH], bias[CH], w[CH], bb[CH];
-      tmem_load_chunk<CH>(tmem_row + c, v);
+      acc_load_chunk<BLOCK_N, CH>(tmem_row + c, v);
       load_vec<CH>(p.bias, c, p.N, bias);
       load_vec<CH>(p.ln_w, c, p.N, w);
       load_vec<CH>(p.ln_b, c, p.N, bb);
@@ -269,14 +283,14 @@ __device__ __forceinline__ void epilogue_tile(const GemmPlan& p, int m_tile, int
     float v[80];
     {
       float t[32];
-      tmem_load_chunk<32>(tmem_row, t);
+      acc_load_chunk<BLOCK_N, 32>(tmem_row, t);
 #pragma unroll
       for (int j = 0; j < 32; ++j) v[j] = t[j];
-      tmem_load_chunk<32>(tmem_row + 32, t);
+      acc_load_chunk<BLOCK_N, 32>(tmem_row + 32, t);
 #pragma unroll
       for (int j = 0; j < 32; ++j) v[32 + j] = t[j];
       float t16[16];
-      tmem_load_chunk<16>(tmem_row + 64, t16);
+      acc_load_chunk<BLOCK_N, 16>(tmem_row + 64, t16);
 #pragma unroll
       for (int j = 0; j < 16; ++j) v[64 + j] = t16[j];
     }
@@ -373,7 +387,7 @@ __device__ __forceinline__ float gelu_tanh_f32(float x) {
 }
 
 // Epilogue for EPI_STORE / EPI_GELU / EPI_RESID / EPI_GNSTATS with coalesced global traffic.
-// Eight warps: warp ew owns TMEM lanes [32*(ew&3), +32) and the column half (ew>>2) of the tile.  A thread owns
+// Eight warps: warp ew owns accumulator rows [32*(ew&3), +32) and the column half (ew>>2) of the tile.  A thread owns
 // one accumulator row; 64-byte row segments (32 bf16 or 16 fp32 columns) are staged in the warp's private
 // shared-memory buffer (pitch 80 B, conflict-free 16-byte accesses) and then written (and, for the residual,
 // first read) with 16-byte accesses in which 4 lanes cover one row segment: every warp-wide access touches
@@ -432,7 +446,7 @@ __device__ __forceinline__ void epilogue_tile_staged_t(const GemmPlan& p, int m_
     }
     float v[CH];
     long long tq0 = trc ? clock64() : 0;
-    tmem_load_chunk<CH>(tmem_row + c, v);
+    acc_load_chunk<BLOCK_N, CH>(tmem_row + c, v);
     if (trc) { const long long t = clock64(); tq_tmem += t - tq0; tq0 = t; }
     if constexpr (EPI == EPI_STORE || EPI == EPI_GELU) {
       const float4* sb = reinterpret_cast<const float4*>(s_bias + c);  // warp-wide broadcast reads
@@ -596,7 +610,7 @@ __device__ __forceinline__ void epilogue_tile_staged_t(const GemmPlan& p, int m_
 
 // Epilogue for rank-2 outputs (EPI_STORE / EPI_GELU / EPI_RESID) with TMA stores.
 // Eight warps as above.  A thread owns one accumulator row; it writes 128-byte row segments (64 bf16 or 32 fp32
-// columns, produced as two 64-byte halves = two tcgen05.ld) into the warp's 32 x 128 B staging tile in the
+// columns, produced as two 64-byte halves) into the warp's 32 x 128 B staging tile in the
 // SWIZZLE_128B layout (16-byte piece j of row r at piece j ^ (r & 7): conflict-free row-wise STS.128), and one lane
 // issues a single cp.async.bulk.tensor store per tile.  No address arithmetic, LDS or STG in the flush; rows beyond
 // M are clipped by the tensor map.  The residual of EPI_RESID is read by its owner thread (64 contiguous bytes per
@@ -609,9 +623,9 @@ __device__ __forceinline__ void epilogue_tile_tma(const GemmPlan& p, int m_tile,
   // [g_begin, g_end): sub-range of this warp's columns (multiples of GW) -- lets a caller interleave the 128-byte groups
   // of a tile with other work so that the wait for the previous TMA store never blocks (fused MLP kernel)
   static_assert(BLOCK_N >= 128, "TMA-store epilogue needs BLOCK_N >= 128");
-  constexpr int CPW = BLOCK_N / (NEW / 4);  // columns per warp (NEW / 4 warps share one TMEM lane quarter)
+  constexpr int CPW = BLOCK_N / (NEW / 4);  // columns per warp (NEW / 4 warps share one quarter of the rows)
   static_assert(CPW * (F32 ? 4 : 2) >= 128, "a warp must own at least one 128-byte row segment");
-  constexpr int CH = F32 ? 16 : 32;     // columns per 64-byte half row (one tcgen05.ld)
+  constexpr int CH = F32 ? 16 : 32;     // columns per 64-byte half row
   constexpr int GW = 2 * CH;            // columns per staged 128-byte row (one TMA store)
   const int q = ew & 3, half = ew >> 2;
   const long long grow = (long long)m_tile * BLOCK_M + q * 32 + lane;
@@ -673,7 +687,7 @@ __device__ __forceinline__ void epilogue_tile_tma(const GemmPlan& p, int m_tile,
       }
       float v[CH];
       long long tq1 = trc ? clock64() : 0;
-      tmem_load_chunk<CH>(tmem_row + c, v);
+      acc_load_chunk<BLOCK_N, CH>(tmem_row + c, v);
       if (trc) { const long long t = clock64(); tq_tmem += t - tq1; }
       uint4* dst = reinterpret_cast<uint4*>(my_row);
       if constexpr (F32) {
@@ -749,7 +763,7 @@ __device__ __forceinline__ void epilogue_tile_tma(const GemmPlan& p, int m_tile,
 }
 
 // Split-bf16 (x3) outputs with TMA stores (EPI_STORE / EPI_GELU, bf16 [M, 2N] = [hi N | lo N] rows).
-// A thread owns one accumulator row.  Per 32-column chunk (one tcgen05.ld) it computes hi = bf16(v) and
+// A thread owns one accumulator row.  Per 32-column chunk it computes hi = bf16(v) and
 // lo = bf16(v - hi) in registers (the long part: exact-erf GELU), THEN waits for the previous chunk's TMA stores to
 // have read the staging buffer (long finished by then), writes hi / lo into two 32-row x 64-byte tiles and one
 // lane issues two stores: hi at column `col`, lo at column N + col.  Rows beyond M are clipped by the tensor map
@@ -776,9 +790,9 @@ __device__ __forceinline__ void epilogue_tile_tma_split(const GemmPlan& p, int m
     if (col >= p.N) break;  // warp-uniform
     float v[CH];
     long long tq0 = trc ? clock64() : 0;
-    tmem_load_chunk<CH>(tmem_row + c, v);
+    acc_load_chunk<BLOCK_N, CH>(tmem_row + c, v);
     if (trc) { const long long t = clock64(); tq_tmem += t - tq0; tq0 = t; }
-    // element PAIRS in packed fp32 (FADD2 / FFMA2 / FMUL2): this epilogue is FMA-pipe bound, see gelu_erf2
+    // element PAIRS (f2_*): this epilogue is FMA-pipe bound, see gelu_erf2
     f32x2_t v2[CH / 2];
 #pragma unroll
     for (int j = 0; j < CH / 2; ++j) v2[j] = f2_pack(v[2 * j], v[2 * j + 1]);
@@ -841,6 +855,12 @@ __device__ __forceinline__ void epilogue_tile_tma_split(const GemmPlan& p, int m
 template <int BLOCK_N, int EPI>
 __device__ __forceinline__ void epilogue_tile_staged(const GemmPlan& p, int m_tile, int n_tile, uint32_t tmem_acc,
                                                      int ew, int lane, uint8_t* stg) {
+  if constexpr (EPI == EPI_GELU) {
+    if (p.use_tma_store && p.split) {  // launch-uniform: split-bf16 output through TMA tile stores
+      epilogue_tile_tma_split<BLOCK_N, EPI, NUM_EPI_WARPS>(p, m_tile, n_tile, tmem_acc, ew, lane, stg);
+      return;
+    }
+  }
   if constexpr (BLOCK_N >= 128 && (EPI == EPI_STORE || EPI == EPI_GELU || EPI == EPI_RESID)) {
     if (p.use_tma_store) {  // launch-uniform
       if constexpr (EPI == EPI_RESID) {

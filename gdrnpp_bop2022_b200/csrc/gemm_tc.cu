@@ -1,12 +1,14 @@
-// tcgen05 + TMA implicit-GEMM kernel for the GDRNPP dense path (sm_100a).
+// wgmma + TMA implicit-GEMM kernel for the GDRNPP dense path (sm_90a).
 //
 // One persistent CTA per SM, warp-specialised:
-//   warp 0 lane 0 : TMA producer  (A pixel boxes + W tiles -> 128B-swizzled smem ring)
-//   warp 1 lane 0 : tcgen05.mma issuer (UMMA 128 x BLOCK_N x 16, bf16 -> fp32 accumulators in TMEM)
-//   warp 2        : TMEM allocate / free
-//   warps 4..11   : epilogue (tcgen05.ld -> registers -> fused math -> TMA store / global; gemm_epilogue.cuh),
-//                   double-buffered against the next tile's MMAs through two TMEM accumulator stages.
-// gemm_tc_launch() also dispatches to the CTA-pair kernel (gemm_pair.cu); the fused MLP block lives in mlp_fused.cu.
+//   warp 0 lane 0   : TMA producer  (A pixel boxes + W tiles -> 128B-swizzled smem ring)
+//   warps 4..11     : two consumer warpgroups.  Warpgroup g issues wgmma m64 x BLOCK_N x 16 (bf16 -> fp32 registers)
+//                     for rows [64g, 64g + 64) of the 128-row tile, releases each ring stage as soon as the MMAs that
+//                     read it retire, then writes its accumulators into the shared-memory accumulator tile; the same
+//                     8 warps then run the fused epilogue from there (gemm_epilogue.cuh) while the producer already
+//                     fills the ring for the next tile.
+// X3 (split-bf16, 64- / 128-wide tiles): a stage holds {A hi, A lo, W hi, W lo} and feeds all three products.
+// The kernel makes no function call: any call makes ptxas serialize the wgmma pipeline (C7510).
 //
 // It replaces, for the reference forward (core/gdrn_modeling/models/GDRN_double_mask.py:102-160), every
 // cuDNN/cuBLAS call made by timm ConvNeXt (Linear fc1/fc2, stem 4x4s4, 2x2s2 downsample), by the geometry
@@ -17,42 +19,47 @@
 #include <string.h>
 #include "gemm_tc.h"
 #include "gemm_epilogue.cuh"
+#include "wgmma.cuh"
 
 namespace {
 
-template <int BLOCK_N>
+// X3: split-bf16 operands with the shared four-tile stage {A hi, A lo, W hi, W lo} of one (tap, k-chunk) feeding the three
+// products A_lo*W_hi + A_hi*W_lo + A_hi*W_hi (4 operand tiles per 3 MMA groups instead of 6 with an expanded tap list).
+template <int BLOCK_N, bool X3>
 struct Cfg {
-  static constexpr int B_STAGE_BYTES = BLOCK_N * BLOCK_K * 2;
-  static constexpr int STAGE_BYTES = A_STAGE_BYTES + B_STAGE_BYTES;
-  static constexpr int STAGES = (SMEM_BUDGET / STAGE_BYTES) > 8 ? 8 : (SMEM_BUDGET / STAGE_BYTES);
-  static constexpr int ACC_COLS = BLOCK_N <= 128 ? 128 : 256;  // TMEM columns per accumulator stage
-  static constexpr int TMEM_COLS = 2 * ACC_COLS;
-  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024 /*align*/ + 256 /*barriers*/ + NUM_EPI_WARPS * EPI_STAGE_BYTES;
+  static constexpr int NOPS = X3 ? 2 : 1;  // hi (and lo) copies of each operand per stage
+  static constexpr int B_TILE_BYTES = BLOCK_N * BLOCK_K * 2;
+  static constexpr int B_STAGE_BYTES = NOPS * B_TILE_BYTES;
+  static constexpr int A_BYTES = NOPS * A_STAGE_BYTES;
+  static constexpr int STAGE_BYTES = A_BYTES + B_STAGE_BYTES;
+  static constexpr int ACC_BYTES = acc_bytes<BLOCK_N>();
+  static constexpr int RING = (SMEM_BUDGET - ACC_BYTES) / STAGE_BYTES;
+  static constexpr int STAGES = RING > 8 ? 8 : RING;
+  static constexpr int SMEM_BYTES = ACC_BYTES + STAGES * STAGE_BYTES + 1024 /*align*/ + 256 /*barriers*/ + NUM_EPI_WARPS * EPI_STAGE_BYTES;
+  static_assert(STAGES >= 2, "gemm: shared-memory ring needs two stages");
 };
 
 constexpr int PREFETCH_AHEAD = 6;  // k-iterations of A/B requested into L2 ahead of the shared-memory ring
+constexpr int CONSUMER_THREADS = 256;
+constexpr int BAR_ACC = 1;         // named barrier of the two consumer warpgroups (accumulator tile hand-over)
 
-template <int BLOCK_N, int EPI>
+template <int BLOCK_N, int EPI, bool X3>
 __global__ void __launch_bounds__(NUM_THREADS, 1) gemm_tc_kernel(const __grid_constant__ GemmPlan p) {
-  using C = Cfg<BLOCK_N>;
-  extern __shared__ uint8_t smem_raw[];
-  // 1024-byte alignment required by SWIZZLE_128B
-  const uint32_t smem_base = (ptx::smem_u32(smem_raw) + 1023u) & ~1023u;
-  const uint32_t bar_base = smem_base + C::STAGES * C::STAGE_BYTES + NUM_EPI_WARPS * EPI_STAGE_BYTES;
+  using C = Cfg<BLOCK_N, X3>;
+  // 1024-byte alignment required by SWIZZLE_128B: [accumulator tile | ring | epilogue staging | barriers]
+  const uint32_t smem_base = (ptx::smem_u32(gemm_smem) + 1023u) & ~1023u;
+  const uint32_t ring_base = smem_base + C::ACC_BYTES;
+  const uint32_t bar_base = ring_base + C::STAGES * C::STAGE_BYTES + NUM_EPI_WARPS * EPI_STAGE_BYTES;
   auto full_bar = [&](int s) { return bar_base + 8u * s; };
   auto empty_bar = [&](int s) { return bar_base + 8u * (C::STAGES + s); };
-  auto tfull_bar = [&](int s) { return bar_base + 8u * (2 * C::STAGES + s); };
-  auto tempty_bar = [&](int s) { return bar_base + 8u * (2 * C::STAGES + 2 + s); };
-  const uint32_t tmem_slot = bar_base + 8u * (2 * C::STAGES + 4);
-  uint8_t* smem_gen = smem_raw + (smem_base - ptx::smem_u32(smem_raw));
-  volatile uint32_t* tmem_slot_ptr = reinterpret_cast<volatile uint32_t*>(
-      smem_gen + C::STAGES * C::STAGE_BYTES + NUM_EPI_WARPS * EPI_STAGE_BYTES + 8 * (2 * C::STAGES + 4));
+  uint8_t* smem_gen = gemm_smem + (smem_base - ptx::smem_u32(gemm_smem));
+  float* acc_smem = reinterpret_cast<float*>(smem_gen);
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
   // epilogues that need the whole row in one thread (LayerNorm, out-conv) or tiny N keep 4 warps + direct stores
   constexpr bool kStaged = (BLOCK_N >= 64) && (EPI == EPI_STORE || EPI == EPI_GELU || EPI == EPI_RESID || EPI == EPI_GNSTATS);
-  uint8_t* stage_base = smem_gen + C::STAGES * C::STAGE_BYTES;  // 1024-aligned (TMA-store tiles are 128B-swizzled)
+  uint8_t* stage_base = smem_gen + C::ACC_BYTES + C::STAGES * C::STAGE_BYTES;  // 1024-aligned (TMA-store tiles are 128B-swizzled)
 
   ptx::griddep_launch();
   if (warp == 0 && lane == 0) {
@@ -62,22 +69,11 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) gemm_tc_kernel(const __grid_co
   if (warp == 1 && lane == 0) {
     for (int s = 0; s < C::STAGES; ++s) {
       ptx::mbar_init(full_bar(s), 1);
-      ptx::mbar_init(empty_bar(s), 1);
-    }
-    for (int s = 0; s < 2; ++s) {
-      ptx::mbar_init(tfull_bar(s), 1);
-      ptx::mbar_init(tempty_bar(s), kStaged ? NUM_EPI_WARPS : 4);
+      ptx::mbar_init(empty_bar(s), 2);  // one arrive per consumer warpgroup
     }
     ptx::fence_barrier_init();
   }
-  if (warp == 2) {
-    ptx::tmem_alloc(tmem_slot, C::TMEM_COLS);
-    ptx::tmem_relinquish();
-  }
-  ptx::tc_fence_before();
   __syncthreads();
-  ptx::tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot_ptr;
   ptx::griddep_wait();
 
   const int total_tiles = p.m_tiles * p.n_tiles;
@@ -113,13 +109,25 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) gemm_tc_kernel(const __grid_co
       for (int tap = 0; tap < p.num_taps; ++tap) {
         const GemmTap tp = p.taps[tap];
         for (int kc = 0; kc < p.k_chunks; ++kc) {
-          { const long long t0 = tr ? clock64() : 0; ptx::mbar_wait(empty_bar(stage), phase ^ 1); if (tr) tr_acc0 += clock64() - t0; }
-          const uint32_t sa = smem_base + stage * C::STAGE_BYTES;
-          const uint32_t sb = sa + A_STAGE_BYTES;
+          { const long long t0 = tr ? clock64() : 0; ptx::mbar_wait_nocall(empty_bar(stage), phase ^ 1); if (tr) tr_acc0 += clock64() - t0; }
+          const uint32_t sa = ring_base + stage * C::STAGE_BYTES;
+          const uint32_t sb = sa + C::A_BYTES;
           ptx::mbar_arrive_expect_tx(full_bar(stage), C::STAGE_BYTES);
           const int k0 = kc * BLOCK_K;
+#pragma unroll
+          for (int h = 0; h < C::NOPS; ++h) {   // h = 1: the lo halves, behind the hi tiles of the stage
+            const uint32_t da = sa + h * A_STAGE_BYTES;
+            const int ca = k0 + tp.c0 + h * p.x3_a_lo;
+            if (p.a_rank == 2) {
+              ptx::tma_load_2d(da, &p.tmap_a, full_bar(stage), ca, m_tile * BLOCK_M + tp.d1);
+            } else if (p.a_rank == 4) {
+              ptx::tma_load_4d(da, &p.tmap_a, full_bar(stage), ca, x0 + tp.d1, y0 + tp.d2, b0);
+            } else {
+              ptx::tma_load_5d(da, &p.tmap_a, full_bar(stage), ca, x0 + tp.d1, tp.d2, y0 + tp.d3, b0);
+            }
+            ptx::tma_load_2d(sb + h * C::B_TILE_BYTES, &p.tmap_b, full_bar(stage), tp.b_off + k0 + h * p.x3_b_lo, brow);
+          }
           if (p.a_rank == 2) {
-            ptx::tma_load_2d(sa, &p.tmap_a, full_bar(stage), k0 + tp.c0, m_tile * BLOCK_M + tp.d1);
             // A is streamed from HBM (it was written by the previous kernel): request it into L2 several
             // k-iterations ahead so the shared-memory ring only has to cover L2 latency, not DRAM latency.
             int pk = kc + PREFETCH_AHEAD, pm = m_tile;
@@ -130,56 +138,57 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) gemm_tc_kernel(const __grid_co
               pm = (nt < total_tiles && nm != m_tile) ? nm : -1;
             }
             if (pm >= 0 && pk < p.k_chunks && p.num_taps == 1) ptx::tma_prefetch_2d(&p.tmap_a, pk * BLOCK_K, pm * BLOCK_M);
-          } else if (p.a_rank == 4) {
-            ptx::tma_load_4d(sa, &p.tmap_a, full_bar(stage), k0 + tp.c0, x0 + tp.d1, y0 + tp.d2, b0);
-          } else {
-            ptx::tma_load_5d(sa, &p.tmap_a, full_bar(stage), k0 + tp.c0, x0 + tp.d1, tp.d2, y0 + tp.d3, b0);
           }
-          ptx::tma_load_2d(sb, &p.tmap_b, full_bar(stage), tp.b_off + k0, brow);
           if (++stage == C::STAGES) { stage = 0; phase ^= 1; }
         }
       }
     }
-  } else if (warp == 1 && lane == 0) {
-    // ================= MMA issuer =================
-    constexpr uint32_t idesc = ptx::make_idesc_bf16(BLOCK_M, BLOCK_N);
+    if (tr) { p.trace[0] = tr_acc0; p.trace[6] = clock64() - tr_start; p.trace[7] = (total_tiles - 1 - (int)blockIdx.x) / (int)gridDim.x + 1; }
+  } else if (warp >= 4) {
+    // ================= consumers: wgmma mainloop, accumulator hand-over, epilogue =================
+    const int ew = warp - 4;
+    const int wg = ew >> 2;             // rows [64 wg, 64 wg + 64) of the tile
+    const int wl = ew & 3;              // warp inside the warpgroup
+    const bool tr_me = tr && ew == 0 && lane == 0;
     int stage = 0;
     uint32_t phase = 0;
-    int it = 0;
-    for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x, ++it) {
-      const int as = it & 1;
-      const uint32_t aphase = (it >> 1) & 1;
-      { const long long t0 = tr ? clock64() : 0; ptx::mbar_wait(tempty_bar(as), aphase ^ 1); if (tr) tr_acc1 += clock64() - t0; }
-      ptx::tc_fence_after();
-      const uint32_t d_tmem = tmem_base + as * C::ACC_COLS;
-      for (int k = 0; k < k_iters; ++k) {
-        { const long long t0 = tr ? clock64() : 0; ptx::mbar_wait(full_bar(stage), phase); if (tr) tr_acc0 += clock64() - t0; }
-        ptx::tc_fence_after();
-        const uint32_t sa = smem_base + stage * C::STAGE_BYTES;
-        const uint32_t sb = sa + A_STAGE_BYTES;
-        const uint64_t adesc = ptx::make_sw128_kmajor_desc(sa);
-        const uint64_t bdesc = ptx::make_sw128_kmajor_desc(sb);
-#pragma unroll
-        for (int kk = 0; kk < BLOCK_K / UMMA_K; ++kk) {
-          // advance 16 bf16 = 32 B inside the 128B swizzle row: +2 in the (addr >> 4) field
-          ptx::tc_mma_bf16(d_tmem, adesc + 2u * kk, bdesc + 2u * kk, idesc, (k | kk) != 0 ? 1u : 0u);
-        }
-        ptx::tc_commit(empty_bar(stage));  // smem slot reusable once these MMAs retire
-        if (++stage == C::STAGES) { stage = 0; phase ^= 1; }
-      }
-      ptx::tc_commit(tfull_bar(as));  // accumulator complete
-    }
-  } else if (warp >= 4 && (kStaged || warp < 8)) {
-    // ================= epilogue =================
-    const int ew = warp - 4;
-    int it = 0;
-    for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x, ++it) {
+    for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
       const int n_tile = p.n_major ? tile / p.m_tiles : tile % p.n_tiles;
       const int m_tile = p.n_major ? tile % p.m_tiles : tile / p.n_tiles;
-      const int as = it & 1;
-      const uint32_t aphase = (it >> 1) & 1;
+      float acc[BLOCK_N / 2];
+#pragma unroll
+      for (int i = 0; i < BLOCK_N / 2; ++i) acc[i] = 0.f;
+      int prev_stage = -1;
+      for (int k = 0; k < k_iters; ++k) {
+        { const long long t0 = tr_me ? clock64() : 0; ptx::mbar_wait_nocall(full_bar(stage), phase); if (tr_me) tr_acc0 += clock64() - t0; }
+        const uint32_t sa = ring_base + stage * C::STAGE_BYTES + wg * (A_STAGE_BYTES / 2);
+        const uint32_t sb = ring_base + stage * C::STAGE_BYTES + C::A_BYTES;
+        ptx::wgmma_fence();
+        // X3: (A lo, W hi), (A hi, W lo), (A hi, W hi) -- small terms first; otherwise the single (A, W) product
+#pragma unroll
+        for (int q = 0; q < (X3 ? 3 : 1); ++q) {
+          const uint32_t a_off = (X3 && q == 0) ? A_STAGE_BYTES : 0u;
+          const uint32_t b_off = (X3 && q == 1) ? C::B_TILE_BYTES : 0u;
+          const uint64_t adesc = ptx::make_sw128_kmajor_desc(sa + a_off);
+          const uint64_t bdesc = ptx::make_sw128_kmajor_desc(sb + b_off);
+#pragma unroll
+          for (int kk = 0; kk < BLOCK_K / MMA_K; ++kk) {
+            // advance 16 bf16 = 32 B inside the 128B swizzle row: +2 in the (addr >> 4) field
+            ptx::Wgmma<BLOCK_N>::mma(acc, adesc + 2u * kk, bdesc + 2u * kk, (k | q | kk) != 0 ? 1u : 0u);
+          }
+        }
+        ptx::wgmma_commit();
+        // the previous stage's MMAs have retired once at most this stage's group is in flight: release that slot
+        ptx::wgmma_wait<1>();
+        if (prev_stage >= 0 && wl == 0 && lane == 0) ptx::mbar_arrive(empty_bar(prev_stage));
+        prev_stage = stage;
+        if (++stage == C::STAGES) { stage = 0; phase ^= 1; }
+      }
+      ptx::wgmma_wait<0>();
+      if (prev_stage >= 0 && wl == 0 && lane == 0) ptx::mbar_arrive(empty_bar(prev_stage));
+
       if (kStaged && EPI != EPI_GNSTATS && !p.use_tma_store) {
-        // this warp's bias (and layer-scale gamma) segment -> its shared-memory slot, before the accumulator wait
+        // this warp's bias (and layer-scale gamma) segment -> its shared-memory slot
         float* sbw = reinterpret_cast<float*>(stage_base + ew * EPI_STAGE_BYTES + 32 * EPI_STAGE_PITCH + 256);
         const int cb = n_tile * BLOCK_N + (ew >> 2) * (BLOCK_N / 2) + lane * 4;
         if (lane * 4 < BLOCK_N / 2) {
@@ -193,52 +202,36 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) gemm_tc_kernel(const __grid_co
         }
         __syncwarp();
       }
-      if (kStaged && EPI == EPI_RESID && !p.resid_reduce) {
-        // the residual rows of this tile are not produced by the MMAs: pull them into L2 while the mainloop runs
-        const RowInfo pri = map_row(p, m_tile, (ew & 3) * 32 + lane);
-        if (pri.valid) {
-          const float* rp = p.resid + pri.orow * p.ldo + n_tile * BLOCK_N + (ew >> 2) * (BLOCK_N / 2);
+      long long t0 = tr_me ? clock64() : 0;
+      // the previous tile's epilogue has finished reading the accumulator tile
+      ptx::named_bar_sync(BAR_ACC, CONSUMER_THREADS);
+      {
+        const int r0 = wg * 64 + wl * 16 + (lane >> 2);
+        const int c0 = (lane & 3) * 2;
 #pragma unroll
-          for (int b = 0; b < (BLOCK_N / 2) * 4; b += 128)
-            asm volatile("prefetch.global.L2 [%0];" ::"l"(reinterpret_cast<const uint8_t*>(rp) + b));
+        for (int j = 0; j < BLOCK_N / 8; ++j) {
+          *reinterpret_cast<float2*>(acc_smem + acc_index<BLOCK_N>(r0, j * 8 + c0)) = make_float2(acc[4 * j], acc[4 * j + 1]);
+          *reinterpret_cast<float2*>(acc_smem + acc_index<BLOCK_N>(r0 + 8, j * 8 + c0)) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
         }
       }
-      long long t0 = tr ? clock64() : 0;
-      ptx::mbar_wait(tfull_bar(as), aphase);
-      if (tr) { const long long t1 = clock64(); tr_acc0 += t1 - t0; t0 = t1; }
-      ptx::tc_fence_after();
+      ptx::named_bar_sync(BAR_ACC, CONSUMER_THREADS);
+      if (tr_me) { const long long t1 = clock64(); tr_acc1 += t1 - t0; }
       if constexpr (kStaged) {
-        epilogue_tile_staged<BLOCK_N, EPI>(p, m_tile, n_tile, tmem_base + as * C::ACC_COLS, ew, lane,
-                                           stage_base + ew * EPI_STAGE_BYTES);
-      } else {
-        const uint32_t tmem_row = tmem_base + ((uint32_t)((ew & 3) * 32) << 16) + as * C::ACC_COLS;
-        epilogue_tile<BLOCK_N, EPI>(p, m_tile, n_tile, tmem_row, lane, stage_base + (ew & 3) * EPI_STAGE_BYTES);
+        epilogue_tile_staged<BLOCK_N, EPI>(p, m_tile, n_tile, 0u, ew, lane, stage_base + ew * EPI_STAGE_BYTES);
+      } else if (ew < 4) {
+        const uint32_t acc_row = (uint32_t)(ew * 32) << 16;
+        epilogue_tile<BLOCK_N, EPI>(p, m_tile, n_tile, acc_row, lane, stage_base + ew * EPI_STAGE_BYTES);
       }
-      ptx::tc_fence_before();
-      __syncwarp();
-      if (lane == 0) ptx::mbar_arrive(tempty_bar(as));
-      if (tr) tr_acc1 += clock64() - t0;
     }
-    if (tr && ew == 0 && lane == 0) { p.trace[3] = tr_acc0; p.trace[4] = tr_acc1; }
+    if (tr_me) { p.trace[1] = tr_acc0; p.trace[3] = tr_acc1; }
     if (lane == 0) ptx::bulk_wait0();  // outstanding TMA stores (no-op when none were issued)
-  }
-  if (tr && lane == 0) {
-    if (warp == 0) { p.trace[0] = tr_acc0; p.trace[6] = clock64() - tr_start; p.trace[7] = (total_tiles - 1 - (int)blockIdx.x) / (int)gridDim.x + 1; }
-    if (warp == 1) { p.trace[1] = tr_acc0; p.trace[2] = tr_acc1; }
-  }
-
-  ptx::tc_fence_before();
-  __syncthreads();
-  if (warp == 2) {
-    ptx::tc_fence_after();
-    ptx::tmem_dealloc(tmem_base, C::TMEM_COLS);
   }
 }
 
-template <int BLOCK_N, int EPI>
+template <int BLOCK_N, int EPI, bool X3 = false>
 int launch_inst(const GemmPlan& plan, cudaStream_t stream) {
-  using C = Cfg<BLOCK_N>;
-  auto kfn = gemm_tc_kernel<BLOCK_N, EPI>;
+  using C = Cfg<BLOCK_N, X3>;
+  auto kfn = gemm_tc_kernel<BLOCK_N, EPI, X3>;
   GDRN_OPT_IN_SMEM(kfn, C::SMEM_BYTES);
   int total = plan.m_tiles * plan.n_tiles;
   if (total <= 0) return GDRN_OK;
@@ -260,39 +253,25 @@ int gemm_tc_launch(const GemmPlan& plan_in, int block_n, cudaStream_t stream) {
   GDRN_REQUIRE(plan.a_rank == 2 || plan.a_rank == 4 || plan.a_rank == 5, "gemm: bad a_rank");
   plan.use_tma_store = 0;
   plan.resid_reduce = 0;
-  if (plan.split && !plan.x3_expanded) {
-    // split-bf16 (x3): taps[] lists the hi operands; either the CTA-pair kernel that shares {A hi, A lo, W hi, W lo}
-    // between the three products of a stage, or the general kernel with a 3x longer tap list.
+  if (block_n > 128) {
+    // 128 x 256 tiles would need a 128 KB accumulator tile next to the operand ring: run them as two 128-wide tiles
+    GDRN_REQUIRE(plan.b_ptr != nullptr, "gemm: block_n 256 needs plan.b_ptr to re-tile W");
+    const uint64_t dims[2] = {(uint64_t)plan.b_ktot, (uint64_t)plan.b_rows};
+    const uint64_t str[1] = {(uint64_t)plan.b_ktot * 2};
+    const uint32_t box[2] = {64, 128};
+    int rc = make_tmap_bf16(&plan.tmap_b, plan.b_ptr, 2, dims, str, box);
+    if (rc != GDRN_OK) return rc;
+    block_n = 128;
+    plan.n_tiles = (plan.N + block_n - 1) / block_n;
+  }
+  // split-bf16 (x3): taps[] lists the hi operands.  64- / 128-wide tiles run the shared four-tile stage (X3 kernel); the
+  // other widths expand every tap to (A lo, W hi) + (A hi, W lo) + (A hi, W hi), small terms first.
+  static int x3_shared_on = -1;  // GDRN_X3_SHARED=0 forces the expanded tap list (A/B experiments)
+  if (x3_shared_on < 0) { const char* e = getenv("GDRN_X3_SHARED"); x3_shared_on = e ? atoi(e) : 1; }
+  const bool x3_shared = x3_shared_on && plan.split && !plan.x3_expanded && (block_n == 64 || block_n == 128) &&
+                         plan.epi != EPI_OUTCONV;
+  if (plan.split && !plan.x3_expanded && !x3_shared) {
     GDRN_REQUIRE(plan.num_taps >= 1 && 3 * plan.num_taps <= GEMM_MAX_TAPS, "gemm: bad num_taps (split)");
-    static int x3_pair = -1;  // GDRN_X3_PAIR=0 forces the general kernel (A/B experiments, parity cross-checks)
-    if (x3_pair < 0) { const char* e = getenv("GDRN_X3_PAIR"); x3_pair = e ? atoi(e) : 1; }
-    if (x3_pair && gemm_pair_x3_supported(plan, block_n)) {
-      {
-        const uint64_t dims[2] = {(uint64_t)plan.b_ktot, (uint64_t)plan.b_rows};
-        const uint64_t str[1] = {(uint64_t)plan.b_ktot * 2};
-        const uint32_t box[2] = {64, (uint32_t)block_n / 2};
-        int rc = make_tmap_bf16(&plan.tmap_b, plan.b_ptr, 2, dims, str, box);
-        if (rc != GDRN_OK) return rc;
-      }
-      if (plan.epi != EPI_GNSTATS) {
-        const bool f32 = plan.epi != EPI_GELU;
-        GDRN_REQUIRE(((uintptr_t)plan.out % 16 == 0) && ((plan.ldo * (f32 ? 4 : 2)) % 16 == 0) && plan.N % 64 == 0,
-                     "gemm (split): output not TMA-store compatible");
-        const uint64_t dims[2] = {(uint64_t)plan.ldo, (uint64_t)plan.M};
-        const uint64_t str[1] = {(uint64_t)plan.ldo * (f32 ? 4 : 2)};
-        const uint32_t box[2] = {32u, 32u};
-        // fp32: 32 x 128-byte swizzled staging rows; split bf16: two dense 32 x 64-byte tiles (hi, lo) per chunk
-        int rc = f32 ? make_tmap_store(&plan.tmap_out, plan.out, 1, dims, str, box)
-                     : make_tmap_store_plain(&plan.tmap_out, plan.out, 0, dims, str, box);
-        if (rc != GDRN_OK) return rc;
-        plan.use_tma_store = 1;
-        static int red = -1;
-        if (red < 0) { const char* e = getenv("GDRN_RESID_REDUCE"); red = e ? atoi(e) : 1; }
-        plan.resid_reduce = (red && plan.epi == EPI_RESID && plan.resid == plan.out) ? 1 : 0;
-      }
-      return gemm_pair_x3_launch(plan, block_n, stream);
-    }
-    // general kernel: every tap becomes (A lo, W hi) + (A hi, W lo) + (A hi, W hi), small terms first
     const int n = plan.num_taps;
     for (int t = n - 1; t >= 0; --t) {
       const GemmTap h = plan.taps[t];
@@ -322,35 +301,31 @@ int gemm_tc_launch(const GemmPlan& plan_in, int block_n, cudaStream_t stream) {
       plan.resid_reduce = (red && plan.epi == EPI_RESID && plan.resid == plan.out) ? 1 : 0;
     }
   }
-  GDRN_REQUIRE(plan.num_taps >= 1 && plan.num_taps <= GEMM_MAX_TAPS, "gemm: bad num_taps");
-  {
-    // CTA-pair path: rank-2, one tap, BLOCK_N = 256, TMA-store epilogue, enough tiles to fill the pairs
-    static int pair_on = -1;  // GDRN_GEMM_PAIR=0 disables (A/B experiments)
-    if (pair_on < 0) { const char* e = getenv("GDRN_GEMM_PAIR"); pair_on = e ? atoi(e) : 1; }
-    // measured (profiles/): the pair kernel wins when the mainloop dominates (K >= 1024: fc2, stage-3 fc1) and loses
-    // a few % on short-K tiles whose time is the GELU epilogue plus per-tile pair handshakes
-    static int gelu16 = -1;   // GDRN_GELU16=0: GELU GEMMs keep the 8-warp epilogue (and the K threshold below)
-    if (gelu16 < 0) { const char* e = getenv("GDRN_GELU16"); gelu16 = e ? atoi(e) : 1; }
-    static int pair_min_k = -1;
-    if (pair_min_k < 0) { const char* e = getenv("GDRN_GEMM_PAIR_MIN_KCHUNKS"); pair_min_k = e ? atoi(e) : 16; }
-    if (pair_on && plan.use_tma_store && block_n == 256 && plan.num_taps == 1 && plan.taps[0].c0 == 0 &&
-        plan.taps[0].d1 == 0 && plan.taps[0].b_off == 0 && plan.b_ptr != nullptr && plan.N % 256 == 0 &&
-        (plan.epi == EPI_GELU || plan.epi == EPI_RESID || plan.epi == EPI_STORE) && plan.M >= 256 * 16 &&
-        (plan.k_chunks >= pair_min_k || (plan.epi == EPI_GELU && gelu16))) {
-      const uint64_t dims[2] = {(uint64_t)plan.b_ktot, (uint64_t)plan.b_rows};
-      const uint64_t str[1] = {(uint64_t)plan.b_ktot * 2};
-      const uint32_t box[2] = {64, 128};
-      int rc = make_tmap_bf16(&plan.tmap_b, plan.b_ptr, 2, dims, str, box);
-      if (rc != GDRN_OK) return rc;
-      return gemm_pair_launch(plan, (plan.epi == EPI_GELU && gelu16) ? 16 : 8, stream);
-    }
+  if (x3_shared && plan.epi == EPI_GELU && plan.a_rank == 2 && plan.N % 64 == 0 && ((uintptr_t)plan.out % 16 == 0) &&
+      ((plan.ldo * 2) % 16 == 0)) {
+    // split-bf16 GELU output [hi N | lo N]: two dense 32 x 64-byte tiles per 32-column chunk, TMA-stored
+    const uint64_t dims[2] = {(uint64_t)plan.ldo, (uint64_t)plan.M};
+    const uint64_t str[1] = {(uint64_t)plan.ldo * 2};
+    const uint32_t box[2] = {32u, 32u};
+    int rc = make_tmap_store_plain(&plan.tmap_out, plan.out, 0, dims, str, box);
+    if (rc != GDRN_OK) return rc;
+    plan.use_tma_store = 1;
   }
+  GDRN_REQUIRE(plan.num_taps >= 1 && plan.num_taps <= GEMM_MAX_TAPS, "gemm: bad num_taps");
+#define GDRN_GEMM_CASE_X3(BN, E) \
+  if (x3_shared && block_n == BN && plan.epi == E) return launch_inst<BN, E, true>(plan, stream);
+  GDRN_GEMM_CASE_X3(128, EPI_GELU)
+  GDRN_GEMM_CASE_X3(128, EPI_RESID)
+  GDRN_GEMM_CASE_X3(128, EPI_STORE)
+  GDRN_GEMM_CASE_X3(128, EPI_GNSTATS)
+  GDRN_GEMM_CASE_X3(128, EPI_BIAS_LN)
+  GDRN_GEMM_CASE_X3(64, EPI_GELU)
+  GDRN_GEMM_CASE_X3(64, EPI_RESID)
+  GDRN_GEMM_CASE_X3(64, EPI_STORE)
+  GDRN_GEMM_CASE_X3(64, EPI_GNSTATS)
+#undef GDRN_GEMM_CASE_X3
 #define GDRN_GEMM_CASE(BN, E) \
   if (block_n == BN && plan.epi == E) return launch_inst<BN, E>(plan, stream);
-  GDRN_GEMM_CASE(256, EPI_GELU)
-  GDRN_GEMM_CASE(256, EPI_RESID)
-  GDRN_GEMM_CASE(256, EPI_STORE)
-  GDRN_GEMM_CASE(256, EPI_GNSTATS)
   GDRN_GEMM_CASE(128, EPI_GELU)
   GDRN_GEMM_CASE(128, EPI_RESID)
   GDRN_GEMM_CASE(128, EPI_STORE)

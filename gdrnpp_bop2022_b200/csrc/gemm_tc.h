@@ -1,6 +1,6 @@
-// Internal C++ interface of the tcgen05/TMA implicit-GEMM kernel (gemm_tc.cu).
+// Internal C++ interface of the wgmma/TMA implicit-GEMM kernel (gemm_tc.cu).
 //
-//   D[m, n] = sum_{tap} sum_{k} A_tap[m, k] * W[n, tap.b_off + k]      (bf16 x bf16 -> fp32 in TMEM)
+//   D[m, n] = sum_{tap} sum_{k} A_tap[m, k] * W[n, tap.b_off + k]      (bf16 x bf16 -> fp32)
 //
 // A rows are pixels of an NHWC activation tensor: a 128-row tile is a (bw x bh x bb) box of pixels
 // fetched by one TMA box load per (tap, 64-channel chunk); conv padding = TMA out-of-bounds zero fill.
@@ -40,7 +40,7 @@ struct GemmPlan {
   // ---- B operand ----
   CUtensorMap tmap_b;   // 2D [rows][K_total] bf16, K-major
   int b_rows_per_class; // EPI_OUTCONV: row offset multiplier for the ROI class (0 otherwise)
-  const void* b_ptr;    // W base / rows / row length (elements): lets gemm_tc_launch re-tile W for the CTA-pair kernel
+  const void* b_ptr;    // W base / rows / row length (elements): lets gemm_tc_launch re-tile W for 128-wide tiles
   long long b_rows, b_ktot;
   // ---- problem ----
   int m_tiles, n_tiles;
@@ -55,20 +55,12 @@ struct GemmPlan {
                         // [hi | lo] pairs (row width 2N, lo = bf16(v - hi))
   int x3_a_lo;          // split: offset of the lo half in A's coordinate 0 (channels / K); taps[] list the hi operands only
   int x3_b_lo;          // split: offset of the lo half inside a row of W (elements)
-  int x3_collect;       // pair kernel: A_hi read once per k-step through the A collector (set by gemm_pair_x3_launch; GDRN_X3_COLLECT)
-  int x3_expanded;      // set by gemm_tc_launch once taps[] has been expanded to the three products (general kernel)
+  int x3_expanded;      // set by gemm_tc_launch once taps[] has been expanded to the three products
   void* out;            // [rows, ldo]
   CUtensorMap tmap_out; // rank-2 outputs: store map (filled by gemm_tc_launch when use_tma_store)
   int use_tma_store;    // set by gemm_tc_launch
   int resid_reduce;     // set by gemm_tc_launch: EPI_RESID in place -> TMA reduce-add (x += gamma*(acc+bias)), x is never read by the SM
   long long ldo;        // output row stride (elements)
-  // pair-x3 kernel, in-place EPI_RESID only: balanced k-split schedule (every CTA pair gets one contiguous, equally long
-  // range of (tile, k-iteration) units instead of whole tiles; partial tiles meet in the L2 reduce-add).  sk_flags =
-  // zeroed device words, one per (tile, CTA of the pair, epilogue warp): order the partial reduce-adds of a tile (highest
-  // k range first) so that the result does not depend on timing; the last writer leaves its word at zero again.
-  unsigned* sk_flags;   // null: whole tiles only
-  int sk_flag_words;    // capacity of sk_flags
-  int streamk;          // set by gemm_pair_x3_launch
   int OH, OW, osy, osx, ooy, oox;  // rank 4/5: out row = (b*OH + y*osy+ooy)*OW + x*osx+oox
   const float* bias;    // [N] or null
   const float* gamma;   // EPI_RESID [N]
@@ -85,29 +77,18 @@ struct GemmPlan {
   const float* roi_extents;      // [B,3]
   const float* roi_coord_2d;     // [B,2,64,64] fp32 NCHW
   void* pnp_in;                  // bf16 [B*4096, 128]
-  // debug: CTA 0 writes [0] producer empty-wait, [1] MMA full-wait, [2] MMA accumulator-wait, [3] epilogue warp 0
-  // accumulator-wait, [4] epilogue warp 0 busy, [6] CTA cycles, [7] tiles of CTA 0 (clock64 cycles)
+  // debug: CTA 0 writes [0] producer empty-wait, [1] consumer full-wait, [3] accumulator hand-over, [6] CTA cycles,
+  // [7] tiles of CTA 0, [8..10] epilogue warp 0 accumulator loads / compute / flush (clock64 cycles)
   long long* trace;
   float* map_mask; float* map_full; float* map_x; float* map_y; float* map_z; float* map_region;  // NCHW or null
 };
 
-// block_n in {16, 64, 80, 128, 256}
+// block_n in {16, 64, 80, 128, 256} (256: run as 128-wide tiles)
 int gemm_tc_launch(const GemmPlan& plan, int block_n, cudaStream_t stream);
 
-// CTA-pair (cta_group::2) kernel for rank-2, single-tap, BLOCK_N = 256 plans (gemm_pair.cu); called by gemm_tc_launch,
-// which also re-tiles plan.tmap_b to 128-row boxes.  epi_warps = 8 or 16 (16: EPI_GELU only).
-int gemm_pair_launch(const GemmPlan& plan, int epi_warps, cudaStream_t stream);
-
-// CTA-pair split-bf16 kernel (gemm_pair_x3.cu): every shared-memory stage holds {A hi, A lo, W hi, W lo} of one
-// (tap, k-chunk) and feeds the three products A_lo*W_hi + A_hi*W_lo + A_hi*W_hi -- 4 operand tiles per 3 MMA groups
-// instead of 6.  rank 2/4/5 A, any tap list; block_n in {128, 256}; epilogues GELU (split out), RESID / STORE (fp32,
-// TMA store / reduce-add), GNSTATS (fp32).  Called by gemm_tc_launch.
-int gemm_pair_x3_supported(const GemmPlan& plan, int block_n);
-int gemm_pair_x3_launch(const GemmPlan& plan, int block_n, cudaStream_t stream);
-
-// Fused ConvNeXt MLP block (C = 128): x += gamma * (W2 . gelu(W1 . A + b1) + b2), hidden activation kept on chip.
-// A bf16 [M, C]; W1 bf16 [4C, C]; W2 bf16 [C, 4C]; x fp32 [M, C] updated in place.
-// split-bf16 (parity mode) twin, mlp_fused_x3.cu: A [M,2C], W1 [4C,2C], W2 [C,8C] hold [hi | lo] halves
+// Fused ConvNeXt MLP block (C = 128, mlp_fused.cu): x += gamma * (W2 . gelu(W1 . A + b1) + b2), hidden activation kept on
+// chip.  A bf16 [M, C]; W1 bf16 [4C, C]; W2 bf16 [C, 4C]; x fp32 [M, C] updated in place.
+// split-bf16 (parity mode) twin: A [M,2C], W1 [4C,2C], W2 [C,8C] hold [hi | lo] halves
 int mlp_fused_x3_supported(int C, long long M);
 int mlp_fused_x3_launch(const void* A, const void* W1, const float* b1, const void* W2, const float* b2, const float* gamma,
                         float* x, long long M, int C, cudaStream_t stream);

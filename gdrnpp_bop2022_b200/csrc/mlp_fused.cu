@@ -1,319 +1,273 @@
-// Fused ConvNeXt MLP block kernel (fc1 -> GELU -> fc2 -> residual on chip); see the banner below and DESIGN.md 3.1.
+// Fused ConvNeXt MLP block (stage 0, C = 128): x += gamma * (W2 . gelu(W1 . A + b1) + b2) with the 4C-wide hidden
+// activation kept on chip (wgmma + TMA, sm_90a).  Reference op: timm ConvNeXtBlock.mlp (Linear C->4C, GELU, Linear 4C->C)
+// * gamma + shortcut (timm 0.6.7, un-vendored), called from models/GDRN_double_mask.py:102 through the backbone.
+//
+// One persistent CTA per SM, 384 threads: warp 0 lane 0 is the TMA producer, warps 4..11 are two consumer warpgroups
+// (rows [0, 64) and [64, 128) of a 128-row tile).  Per tile the A rows stay resident in shared memory and the 512 hidden
+// columns are processed in eight chunks of 64:
+//   fc1   h[64 x 64] = A . W1[chunk]^T                      (wgmma, registers)
+//         + b1, GELU, bf16 -> the warpgroup's rows of the H tile in shared memory, written directly in the
+//         128B-swizzled K-major operand layout the TMA would produce
+//   fc2   o[64 x 128] += H . W2[:, chunk]^T                  (wgmma, H tile as the A operand, accumulator in registers)
+// and after the last chunk every thread adds gamma * (o + b2) to its x elements.  Weight chunks {W1 rows, W2 columns}
+// stream through a ring of stages; the weights (256 KB, 512 KB split) stay in L2 across tiles.
+// X3 (split-bf16 parity mode): A [M, 2C], W1 [4C, 2C], W2 [C, 8C] hold [hi | lo] halves; every contraction is the three
+// products lo.hi + hi.lo + hi.hi of one k-chunk (the order of the X3 GEMM kernel), GELU is the exact erf form and the
+// hidden activation is stored as its hi / lo bf16 pair -- the same arithmetic as the two-GEMM path.
 #include <stdio.h>
 #include <stdlib.h>
 #include <string.h>
+#include "gemm_tc.h"
 #include "gemm_epilogue.cuh"
+#include "wgmma.cuh"
 
 namespace {
 
-// ================================================================================================================
-// Fused ConvNeXt MLP for the wide-and-shallow stage (C = 128):  x += gamma * (W2 . gelu(W1 . a + b1) + b2)
-// in ONE kernel per block; the 4C-wide hidden activation never leaves the SM.  Unfused, stage 0 writes and re-reads a
-// 268 MB bf16 `Hb` per block (fc1 HBM-write bound, fc2 HBM-read bound: 190 us for 69 GFLOP).
-// One persistent CTA per SM; per 128-row tile the hidden dimension is processed in four rounds of 128 columns, software
-// pipelined over a flat sequence of global rounds G (tile boundaries included):
-//   MMA-1(G)  H[G&1][128x128] = A[128xC] . W1[r]^T                   TMEM columns [ (G&1)*128, +128 )
-//   E1(G)     8 warps: tcgen05.ld -> +b1 -> GELU -> bf16 -> A'[G&1] in shared memory, written directly in the
-//             128B-swizzled K-major UMMA operand layout (16-byte piece j of row r at j ^ (r & 7))
-//   MMA-2(G)  O[ob][128xC]   += A'[G&1][128x128] . W2[:, r]^T        TMEM columns [ 256 + ob*128, +128 )
-//   E2        after round 3: gamma*(O+b2) -> staging -> TMA reduce-add into x  (epilogue_tile_tma)
-// The MMA thread issues MMA-1(G+1) BEFORE it waits for A'(G): the tensor core, the weight stream (ring of 32 KB slots
-// in consumption order W1(0), {W1(G+1), W2(G)}...) and the A-tile load of the next row block all run underneath E1,
-// which is the critical path (GELU at ~0.5 IPC on 8 warps).  H, A' and O are double-buffered.
-// ================================================================================================================
-struct MlpFusedPlan {
-  GemmPlan g;            // fields used by E2: tmap_out, M, N (= C), bias (= b2), gamma, resid/out (= x), ldo, resid_reduce
-  CUtensorMap tmap_a;    // A   [M, C]   bf16, box {64, 128}
-  CUtensorMap tmap_w1;   // W1  [4C, C]  bf16, box {64, 128}
-  CUtensorMap tmap_w2;   // W2  [C, 4C]  bf16, box {64, 128}
+constexpr int MF_C = 128;
+constexpr int MF_HC = 64;                         // hidden columns per chunk
+constexpr int MF_CHUNKS = 4 * MF_C / MF_HC;       // 8
+constexpr int MF_KC1 = MF_C / BLOCK_K;            // k-chunks of fc1 (2)
+constexpr int MF_W1_TILE = MF_HC * BLOCK_K * 2;   // 64 rows x 64 k: 8 KB
+constexpr int MF_W2_TILE = MF_C * BLOCK_K * 2;    // 128 rows x 64 k: 16 KB
+
+struct MlpPlan {
+  CUtensorMap tmap_a;    // A  [M, S*C]   bf16, box {64, 128}
+  CUtensorMap tmap_w1;   // W1 [4C, S*C]  bf16, box {64, 64}
+  CUtensorMap tmap_w2;   // W2 [C, S*4C]  bf16, box {64, 128}
   const float* b1;       // [4C]
+  const float* b2;       // [C]
+  const float* gamma;    // [C]
+  float* x;              // [M, C] fp32, updated in place
   int m_tiles;
 };
 
-constexpr int MF_SLOT_BYTES = 32768;
-constexpr int MF_SLOTS = 3;
+template <bool X3>
+struct MfCfg {
+  static constexpr int S = X3 ? 2 : 1;
+  static constexpr int A_BYTES = S * MF_KC1 * A_STAGE_BYTES;            // 32 / 64 KB
+  static constexpr int H_BYTES = S * A_STAGE_BYTES;                     // 128 rows x 64 hidden columns: 16 / 32 KB
+  static constexpr int STAGE_BYTES = S * (MF_KC1 * MF_W1_TILE + MF_W2_TILE);
+  static constexpr int RING = (227 * 1024 - 1024 - 256 - A_BYTES - H_BYTES) / STAGE_BYTES;
+  static constexpr int STAGES = RING > 6 ? 6 : RING;
+  static constexpr int SMEM_BYTES = A_BYTES + H_BYTES + STAGES * STAGE_BYTES + 1024 + 256;
+  static_assert(STAGES >= 2, "fused MLP: shared-memory ring needs two stages");
+};
 
-template <int C>
-__global__ void __launch_bounds__(NUM_THREADS, 1) mlp_fused_kernel(const __grid_constant__ MlpFusedPlan fp) {
-  static_assert(C == 128, "fused MLP: only C = 128 is instantiated");
-  constexpr int KC1 = C / 64;                 // k-chunks of fc1 (2)
-  constexpr int ROUNDS = 4 * C / 128;         // hidden rounds of 128 columns (4)
-  constexpr int A_BYTES = KC1 * A_STAGE_BYTES;            // 32 KB
-  constexpr int AP_BYTES = 2 * A_STAGE_BYTES;             // one A' buffer: 128 rows x 128 hidden columns
-  constexpr int CHUNK_BYTES = 128 * BLOCK_K * 2;          // a 128-row x 64-k weight chunk (16 KB); two per slot
-  constexpr int O_COL = 256;
-  const GemmPlan& p = fp.g;
-  extern __shared__ uint8_t smem_raw[];
-  const uint32_t smem_base = (ptx::smem_u32(smem_raw) + 1023u) & ~1023u;
-  uint8_t* smem_gen = smem_raw + (smem_base - ptx::smem_u32(smem_raw));
-  // layout: [A][A' x2][ring][E2 staging 8 x 4 KB][barriers]
-  const uint32_t a_smem = smem_base;
-  const uint32_t ap_smem = a_smem + A_BYTES;
-  const uint32_t ring_smem = ap_smem + 2 * AP_BYTES;
-  const uint32_t stg_off = A_BYTES + 2 * AP_BYTES + MF_SLOTS * MF_SLOT_BYTES;
-  const uint32_t bar_base = smem_base + stg_off + NUM_EPI_WARPS * EPI_STAGE_BYTES;
-  enum { B_AFULL = 0, B_AEMPTY = 1, B_HFULL = 2, B_HEMPTY = 4, B_APFULL = 6, B_APEMPTY = 8, B_OFULL = 10, B_OEMPTY = 12,
-         B_RFULL = 14, B_REMPTY = B_RFULL + MF_SLOTS, B_END = B_REMPTY + MF_SLOTS };
-  auto bar = [&](int i) { return bar_base + 8u * i; };
-  const uint32_t tmem_slot = bar_base + 8u * B_END;
-  volatile uint32_t* tmem_slot_ptr =
-      reinterpret_cast<volatile uint32_t*>(smem_gen + stg_off + NUM_EPI_WARPS * EPI_STAGE_BYTES + 8 * B_END);
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+// byte offset of bf16 element (r, c) in a 128B-swizzled K-major tile of 64-column rows (the TMA SWIZZLE_128B layout)
+__device__ __forceinline__ uint32_t sw128_off(int r, int c) {
+  return (uint32_t)((r >> 3) * 1024 + (r & 7) * 128 + ((((c >> 3) ^ (r & 7)) & 7) << 4) + (c & 7) * 2);
+}
+
+template <bool X3>
+__global__ void __launch_bounds__(NUM_THREADS, 1) mlp_fused_kernel(const __grid_constant__ MlpPlan fp) {
+  using C = MfCfg<X3>;
+  const uint32_t smem_base = (ptx::smem_u32(gemm_smem) + 1023u) & ~1023u;
+  uint8_t* smem_gen = gemm_smem + (smem_base - ptx::smem_u32(gemm_smem));
+  const uint32_t a_base = smem_base;                       // [h][kc] tiles of 128 rows x 64 k
+  const uint32_t h_base = a_base + C::A_BYTES;             // [h] tiles of 128 rows x 64 hidden columns
+  const uint32_t ring_base = h_base + C::H_BYTES;          // stage: [h][kc] W1 tiles, then [h] W2 tiles
+  const uint32_t bar_base = ring_base + C::STAGES * C::STAGE_BYTES;
+  auto full_bar = [&](int s) { return bar_base + 8u * s; };
+  auto empty_bar = [&](int s) { return bar_base + 8u * (C::STAGES + s); };
+  const uint32_t a_full = bar_base + 8u * (2 * C::STAGES);
+  const uint32_t a_empty = a_full + 8u;
+
+  const int warp = threadIdx.x >> 5;
+  const int lane = threadIdx.x & 31;
   ptx::griddep_launch();
   if (warp == 0 && lane == 0) {
-    ptx::prefetch_tmap(&fp.tmap_a); ptx::prefetch_tmap(&fp.tmap_w1); ptx::prefetch_tmap(&fp.tmap_w2);
-    ptx::prefetch_tmap(&p.tmap_out);
+    ptx::prefetch_tmap(&fp.tmap_a);
+    ptx::prefetch_tmap(&fp.tmap_w1);
+    ptx::prefetch_tmap(&fp.tmap_w2);
   }
   if (warp == 1 && lane == 0) {
-    ptx::mbar_init(bar(B_AFULL), 1); ptx::mbar_init(bar(B_AEMPTY), 1);
-    for (int i = 0; i < 2; ++i) {
-      ptx::mbar_init(bar(B_HFULL + i), 1); ptx::mbar_init(bar(B_HEMPTY + i), NUM_EPI_WARPS);
-      ptx::mbar_init(bar(B_APFULL + i), NUM_EPI_WARPS); ptx::mbar_init(bar(B_APEMPTY + i), 1);
-      ptx::mbar_init(bar(B_OFULL + i), 1); ptx::mbar_init(bar(B_OEMPTY + i), NUM_EPI_WARPS);
+    for (int s = 0; s < C::STAGES; ++s) {
+      ptx::mbar_init(full_bar(s), 1);
+      ptx::mbar_init(empty_bar(s), 2);   // one arrive per consumer warpgroup
     }
-    for (int s = 0; s < MF_SLOTS; ++s) { ptx::mbar_init(bar(B_RFULL + s), 1); ptx::mbar_init(bar(B_REMPTY + s), 1); }
+    ptx::mbar_init(a_full, 1);
+    ptx::mbar_init(a_empty, 2);
     ptx::fence_barrier_init();
   }
-  if (warp == 2) {
-    ptx::tmem_alloc(tmem_slot, 512);
-    ptx::tmem_relinquish();
-  }
-  ptx::tc_fence_before();
   __syncthreads();
-  ptx::tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot_ptr;
   ptx::griddep_wait();
-  const int my_tiles = (int)blockIdx.x < fp.m_tiles ? (fp.m_tiles - 1 - (int)blockIdx.x) / (int)gridDim.x + 1 : 0;
-  const uint32_t total_rounds = (uint32_t)my_tiles * ROUNDS;
-  const bool tr = p.trace != nullptr && blockIdx.x == 0;   // GDRN_MLP_TRACE: cycle accounting of CTA 0
-  long long tw[6] = {0, 0, 0, 0, 0, 0};
-  const long long tr_start = tr ? clock64() : 0;
-#define MF_TIMED_WAIT(slot_, b_, par_) do { const long long t0_ = tr ? clock64() : 0; ptx::mbar_wait((b_), (par_)); \
-                                            if (tr) tw[slot_] += clock64() - t0_; } while (0)
 
   if (warp == 0 && lane == 0) {
-    // ================= TMA producer: A(it), then slots in the MMA thread's consumption order =================
-    int slot = 0;
-    uint32_t sphase = 0;
-    auto load_w1 = [&](uint32_t G) {       // W1 rows [r*128, +128), both k-chunks -> one slot
-      const int r = (int)(G % ROUNDS);
-      ptx::mbar_wait(bar(B_REMPTY + slot), sphase ^ 1);
-      ptx::mbar_arrive_expect_tx(bar(B_RFULL + slot), MF_SLOT_BYTES);
-      for (int kc = 0; kc < KC1; ++kc)
-        ptx::tma_load_2d(ring_smem + slot * MF_SLOT_BYTES + kc * CHUNK_BYTES, &fp.tmap_w1, bar(B_RFULL + slot), kc * BLOCK_K, r * 128);
-      if (++slot == MF_SLOTS) { slot = 0; sphase ^= 1; }
-    };
-    auto load_w2 = [&](uint32_t G) {       // W2 all C rows, hidden k-chunks 2r, 2r+1 -> one slot
-      const int r = (int)(G % ROUNDS);
-      ptx::mbar_wait(bar(B_REMPTY + slot), sphase ^ 1);
-      ptx::mbar_arrive_expect_tx(bar(B_RFULL + slot), MF_SLOT_BYTES);
-      for (int c = 0; c < 2; ++c)
-        ptx::tma_load_2d(ring_smem + slot * MF_SLOT_BYTES + c * CHUNK_BYTES, &fp.tmap_w2, bar(B_RFULL + slot), (2 * r + c) * BLOCK_K, 0);
-      if (++slot == MF_SLOTS) { slot = 0; sphase ^= 1; }
-    };
-    auto load_a = [&](uint32_t it) {
-      const int tile = (int)blockIdx.x + (int)it * (int)gridDim.x;
-      ptx::mbar_wait(bar(B_AEMPTY), (it & 1u) ^ 1u);
-      ptx::mbar_arrive_expect_tx(bar(B_AFULL), A_BYTES);
-      for (int kc = 0; kc < KC1; ++kc)
-        ptx::tma_load_2d(a_smem + kc * A_STAGE_BYTES, &fp.tmap_a, bar(B_AFULL), kc * BLOCK_K, tile * BLOCK_M);
-    };
-    if (total_rounds > 0) {
-      load_a(0);
-      load_w1(0);
-      for (uint32_t G = 0; G < total_rounds; ++G) {
-        if (G + 1 < total_rounds) {
-          if ((G + 1) % ROUNDS == 0) load_a((G + 1) / ROUNDS);
-          load_w1(G + 1);
+    // ================= TMA producer =================
+    int stage = 0;
+    uint32_t phase = 0, aphase = 0;
+    for (int tile = blockIdx.x; tile < fp.m_tiles; tile += gridDim.x) {
+      ptx::mbar_wait_nocall(a_empty, aphase ^ 1);
+      ptx::mbar_arrive_expect_tx(a_full, C::A_BYTES);
+      for (int h = 0; h < C::S; ++h)
+        for (int kc = 0; kc < MF_KC1; ++kc)
+          ptx::tma_load_2d(a_base + (h * MF_KC1 + kc) * A_STAGE_BYTES, &fp.tmap_a, a_full, h * MF_C + kc * BLOCK_K,
+                           tile * BLOCK_M);
+      aphase ^= 1;
+      for (int j = 0; j < MF_CHUNKS; ++j) {
+        ptx::mbar_wait_nocall(empty_bar(stage), phase ^ 1);
+        const uint32_t sw = ring_base + stage * C::STAGE_BYTES;
+        ptx::mbar_arrive_expect_tx(full_bar(stage), C::STAGE_BYTES);
+        for (int h = 0; h < C::S; ++h) {
+          for (int kc = 0; kc < MF_KC1; ++kc)
+            ptx::tma_load_2d(sw + (h * MF_KC1 + kc) * MF_W1_TILE, &fp.tmap_w1, full_bar(stage), h * MF_C + kc * BLOCK_K,
+                             j * MF_HC);
+          ptx::tma_load_2d(sw + C::S * MF_KC1 * MF_W1_TILE + h * MF_W2_TILE, &fp.tmap_w2, full_bar(stage),
+                           h * 4 * MF_C + j * MF_HC, 0);
         }
-        load_w2(G);
+        if (++stage == C::STAGES) { stage = 0; phase ^= 1; }
       }
     }
-  } else if (warp == 1 && lane == 0) {
-    // ================= MMA issuer =================
-    constexpr uint32_t idesc = ptx::make_idesc_bf16(BLOCK_M, 128);
-    int slot = 0;
-    uint32_t sphase = 0;
-    auto mma1 = [&](uint32_t G) {
-      const uint32_t hb = G & 1u, n = G >> 1;
-      const int r = (int)(G % ROUNDS);
-      if (r == 0) MF_TIMED_WAIT(0, bar(B_AFULL), (G / ROUNDS) & 1u);
-      MF_TIMED_WAIT(1, bar(B_HEMPTY + hb), (n & 1u) ^ 1u);
-      MF_TIMED_WAIT(2, bar(B_RFULL + slot), sphase);
-      ptx::tc_fence_after();
-#pragma unroll
-      for (int kc = 0; kc < KC1; ++kc) {
-        const uint64_t adesc = ptx::make_sw128_kmajor_desc(a_smem + kc * A_STAGE_BYTES);
-        const uint64_t bdesc = ptx::make_sw128_kmajor_desc(ring_smem + slot * MF_SLOT_BYTES + kc * CHUNK_BYTES);
-#pragma unroll
-        for (int kk = 0; kk < BLOCK_K / UMMA_K; ++kk)
-          ptx::tc_mma_bf16(tmem_base + hb * 128, adesc + 2u * kk, bdesc + 2u * kk, idesc, (kc | kk) != 0 ? 1u : 0u);
-      }
-      ptx::tc_commit(bar(B_REMPTY + slot));
-      if (++slot == MF_SLOTS) { slot = 0; sphase ^= 1; }
-      if (r == ROUNDS - 1) ptx::tc_commit(bar(B_AEMPTY));   // A tile consumed
-      ptx::tc_commit(bar(B_HFULL + hb));
-    };
-    auto mma2 = [&](uint32_t G) {
-      const uint32_t hb = G & 1u, n = G >> 1;
-      const int r = (int)(G % ROUNDS);
-      const uint32_t it = G / ROUNDS, ob = it & 1u;
-      MF_TIMED_WAIT(3, bar(B_APFULL + hb), n & 1u);
-      if (r == 0) MF_TIMED_WAIT(4, bar(B_OEMPTY + ob), ((it >> 1) & 1u) ^ 1u);
-      MF_TIMED_WAIT(2, bar(B_RFULL + slot), sphase);
-      ptx::tc_fence_after();
-#pragma unroll
-      for (int c = 0; c < 2; ++c) {
-        const uint64_t adesc = ptx::make_sw128_kmajor_desc(ap_smem + hb * AP_BYTES + c * A_STAGE_BYTES);
-        const uint64_t bdesc = ptx::make_sw128_kmajor_desc(ring_smem + slot * MF_SLOT_BYTES + c * CHUNK_BYTES);
-#pragma unroll
-        for (int kk = 0; kk < BLOCK_K / UMMA_K; ++kk)
-          ptx::tc_mma_bf16(tmem_base + O_COL + ob * 128, adesc + 2u * kk, bdesc + 2u * kk, idesc, (r | c | kk) != 0 ? 1u : 0u);
-      }
-      ptx::tc_commit(bar(B_REMPTY + slot));
-      if (++slot == MF_SLOTS) { slot = 0; sphase ^= 1; }
-      ptx::tc_commit(bar(B_APEMPTY + hb));
-      if (r == ROUNDS - 1) ptx::tc_commit(bar(B_OFULL + ob));
-    };
-    if (total_rounds > 0) {
-      mma1(0);
-      for (uint32_t G = 0; G < total_rounds; ++G) {
-        if (G + 1 < total_rounds) mma1(G + 1);
-        mma2(G);
-      }
-    }
-    if (tr) { for (int i = 0; i < 5; ++i) p.trace[i] = tw[i]; p.trace[5] = clock64() - tr_start; p.trace[6] = my_tiles; }
   } else if (warp >= 4) {
-    // ================= epilogue warps: E1 per round, E2 per tile =================
+    // ================= consumers =================
     const int ew = warp - 4;
-    const int q = ew & 3, half = ew >> 2;      // TMEM lane quarter / 64-column half of the round = A' k-chunk
-    const int row = q * 32 + lane;
-    const int sw = row & 7;
-    uint8_t* ap_gen = smem_gen + A_BYTES;
-    uint32_t G = 0;
-    // E2 (x += gamma * (O + b2)) of a tile is issued one tile LATE, as two 128-byte-column groups interleaved with the
-    // E1 rounds of the next tile: by then O is long complete (no wait on the last MMA-2) and the TMA reduce-add of the
-    // previous group has long finished reading the staging buffer (the L2 reduce path sustains only ~16 B/clk per SM).
-    auto e2_group = [&](int jt, int grp) {
-      if (jt < 0) return;
-      const uint32_t job = (uint32_t)jt & 1u;
-      const long long te1 = tr ? clock64() : 0;
-      if (grp == 0) {
-        ptx::mbar_wait(bar(B_OFULL + job), ((uint32_t)jt >> 1) & 1u);
-        ptx::tc_fence_after();
-      }
-      const int jtile = (int)blockIdx.x + jt * (int)gridDim.x;
-      epilogue_tile_tma<C, EPI_RESID, true, NUM_EPI_WARPS>(p, jtile, 0, tmem_base + O_COL + job * 128, ew, lane,
-                                                           smem_gen + stg_off + ew * EPI_STAGE_BYTES, grp * 32, grp * 32 + 32);
-      if (grp == 1) {
-        ptx::tc_fence_before();
-        __syncwarp();
-        if (lane == 0) ptx::mbar_arrive(bar(B_OEMPTY + job));
-      }
-      if (tr) tw[4] += clock64() - te1;
-    };
-    for (int it = 0; it < my_tiles; ++it) {
-      for (int r = 0; r < ROUNDS; ++r, ++G) {
-        const uint32_t hb = G & 1u, n = G >> 1;
-        MF_TIMED_WAIT(0, bar(B_HFULL + hb), n & 1u);
-        MF_TIMED_WAIT(1, bar(B_APEMPTY + hb), (n & 1u) ^ 1u);   // MMA-2 that last read this A' buffer has retired
-        ptx::tc_fence_after();
-        const long long te0 = tr ? clock64() : 0;
-        const uint32_t tmem_row = tmem_base + hb * 128 + ((uint32_t)(q * 32) << 16) + half * 64;
-        uint4* dst = reinterpret_cast<uint4*>(ap_gen + hb * AP_BYTES + half * A_STAGE_BYTES + row * 128);
-        const float* b1 = fp.b1 + r * 128 + half * 64;
+    const int wg = ew >> 2;              // rows [64 wg, 64 wg + 64) of the tile
+    const int wl = ew & 3;
+    const int bar_id = 2 + wg;           // named barrier of this warpgroup (128 threads)
+    const bool leader = (wl == 0 && lane == 0);
+    int stage = 0;
+    uint32_t phase = 0, aphase = 0;
+    for (int tile = blockIdx.x; tile < fp.m_tiles; tile += gridDim.x) {
+      ptx::mbar_wait_nocall(a_full, aphase);
+      aphase ^= 1;
+      float o[MF_C / 2];
 #pragma unroll
-        for (int c = 0; c < 2; ++c) {
-          float v[32];
-          tmem_load_chunk<32>(tmem_row + c * 32, v);
+      for (int i = 0; i < MF_C / 2; ++i) o[i] = 0.f;
+      for (int j = 0; j < MF_CHUNKS; ++j) {
+        ptx::mbar_wait_nocall(full_bar(stage), phase);
+        const uint32_t sw = ring_base + stage * C::STAGE_BYTES;
+        // ---- fc1: h = A . W1[chunk]^T (X3: lo.hi + hi.lo + hi.hi per k-chunk) ----
+        float hacc[MF_HC / 2];
 #pragma unroll
-          for (int j = 0; j < 32; j += 8) {
-            const float4 ba = __ldg(reinterpret_cast<const float4*>(b1 + c * 32 + j));
-            const float4 bb = __ldg(reinterpret_cast<const float4*>(b1 + c * 32 + j + 4));
-            uint4 w;
-            w.x = gelu_pack2_f16(v[j] + ba.x, v[j + 1] + ba.y); w.y = gelu_pack2_f16(v[j + 2] + ba.z, v[j + 3] + ba.w);
-            w.z = gelu_pack2_f16(v[j + 4] + bb.x, v[j + 5] + bb.y); w.w = gelu_pack2_f16(v[j + 6] + bb.z, v[j + 7] + bb.w);
-            dst[((c * 4) + (j >> 3)) ^ sw] = w;
+        for (int i = 0; i < MF_HC / 2; ++i) hacc[i] = 0.f;
+        ptx::wgmma_fence();
+#pragma unroll
+        for (int kc = 0; kc < MF_KC1; ++kc) {
+#pragma unroll
+          for (int q = 0; q < (X3 ? 3 : 1); ++q) {
+            const int ah = (X3 && q == 0) ? 1 : 0, bh = (X3 && q == 1) ? 1 : 0;
+            const uint64_t ad = ptx::make_sw128_kmajor_desc(a_base + (ah * MF_KC1 + kc) * A_STAGE_BYTES + wg * (A_STAGE_BYTES / 2));
+            const uint64_t bd = ptx::make_sw128_kmajor_desc(sw + (bh * MF_KC1 + kc) * MF_W1_TILE);
+#pragma unroll
+            for (int kk = 0; kk < BLOCK_K / MMA_K; ++kk)
+              ptx::Wgmma<MF_HC>::mma(hacc, ad + 2u * kk, bd + 2u * kk, (kc | q | kk) != 0 ? 1u : 0u);
           }
         }
-        ptx::tc_fence_before();
-        ptx::fence_proxy_async();   // A' was written through the generic proxy, tcgen05.mma reads it through the async proxy
-        __syncwarp();
-        if (lane == 0) { ptx::mbar_arrive(bar(B_HEMPTY + hb)); ptx::mbar_arrive(bar(B_APFULL + hb)); }
-        if (tr) tw[2] += clock64() - te0;
-        if (r == 0) e2_group(it - 1, 0);   // two rounds apart: each 32 KB batch of reduce-adds drains (~16 B/clk) before the next
-        if (r == 2) e2_group(it - 1, 1);
+        ptx::wgmma_commit();
+        ptx::wgmma_wait<0>();
+        if (j == MF_CHUNKS - 1 && leader) ptx::mbar_arrive(a_empty);   // A of this tile is no longer read
+        // ---- + b1, GELU, bf16 (hi / lo) -> this warpgroup's rows of the H tile ----
+        ptx::named_bar_sync(bar_id, 128);    // the previous chunk's fc2 of the whole warpgroup has retired
+        {
+          const int r0 = wg * 64 + wl * 16 + (lane >> 2);
+          uint8_t* hgen = smem_gen + (h_base - smem_base);
+#pragma unroll
+          for (int t = 0; t < MF_HC / 8; ++t) {
+            const int c = t * 8 + (lane & 3) * 2;
+            const float2 b = __ldg(reinterpret_cast<const float2*>(fp.b1 + j * MF_HC + c));
+#pragma unroll
+            for (int half = 0; half < 2; ++half) {
+              const int r = r0 + 8 * half;
+              const float v0 = hacc[4 * t + 2 * half], v1 = hacc[4 * t + 2 * half + 1];
+              if constexpr (X3) {
+                f32x2_t v2 = gelu_erf2(f2_add(f2_pack(v0, v1), f2_pack(b.x, b.y)));
+                const float2 f = f2_unpack(v2);
+                const uint32_t hb = pack_bf16(f.x, f.y);
+                const float2 d = f2_unpack(f2_sub(v2, f2_pack(__uint_as_float(hb << 16), __uint_as_float(hb & 0xffff0000u))));
+                *reinterpret_cast<uint32_t*>(hgen + sw128_off(r, c)) = hb;
+                *reinterpret_cast<uint32_t*>(hgen + A_STAGE_BYTES + sw128_off(r, c)) = pack_bf16(d.x, d.y);
+              } else {
+                *reinterpret_cast<uint32_t*>(hgen + sw128_off(r, c)) = gelu_pack2_f16(v0 + b.x, v1 + b.y);
+              }
+            }
+          }
+        }
+        ptx::fence_proxy_async();            // generic-proxy stores -> visible to wgmma (async proxy)
+        ptx::named_bar_sync(bar_id, 128);
+        // ---- fc2: o += H . W2[:, chunk]^T (X3: lo.hi + hi.lo + hi.hi) ----
+        ptx::wgmma_fence();
+#pragma unroll
+        for (int q = 0; q < (X3 ? 3 : 1); ++q) {
+          const int ah = (X3 && q == 0) ? 1 : 0, bh = (X3 && q == 1) ? 1 : 0;
+          const uint64_t ad = ptx::make_sw128_kmajor_desc(h_base + ah * A_STAGE_BYTES + wg * (A_STAGE_BYTES / 2));
+          const uint64_t bd = ptx::make_sw128_kmajor_desc(sw + C::S * MF_KC1 * MF_W1_TILE + bh * MF_W2_TILE);
+#pragma unroll
+          for (int kk = 0; kk < BLOCK_K / MMA_K; ++kk)
+            ptx::Wgmma<MF_C>::mma(o, ad + 2u * kk, bd + 2u * kk, (j | q | kk) != 0 ? 1u : 0u);
+        }
+        ptx::wgmma_commit();
+        ptx::wgmma_wait<0>();
+        if (leader) ptx::mbar_arrive(empty_bar(stage));
+        if (++stage == C::STAGES) { stage = 0; phase ^= 1; }
+      }
+      // ---- x += gamma * (o + b2): the same rounding as the residual GEMM's L2 reduce-add ----
+      const long long r0 = (long long)tile * BLOCK_M + wg * 64 + wl * 16 + (lane >> 2);
+#pragma unroll
+      for (int t = 0; t < MF_C / 8; ++t) {
+        const int c = t * 8 + (lane & 3) * 2;
+        const float2 b = __ldg(reinterpret_cast<const float2*>(fp.b2 + c));
+        const float2 g = __ldg(reinterpret_cast<const float2*>(fp.gamma + c));
+#pragma unroll
+        for (int half = 0; half < 2; ++half) {
+          float2* xp = reinterpret_cast<float2*>(fp.x + (r0 + 8 * half) * MF_C + c);
+          float2 xv = *xp;
+          xv.x = __fadd_rn(xv.x, __fmul_rn(g.x, __fadd_rn(o[4 * t + 2 * half], b.x)));
+          xv.y = __fadd_rn(xv.y, __fmul_rn(g.y, __fadd_rn(o[4 * t + 2 * half + 1], b.y)));
+          *xp = xv;
+        }
       }
     }
-    e2_group(my_tiles - 1, 0);
-    e2_group(my_tiles - 1, 1);
-    if (lane == 0) ptx::bulk_wait0();
-    if (tr && ew == 0 && lane == 0) for (int i = 0; i < 5; ++i) p.trace[8 + i] = tw[i];
   }
-#undef MF_TIMED_WAIT
-  ptx::tc_fence_before();
-  __syncthreads();
-  if (warp == 2) {
-    ptx::tc_fence_after();
-    ptx::tmem_dealloc(tmem_base, 512);
+}
+
+template <bool X3>
+int mlp_launch(const void* A, const void* W1, const float* b1, const void* W2, const float* b2, const float* gamma,
+               float* x, long long M, cudaStream_t stream) {
+  using C = MfCfg<X3>;
+  MlpPlan fp;
+  memset(&fp, 0, sizeof(fp));
+  const uint64_t S = C::S;
+  {
+    const uint64_t dims[2] = {S * MF_C, (uint64_t)M}, str[1] = {S * MF_C * 2};
+    const uint32_t box[2] = {64, 128};
+    int rc = make_tmap_bf16(&fp.tmap_a, A, 2, dims, str, box);
+    if (rc != GDRN_OK) return rc;
   }
+  {
+    const uint64_t dims[2] = {S * MF_C, 4 * MF_C}, str[1] = {S * MF_C * 2};
+    const uint32_t box[2] = {64, 64};
+    int rc = make_tmap_bf16(&fp.tmap_w1, W1, 2, dims, str, box);
+    if (rc != GDRN_OK) return rc;
+  }
+  {
+    const uint64_t dims[2] = {S * 4 * MF_C, MF_C}, str[1] = {S * 4 * MF_C * 2};
+    const uint32_t box[2] = {64, 128};
+    int rc = make_tmap_bf16(&fp.tmap_w2, W2, 2, dims, str, box);
+    if (rc != GDRN_OK) return rc;
+  }
+  fp.b1 = b1; fp.b2 = b2; fp.gamma = gamma; fp.x = x;
+  fp.m_tiles = (int)(M / BLOCK_M);
+  auto kfn = mlp_fused_kernel<X3>;
+  GDRN_OPT_IN_SMEM(kfn, C::SMEM_BYTES);
+  const int grid = fp.m_tiles < gdrn_num_sms() ? fp.m_tiles : gdrn_num_sms();
+  GDRN_CHECK_CUDA(gdrn_launch_dep(kfn, dim3(grid), dim3(NUM_THREADS), C::SMEM_BYTES, stream, fp));
+  gdrn_count_launch(1);
+  return GDRN_OK;
 }
 
 }  // namespace
 
-int mlp_fused_supported(int C, long long M) { return C == 128 && M % 128 == 0 && M >= 128 * 148; }
+int mlp_fused_supported(int C, long long M) { return C == MF_C && M % BLOCK_M == 0 && M >= BLOCK_M; }
+int mlp_fused_x3_supported(int C, long long M) { return mlp_fused_supported(C, M); }
 
 int mlp_fused_launch(const void* A, const void* W1, const float* b1, const void* W2, const float* b2, const float* gamma,
                      float* x, long long M, int C, cudaStream_t stream) {
-  GDRN_REQUIRE(mlp_fused_supported(C, M), "mlp_fused: unsupported shape");
-  MlpFusedPlan fp;
-  memset(&fp, 0, sizeof(fp));
-  {
-    const uint64_t d[2] = {(uint64_t)C, (uint64_t)M}; const uint64_t st[1] = {(uint64_t)C * 2}; const uint32_t bx[2] = {64, 128};
-    int rc = make_tmap_bf16(&fp.tmap_a, A, 2, d, st, bx);
-    if (rc != GDRN_OK) return rc;
-  }
-  {
-    const uint64_t d[2] = {(uint64_t)C, (uint64_t)4 * C}; const uint64_t st[1] = {(uint64_t)C * 2}; const uint32_t bx[2] = {64, 128};
-    int rc = make_tmap_bf16(&fp.tmap_w1, W1, 2, d, st, bx);
-    if (rc != GDRN_OK) return rc;
-  }
-  {
-    const uint64_t d[2] = {(uint64_t)4 * C, (uint64_t)C}; const uint64_t st[1] = {(uint64_t)4 * C * 2}; const uint32_t bx[2] = {64, (uint32_t)C};
-    int rc = make_tmap_bf16(&fp.tmap_w2, W2, 2, d, st, bx);
-    if (rc != GDRN_OK) return rc;
-  }
-  {
-    const uint64_t d[2] = {(uint64_t)C, (uint64_t)M}; const uint64_t st[1] = {(uint64_t)C * 4}; const uint32_t bx[2] = {32, 32};
-    int rc = make_tmap_store(&fp.g.tmap_out, x, 1, d, st, bx);
-    if (rc != GDRN_OK) return rc;
-  }
-  fp.g.a_rank = 2; fp.g.M = (int)M; fp.g.N = C; fp.g.epi = EPI_RESID; fp.g.out_f32 = 1; fp.g.out = x; fp.g.resid = x;
-  fp.g.ldo = C; fp.g.bias = b2; fp.g.gamma = gamma; fp.g.use_tma_store = 1; fp.g.resid_reduce = 1;
-  fp.b1 = b1;
-  fp.m_tiles = (int)(M / 128);
-  constexpr int C_ = 128;
-  constexpr int SMEM = (C_ / 64) * A_STAGE_BYTES + 2 * 2 * A_STAGE_BYTES + MF_SLOTS * MF_SLOT_BYTES + NUM_EPI_WARPS * EPI_STAGE_BYTES + 256 + 1024;
-  auto kfn = mlp_fused_kernel<C_>;
-  GDRN_OPT_IN_SMEM(kfn, SMEM);
-  const int grid = fp.m_tiles < gdrn_num_sms() ? fp.m_tiles : gdrn_num_sms();
-  static int trace_on = -1;
-  if (trace_on < 0) trace_on = getenv("GDRN_MLP_TRACE") ? 1 : 0;
-  static long long* d_trace = nullptr;
-  if (trace_on) {
-    if (!d_trace) GDRN_CHECK_CUDA(cudaMalloc(&d_trace, 16 * sizeof(long long)));
-    GDRN_CHECK_CUDA(cudaMemsetAsync(d_trace, 0, 16 * sizeof(long long), stream));
-    fp.g.trace = d_trace;
-  }
-  GDRN_CHECK_CUDA(gdrn_launch_dep(kfn, dim3(grid), dim3(NUM_THREADS), SMEM, stream, fp));
-  gdrn_count_launch(1);
-  if (trace_on) {
-    long long h[16];
-    GDRN_CHECK_CUDA(cudaMemcpyAsync(h, d_trace, sizeof(h), cudaMemcpyDeviceToHost, stream));
-    GDRN_CHECK_CUDA(cudaStreamSynchronize(stream));
-    fprintf(stderr, "[mlp fused trace] cta0 cycles=%lld tiles=%lld | mma waits: A=%lld H-empty=%lld ring=%lld A'-full=%lld O-empty=%lld | "
-                    "epi0: H-full wait=%lld A'-empty wait=%lld E1 busy=%lld O-full wait=%lld E2 busy=%lld\n",
-            h[5], h[6], h[0], h[1], h[2], h[3], h[4], h[8], h[9], h[10], h[11], h[12]);
-  }
-  return GDRN_OK;
+  GDRN_REQUIRE(mlp_fused_supported(C, M), "mlp_fused: needs C == 128 and M a positive multiple of 128");
+  return mlp_launch<false>(A, W1, b1, W2, b2, gamma, x, M, stream);
+}
+
+int mlp_fused_x3_launch(const void* A, const void* W1, const float* b1, const void* W2, const float* b2, const float* gamma,
+                        float* x, long long M, int C, cudaStream_t stream) {
+  GDRN_REQUIRE(mlp_fused_x3_supported(C, M), "mlp_fused_x3: needs C == 128 and M a positive multiple of 128");
+  return mlp_launch<true>(A, W1, b1, W2, b2, gamma, x, M, stream);
 }

@@ -3,9 +3,9 @@
 //
 // Bit-exactness: the reference kernels are built by nvcc with the default --fmad=true, so WHICH products
 // are fused is decided by ptxas.  The arithmetic below spells out, with explicit round-to-nearest
-// intrinsics, the contraction ptxas 12.9 applies to the reference source for sm_100a (read from the SASS
-// of the reference file compiled here; see DESIGN.md "voting: FMA placement") so that inlier sets are
-// bit-identical to the reference build on B200.  sqrtf / __fdiv_rn are IEEE correctly rounded, as are
+// intrinsics, the contraction ptxas 12.9 applies to the reference source for sm_90a (read from the SASS
+// of the reference file compiled for sm_90a) so that hypotheses and inlier sets are bit-identical to the
+// reference build on H100 (tests/golden/ref_cuda_golden.json).  sqrtf / __fdiv_rn are IEEE correctly rounded, as are
 // sqrt.rn / div.rn in the reference.  The `< 1e-6` tests compare in double like the reference
 // (1e-6 is a double literal, ransac_voting_kernel.cu:42-43,121).
 //
@@ -39,7 +39,7 @@ __global__ void gen_hyp_kernel(const float* __restrict__ direct, const float* __
   float s1 = __fmaf_rn(d1y, cx1, -__fmul_rn(d1x, cy1));  // nx1*cx1 + ny1*cy1
   float s0 = __fmaf_rn(d0y, cx0, -__fmul_rn(d0x, cy0));  // nx0*cx0 + ny0*cy0
   float num_y = __fmaf_rn(d1y, s0, -__fmul_rn(d0y, s1));
-  float num_x = __fmaf_rn(d0x, s1, -__fmul_rn(d1x, s0));
+  float num_x = __fmaf_rn(-d1x, s0, __fmul_rn(d0x, s1));
   hypo[hvi * 2] = __fdiv_rn(num_x, det_x);
   hypo[hvi * 2 + 1] = __fdiv_rn(num_y, det_y);
 }

@@ -42,7 +42,7 @@ __device__ __forceinline__ bool rv_hypothesis(float d0x, float d0y, float d1x, f
   float s1 = __fmaf_rn(d1y, cx1, -__fmul_rn(d1x, cy1));
   float s0 = __fmaf_rn(d0y, cx0, -__fmul_rn(d0x, cy0));
   float num_y = __fmaf_rn(d1y, s0, -__fmul_rn(d0y, s1));
-  float num_x = __fmaf_rn(d0x, s1, -__fmul_rn(d1x, s0));
+  float num_x = __fmaf_rn(-d1x, s0, __fmul_rn(d0x, s1));
   *hx = __fdiv_rn(num_x, det_x);
   *hy = __fdiv_rn(num_y, det_y);
   return true;

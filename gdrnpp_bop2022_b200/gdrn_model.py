@@ -9,7 +9,7 @@ Reference interface mirrored (paths relative to the reference tree):
   * ``state_dict`` key names / shapes of a reference checkpoint (SURVEY.md Appendix A), so
     ``MyCheckpointer(model).resume_or_load`` (core/utils/my_checkpoint.py:35-83) works unchanged.
 
-All arithmetic happens in libgdrn_b200.so (hand-written sm_100a CUDA behind the C ABI of
+All arithmetic happens in libgdrn_b200.so (hand-written sm_90a CUDA behind the C ABI of
 include/gdrn_b200.h).  There is no PyTorch/CPU fallback: without the library or a CUDA device the
 forward raises.
 """
@@ -145,10 +145,10 @@ class GDRN_DoubleMask(nn.Module):
             raise ValueError(f"unknown backbone {arch}")
         pnp = net_cfg.PNP_NET
         if pnp.ROT_TYPE != "allo_rot6d" or pnp.TRANS_TYPE != "centroid_z" or _cfg_get(pnp, "Z_TYPE", "REL") != "REL":
-            raise NotImplementedError("the B200 path implements ROT_TYPE=allo_rot6d, TRANS_TYPE=centroid_z, Z_TYPE=REL")
+            raise NotImplementedError("this path implements ROT_TYPE=allo_rot6d, TRANS_TYPE=centroid_z, Z_TYPE=REL")
         g = net_cfg.GEO_HEAD
         if not (g.XYZ_CLASS_AWARE and g.MASK_CLASS_AWARE and g.REGION_CLASS_AWARE and g.NUM_REGIONS == 64):
-            raise NotImplementedError("the B200 path implements the class-aware, 64-region geometry head")
+            raise NotImplementedError("this path implements the class-aware, 64-region geometry head")
         shapes = state_dict_shapes(arch, self.num_classes)
         _build_param_tree(self, shapes)
         self._handle = None
@@ -223,7 +223,7 @@ class GDRN_DoubleMask(nn.Module):
                 roi_centers=None, roi_whs=None, roi_extents=None, resize_ratios=None, do_loss=False,
                 return_raw=False, _workspace=None):
         if do_loss:
-            raise NotImplementedError("training (do_loss=True) is out of scope of the B200 hot path")
+            raise NotImplementedError("training (do_loss=True) is out of scope of the inference hot path")
         if not x.is_cuda:
             raise _lib.GdrnError("GDRN_DoubleMask.forward needs CUDA tensors (no CPU fallback)")
         for name, t in (("roi_classes", roi_classes), ("roi_coord_2d", roi_coord_2d), ("roi_cams", roi_cams),
@@ -331,7 +331,7 @@ class GDRN_DoubleMask(nn.Module):
 def build_model_optimizer(cfg, is_test=True):
     """Reference entry point (GDRN_double_mask.py:539-615).  Only the test-time build is in scope."""
     if not is_test:
-        raise NotImplementedError("training is out of scope of the B200 hot path (SURVEY.md §2 row 17/19)")
+        raise NotImplementedError("training is out of scope of the inference hot path (SURVEY.md §2 row 17/19)")
     bb_type = _cfg_get(cfg, "MODEL.POSE_NET.BACKBONE.INIT_CFG.type", "timm/convnext_base")
     arch = bb_type.split("/")[-1]
     model = GDRN_DoubleMask(cfg, arch=arch)

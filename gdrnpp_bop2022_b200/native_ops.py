@@ -290,7 +290,7 @@ class _FlowModule:
         for t, n in ((depth_src, "depth_src"), (depth_tgt, "depth_tgt"), (KT, "KT"), (Kinv, "Kinv")):
             _check_cuda_contig(t, n)
         if depth_src.dtype != torch.float32:
-            raise RuntimeError("flow_cuda.forward: float32 only on the B200 path")
+            raise RuntimeError("flow_cuda.forward: float32 only on the CUDA path")
         B, _, H, W = depth_src.shape
         flow = torch.empty((B, 2, H, W), dtype=torch.float32, device=depth_src.device)
         valid = torch.empty((B, 1, H, W), dtype=torch.float32, device=depth_src.device)

@@ -1,5 +1,5 @@
 """GdrnPredictor -- the single-image API of the reference (core/gdrn_modeling/demo/predictor_gdrn.py:44-476),
-routed to the B200 hot path.
+routed to the CUDA hot path.
 
 Same constructor signature, method names and data contracts as the reference:
 ``GdrnPredictor(config_file_path, ckpt_file_path, camera_json_path, path_to_obj_models)``;

@@ -1,4 +1,4 @@
-/* libgdrn_b200.so -- C ABI of the B200-native GDRNPP per-ROI pose-inference hot path.
+/* libgdrn_b200.so -- C ABI of the H100-native GDRNPP per-ROI pose-inference hot path.
  *
  * Plain pointers and sizes only (no torch types).  Unless stated otherwise every pointer is a DEVICE
  * pointer, every call is asynchronous on the given CUDA stream (passed as void* = cudaStream_t), never
@@ -81,7 +81,7 @@ int gdrn_model_forward(GdrnModel* m, const float* roi_img, const int64_t* roi_cl
                        size_t workspace_bytes, void* stream);
 
 /* Per-category device timing of the LAST forward (CUDA events on the launch stream): categories
- * 0 = tcgen05 GEMM kernel, 1 = depthwise-7x7+LayerNorm kernel, 2 = other CUDA-core kernels.
+ * 0 = wgmma GEMM kernel, 1 = depthwise-7x7+LayerNorm kernel, 2 = other CUDA-core kernels.
  * get_profile blocks until that forward has finished. */
 int gdrn_model_set_profiling(GdrnModel* m, int enable);
 int gdrn_model_get_profile(GdrnModel* m, float* ms_out, int* launches_out);
@@ -91,7 +91,7 @@ int gdrn_model_get_profile(GdrnModel* m, float* ms_out, int* launches_out);
  * ([B,h,w,256] NHWC, post GN+GELU) | "pnp_in" ([B,64,64,128]) . Returns element count or <0. */
 int64_t gdrn_model_debug_read(GdrnModel* m, const char* name, int batch, float* dst, void* workspace, void* stream);
 
-/* Plain GEMM through the same tcgen05 kernel, exported for tests and roofline measurement:
+/* Plain GEMM through the same wgmma kernel, exported for tests and roofline measurement:
  * out[M,N] = epi(A[M,K] @ W[N,K]^T + bias); A, W bf16 row-major (K contiguous, lda/ldw = K).
  * epi: 0 = store (out bf16 or fp32 by out_f32), 1 = GELU -> bf16, 2 = resid + gamma*(.) -> fp32. */
 int gdrn_gemm_bf16(const void* A, const void* W, const float* bias, const float* gamma, const float* resid,
@@ -104,12 +104,9 @@ int gdrn_gemm_bf16(const void* A, const void* W, const float* bias, const float*
 int gdrn_gemm_x3(const void* A, const void* W, const float* bias, const float* gamma, const float* resid, void* out,
                  int M, int N, int K, int epi, int block_n, void* stream);
 
-/* In-place residual form (epi 2) of gdrn_gemm_x3 with the balanced k-split schedule of the CTA-pair kernel allowed:
- * x [M,N] fp32 += gamma * (A @ W^T + bias).  `flags` = flag_words ZEROED device words (>= 16 per 256 x block_n tile); the
- * kernel leaves them zeroed.  Tiles whose K range is split between two CTA pairs are reduce-added in a fixed order, so the
- * result is run-to-run deterministic.  The schedule is used when GDRN_X3_KSPLIT=1 (default 0 = whole tiles: measured no
- * faster, the GEMMs are clock-limited by the power cap, DESIGN.md 4.1).  Exported for tests and measurement (the model forward
- * passes the same flag words for its fc2 GEMMs: timm ConvNeXtBlock.mlp.fc2 + layer scale + shortcut). */
+/* DEPRECATED: same as gdrn_gemm_x3 with epi 2 and out == resid, x [M,N] fp32 += gamma * (A @ W^T + bias); kept for
+ * callers of the earlier k-split schedule, which is no longer implemented.  `flags` must still be flag_words ZEROED device
+ * words; they are not used and stay zeroed.  Run-to-run deterministic. */
 int gdrn_gemm_x3_ksplit(const void* A, const void* W, const float* bias, const float* gamma, float* x, int M, int N, int K,
                         int block_n, unsigned* flags, int flag_words, void* stream);
 

@@ -6,17 +6,17 @@
   * oracle/_ref/libupnp_ceres_ref.so -- uncertainty-PnP solved with the REFERENCE's vendored Ceres 2.0 headers (Jet
                                     autodiff + TinySolver LM), see upnp_ceres_ref.cpp.
   * oracle/_ref/<mod>/<mod>.so   -- the REFERENCE's own CUDA extensions (ransac_voting, torch_nndistance_aten,
-                                    flow_cuda) compiled unmodified from /root/reference for sm_100a: the GPU-side
-                                    ground truth for the bit-exactness tests on the B200 box.
-The _ref outputs are only (re)built when /root/reference exists (i.e. in the build container); they are
-git-ignored but travel to the GPU box with the snapshot.  No reference source is copied into the repo.
+                                    flow_cuda) compiled unmodified for sm_90a: the GPU-side ground truth that
+                                    tools/make_golden_ref.py turns into tests/golden/ fixtures.
+The _ref outputs are only (re)built when GDRN_REFERENCE_SRC names a checkout of the reference project; they are
+git-ignored.  The tests read the stored fixtures, never oracle/_ref.  No reference source is copied into the repo.
 """
 import os
 import subprocess
 import sys
 
 HERE = os.path.dirname(os.path.abspath(__file__))
-REF = "/root/reference"
+REF = os.environ.get("GDRN_REFERENCE_SRC", "")
 REFDIR = os.path.join(HERE, "_ref")
 
 
@@ -36,7 +36,7 @@ def build_oracle_ops():
 
 def build_fps_ref():
     src = os.path.join(REF, "core/csrc/fps/src/farthest_point_sampling.cpp")
-    if not os.path.exists(src):
+    if not REF or not os.path.exists(src):
         return None
     os.makedirs(REFDIR, exist_ok=True)
     out = os.path.join(REFDIR, "libfps_ref.so")
@@ -50,7 +50,7 @@ def build_upnp_ceres_ref():
     Ceres 2.0 headers (jet.h autodiff, rotation.h, tiny_solver.h LM) and Eigen, included where they lie; glog is stubbed
     (oracle/stubs).  libceres.so itself is absent, so the reference's own uncertainty_pnp.cpp cannot be linked."""
     inc = os.path.join(REF, "core/csrc/uncertainty_pnp/include")
-    if not os.path.isdir(inc):
+    if not REF or not os.path.isdir(inc):
         return None
     os.makedirs(REFDIR, exist_ok=True)
     out = os.path.join(REFDIR, "libupnp_ceres_ref.so")
@@ -69,9 +69,9 @@ CUDA_EXTS = {
 
 
 def build_cuda_refs(names=None):
-    if not os.path.isdir(REF):
+    if not REF or not os.path.isdir(REF):
         return {}
-    os.environ.setdefault("TORCH_CUDA_ARCH_LIST", "10.0a")
+    os.environ.setdefault("TORCH_CUDA_ARCH_LIST", "9.0a")
     os.environ.setdefault("MAX_JOBS", "4")
     from torch.utils.cpp_extension import load
 
@@ -88,7 +88,7 @@ def build_cuda_refs(names=None):
         extra_inc = [os.path.join(REF, os.path.dirname(srcs[0]))]
         try:
             load(name=name, sources=[os.path.join(REF, s) for s in srcs], extra_include_paths=extra_inc,
-                 extra_cuda_cflags=["-gencode", "arch=compute_100a,code=sm_100a"], build_directory=bdir,
+                 extra_cuda_cflags=["-gencode", "arch=compute_90a,code=sm_90a"], build_directory=bdir,
                  with_cuda=True, is_python_module=False, verbose=False)
         except Exception as e:  # loading a CUDA .so can fail on a CPU-only box after a successful build
             if not os.path.exists(so):

@@ -5,11 +5,10 @@
  *
  * Each function cites the reference lines it follows (paths relative to the reference tree).
  * Where the reference is CUDA built with nvcc's default --fmad=true, the fused-multiply-add placement
- * that ptxas 12.9 produces for sm_100a (inspected in the SASS of the reference file compiled in the
- * build container) is written out with fmaf() so the results are bit-identical to that build; see
- * DESIGN.md "FMA placement".  Pinned against the real reference in tests/test_oracle_pinning.py
- * (FPS: the reference .cpp compiled into oracle/_ref; voting/nnd/flow: the reference .cu built for
- * sm_100a into oracle/_ref and run on the GPU box).
+ * that ptxas 12.9 produces for sm_90a (inspected in the SASS of the reference file compiled for sm_90a)
+ * is written out with fmaf() so the results are bit-identical to that build.  Pinned against what the
+ * real reference computes (tests/golden/: FPS from the reference .cpp, voting/nnd/flow from the reference
+ * .cu built for sm_90a and run on an H100, tools/make_golden_ref.py).
  */
 #include <float.h>
 #include <math.h>
@@ -95,7 +94,7 @@ void oracle_generate_hypothesis(const float* direct, const float* coords, const 
     float s1 = fmaf(d1y, cx1, -(d1x * cy1));
     float s0 = fmaf(d0y, cx0, -(d0x * cy0));
     float num_y = fmaf(d1y, s0, -(d0y * s1));
-    float num_x = fmaf(d0x, s1, -(d1x * s0));
+    float num_x = fmaf(-d1x, s0, d0x * s1);
     hypo[hvi * 2] = num_x / det_x;
     hypo[hvi * 2 + 1] = num_y / det_y;
   }

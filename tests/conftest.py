@@ -9,7 +9,7 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (an H100)")
 
 
 @pytest.fixture(scope="session")
@@ -29,17 +29,3 @@ def dev():
         pytest.skip("no CUDA device")
     return torch.device("cuda:0")
 
-
-def load_ref_ext(name):
-    """Import one of the REFERENCE's own CUDA extensions prebuilt into oracle/_ref (or return None)."""
-    import importlib.util
-
-    import torch  # noqa: F401  (libtorch must be loaded first)
-
-    path = os.path.join(ROOT, "oracle", "_ref", name, name + ".so")
-    if not os.path.exists(path):
-        return None
-    spec = importlib.util.spec_from_file_location(name, path)
-    mod = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(mod)
-    return mod

@@ -1,14 +1,16 @@
-"""GPU parity tests (run on the B200 box): the CUDA path, called through the C ABI, against the oracle on the
+"""GPU parity tests (run on an H100): the CUDA path, called through the C ABI, against the oracle on the
 same seeded inputs -- bit-exact for integer / index / mask work, stated tolerances for floating point.
-Where oracle/_ref holds the REFERENCE's own CUDA extensions (built for sm_100a), they are run side by side."""
+Outputs of the REFERENCE's own CUDA extensions are stored under tests/golden/ and compared bit for bit."""
 import ctypes
+import hashlib
+import json
 import os
 
 import numpy as np
 import pytest
 import torch
 
-from conftest import ROOT, load_ref_ext
+from conftest import ROOT
 from oracle import gdrn_model_oracle as O
 from oracle import ops_oracle as OO
 
@@ -21,17 +23,32 @@ def _lib():
     return _lib
 
 
+def _digest(t):
+    """First 64 bits of the SHA-256 of the raw bytes of a tensor (bool as uint8), as tools/make_golden_ref.py stores them."""
+    t = t.detach().cpu()
+    if t.dtype == torch.bool:
+        t = t.to(torch.uint8)
+    return hashlib.sha256(np.ascontiguousarray(t.contiguous().numpy()).tobytes()).hexdigest()[:16]
+
+
+def _ref_cuda_golden():
+    """Digests of the outputs of the REFERENCE's own CUDA extensions (ransac_voting_kernel.cu, nnd_cuda_kernel.cu,
+    flow_cuda_kernel.cu compiled unmodified for sm_90a) on the seeded inputs below, tools/make_golden_ref.py --cuda."""
+    with open(os.path.join(ROOT, "tests", "golden", "ref_cuda_golden.json")) as f:
+        return json.load(f)
+
+
 # ------------------------------------------------------------------------------------------------ GEMM
 @pytest.mark.parametrize("M,N,K,bn,epi,f32", [
     (128, 128, 64, 128, 0, 1), (300, 128, 64, 128, 0, 0), (128, 256, 256, 256, 0, 1), (1000, 512, 128, 256, 1, 0),
     (4096, 128, 512, 128, 2, 1), (4096, 256, 1024, 256, 2, 1), (64, 1024, 8192, 64, 1, 0), (64, 9, 256, 16, 0, 1),
     (1, 256, 64, 256, 0, 1), (129, 512, 2048, 256, 1, 0),
-    # CTA-pair (cta_group::2) kernel: M >= 4096, BLOCK_N 256; ragged M (odd number of 128-row tiles + a partial tile),
-    # short K with the 16-warp GELU epilogue, fp32 and bf16 plain stores
+    # M >= 4096, BLOCK_N 256 (run as 128-wide tiles); ragged M (odd number of 128-row tiles + a partial tile),
+    # short-K GELU, fp32 and bf16 plain stores
     (4296, 512, 1024, 256, 1, 0), (4224, 256, 128, 256, 1, 0), (8192, 256, 2048, 256, 0, 1), (4100, 256, 1024, 256, 0, 0),
 ])
 def test_gemm_vs_torch(dev, lib, M, N, K, bn, epi, f32):
-    """tcgen05 kernel vs a plain fp32 torch reference of the same op (bf16 operands, fp32 accumulate)."""
+    """wgmma kernel vs a plain fp32 torch reference of the same op (bf16 operands, fp32 accumulate)."""
     L = _lib()
     g = torch.Generator().manual_seed(M * 7 + N * 3 + K)
     A = (torch.randn(M, K, generator=g) * 0.5).to(dev).bfloat16()
@@ -100,11 +117,11 @@ def _split_bf16(t):
 
 
 @pytest.mark.parametrize("M,N,K,bn,epi", [
-    # CTA-pair split kernel (>= 48 pair tiles): GELU -> split bf16, fp32 store, in-place residual (TMA reduce-add),
-    # BLOCK_N 128, ragged M (odd tile count + partial tile: the peer CTA of the last pair has no rows)
+    # shared four-tile split stage, many tiles: GELU -> split bf16 (TMA split stores), fp32 store, in-place residual,
+    # BLOCK_N 128, ragged M (odd tile count + partial tile)
     (8192, 512, 256, 256, 1), (8192, 1024, 128, 256, 0), (12417, 256, 512, 256, 2), (16384, 128, 512, 128, 2),
     (12300, 128, 128, 128, 1), (16384, 512, 2048, 256, 2),
-    # general kernel with the 3x tap list (too few tiles for the pairs, or BLOCK_N 64)
+    # few tiles, BLOCK_N 64 / 256
     (300, 128, 64, 128, 0), (1000, 512, 128, 256, 1), (64, 1024, 8192, 64, 1), (4096, 256, 1024, 256, 2),
     # narrow tiles the forward picks for small batches (B = 5: stage-2 / stage-3 fc2, stage-3 fc1)
     (1280, 512, 2048, 64, 2), (320, 1024, 4096, 64, 2), (320, 4096, 1024, 128, 1), (1280, 256, 512, 64, 0),
@@ -145,16 +162,15 @@ def test_gemm_x3_vs_fp64(dev, lib, M, N, K, bn, epi):
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("M,N,K,bn", [
-    (16384, 512, 2048, 256),    # stage-2 fc2 at B = 64: 128 tiles x 32 k-iterations on 74 pairs (tiles cut in two)
-    (65536, 256, 1024, 256),    # stage-1 fc2: 256 tiles x 16
-    (4096, 1024, 4096, 256),    # stage-3 fc2: 64 tiles x 64 (fewer tiles than pairs: some tiles are cut in THREE)
-    (20000, 256, 1024, 256),    # ragged M, odd tile count (the peer CTA of the last pair has no rows)
+    (16384, 512, 2048, 256),    # stage-2 fc2 at B = 64
+    (65536, 256, 1024, 256),    # stage-1 fc2
+    (4096, 1024, 4096, 256),    # stage-3 fc2 (fewer tiles than SMs)
+    (20000, 256, 1024, 256),    # ragged M, odd tile count
     (16384, 128, 512, 128),     # BLOCK_N 128
 ])
 def test_gemm_x3_ksplit_residual(dev, lib, M, N, K, bn):
-    """Balanced k-split schedule of the CTA-pair split-bf16 kernel (in-place residual GEMMs whose tile count leaves the
-    last wave partly empty): same result as the fp64 reference, run-to-run bit-identical (partial tiles are reduce-added
-    in a fixed order), ordering words left at zero."""
+    """The deprecated k-split entry (now the whole-tile in-place residual GEMM): same result as the fp64 reference and as
+    gdrn_gemm_x3, run-to-run bit-identical, flag words left at zero."""
     L = _lib()
     g = torch.Generator().manual_seed(M + N + K)
     A = (torch.randn(M, K, generator=g) * 0.5).to(dev)
@@ -192,7 +208,7 @@ def test_mlp_fused_x3_vs_unfused_and_fp64(dev, lib):
     chip) against (a) the two-kernel path it replaces -- same products in the same accumulation order -- and (b) an fp64
     torch reference of timm's ConvNeXtBlock MLP half on the original fp32 operands."""
     L = _lib()
-    C, M = 128, 128 * 148 * 2 + 128 * 5          # two full waves + a ragged third
+    C, M = 128, 128 * 132 * 2 + 128 * 5          # two full waves of 132 SMs + a ragged third
     g = torch.Generator().manual_seed(11)
     A = (torch.randn(M, C, generator=g) * 0.7).to(dev)
     W1 = (torch.randn(4 * C, C, generator=g) / np.sqrt(C)).to(dev)
@@ -346,8 +362,8 @@ def test_forward_vs_oracle_convnext_tiny_small(dev, arch, B):
 @pytest.mark.parametrize("precision", ["bf16x3", "bf16"])
 def test_forward_vs_oracle_b64(dev, precision):
     """BASELINE.json configs[1] at its full size: the bench's own first batch (B = 64, seed 0, unmodified
-    make_state_dict() weights) against the fp32 oracle.  At B = 64 every GEMM takes the kernel the bench times (CTA-pair
-    kernels from M >= 4096 rows, the fused stage-0 MLP in bf16 mode) -- paths the small-batch tests do not reach.
+    make_state_dict() weights) against the fp32 oracle.  At B = 64 every GEMM runs at the tile counts the bench times
+    (and the fused stage-0 MLP in both modes) -- sizes the small-batch tests do not reach.
     bf16x3 (the mode of record): north-star bar R < 1e-4 rad, t < 1e-3.  bf16 (secondary throughput mode): its own
     documented tolerances."""
     sd, batch, model, out = _run_model(dev, 64, seed=0, precision=precision)
@@ -364,8 +380,8 @@ def test_forward_vs_oracle_b64(dev, precision):
         assert (raw[:, :6] - ref["rot6d"]).abs().max().item() < 1e-4
         assert rerr < 1e-4, rerr
         assert terr < 1e-3, terr
-        # run-to-run determinism at the bench's batch size (the k-split fc2 GEMMs add partial tiles in a fixed order; the
-        # GroupNorm sums are double atomics whose order noise disappears in the float rounding of mean / rstd)
+        # run-to-run determinism at the bench's batch size (the GroupNorm sums are double atomics whose order noise
+        # disappears in the float rounding of mean / rstd)
         gb = {k: v.to(dev) for k, v in batch.items()}
         out2 = model(gb["roi_img"], roi_classes=gb["roi_classes"], roi_coord_2d=gb["roi_coord_2d"], roi_cams=gb["roi_cams"],
                      roi_centers=gb["roi_centers"], roi_whs=gb["roi_whs"], roi_extents=gb["roi_extents"],
@@ -603,31 +619,27 @@ def test_voting_bit_exact(dev, tn, vn, hn, vp):
     assert int(inl2.min()) == 1
 
 
+VOTING_REF_CASES = ((2048, 9, 128, 1), (30000, 9, 128, 2), (777, 3, 64, 3))
+
+
 def test_voting_vs_reference_cuda_build(dev):
-    """The REFERENCE's own kernels (ransac_voting_kernel.cu compiled unmodified for sm_100a into oracle/_ref)."""
-    ref = load_ref_ext("ransac_voting")
-    if ref is None:
-        pytest.xfail("oracle/_ref/ransac_voting not built (python oracle/build_ref.py --cuda-refs in the build container)")
+    """Bit-identical hypotheses and inlier masks to the REFERENCE's own kernels (ransac_voting_kernel.cu)."""
     from gdrnpp_bop2022_b200.native_ops import ransac_voting as rv
 
-    for tn, vn, hn, seed in ((2048, 9, 128, 1), (30000, 9, 128, 2), (777, 3, 64, 3)):
+    gold = _ref_cuda_golden()
+    for tn, vn, hn, seed in VOTING_REF_CASES:
         direct, coords, idxs = _voting_inputs(tn, vn, hn, seed)
         D, C, I = (torch.from_numpy(a).to(dev) for a in (direct, coords, idxs))
         for vp in (False, True):
-            gen_r = ref.generate_hypothesis_vanishing_point if vp else ref.generate_hypothesis
-            vote_r = ref.voting_for_hypothesis_vanishing_point if vp else ref.voting_for_hypothesis
             gen_m = rv.generate_hypothesis_vanishing_point if vp else rv.generate_hypothesis
             vote_m = rv.voting_for_hypothesis_vanishing_point if vp else rv.voting_for_hypothesis
-            h_r, h_m = gen_r(D, C, I), gen_m(D, C, I)
+            h_m = gen_m(D, C, I)
+            i_m = torch.zeros((hn, vn, tn), dtype=torch.uint8, device=dev)
+            vote_m(D, C, h_m, i_m, 0.99 if vp else 0.999)
             torch.cuda.synchronize()
-            assert torch.equal(h_r.view(torch.int32), h_m.view(torch.int32)), (tn, vp)
-            i_r = torch.zeros((hn, vn, tn), dtype=torch.uint8, device=dev)
-            i_m = torch.zeros_like(i_r)
-            thr = 0.99 if vp else 0.999
-            vote_r(D, C, h_r, i_r, thr)
-            vote_m(D, C, h_m, i_m, thr)
-            torch.cuda.synchronize()
-            assert torch.equal(i_r, i_m), (tn, vp)
+            key = "voting_%d_%d_%d_%d_vp%d" % (tn, vn, hn, seed, int(vp))
+            assert _digest(h_m) == gold[key + "_hyp"], (tn, vp)
+            assert _digest(i_m) == gold[key + "_inliers"], (tn, vp)
 
 
 def _voting_field(h, w, kp, noise, rs):
@@ -639,14 +651,14 @@ def _voting_field(h, w, kp, noise, rs):
 
 def test_ransac_voting_layer_device_side_vs_reference_driver(dev):
     """ransac_voting_layer / _v3 (ONE device call: compaction, hypotheses, fused vote + count, winner, refit) against the
-    reference's driver loop (ransac_voting_gpu.py:24-104) restated in the test on top of the op-level entry points --
-    the reference's own CUDA extension when oracle/_ref holds it, else ours (bit-identical to it, see
-    test_voting_vs_reference_cuda_build) -- fed with the SAME pixel pairs: identical winners, bit-identical inlier
+    reference's driver loop (ransac_voting_gpu.py:24-104) restated in the test on top of the op-level entry points
+    (ours, bit-identical to the reference's own CUDA extension, see test_voting_vs_reference_cuda_build) -- fed with the
+    SAME pixel pairs: identical winners, bit-identical inlier
     sets, final keypoints equal to fp32 rounding.  Also: keypoint recovery, empty / tiny masks, batch invariance."""
     from gdrnpp_bop2022_b200.native_ops import ransac_voting as rv_mine
     from gdrnpp_bop2022_b200.native_ops import ransac_voting_layer, ransac_voting_layer_v3
 
-    ops = load_ref_ext("ransac_voting") or rv_mine
+    ops = rv_mine
     rs = np.random.RandomState(0)
     h = w = 64
     kp = np.array([[20.3, 30.1], [50.2, 10.4], [5.5, 60.0], [40.0, 40.0]], np.float32)
@@ -760,23 +772,26 @@ def test_nnd_bit_exact(dev, b, n, m):
     assert ga_only1.shape == A.shape
 
 
+NND_REF_SHAPE = (10, 1000, 1500)   # the reference's test.py sizes
+
+
+def nnd_ref_inputs():
+    b, n, m = NND_REF_SHAPE
+    rs = np.random.RandomState(0)
+    return rs.rand(b, n, 3).astype(np.float32), rs.rand(b, m, 3).astype(np.float32)
+
+
 def test_nnd_vs_reference_cuda_build(dev):
-    ref = load_ref_ext("torch_nndistance_aten")
-    if ref is None:
-        pytest.xfail("oracle/_ref/torch_nndistance_aten not built (python oracle/build_ref.py --cuda-refs in the build container)")
+    """Bit-identical distances and indices to the REFERENCE's own kernel (nnd_cuda_kernel.cu)."""
     from gdrnpp_bop2022_b200.native_ops import torch_nndistance_aten as mine
 
-    torch.manual_seed(0)
-    a, b = torch.rand(10, 1000, 3, device=dev), torch.rand(10, 1500, 3, device=dev)  # the reference's test.py recipe
-    outs = []
-    for mod in (ref, mine):
-        d1 = torch.zeros(10, 1000, device=dev); d2 = torch.zeros(10, 1500, device=dev)
-        i1 = torch.zeros(10, 1000, dtype=torch.int32, device=dev); i2 = torch.zeros(10, 1500, dtype=torch.int32, device=dev)
-        assert mod.nnd_forward_cuda(a, b, d1, d2, i1, i2) == 1
-        torch.cuda.synchronize()
-        outs.append((d1, d2, i1, i2))
-    for x, y in zip(*outs):
-        assert torch.equal(x, y)
+    b, n, m = NND_REF_SHAPE
+    a, bb = (torch.from_numpy(x).to(dev) for x in nnd_ref_inputs())
+    d1 = torch.zeros(b, n, device=dev); d2 = torch.zeros(b, m, device=dev)
+    i1 = torch.zeros(b, n, dtype=torch.int32, device=dev); i2 = torch.zeros(b, m, dtype=torch.int32, device=dev)
+    assert mine.nnd_forward_cuda(a, bb, d1, d2, i1, i2) == 1
+    torch.cuda.synchronize()
+    assert [_digest(x) for x in (d1, d2, i1, i2)] == _ref_cuda_golden()["nnd"]
 
 
 def _flow_inputs(B, H, W, seed):
@@ -805,11 +820,8 @@ def test_flow_bit_exact(dev, B, H, W):
     assert np.array_equal(va.cpu().numpy(), ova)
     assert np.array_equal(fl.cpu().numpy().view(np.uint32), ofl.view(np.uint32))
     assert 0.2 < ova.mean() < 0.9  # the case exercises both branches
-    ref = load_ref_ext("flow_cuda")
-    if ref is not None:
-        rfl, rva = ref.forward(*(torch.from_numpy(x).to(dev) for x in (ds, dt, KT, Kinv)))
-        torch.cuda.synchronize()
-        assert torch.equal(rva, va) and torch.equal(rfl.view(torch.int32), fl.view(torch.int32))
+    # bit-identical to the REFERENCE's own kernel (flow_cuda_kernel.cu)
+    assert [_digest(fl), _digest(va)] == _ref_cuda_golden()["flow_%d_%d_%d" % (B, H, W)]
 
 
 # --------------------------------------------------------------------------------- uncertainty PnP
@@ -1292,19 +1304,18 @@ def test_dwconv_ln_pingpong_vs_cluster_kernel_and_torch(dev, lib, B, H, C, split
 
 def test_upnp_vs_vendored_ceres_and_epnp_wrapper(dev):
     """csrc/upnp.cu (batched device LM) and the reference-signature host entry against the REFERENCE's vendored Ceres 2.0
-    (oracle/_ref/libupnp_ceres_ref.so: ceres::Jet autodiff + ceres::TinySolver on the residual of uncertainty_pnp.cpp:16-34)
+    (ceres::Jet autodiff + ceres::TinySolver on the residual of uncertainty_pnp.cpp:16-34, minimisers stored in
+    tests/golden/ref_cpu_golden.npz)
     on noise-free and noisy problems; and native_ops.uncertainty_pnp -- the un_pnp_utils.py:11-78 wrapper (EPnP init on the 4
     highest-weight points via cv2, then the weighted refine) -- recovers a known pose."""
-    from test_oracle_pinning import _upnp_problem, upnp_ceres_ref
+    from test_oracle_pinning import _upnp_problem, ref_cpu_golden
 
     from gdrnpp_bop2022_b200 import native_ops
 
     rs = np.random.RandomState(21)
     probs = [_upnp_problem(rs, 9, 0.0 if i % 2 == 0 else 0.4) for i in range(10)]
     K = probs[0][0]
-    refs = [upnp_ceres_ref(p2, p3, w, K, init) for (_, _, p2, p3, w, init) in probs]
-    if refs[0] is None:
-        pytest.xfail("oracle/_ref/libupnp_ceres_ref.so not built (python oracle/build_ref.py in the build container)")
+    refs = ref_cpu_golden()["upnp_device"]
     t = lambda k: torch.from_numpy(np.stack([p[k] for p in probs])).to(dev)
     res = native_ops.uncertainty_pnp_batched(t(2), t(3), t(4), torch.from_numpy(np.tile(K[None], (len(probs), 1, 1))).to(dev), t(5)).cpu().numpy()
     for i, (_, rt, p2, p3, w, init) in enumerate(probs):

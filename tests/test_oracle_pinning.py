@@ -1,7 +1,6 @@
-"""Pin the oracle: against the reference's own code where it runs here (FPS .cpp compiled into oracle/_ref,
+"""Pin the oracle: against stored outputs of the reference's own code (FPS .cpp, vendored-Ceres uPnP,
 Python head/PnP/pose classes imported with stubbed third-party deps -> tests/golden/*.npz), and against
 independent formulations elsewhere."""
-import ctypes
 import math
 import os
 import sys
@@ -30,19 +29,39 @@ def test_fps_oracle_matches_golden_fixture():
         assert (OO.fps(pts, len(idx)) == idx).all(), i
 
 
-def test_fps_oracle_matches_reference_build_when_present():
-    path = os.path.join(ROOT, "oracle", "_ref", "libfps_ref.so")
-    if not os.path.exists(path):
-        pytest.skip("oracle/_ref/libfps_ref.so not built (no /root/reference)")
-    ref = ctypes.CDLL(path)
+def ref_cpu_golden():
+    """What the reference's own CPU code computes (core/csrc/fps farthest_point_sampling.cpp; uncertainty-PnP on its
+    vendored Ceres 2.0), stored by tools/make_golden_ref.py --cpu."""
+    return np.load(os.path.join(GOLD, "ref_cpu_golden.npz"))
+
+
+def test_fps_oracle_matches_reference_build():
+    g = ref_cpu_golden()
     rs = np.random.RandomState(5)
     for pn, sn in ((1, 1), (7, 7), (100, 16), (3000, 64), (20000, 128)):
         pts = (rs.rand(pn, 3).astype(np.float32) - 0.5) * 0.3
         if pn == 100:
             pts[10:20] = pts[0]  # duplicates -> zero distances / ties
-        idx = np.zeros(sn, np.int32)
-        ref.farthest_point_sampling_init_center(pts.ctypes.data_as(ctypes.c_void_p), idx.ctypes.data_as(ctypes.c_void_p), pn, sn)
-        assert (OO.fps(pts, sn) == idx).all(), (pn, sn)
+        assert (OO.fps(pts, sn) == g["fps_%d_%d" % (pn, sn)]).all(), (pn, sn)
+
+
+def _ref_heads_state_dict(g):
+    """The weights tools/make_golden_ref_heads.py drew for the reference modules: same generator, same parameter order."""
+    gen = torch.Generator().manual_seed(1)
+    sd = {}
+    for key, shape in zip(g["param_names"].tolist(), g["param_shapes"].tolist()):
+        shape = tuple(int(d) for d in shape.split(","))
+        prefix, n_ = key.split(".", 1)
+        if len(shape) > 1:
+            fan_in = math.prod(shape[1:]) if not n_.startswith("features.0.weight") or prefix == "pnp_net" else shape[0] * 9 / 4
+            sd[key] = torch.randn(shape, generator=gen) * math.sqrt(2.0 / fan_in)
+        elif n_.endswith("weight"):
+            sd[key] = torch.rand(shape, generator=gen) * 0.4 + 0.8
+        else:
+            sd[key] = torch.randn(shape, generator=gen) * 0.1
+    for alias, target in zip(g["alias_names"].tolist(), g["alias_targets"].tolist()):
+        sd[alias] = sd[target]
+    return sd
 
 
 def test_head_pnp_pose_oracle_matches_reference_classes():
@@ -50,7 +69,7 @@ def test_head_pnp_pose_oracle_matches_reference_classes():
     own TopDownDoubleMaskXyzRegionHead / ConvPnPNet / rot6d / pose_from_predictions_test / allo->ego code."""
     path = os.path.join(GOLD, "ref_heads.npz")
     g = np.load(path)
-    sd = {k[3:]: torch.from_numpy(g[k]) for k in g.files if k.startswith("sd/")}
+    sd = _ref_heads_state_dict(g)
     feat = torch.from_numpy(g["in/feat"])
     with torch.no_grad():
         outs = O.geo_head(sd, feat, num_classes=int(g["num_classes"]))
@@ -282,12 +301,7 @@ def test_baseline_config0_cpu_plumbing():
     pts = rng.uniform(-0.1, 0.1, (8192, 3)).astype(np.float32)
     idx = OO.fps(pts, 64)
     assert len(set(idx.tolist())) == 64 and idx.min() >= 0 and idx.max() < 8192
-    ref_so = os.path.join(ROOT, "oracle", "_ref", "libfps_ref.so")
-    if os.path.exists(ref_so):
-        L = ctypes.CDLL(ref_so)
-        ref = np.zeros(64, np.int32)
-        L.farthest_point_sampling_init_center(pts.ctypes.data_as(ctypes.c_void_p), ref.ctypes.data_as(ctypes.c_void_p), 8192, 64)
-        assert np.array_equal(ref, idx)
+    assert np.array_equal(ref_cpu_golden()["fps_8192_64"], idx)
 
     tn, vn, hn = 2048, 9, 128
     coords = rng.uniform(0, 64, (tn, 2)).astype(np.float32)
@@ -371,33 +385,16 @@ def _upnp_problem(rs, pn, noise):
     return K, rt, p2, p3, w, rt + rs.rand(6) * 0.05
 
 
-def upnp_ceres_ref(p2, p3, w, K, init):
-    """oracle/_ref/libupnp_ceres_ref.so: the reference's vendored Ceres (Jet autodiff + TinySolver LM); None if not built."""
-    so = os.path.join(ROOT, "oracle", "_ref", "libupnp_ceres_ref.so")
-    if not os.path.exists(so):
-        return None
-    L = ctypes.CDLL(so)
-    L.upnp_ceres_ref.restype = ctypes.c_int
-    c = lambda a: np.ascontiguousarray(a, np.float64).ctypes.data_as(ctypes.c_void_p)
-    res = np.zeros(6)
-    a2, a3, aw, aK, ai = (np.ascontiguousarray(x, np.float64) for x in (p2, p3, w, K, init))
-    L.upnp_ceres_ref(a2.ctypes.data_as(ctypes.c_void_p), a3.ctypes.data_as(ctypes.c_void_p), aw.ctypes.data_as(ctypes.c_void_p),
-                     aK.ctypes.data_as(ctypes.c_void_p), ai.ctypes.data_as(ctypes.c_void_p), res.ctypes.data_as(ctypes.c_void_p),
-                     int(p2.shape[0]), None)
-    return res
-
-
 def test_upnp_oracle_pinned_to_vendored_ceres():
     """Pins the uncertainty-PnP oracle (numpy LM) against the REFERENCE's own vendored Ceres 2.0: ceres::Jet autodiff of
     the residual of uncertainty_pnp.cpp:16-34 + ceres::AngleAxisRotatePoint + ceres::TinySolver, built from the headers
-    under /root/reference/core/csrc/uncertainty_pnp/include (oracle/build_ref.py).  Noise-free (the reference main()
-    recipe, :98-156) and noisy problems: same minimiser to 1e-7."""
+    under core/csrc/uncertainty_pnp/include (oracle/build_ref.py; minimisers in tests/golden/ref_cpu_golden.npz).
+    Noise-free (the reference main() recipe, :98-156) and noisy problems: same minimiser to 1e-7."""
+    refs = ref_cpu_golden()["upnp_pinning"]
     rs = np.random.RandomState(3)
-    if upnp_ceres_ref(*_upnp_problem(rs, 8, 0.0)[2:5], _upnp_problem(rs, 8, 0.0)[0], np.zeros(6) + 0.5) is None:
-        pytest.xfail("oracle/_ref/libupnp_ceres_ref.so not built (python oracle/build_ref.py in the build container)")
     for trial in range(12):
         K, rt, p2, p3, w, init = _upnp_problem(rs, 8 + trial, 0.0 if trial % 2 == 0 else 0.5)
-        ref = upnp_ceres_ref(p2, p3, w, K, init)
+        ref = refs[trial]
         mine = OO.uncertainty_pnp(p2, p3, w, K, init)
         assert np.abs(ref - mine).max() < 1e-7, (trial, ref, mine)
         if trial % 2 == 0:

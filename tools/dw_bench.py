@@ -1,6 +1,6 @@
 """Depthwise 7x7 + LayerNorm kernels at the four ConvNeXt stage shapes (B = 64): us / launch of the one-tile-per-CTA
 cluster kernel (variant 0) and the persistent ping-pong kernel (variant 1), bf16 and split output.
-Usage (under gpurun): [GDRN_DW_TRACE=1] python tools/dw_bench.py"""
+Usage (on the GPU): [GDRN_DW_TRACE=1] python tools/dw_bench.py"""
 import os
 import sys
 

@@ -1,5 +1,5 @@
 """One parity-mode forward at a small batch (default B = 5, the per-image case of BASELINE configs[4]) repeated N times, for
-ncu launch lists (tools/r02b_ncu_small.sh) and a CUDA-event timing of the graph replay.  Usage: python tools/fwd_small.py [B] [reps]"""
+a CUDA-event timing of the graph replay.  Usage: python tools/fwd_small.py [B] [reps]"""
 import os
 import sys
 

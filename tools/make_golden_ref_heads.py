@@ -1,5 +1,5 @@
-"""Generate tests/golden/ref_heads.npz by running the REFERENCE's own Python code (imported from
-/root/reference, read-only) on small seeded inputs:
+"""Generate tests/golden/ref_heads.npz by running the REFERENCE's own Python code (imported read-only from the checkout
+that GDRN_REFERENCE_SRC names) on small seeded inputs:
 
   * TopDownDoubleMaskXyzRegionHead   (core/gdrn_modeling/models/heads/top_down_doublemask_xyz_region_head.py)
   * ConvPnPNet                        (core/gdrn_modeling/models/heads/conv_pnp_net.py)
@@ -11,9 +11,11 @@ Third-party packages the reference imports but which are absent here (mmcv, dete
 numba, ...) are replaced by import stubs: a permissive dummy for everything that is only imported, and small
 real implementations for the handful of functions the path executes (weight-init helpers, conv registry,
 transforms3d.axangles.axangle2mat restated from its published formula).  No reference file is modified or
-copied.  Reduced widths keep the fixture small (in_dim = feat_dim = 32, 3 classes, PnP featdim 32, 16x16 maps).
+copied.  Reduced widths keep the fixture small (in_dim = feat_dim = 32, 3 classes, PnP featdim 32, 16x16 maps); the
+weights are not stored but drawn from a seeded generator in parameter order (param_names / param_shapes), which
+tests/test_oracle_pinning.py repeats.
 
-Run in the build container only:   python tools/make_golden_ref_heads.py
+  GDRN_REFERENCE_SRC=<reference checkout> python tools/make_golden_ref_heads.py
 """
 import importlib.abc
 import importlib.machinery
@@ -27,7 +29,7 @@ import torch
 import torch.nn as nn
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-REF = "/root/reference"
+REF = os.environ.get("GDRN_REFERENCE_SRC", "")
 STUB_TOPLEVEL = {"mmcv", "detectron2", "timm", "transforms3d", "numba", "fvcore", "pytorch_lightning", "loguru",
                  "termcolor", "tabulate", "imgaug", "vispy", "OpenGL", "pyassimp", "plyfile", "glumpy", "pypng", "png",
                  "ruamel", "setproctitle", "thop", "einops_exts", "open3d", "horovod", "fairscale", "tensorboardX",
@@ -153,6 +155,7 @@ class StubFinder(importlib.abc.MetaPathFinder, importlib.abc.Loader):
 
 
 def main():
+    assert REF and os.path.isdir(REF), "set GDRN_REFERENCE_SRC to a checkout of the reference project"
     sys.meta_path.insert(0, StubFinder())
     sys.path.insert(0, REF)
     # NumPy-1.x names the reference still uses (lib/pysixd/RT_transform.py:298 etc.)
@@ -202,10 +205,18 @@ def main():
                                            roi_centers=centers, resize_ratios=ratios, roi_whs=whs, eps=1e-4,
                                            is_allo=True, z_type="REL", is_train=False)
     out = {"num_classes": np.int64(nc)}
-    for k, v in head.state_dict().items():
-        out["sd/geo_head_net." + k] = v.numpy()
-    for k, v in pnp.state_dict().items():
-        out["sd/pnp_net." + k] = v.numpy()
+    names, shapes, aliases, targets = [], [], [], []
+    for prefix, mod in (("geo_head_net.", head), ("pnp_net.", pnp)):
+        params = dict(mod.named_parameters())
+        for n_, p in params.items():
+            names.append(prefix + n_)
+            shapes.append(",".join(str(d) for d in p.shape))
+        for k, v in mod.state_dict().items():   # the same module registered twice (norm / gn): no buffers of its own
+            if k not in params:
+                aliases.append(prefix + k)
+                targets.append(prefix + next(n_ for n_, p in params.items() if p.data_ptr() == v.data_ptr()))
+    out["param_names"], out["param_shapes"] = np.array(names), np.array(shapes)
+    out["alias_names"], out["alias_targets"] = np.array(aliases), np.array(targets)
     out.update({"in/feat": feat.numpy(), "in/coor_feat": coor_feat.numpy(), "in/region": region_in.numpy(),
                 "in/extents": extents.numpy(), "in/cams": cams.numpy(), "in/centers": centers.numpy(),
                 "in/whs": whs.numpy(), "in/ratios": ratios.numpy()})

@@ -1,5 +1,5 @@
 """Per-shape timing of the split-bf16 GEMMs of the ConvNeXt stages (gdrn_gemm_x3): us / call and executed TFLOP/s (3 products).
-Usage (under gpurun): python tools/x3_shapes_bench.py [--trace]"""
+Usage (on the GPU): python tools/x3_shapes_bench.py [--trace]"""
 import json
 import os
 import sys
@@ -31,7 +31,7 @@ def main():
         W = (torch.randn(N, 2 * K, generator=g) / np.sqrt(K)).to(dev).bfloat16()
         bias, gamma = torch.randn(N).to(dev), torch.rand(N).to(dev)
         o = torch.zeros((M, 2 * N), dtype=torch.bfloat16, device=dev) if epi == 1 else torch.zeros((M, N), dtype=torch.float32, device=dev)
-        if epi == 2:   # in-place residual: the entry that may use the balanced k-split schedule (GDRN_X3_KSPLIT)
+        if epi == 2:   # in-place residual entry (the fc2 GEMMs of the forward)
             flags = torch.zeros(8192, dtype=torch.int32, device=dev)
             call = lambda: L.check(lib.gdrn_gemm_x3_ksplit(L.ptr(A), L.ptr(W), L.ptr(bias), L.ptr(gamma), L.ptr(o), M, N, K, bn,
                                                            L.ptr(flags), 8192, L.current_stream()), "gemm_x3_ksplit")
