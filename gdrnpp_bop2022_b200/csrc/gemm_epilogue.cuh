@@ -297,7 +297,7 @@ __device__ __forceinline__ void epilogue_tile(const GemmPlan& p, int m_tile, int
     if (ri.valid) {
       const int b = ri.b;
       const int pix = (int)(ri.orow - (long long)b * p.rows_per_roi);
-      int cls = (int)p.roi_classes[b];
+      int cls = p.roi_classes ? (int)p.roi_classes[b] : 0;
       cls = cls < 0 ? 0 : (cls >= p.num_classes ? p.num_classes - 1 : cls);
       const float* ob = p.oc_bias + cls * 80;
 #pragma unroll

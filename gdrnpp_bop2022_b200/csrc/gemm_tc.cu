@@ -102,7 +102,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) gemm_tc_kernel(const __grid_co
       if (EPI == EPI_OUTCONV) {
         long long grow = (long long)m_tile * BLOCK_M;
         int b = (int)(grow / p.rows_per_roi);
-        int cls = (int)p.roi_classes[b];
+        int cls = p.roi_classes ? (int)p.roi_classes[b] : 0;   // NULL: class-agnostic head (one slab)
         cls = cls < 0 ? 0 : (cls >= p.num_classes ? p.num_classes - 1 : cls);  // never index outside the weights
         brow += cls * p.b_rows_per_class;
       }

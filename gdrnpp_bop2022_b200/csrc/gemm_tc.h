@@ -70,7 +70,7 @@ struct GemmPlan {
   const float* ln_w; const float* ln_b; float ln_eps;  // EPI_BIAS_LN
   int ln_n;             // EPI_BIAS_LN: LayerNorm width (0 = N); columns [ln_n, N) are zero PAD channels (zero weight rows / bias / affine)
   // EPI_OUTCONV
-  const long long* roi_classes;  // [B]
+  const long long* roi_classes;  // [B]; NULL = class 0 for every ROI (class-agnostic head)
   int num_classes;               // roi_classes are clamped to [0, num_classes)
   int rows_per_roi;              // 4096
   const float* oc_bias;          // [num_classes, 80]

@@ -514,9 +514,11 @@ extern "C" int gdrn_model_forward(GdrnModel* m, const float* roi_img, const int6
     return GDRN_ERR_STATE;
   }
   GDRN_REQUIRE(batch >= 1 && batch <= m->max_batch, "forward: batch out of range");
-  GDRN_REQUIRE(roi_img && roi_classes && roi_coord_2d && roi_cams && roi_centers && roi_whs && resize_ratios &&
+  GDRN_REQUIRE(roi_img && roi_coord_2d && roi_cams && roi_centers && roi_whs && resize_ratios &&
                    roi_extents && out_rot && out_trans && workspace,
                "forward: null argument");
+  // a class-agnostic head (one class slab) reads no labels; a class-aware one needs them
+  GDRN_REQUIRE(roi_classes || m->num_classes == 1, "forward: roi_classes is NULL but the head is class-aware");
   const size_t need = gdrn_model_workspace_bytes(m, batch);
   if (workspace_bytes < need) {
     gdrn_set_last_error(__FILE__, __LINE__, "forward: workspace too small");

@@ -147,9 +147,15 @@ class GDRN_DoubleMask(nn.Module):
         if pnp.ROT_TYPE != "allo_rot6d" or pnp.TRANS_TYPE != "centroid_z" or _cfg_get(pnp, "Z_TYPE", "REL") != "REL":
             raise NotImplementedError("this path implements ROT_TYPE=allo_rot6d, TRANS_TYPE=centroid_z, Z_TYPE=REL")
         g = net_cfg.GEO_HEAD
-        if not (g.XYZ_CLASS_AWARE and g.MASK_CLASS_AWARE and g.REGION_CLASS_AWARE and g.NUM_REGIONS == 64):
-            raise NotImplementedError("this path implements the class-aware, 64-region geometry head")
-        shapes = state_dict_shapes(arch, self.num_classes)
+        aware = (bool(g.XYZ_CLASS_AWARE), bool(g.MASK_CLASS_AWARE), bool(g.REGION_CLASS_AWARE))
+        if len(set(aware)) != 1 or g.NUM_REGIONS != 64:
+            raise NotImplementedError("this path implements the 64-region geometry head, either class-aware or "
+                                      "class-agnostic in all of xyz / mask / region")
+        # class-agnostic (the reference's per-object models, model_utils.get_geo_head): one class slab of 70 channels,
+        # the class gather is skipped and roi_classes is not read
+        self.class_aware = aware[0]
+        self.head_classes = self.num_classes if self.class_aware else 1
+        shapes = state_dict_shapes(arch, self.head_classes)
         _build_param_tree(self, shapes)
         self._handle = None
         self._engine_device = None   # the CUDA device the engine's weights live on (cudaMalloc'ed on first use)
@@ -180,7 +186,7 @@ class GDRN_DoubleMask(nn.Module):
                                  "(build one GDRN_DoubleMask per device)")
         if self._handle is None:
             h = ctypes.c_void_p()
-            _lib.check(L.gdrn_model_create_ex(ctypes.byref(h), self.arch.encode(), self.num_classes, self.max_batch,
+            _lib.check(L.gdrn_model_create_ex(ctypes.byref(h), self.arch.encode(), self.head_classes, self.max_batch,
                                               1 if self.precision == "bf16x3" else 0), "gdrn_model_create_ex")
             self._handle = h
             self._engine_device = device
@@ -216,6 +222,13 @@ class GDRN_DoubleMask(nn.Module):
         except Exception:
             pass
 
+    @property
+    def wants_maps(self):
+        """True when the config asks for the geometry maps (PnP, result saving or depth refine read them)."""
+        cfg = self.cfg
+        return bool(_cfg_get(cfg, "TEST.USE_PNP", False) or _cfg_get(cfg, "TEST.SAVE_RESULTS_ONLY", False)
+                    or _cfg_get(cfg, "TEST.USE_DEPTH_REFINE", False))
+
     # --- forward ---------------------------------------------------------------------------------
     def forward(self, x, gt_xyz=None, gt_xyz_bin=None, gt_mask_trunc=None, gt_mask_visib=None, gt_mask_obj=None,
                 gt_mask_full=None, gt_region=None, gt_ego_rot=None, gt_points=None, sym_infos=None, gt_trans=None,
@@ -226,18 +239,16 @@ class GDRN_DoubleMask(nn.Module):
             raise NotImplementedError("training (do_loss=True) is out of scope of the inference hot path")
         if not x.is_cuda:
             raise _lib.GdrnError("GDRN_DoubleMask.forward needs CUDA tensors (no CPU fallback)")
-        for name, t in (("roi_classes", roi_classes), ("roi_coord_2d", roi_coord_2d), ("roi_cams", roi_cams),
-                        ("roi_centers", roi_centers), ("roi_whs", roi_whs), ("roi_extents", roi_extents),
-                        ("resize_ratios", resize_ratios)):
+        for name, t in (("roi_classes", roi_classes if self.class_aware else 0), ("roi_coord_2d", roi_coord_2d),
+                        ("roi_cams", roi_cams), ("roi_centers", roi_centers), ("roi_whs", roi_whs),
+                        ("roi_extents", roi_extents), ("resize_ratios", resize_ratios)):
             if t is None:
                 raise ValueError(f"{name} is required")
         dev = x.device
         B = x.shape[0]
         if tuple(x.shape[1:]) != (3, 256, 256):
             raise ValueError(f"roi_img must be [B,3,256,256], got {tuple(x.shape)}")
-        cfg = self.cfg
-        want_maps = bool(_cfg_get(cfg, "TEST.USE_PNP", False) or _cfg_get(cfg, "TEST.SAVE_RESULTS_ONLY", False)
-                         or _cfg_get(cfg, "TEST.USE_DEPTH_REFINE", False))
+        want_maps = self.wants_maps
         map_names = (("mask", 1), ("full_mask", 1), ("coor_x", 1), ("coor_y", 1), ("coor_z", 1), ("region", 65))
         out_rot = torch.empty((B, 3, 3), dtype=torch.float32, device=dev)
         out_trans = torch.empty((B, 3), dtype=torch.float32, device=dev)
@@ -256,7 +267,8 @@ class GDRN_DoubleMask(nn.Module):
             self._ensure_engine(dev)
             f32 = lambda t: t.detach().to(device=dev, dtype=torch.float32).contiguous()
             x = f32(x)
-            cls = roi_classes.detach().to(device=dev, dtype=torch.int64).contiguous()
+            # class-agnostic head: the labels are not read (GDRN_double_mask.py skips the class gathers), NULL to the engine
+            cls = roi_classes.detach().to(device=dev, dtype=torch.int64).contiguous() if self.class_aware else None
             if roi_cams.dim() == 2:
                 roi_cams = roi_cams.unsqueeze(0).expand(B, 3, 3)
             c2d, cams, ctr, whs, ext, rr = (f32(roi_coord_2d), f32(roi_cams), f32(roi_centers), f32(roi_whs),
@@ -271,7 +283,8 @@ class GDRN_DoubleMask(nn.Module):
                     maps = _lib.GdrnMaps(*[tensors[nm][sl].data_ptr() for nm, _ in map_names])
                 ws = _workspace if _workspace is not None else self._get_workspace(n, dev)
                 rc = L.gdrn_model_forward(
-                    self._handle, _lib.ptr(x[sl]), _lib.ptr(cls[sl]), _lib.ptr(c2d[sl]), _lib.ptr(cams[sl]),
+                    self._handle, _lib.ptr(x[sl]), _lib.ptr(cls[sl]) if cls is not None else None, _lib.ptr(c2d[sl]),
+                    _lib.ptr(cams[sl]),
                     _lib.ptr(ctr[sl]), _lib.ptr(whs[sl]), _lib.ptr(rr[sl]), _lib.ptr(ext[sl]), n, _lib.ptr(out_rot[sl]),
                     _lib.ptr(out_trans[sl]), _lib.ptr(out_raw[sl]) if out_raw is not None else None,
                     ctypes.byref(maps) if maps is not None else None, _lib.ptr(ws), ws.numel(), _lib.current_stream())
@@ -284,14 +297,17 @@ class GDRN_DoubleMask(nn.Module):
 
         Returns ``(replay, out_dict)``: ``replay()`` re-runs the ~150 kernel launches of the forward as one graph
         launch on the current stream (inputs are read from the same tensors, so refill them in place);
-        ``out_dict`` holds the static output tensors.  CUDA streams and graphs replace a tracing compiler here."""
-        kw = dict(roi_classes=batch["roi_classes"], roi_coord_2d=batch["roi_coord_2d"], roi_cams=batch["roi_cams"],
-                  roi_centers=batch["roi_centers"], roi_whs=batch["roi_whs"], roi_extents=batch["roi_extents"],
-                  resize_ratios=batch["resize_ratios"])
+        ``out_dict`` holds the static output tensors.  CUDA streams and graphs replace a tracing compiler here.
+        A class-agnostic model does not read roi_classes, which may then be absent or None."""
+        kw = dict(roi_classes=batch["roi_classes"] if self.class_aware else None, roi_coord_2d=batch["roi_coord_2d"],
+                  roi_cams=batch["roi_cams"], roi_centers=batch["roi_centers"], roi_whs=batch["roi_whs"],
+                  roi_extents=batch["roi_extents"], resize_ratios=batch["resize_ratios"])
         for k, v in list(kw.items()) + [("roi_img", batch["roi_img"])]:
-            if not (v.is_cuda and v.is_contiguous()):
+            if k == "roi_classes" and not self.class_aware:
+                continue
+            if not (v is not None and v.is_cuda and v.is_contiguous()):
                 raise _lib.GdrnError(f"capture_graph: {k} must be a contiguous CUDA tensor")
-        if batch["roi_img"].dtype != torch.float32 or batch["roi_classes"].dtype != torch.int64:
+        if batch["roi_img"].dtype != torch.float32 or (self.class_aware and batch["roi_classes"].dtype != torch.int64):
             raise _lib.GdrnError("capture_graph: roi_img must be float32 and roi_classes int64 (no hidden copies)")
         dev = batch["roi_img"].device
         B = batch["roi_img"].shape[0]

@@ -16,12 +16,14 @@ import glob
 import json
 import os
 import re
+from collections.abc import Mapping
 
 import numpy as np
 import torch
 
 from .gdrn_model import GDRN_DoubleMask, _cfg_get, default_cfg, load_py_config
 from .native_ops import crop_resize_float, crop_resize_image, get_affine_transform
+from .per_object import PerObjectGDRN
 from .ply import load_ply
 from .renderer import Model3D, depth_refine, get_K_crop_resize
 
@@ -40,9 +42,20 @@ class GdrnPredictor:
                              reference's args.vertex_scale): extents come from the vertex bounding boxes (_get_extents,
                              :478-498) and the meshes feed depth refine
         Keyword-only: the same pieces already loaded (cam 3x3, objs {obj_id: name}, extents {obj_id: (3,)} metres,
-        models {obj_id: (verts [V,3] metres, faces [F,3])}, state_dict)."""
+        models {obj_id: (verts [V,3] metres, faces [F,3])}, state_dict).
+
+        Per-object models (the reference's configs/gdrn/*SO/**: one class-agnostic network per object): pass
+        ckpt_file_path={obj_id: path} or state_dict={obj_id: state_dict}, and config_file_path as one per-object config
+        shared by all of them or {obj_id: path}.  inference() then sends every ROI to its object's network
+        (PerObjectGDRN); preprocessing and post-processing are unchanged."""
         self.device = torch.device(device)
         # ---- config (predictor_gdrn.py:52-72: eval_only, TEST.USE_PNP=True, TEST.USE_DEPTH_REFINE=False, ...) ----
+        obj_cfgs = None
+        if isinstance(config_file_path, Mapping):
+            obj_cfgs = {int(k): load_py_config(v) for k, v in config_file_path.items()}
+            if cfg is None:
+                cfg = next(iter(obj_cfgs.values()))   # predictor-level settings (TEST.*, INPUT.*) come from the first
+            config_file_path = None
         if cfg is None and config_file_path is not None:
             cfg = load_py_config(config_file_path)
         self.objs_dir = path_to_obj_models
@@ -97,15 +110,14 @@ class GdrnPredictor:
                 models = loaded
         self.extents = {k: np.asarray(v, np.float32) for k, v in extents.items()}
         # ---- model (set_eval_model, predictor_gdrn.py:113-122) ----
-        arch = str(_cfg_get(cfg, "MODEL.POSE_NET.BACKBONE.INIT_CFG.type", "timm/convnext_base")).split("/")[-1]
-        self.model = GDRN_DoubleMask(self.cfg, arch=arch, max_batch=max_batch, precision=precision)
-        if state_dict is None and ckpt_file_path is not None:
-            ck = torch.load(ckpt_file_path, map_location="cpu")
-            state_dict = ck.get("model", ck)
-            state_dict = {k[len("_module."):] if k.startswith("_module.") else k: v for k, v in state_dict.items()}
-        if state_dict is not None:
-            self.model.load_state_dict(state_dict)
-        self.model.to(self.device)
+        per_object_sd = isinstance(state_dict, Mapping) and bool(state_dict) and all(
+            isinstance(v, Mapping) for v in state_dict.values())
+        if obj_cfgs is not None or isinstance(ckpt_file_path, Mapping) or per_object_sd:
+            self.model = self._per_object_model(obj_cfgs, ckpt_file_path, state_dict if per_object_sd else None,
+                                                max_batch, precision, use_cuda_graph)
+        else:
+            self.model = self._load(GDRN_DoubleMask(self.cfg, arch=_arch(self.cfg), max_batch=max_batch,
+                                                    precision=precision), ckpt_file_path, state_dict)
         self.ren_models = None
         if models is not None:
             self.ren_models = [Model3D(*models[i], device=self.device) for i in self.obj_ids]
@@ -115,6 +127,34 @@ class GdrnPredictor:
         self.use_cuda_graph = bool(use_cuda_graph)
         self._coord_grids = {}     # (H, W) -> [H,W,2] normalised coordinate grid on the device
         self._static = {}          # n -> dict of static input tensors (+ pinned staging, + captured graph)
+
+    def _load(self, model, ckpt_file_path, state_dict):
+        if state_dict is None and ckpt_file_path is not None:
+            ck = torch.load(ckpt_file_path, map_location="cpu")
+            state_dict = ck.get("model", ck)
+            state_dict = {k[len("_module."):] if k.startswith("_module.") else k: v for k, v in state_dict.items()}
+        if state_dict is not None:
+            model.load_state_dict(state_dict)
+        return model.to(self.device)
+
+    def _per_object_model(self, obj_cfgs, ckpts, state_dicts, max_batch, precision, use_cuda_graph):
+        """One class-agnostic GDRN_DoubleMask per object, keyed by the detector label (the index of the object in
+        obj_ids, which is what preprocessing() stores in roi_cls)."""
+        ckpts = {int(k): v for k, v in (ckpts or {}).items()}
+        state_dicts = {int(k): v for k, v in (state_dicts or {}).items()}
+        ids = sorted(set(ckpts) | set(state_dicts) or set(obj_cfgs or {}))
+        unknown = [i for i in ids if i not in self.objs]
+        if unknown:
+            raise ValueError(f"per-object weights / configs for obj_id(s) {unknown} that are not in objs {self.obj_ids}")
+        T = self.cfg.TEST
+        members = {}
+        for oid in ids:
+            mcfg = (obj_cfgs or {}).get(oid, self.cfg)
+            for k in ("USE_PNP", "USE_DEPTH_REFINE", "DEPTH_REFINE_ITER", "DEPTH_REFINE_THRESHOLD"):
+                setattr(mcfg.TEST, k, getattr(T, k))   # the predictor's settings apply to every member
+            m = GDRN_DoubleMask(mcfg, arch=_arch(mcfg), max_batch=max_batch, precision=precision)
+            members[self.obj_ids.index(oid)] = self._load(m, ckpts.get(oid), state_dicts.get(oid))
+        return PerObjectGDRN(members, use_cuda_graph=use_cuda_graph)
 
     # ---- preprocessing (predictor_gdrn.py:301-476) ---------------------------------------------
     def preprocessing(self, outputs, image, depth_img=None):
@@ -202,6 +242,13 @@ class GdrnPredictor:
     @torch.no_grad()
     def inference(self, data_dict):
         n = data_dict["roi_img"].shape[0]
+        if isinstance(self.model, PerObjectGDRN):   # each ROI to its object's network (graphs per member and size)
+            out = self.model(
+                data_dict["roi_img"], roi_classes=data_dict["roi_cls"], roi_cams=data_dict["roi_cam"],
+                roi_whs=data_dict["roi_wh"], roi_centers=data_dict["roi_center"], resize_ratios=data_dict["resize_ratio"],
+                roi_coord_2d=data_dict.get("roi_coord_2d"), roi_extents=data_dict.get("roi_extent"))
+            torch.cuda.synchronize(self.device)
+            return out
         st = self._static.get(data_dict.get("_static_n", -1))
         graph_ok = (self.use_cuda_graph and st is not None and 1 <= n <= self.model.max_batch
                     and data_dict["roi_img"] is st["roi_img"])       # the batch still lives in the static buffers
@@ -273,3 +320,7 @@ class GdrnPredictor:
                             out_dict["trans"], K_crop, xyz, out_dict["mask"], d.contiguous(),
                             iters=self.cfg.TEST.DEPTH_REFINE_ITER, thresh=self.cfg.TEST.DEPTH_REFINE_THRESHOLD,
                             mesh_ids=inputs["roi_cls"])
+
+
+def _arch(cfg):
+    return str(_cfg_get(cfg, "MODEL.POSE_NET.BACKBONE.INIT_CFG.type", "timm/convnext_base")).split("/")[-1]

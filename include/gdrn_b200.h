@@ -39,7 +39,9 @@ long long gdrn_launch_count(void);
  * ------------------------------------------------------------------------------------------- */
 typedef struct GdrnModel GdrnModel;
 
-/* arch: "convnext_base" | "convnext_small" | "convnext_tiny"; num_classes: class-aware head size (21). */
+/* arch: "convnext_base" | "convnext_small" | "convnext_tiny"; num_classes: class-aware head size (21), or 1 for the
+ * class-agnostic head of the reference's per-object models (XYZ/MASK/REGION_CLASS_AWARE all false: out_layer
+ * [70,256,1,1], channels vis 0, full 1, x/y/z 2..4, region 5..69). */
 int gdrn_model_create(GdrnModel** out, const char* arch, int num_classes, int max_batch);
 /* precision: 0 = bf16 tensor-core operands, fp32 accumulate / residual stream (the throughput mode; what the
  *               reference's AMP test path does, engine_utils.py autocast);
@@ -73,7 +75,10 @@ typedef struct GdrnMaps { /* optional class-gathered maps (GDRN_double_mask.py:2
 
 /* roi_img [B,3,256,256] fp32 NCHW in [0,1]; roi_classes [B] int64; roi_coord_2d [B,2,64,64]; roi_cams [B,3,3];
  * roi_centers [B,2]; roi_whs [B,2]; resize_ratios [B]; roi_extents [B,3]  ->  out_rot [B,3,3] (egocentric,
- * row-major), out_trans [B,3].  out_raw (optional, [B,9]) receives the Patch-PnP head output (rot6d, t_). */
+ * row-major), out_trans [B,3].  out_raw (optional, [B,9]) receives the Patch-PnP head output (rot6d, t_).
+ * roi_classes may be NULL only for a model created with num_classes = 1 (class-agnostic head): the head then reads
+ * no labels and every ROI uses the one class slab.  A class-aware model rejects NULL with GDRN_ERR_INVALID.  Non-NULL
+ * labels are clamped into [0, num_classes) as before. */
 int gdrn_model_forward(GdrnModel* m, const float* roi_img, const int64_t* roi_classes, const float* roi_coord_2d,
                        const float* roi_cams, const float* roi_centers, const float* roi_whs,
                        const float* resize_ratios, const float* roi_extents, int batch, float* out_rot,

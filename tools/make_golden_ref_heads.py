@@ -15,7 +15,11 @@ copied.  Reduced widths keep the fixture small (in_dim = feat_dim = 32, 3 classe
 weights are not stored but drawn from a seeded generator in parameter order (param_names / param_shapes), which
 tests/test_oracle_pinning.py repeats.
 
-  GDRN_REFERENCE_SRC=<reference checkout> python tools/make_golden_ref_heads.py
+  GDRN_REFERENCE_SRC=<reference checkout> python tools/make_golden_ref_heads.py [--agnostic]
+
+--agnostic writes tests/golden/ref_heads_agnostic.npz instead: the class-agnostic head of the reference's per-object
+models (mask / xyz / region_num_classes = 1, model_utils.py get_geo_head with the *_CLASS_AWARE flags false), same
+stubs, same seeds and the same recipe, so that the channel order of a one-slab out_layer is pinned by the reference too.
 """
 import importlib.abc
 import importlib.machinery
@@ -154,7 +158,7 @@ class StubFinder(importlib.abc.MetaPathFinder, importlib.abc.Loader):
             module.axangle2mat = axangle2mat
 
 
-def main():
+def main(agnostic=False):
     assert REF and os.path.isdir(REF), "set GDRN_REFERENCE_SRC to a checkout of the reference project"
     sys.meta_path.insert(0, StubFinder())
     sys.path.insert(0, REF)
@@ -168,7 +172,7 @@ def main():
     from core.utils.rot_reps import rot6d_to_mat_batch
     from core.gdrn_modeling.models.pose_from_pred_centroid_z import pose_from_pred_centroid_z
 
-    nc = 3
+    nc = 1 if agnostic else 3
     head = TopDownDoubleMaskXyzRegionHead(in_dim=32, feat_dim=32, norm="GN", num_gn_groups=32, act="GELU",
                                           mask_num_classes=nc, xyz_num_classes=nc, region_num_classes=nc,
                                           mask_out_dim=2, xyz_out_dim=3, region_out_dim=65).eval()
@@ -224,10 +228,10 @@ def main():
         out["out/" + name] = o.contiguous().numpy()
     out.update({"out/pnp_rot": rot.numpy(), "out/pnp_t_raw": t.numpy(), "out/pnp_t": t_use.numpy(), "out/rot_m": rot_m.numpy(),
                 "out/ego_rot": ego.numpy(), "out/trans": trans.numpy()})
-    path = os.path.join(ROOT, "tests", "golden", "ref_heads.npz")
+    path = os.path.join(ROOT, "tests", "golden", "ref_heads_agnostic.npz" if agnostic else "ref_heads.npz")
     np.savez_compressed(path, **out)
     print("wrote", path, os.path.getsize(path), "bytes")
 
 
 if __name__ == "__main__":
-    main()
+    main(agnostic="--agnostic" in sys.argv[1:])
