@@ -20,6 +20,10 @@
 // OpenCV's final step is EPnP on the inliers (an algebraic solution + Gauss-Newton); both minimise the same residual, so
 // poses agree to the tolerance tests/test_gpu_parity.py states, not bit-exactly.  < 4 correspondences -> the
 // reference's sentinel pose (-100 everywhere, gdrn_evaluator.py:1178-1179).
+//
+// The network-initialised types of TEST.PNP_TYPE (process_net_and_pnp, gdrn_evaluator.py:241-371) reuse steps 1 and 4:
+// net_iter_pnp is pnp_iterative_kernel (step 1, then the step-4 LM over all correspondences from the network pose);
+// net_ransac_pnp / _rot are pnp_ransac_kernel at 20 iterations followed by pnp_net_select_kernel.
 #include "common.cuh"
 
 namespace {
@@ -27,6 +31,8 @@ namespace {
 constexpr int PR_THREADS = 512;
 constexpr int PR_MAX_PTS = 4096;   // 64 x 64 maps
 constexpr int PR_MAX_HYP = 256;
+constexpr int PNP_ITERATIVE_MAX_ITERS = 20;   // OpenCV's SOLVEPNP_ITERATIVE cap (cvFindExtrinsicCameraParams2 max_iter)
+enum { PNP_NET_ITER = 0, PNP_NET_RANSAC = 1, PNP_NET_RANSAC_ROT = 2 };   // gdrn_pnp_net_maps pnp_type
 
 struct PnpParams {
   const float* coor_x; const float* coor_y; const float* coor_z;   // [n, hw*hw] network outputs in [0,1]
@@ -244,26 +250,31 @@ __device__ void apply_update(double* Rt, const double* d) {
   }
 }
 
-__global__ void __launch_bounds__(PR_THREADS)
-pnp_ransac_kernel(const PnpParams p) {
-  extern __shared__ float sm_f[];
-  float* s3 = sm_f;                         // [PR_MAX_PTS][3] model points
-  float* s2 = s3 + 3 * PR_MAX_PTS;          // [PR_MAX_PTS][2] image points
-  unsigned short* s_src = reinterpret_cast<unsigned short*>(s2 + 2 * PR_MAX_PTS);   // [PR_MAX_PTS] source pixel of entry i
-  unsigned char* s_inl = reinterpret_cast<unsigned char*>(s_src + PR_MAX_PTS);      // [PR_MAX_PTS] inlier flags
-  __shared__ double s_hyp[PR_MAX_HYP][12];
-  __shared__ int s_cnt[PR_MAX_HYP];
-  __shared__ double s_red[PR_THREADS / 32][28];
-  __shared__ double s_pose[12], s_K[9], s_step[8];
-  __shared__ float s_mm[2];
-  __shared__ int s_count, s_scan[PR_THREADS / 32 + 1], s_flag;
+// Shared-memory workspace of one ROI's correspondences (the dynamic smem of both PnP kernels) and of the CTA reductions.
+struct PnpShared {
+  float* s3;                      // [PR_MAX_PTS][3] model points
+  float* s2;                      // [PR_MAX_PTS][2] image points
+  unsigned short* s_src;          // [PR_MAX_PTS] source pixel / point of entry i
+  double (*s_red)[28];            // [PR_THREADS / 32][28] per-warp partial sums
+  double* s_K;                    // [9]
+  double* s_step;                 // [8] LM decisions broadcast by thread 0
+  float* s_mm;                    // [2] mask min / max
+  int* s_count;
+  int* s_scan;                    // [PR_THREADS / 32 + 1]
+};
 
-  const int roi = blockIdx.x;
+// Step 1 of both kernels: the selected correspondences of ROI `roi` compacted into sh.s3 / s2 / s_src in row-major
+// order; returns their count (in every thread).
+__device__ __forceinline__ int gather_correspondences(const PnpParams& p, int roi, const PnpShared& sh) {
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int npts = p.npts;
-  if (tid < 9) s_K[tid] = (double)p.Ks[roi * 9 + tid];
-
-  // ---------------- 1. correspondences ----------------
+  float* s3 = sh.s3;
+  float* s2 = sh.s2;
+  unsigned short* s_src = sh.s_src;
+  double (*s_red)[28] = sh.s_red;
+  float* s_mm = sh.s_mm;
+  int& s_count = *sh.s_count;
+  int* s_scan = sh.s_scan;
   if (p.pts3d == nullptr) {
     float mn = INFINITY, mx = -INFINITY;
     for (int i = tid; i < npts; i += PR_THREADS) {
@@ -326,7 +337,130 @@ pnp_ransac_kernel(const PnpParams p) {
       __syncthreads();
     }
   }
-  const int N = s_count;
+  return s_count;
+}
+
+// Levenberg-Marquardt on the reprojection error of the N compacted correspondences (those with inl[i] != 0, or all of
+// them when inl is null), starting from and updating s_pose [12] in place; s_save [12] holds the last accepted pose.
+// Every thread must call it; thread 0 makes the decisions.
+//   kFromGuess = false (RANSAC refit): points at z <= 1e-9 are left out, at most `max_iters` normal-equation solves.
+//   kFromGuess = true (network-initialised PnP): like OpenCV's iterative solver, every point with z != 0 counts (from a
+//     poor start some may lie behind the camera; dropping them would reward steps that push points there), and only
+//     accepted steps count towards `max_iters` (at most 4 * max_iters solves in all).
+template <bool kFromGuess>
+__device__ __forceinline__ void lm_refine(double* s_pose, double* s_save, const unsigned char* inl, int N, int max_iters,
+                                          const PnpShared& sh) {
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const float* s3 = sh.s3;
+  const float* s2 = sh.s2;
+  const double* s_K = sh.s_K;
+  double (*s_red)[28] = sh.s_red;
+  double* s_step = sh.s_step;
+  double lambda = 1e-4, prev_cost = -1.0;
+  for (int it = 0, solves = 0; it < max_iters && solves < 4 * max_iters; ++it, ++solves) {
+    // normal equations: 21 (upper JtJ) + 6 (Jt r) + 1 (cost) sums
+    double acc[28];
+    for (int k = 0; k < 28; ++k) acc[k] = 0.0;
+    for (int i = tid; i < N; i += PR_THREADS) {
+      if (inl && !inl[i]) continue;
+      const double X = s3[i * 3], Y = s3[i * 3 + 1], Z = s3[i * 3 + 2];
+      const double rx = s_pose[0] * X + s_pose[1] * Y + s_pose[2] * Z;
+      const double ry = s_pose[4] * X + s_pose[5] * Y + s_pose[6] * Z;
+      const double rz = s_pose[8] * X + s_pose[9] * Y + s_pose[10] * Z;
+      const double xc = rx + s_pose[3], yc = ry + s_pose[7], zc = rz + s_pose[11];
+      if (kFromGuess ? zc == 0.0 : !(zc > 1e-9)) continue;
+      const double iz = 1.0 / zc;
+      const double u = s_K[0] * xc * iz + s_K[1] * yc * iz + s_K[2], v = s_K[4] * yc * iz + s_K[5];
+      const double eu = u - s2[i * 2], ev = v - s2[i * 2 + 1];
+      // d(u,v)/d(xc,yc,zc)
+      const double ux = s_K[0] * iz, uy = s_K[1] * iz, uz = -(s_K[0] * xc + s_K[1] * yc) * iz * iz;
+      const double vy = s_K[4] * iz, vz = -s_K[4] * yc * iz * iz;
+      // d xc / d w = -[R X]x  (left perturbation), d xc / d t = I
+      double Ju[6], Jv[6];
+      Ju[0] = uy * (-rz) + uz * ry;           // column 0 of -[r]x = (0, -rz... ) see below
+      Ju[1] = ux * rz + uz * (-rx);
+      Ju[2] = ux * (-ry) + uy * rx;
+      Jv[0] = vy * (-rz) + vz * ry;
+      Jv[1] = vz * (-rx);
+      Jv[2] = vy * rx;
+      Ju[3] = ux; Ju[4] = uy; Ju[5] = uz;
+      Jv[3] = 0.0; Jv[4] = vy; Jv[5] = vz;
+      int k = 0;
+      for (int a = 0; a < 6; ++a)
+        for (int b = a; b < 6; ++b) acc[k++] += Ju[a] * Ju[b] + Jv[a] * Jv[b];
+      for (int a = 0; a < 6; ++a) acc[21 + a] += Ju[a] * eu + Jv[a] * ev;
+      acc[27] += eu * eu + ev * ev;
+    }
+    for (int k = 0; k < 28; ++k)
+      for (int o = 16; o > 0; o >>= 1) acc[k] += __shfl_xor_sync(0xffffffffu, acc[k], o);
+    if (lane == 0) for (int k = 0; k < 28; ++k) s_red[warp][k] = acc[k];
+    __syncthreads();
+    if (tid == 0) {
+      double tot[28];
+      for (int k = 0; k < 28; ++k) { tot[k] = 0.0; for (int w = 0; w < PR_THREADS / 32; ++w) tot[k] += s_red[w][k]; }
+      double A[36], g[6], dx[6];
+      int k = 0;
+      for (int a = 0; a < 6; ++a)
+        for (int b = a; b < 6; ++b) { A[a * 6 + b] = tot[k]; A[b * 6 + a] = tot[k]; ++k; }
+      for (int a = 0; a < 6; ++a) g[a] = -tot[21 + a];
+      const double cost = tot[27];
+      int stop = 0;
+      if (prev_cost >= 0.0 && cost > prev_cost) {
+        // the previous step made it worse: undo it and raise the damping
+        for (int a = 0; a < 12; ++a) s_pose[a] = s_save[a];
+        lambda *= 10.0;
+        s_step[6] = 0.0;   // do not update prev_cost
+        stop = lambda > 1e6;
+        s_step[7] = stop ? 1.0 : 2.0;   // 2 = retry with the saved pose (normal equations recomputed next iteration)
+      } else {
+        for (int a = 0; a < 12; ++a) s_save[a] = s_pose[a];   // save
+        if (solve6(A, g, lambda, dx)) {
+          apply_update(s_pose, dx);
+          double nrm = 0.0;
+          for (int a = 0; a < 6; ++a) nrm += dx[a] * dx[a];
+          stop = nrm < 1e-20;
+          lambda = fmax(lambda * 0.3, 1e-9);
+        } else {
+          lambda *= 10.0;
+          stop = lambda > 1e6;
+        }
+        s_step[6] = 1.0;
+        s_step[5] = cost;
+        s_step[7] = stop ? 1.0 : 0.0;
+      }
+    }
+    __syncthreads();
+    const bool accepted = s_step[6] != 0.0;
+    if (accepted) prev_cost = s_step[5];
+    const bool stop = s_step[7] == 1.0;
+    __syncthreads();
+    if (stop) break;
+    if (kFromGuess && !accepted) --it;   // a rejected step does not count
+  }
+}
+
+__global__ void __launch_bounds__(PR_THREADS)
+pnp_ransac_kernel(const PnpParams p) {
+  extern __shared__ float sm_f[];
+  float* s3 = sm_f;                         // [PR_MAX_PTS][3] model points
+  float* s2 = s3 + 3 * PR_MAX_PTS;          // [PR_MAX_PTS][2] image points
+  unsigned short* s_src = reinterpret_cast<unsigned short*>(s2 + 2 * PR_MAX_PTS);   // [PR_MAX_PTS] source pixel of entry i
+  unsigned char* s_inl = reinterpret_cast<unsigned char*>(s_src + PR_MAX_PTS);      // [PR_MAX_PTS] inlier flags
+  __shared__ double s_hyp[PR_MAX_HYP][12];
+  __shared__ int s_cnt[PR_MAX_HYP];
+  __shared__ double s_red[PR_THREADS / 32][28];
+  __shared__ double s_pose[12], s_K[9], s_step[8];
+  __shared__ float s_mm[2];
+  __shared__ int s_count, s_scan[PR_THREADS / 32 + 1], s_flag;
+  const PnpShared sh = {s3, s2, s_src, s_red, s_K, s_step, s_mm, &s_count, s_scan};
+
+  const int roi = blockIdx.x;
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const int npts = p.npts;
+  if (tid < 9) s_K[tid] = (double)p.Ks[roi * 9 + tid];
+
+  // ---------------- 1. correspondences ----------------
+  const int N = gather_correspondences(p, roi, sh);
   float* out = p.poses + (long long)roi * 12;
   if (p.inlier_mask) for (int i = tid; i < npts; i += PR_THREADS) p.inlier_mask[(long long)roi * npts + i] = 0;
   if (N < 4) {   // gdrn_evaluator.py:1178-1179
@@ -424,85 +558,7 @@ pnp_ransac_kernel(const PnpParams p) {
       s_inl[i] = in ? 1 : 0;
     }
     __syncthreads();
-    double lambda = 1e-4, prev_cost = -1.0;
-    for (int it = 0; it < 12; ++it) {
-      // normal equations over the inliers: 21 (upper JtJ) + 6 (Jt r) + 1 (cost) sums
-      double acc[28];
-      for (int k = 0; k < 28; ++k) acc[k] = 0.0;
-      for (int i = tid; i < N; i += PR_THREADS) {
-        if (!s_inl[i]) continue;
-        const double X = s3[i * 3], Y = s3[i * 3 + 1], Z = s3[i * 3 + 2];
-        const double rx = s_pose[0] * X + s_pose[1] * Y + s_pose[2] * Z;
-        const double ry = s_pose[4] * X + s_pose[5] * Y + s_pose[6] * Z;
-        const double rz = s_pose[8] * X + s_pose[9] * Y + s_pose[10] * Z;
-        const double xc = rx + s_pose[3], yc = ry + s_pose[7], zc = rz + s_pose[11];
-        if (!(zc > 1e-9)) continue;
-        const double iz = 1.0 / zc;
-        const double u = s_K[0] * xc * iz + s_K[1] * yc * iz + s_K[2], v = s_K[4] * yc * iz + s_K[5];
-        const double eu = u - s2[i * 2], ev = v - s2[i * 2 + 1];
-        // d(u,v)/d(xc,yc,zc)
-        const double ux = s_K[0] * iz, uy = s_K[1] * iz, uz = -(s_K[0] * xc + s_K[1] * yc) * iz * iz;
-        const double vy = s_K[4] * iz, vz = -s_K[4] * yc * iz * iz;
-        // d xc / d w = -[R X]x  (left perturbation), d xc / d t = I
-        double Ju[6], Jv[6];
-        Ju[0] = uy * (-rz) + uz * ry;           // column 0 of -[r]x = (0, -rz... ) see below
-        Ju[1] = ux * rz + uz * (-rx);
-        Ju[2] = ux * (-ry) + uy * rx;
-        Jv[0] = vy * (-rz) + vz * ry;
-        Jv[1] = vz * (-rx);
-        Jv[2] = vy * rx;
-        Ju[3] = ux; Ju[4] = uy; Ju[5] = uz;
-        Jv[3] = 0.0; Jv[4] = vy; Jv[5] = vz;
-        int k = 0;
-        for (int a = 0; a < 6; ++a)
-          for (int b = a; b < 6; ++b) acc[k++] += Ju[a] * Ju[b] + Jv[a] * Jv[b];
-        for (int a = 0; a < 6; ++a) acc[21 + a] += Ju[a] * eu + Jv[a] * ev;
-        acc[27] += eu * eu + ev * ev;
-      }
-      for (int k = 0; k < 28; ++k)
-        for (int o = 16; o > 0; o >>= 1) acc[k] += __shfl_xor_sync(0xffffffffu, acc[k], o);
-      if (lane == 0) for (int k = 0; k < 28; ++k) s_red[warp][k] = acc[k];
-      __syncthreads();
-      if (tid == 0) {
-        double tot[28];
-        for (int k = 0; k < 28; ++k) { tot[k] = 0.0; for (int w = 0; w < PR_THREADS / 32; ++w) tot[k] += s_red[w][k]; }
-        double A[36], g[6], dx[6];
-        int k = 0;
-        for (int a = 0; a < 6; ++a)
-          for (int b = a; b < 6; ++b) { A[a * 6 + b] = tot[k]; A[b * 6 + a] = tot[k]; ++k; }
-        for (int a = 0; a < 6; ++a) g[a] = -tot[21 + a];
-        const double cost = tot[27];
-        int stop = 0;
-        if (prev_cost >= 0.0 && cost > prev_cost) {
-          // the previous step made it worse: undo it and raise the damping
-          for (int a = 0; a < 12; ++a) s_pose[a] = s_hyp[0][a];   // s_hyp[0] doubles as the saved pose below
-          lambda *= 10.0;
-          s_step[6] = 0.0;   // do not update prev_cost
-          stop = lambda > 1e6;
-          s_step[7] = stop ? 1.0 : 2.0;   // 2 = retry with the saved pose (normal equations recomputed next iteration)
-        } else {
-          for (int a = 0; a < 12; ++a) s_hyp[0][a] = s_pose[a];   // save
-          if (solve6(A, g, lambda, dx)) {
-            apply_update(s_pose, dx);
-            double nrm = 0.0;
-            for (int a = 0; a < 6; ++a) nrm += dx[a] * dx[a];
-            stop = nrm < 1e-20;
-            lambda = fmax(lambda * 0.3, 1e-9);
-          } else {
-            lambda *= 10.0;
-            stop = lambda > 1e6;
-          }
-          s_step[6] = 1.0;
-          s_step[5] = cost;
-          s_step[7] = stop ? 1.0 : 0.0;
-        }
-      }
-      __syncthreads();
-      if (s_step[6] != 0.0) prev_cost = s_step[5];
-      const bool stop = s_step[7] == 1.0;
-      __syncthreads();
-      if (stop) break;
-    }
+    lm_refine<false>(s_pose, s_hyp[0], s_inl, N, 12, sh);   // s_hyp[0] doubles as the saved pose
     __syncthreads();
   }
   // final inlier set of the refined pose
@@ -528,10 +584,77 @@ pnp_ransac_kernel(const PnpParams p) {
   if (tid < 12) out[tid] = (float)s_pose[tid];
 }
 
+// Network-initialised iterative PnP (TEST.PNP_TYPE = "net_iter_pnp", gdrn_evaluator.py:241-371): the reference calls
+// cv2.solvePnP(SOLVEPNP_ITERATIVE, useExtrinsicGuess=True) from the network pose on ALL selected correspondences, i.e.
+// LM on the reprojection error (at most 20 iterations in OpenCV's cvFindExtrinsicCameraParams2).  Same compaction and
+// LM as pnp_ransac_kernel, no sampling.  < 4 correspondences -> the initial pose unchanged (gdrn_evaluator.py:355-358).
+__global__ void __launch_bounds__(PR_THREADS)
+pnp_iterative_kernel(const PnpParams p, const float* __restrict__ rot0, const float* __restrict__ trans0) {
+  extern __shared__ float sm_f[];
+  float* s3 = sm_f;
+  float* s2 = s3 + 3 * PR_MAX_PTS;
+  unsigned short* s_src = reinterpret_cast<unsigned short*>(s2 + 2 * PR_MAX_PTS);
+  __shared__ double s_red[PR_THREADS / 32][28];
+  __shared__ double s_pose[12], s_save[12], s_K[9], s_step[8];
+  __shared__ float s_mm[2];
+  __shared__ int s_count, s_scan[PR_THREADS / 32 + 1];
+  const PnpShared sh = {s3, s2, s_src, s_red, s_K, s_step, s_mm, &s_count, s_scan};
+
+  const int roi = blockIdx.x;
+  const int tid = threadIdx.x;
+  if (tid < 9) s_K[tid] = (double)p.Ks[roi * 9 + tid];
+  if (tid < 12) s_pose[tid] = (tid & 3) == 3 ? (double)trans0[roi * 3 + (tid >> 2)] : (double)rot0[roi * 9 + (tid >> 2) * 3 + (tid & 3)];
+  const int N = gather_correspondences(p, roi, sh);
+  float* out = p.poses + (long long)roi * 12;
+  if (N < 4) {
+    if (tid < 12) out[tid] = (float)s_pose[tid];   // exact: the pose came in as float
+    if (tid == 0 && p.n_inliers) p.n_inliers[roi] = 0;
+    return;
+  }
+  lm_refine<true>(s_pose, s_save, nullptr, N, PNP_ITERATIVE_MAX_ITERS, sh);
+  if (tid < 12) out[tid] = (float)s_pose[tid];
+  if (tid == 0 && p.n_inliers) p.n_inliers[roi] = N;
+}
+
+// The rules the reference's process_net_and_pnp applies after cv2.solvePnPRansac(EPNP, useExtrinsicGuess=True), one
+// thread per ROI on the pose pnp_ransac_kernel wrote:
+//   * < 4 correspondences or no RANSAC model (the -100 sentinel) -> the network pose (cv2 hands the guess back);
+//   * net_ransac_pnp: ||t_pnp - t_net|| > 1 -> t = t_net, R stays the PnP rotation;
+//   * net_ransac_pnp_rot: t = t_net always.
+__global__ void pnp_net_select_kernel(float* __restrict__ poses, const float* __restrict__ rot_net,
+                                      const float* __restrict__ trans_net, int n, int pnp_type) {
+  const int roi = blockIdx.x * blockDim.x + threadIdx.x;
+  if (roi >= n) return;
+  float* P = poses + (long long)roi * 12;
+  const float* tn = trans_net + roi * 3;
+  if (P[0] == -100.f) {   // a rotation entry is never -100: this is the sentinel
+    for (int r = 0; r < 3; ++r) {
+      for (int c = 0; c < 3; ++c) P[r * 4 + c] = rot_net[roi * 9 + r * 3 + c];
+      P[r * 4 + 3] = tn[r];
+    }
+    return;
+  }
+  bool use_net_t = pnp_type == PNP_NET_RANSAC_ROT;
+  if (!use_net_t) {
+    const double dx = (double)P[3] - tn[0], dy = (double)P[7] - tn[1], dz = (double)P[11] - tn[2];
+    use_net_t = sqrt(dx * dx + dy * dy + dz * dz) > 1.0;   // gdrn_evaluator.py:347-351
+  }
+  if (use_net_t) { P[3] = tn[0]; P[7] = tn[1]; P[11] = tn[2]; }
+}
+
+constexpr size_t PR_SMEM = (size_t)PR_MAX_PTS * (5 * sizeof(float) + sizeof(unsigned short) + 1);
+
 int launch_pnp(const PnpParams& p, int n, cudaStream_t st) {
-  const size_t smem = (size_t)PR_MAX_PTS * (5 * sizeof(float) + sizeof(unsigned short) + 1);
-  GDRN_OPT_IN_SMEM(pnp_ransac_kernel, smem);
-  pnp_ransac_kernel<<<n, PR_THREADS, smem, st>>>(p);
+  GDRN_OPT_IN_SMEM(pnp_ransac_kernel, PR_SMEM);
+  pnp_ransac_kernel<<<n, PR_THREADS, PR_SMEM, st>>>(p);
+  GDRN_CHECK_CUDA(cudaGetLastError());
+  gdrn_count_launch(1);
+  return GDRN_OK;
+}
+
+int launch_pnp_iterative(const PnpParams& p, const float* rot0, const float* trans0, int n, cudaStream_t st) {
+  GDRN_OPT_IN_SMEM(pnp_iterative_kernel, PR_SMEM);
+  pnp_iterative_kernel<<<n, PR_THREADS, PR_SMEM, st>>>(p, rot0, trans0);
   GDRN_CHECK_CUDA(cudaGetLastError());
   gdrn_count_launch(1);
   return GDRN_OK;
@@ -563,4 +686,38 @@ extern "C" int gdrn_pnp_ransac_points(const float* pts3d, const float* pts2d, co
   p.pts3d = pts3d; p.pts2d = pts2d; p.Ks = Ks; p.idxs = idxs; p.npts = npts; p.iters = iters; p.reproj_thr = reproj_thr;
   p.seed = seed; p.poses = poses; p.n_inliers = n_inliers; p.inlier_mask = inlier_mask;
   return launch_pnp(p, n, (cudaStream_t)stream);
+}
+
+extern "C" int gdrn_pnp_net_maps(const float* coor_x, const float* coor_y, const float* coor_z, const float* mask,
+                                 const float* roi_coord_2d, const float* im_hw, const float* extents, const float* Ks,
+                                 const float* rot_net, const float* trans_net, int n, int hw, int pnp_type, float mask_thr,
+                                 float reproj_thr, int ransac_iters, unsigned seed, float* poses, int* n_used, void* stream) {
+  GDRN_REQUIRE(coor_x && coor_y && coor_z && mask && roi_coord_2d && im_hw && extents && Ks && rot_net && trans_net && poses,
+               "pnp_net: null argument");
+  GDRN_REQUIRE(n > 0 && hw > 0 && hw * hw <= PR_MAX_PTS, "pnp_net: need n > 0 and hw*hw <= 4096");
+  GDRN_REQUIRE(pnp_type == PNP_NET_ITER || pnp_type == PNP_NET_RANSAC || pnp_type == PNP_NET_RANSAC_ROT,
+               "pnp_net: pnp_type must be 0 (net_iter_pnp), 1 (net_ransac_pnp) or 2 (net_ransac_pnp_rot)");
+  GDRN_REQUIRE(pnp_type == PNP_NET_ITER || (ransac_iters >= 1 && ransac_iters <= PR_MAX_HYP),
+               "pnp_net: ransac_iters must be in [1, 256]");
+  cudaStream_t st = (cudaStream_t)stream;
+  PnpParams p = {};
+  p.coor_x = coor_x; p.coor_y = coor_y; p.coor_z = coor_z; p.mask = mask; p.coord2d = roi_coord_2d; p.im_hw = im_hw;
+  p.extents = extents; p.Ks = Ks; p.npts = hw * hw; p.iters = ransac_iters; p.mask_thr = mask_thr;
+  p.reproj_thr = reproj_thr; p.seed = seed; p.poses = poses; p.n_inliers = n_used;
+  if (pnp_type == PNP_NET_ITER) return launch_pnp_iterative(p, rot_net, trans_net, n, st);
+  const int rc = launch_pnp(p, n, st);
+  if (rc != GDRN_OK) return rc;
+  pnp_net_select_kernel<<<(n + 127) / 128, 128, 0, st>>>(poses, rot_net, trans_net, n, pnp_type);
+  GDRN_CHECK_CUDA(cudaGetLastError());
+  gdrn_count_launch(1);
+  return GDRN_OK;
+}
+
+extern "C" int gdrn_pnp_iterative_points(const float* pts3d, const float* pts2d, const float* Ks, const float* rot0,
+                                         const float* trans0, int n, int npts, float* poses, void* stream) {
+  GDRN_REQUIRE(pts3d && pts2d && Ks && rot0 && trans0 && poses, "pnp_iterative: null argument");
+  GDRN_REQUIRE(n > 0 && npts >= 1 && npts <= PR_MAX_PTS, "pnp_iterative: need n > 0 and 1 <= npts <= 4096");
+  PnpParams p = {};
+  p.pts3d = pts3d; p.pts2d = pts2d; p.Ks = Ks; p.npts = npts; p.iters = 1; p.poses = poses;
+  return launch_pnp_iterative(p, rot0, trans0, n, (cudaStream_t)stream);
 }

@@ -169,18 +169,22 @@ __global__ void rast_resolve_kernel(const unsigned long long* __restrict__ zbuf,
 // Fast depth refine, one CTA per ROI (gdrn_evaluator.py:539-561):
 //   w = ||xyz|| * mask * (ren>0) * (sensor>0);  w /= sum(w);  sel = w > thresh*max(w)
 //   dz = median(sensor[sel] - ren[sel]);  (y,x) = sum(w * (row, col));  ray = K^-1 (x,y,1) / z;  t += ray * dz
+// weight_mode 1 (TEST.USE_COOR_Z_REFINE, gdrn_evaluator.py:528-537) replaces ||xyz|| by (R xyz)_z with the ROI's
+// rotation R [n,3,3].  Those weights can be negative, and so can their sum: the reference divides by the sum first and
+// takes the max over ALL pixels (zeros included) afterwards, so a negative sum takes its cut from the most negative
+// raw weight.
 constexpr int DR_THREADS = 1024;
 
 __global__ void __launch_bounds__(DR_THREADS)
 depth_refine_kernel(const float* __restrict__ xyz, const float* __restrict__ mask, const float* __restrict__ sensor,
                     const float* __restrict__ ren, const float* __restrict__ Kc, float* __restrict__ trans, int hw,
-                    float thresh, int mask_mode) {
+                    float thresh, int mask_mode, const float* __restrict__ rot, int weight_mode) {
   extern __shared__ float sm[];  // [npix] weights, then [npow2] diffs for the sort
   const int roi = blockIdx.x;
   const int npix = hw * hw;
   float* sw = sm;
   __shared__ double red_d[32];
-  __shared__ float red_f[32];
+  __shared__ float red_f[32], red_n[32];
   __shared__ int s_count;
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const float* X = xyz + (long long)roi * 3 * npix;
@@ -204,34 +208,40 @@ depth_refine_kernel(const float* __restrict__ xyz, const float* __restrict__ mas
     for (int k = 0; k < DR_THREADS / 32; ++k) { mn = fminf(mn, red_mm[0][k]); mx = fmaxf(mx, red_mm[1][k]); }
     m_lo = mn; m_scale = mx - mn;    // applied as a DIVISION below, like torch's (mask - min) / (max - min)
   }
-  // pass 1: weights, sum (double), max
+  // pass 1: weights, sum (double), max (and min for the signed coor-z weights)
+  const float Rz0 = weight_mode == 1 ? rot[roi * 9 + 6] : 0.f, Rz1 = weight_mode == 1 ? rot[roi * 9 + 7] : 0.f,
+              Rz2 = weight_mode == 1 ? rot[roi * 9 + 8] : 0.f;
   double lsum = 0.0;
-  float lmax = 0.f;
+  float lmax = 0.f, lmin = 0.f;
   for (int i = tid; i < npix; i += DR_THREADS) {
     const float a = X[i], b = X[npix + i], c = X[2 * npix + i];
     float mv = mask[(long long)roi * npix + i];
     if (mask_mode == 1) mv = (mv - m_lo) / m_scale;
     else if (mask_mode == 2) mv = 1.0f / (1.0f + expf(-mv));
-    float wv = sqrtf(a * a + b * b + c * c) * mv;
+    float wv = weight_mode == 1 ? (Rz0 * a + Rz1 * b + Rz2 * c) * mv : sqrtf(a * a + b * b + c * c) * mv;
     const float rd = ren[(long long)roi * npix + i], sd = sensor[(long long)roi * npix + i];
     if (!(rd > 0.f) || !(sd > 0.f)) wv = 0.f;
     sw[i] = wv;
     lsum += (double)wv;
     lmax = fmaxf(lmax, wv);
+    lmin = fminf(lmin, wv);
   }
   for (int o = 16; o > 0; o >>= 1) {
     lsum += __shfl_xor_sync(0xffffffffu, lsum, o);
     lmax = fmaxf(lmax, __shfl_xor_sync(0xffffffffu, lmax, o));
+    lmin = fminf(lmin, __shfl_xor_sync(0xffffffffu, lmin, o));
   }
-  if (lane == 0) { red_d[warp] = lsum; red_f[warp] = lmax; }
+  if (lane == 0) { red_d[warp] = lsum; red_f[warp] = lmax; red_n[warp] = lmin; }
   if (tid == 0) s_count = 0;
   __syncthreads();
   double tsum = 0.0;
-  float tmax = 0.f;
-  for (int k = 0; k < DR_THREADS / 32; ++k) { tsum += red_d[k]; tmax = fmaxf(tmax, red_f[k]); }
+  float tmax = 0.f, tmin = 0.f;
+  for (int k = 0; k < DR_THREADS / 32; ++k) { tsum += red_d[k]; tmax = fmaxf(tmax, red_f[k]); tmin = fminf(tmin, red_n[k]); }
   if (tsum == 0.0) return;  // reference: `continue` (pose unchanged)
   const float inv = (float)(1.0 / tsum);
-  const float cut = (tmax * inv) * thresh;
+  // max over all pixels of w / sum: from the largest raw weight when the sum is positive, from the most negative one
+  // (zeros included in both) when it is negative
+  const float cut = ((weight_mode == 1 && inv < 0.f ? tmin : tmax) * inv) * thresh;
   // pass 2: weighted centroid (double) and selection of depth differences
   int npow2 = 1;
   while (npow2 < npix) npow2 <<= 1;
@@ -399,15 +409,24 @@ extern "C" int gdrn_depth_refine_step(const float* xyz, const float* mask, const
 extern "C" int gdrn_depth_refine_step_ex(const float* xyz, const float* mask, int mask_mode, const float* depth_sensor,
                                          const float* ren_depth, const float* K_crop, float* trans, int n, int hw,
                                          float thresh, void* stream) {
+  return gdrn_depth_refine_step_weighted(xyz, mask, mask_mode, depth_sensor, ren_depth, K_crop, nullptr, 0, trans, n, hw,
+                                         thresh, stream);
+}
+
+extern "C" int gdrn_depth_refine_step_weighted(const float* xyz, const float* mask, int mask_mode, const float* depth_sensor,
+                                               const float* ren_depth, const float* K_crop, const float* rot,
+                                               int weight_mode, float* trans, int n, int hw, float thresh, void* stream) {
   GDRN_REQUIRE(xyz && mask && depth_sensor && ren_depth && K_crop && trans, "depth_refine: null argument");
   GDRN_REQUIRE(mask_mode >= 0 && mask_mode <= 2, "depth_refine: mask_mode must be 0 (normalised), 1 (raw L1) or 2 (logits)");
+  GDRN_REQUIRE(weight_mode == 0 || weight_mode == 1, "depth_refine: weight_mode must be 0 (||xyz||) or 1 (coor-z)");
+  GDRN_REQUIRE(weight_mode == 0 || rot, "depth_refine: the coor-z weighting needs the rotations");
   GDRN_REQUIRE(n > 0 && hw > 0 && hw <= 128, "depth_refine: need 0 < hw <= 128");
   int npix = hw * hw, npow2 = 1;
   while (npow2 < npix) npow2 <<= 1;
   size_t smem = (size_t)(npix + npow2) * 4;
   GDRN_OPT_IN_SMEM(depth_refine_kernel, 160 * 1024);
   depth_refine_kernel<<<n, DR_THREADS, smem, (cudaStream_t)stream>>>(xyz, mask, depth_sensor, ren_depth, K_crop, trans,
-                                                                    hw, thresh, mask_mode);
+                                                                    hw, thresh, mask_mode, rot, weight_mode);
   GDRN_CHECK_CUDA(cudaGetLastError());
   gdrn_count_launch(1);
   return GDRN_OK;

@@ -10,7 +10,9 @@ Keyword-only extras let a caller hand over already-loaded pieces instead of path
 ``inference`` and ``process_depth_refine`` run entirely in libgdrn_b200.so; ``preprocessing`` crops the ROIs with the
 batched GPU restatement of cv2.warpAffine (crop_resize_by_warp_affine, SURVEY.md §8f rank 1); ``postprocessing`` with
 ``TEST.USE_PNP`` (the reference predictor's default, predictor_gdrn.py:58) runs the batched GPU RANSAC-PnP
-(``pnp_ransac.py``) instead of the per-ROI ``cv2.solvePnPRansac`` loop (engine/gdrn_evaluator.py:1122-1221).
+(``pnp_ransac.py``) instead of the per-ROI ``cv2.solvePnPRansac`` loop (engine/gdrn_evaluator.py:1122-1221), or the
+network-initialised variant ``TEST.PNP_TYPE`` names (``net_iter_pnp`` / ``net_ransac_pnp`` / ``net_ransac_pnp_rot``,
+:164-175, 241-371); depth refine honours ``TEST.USE_COOR_Z_REFINE`` (:528-537).
 """
 import glob
 import json
@@ -32,7 +34,8 @@ class GdrnPredictor:
     def __init__(self, config_file_path=None, ckpt_file_path=None, camera_json_path=None, path_to_obj_models=None, *,
                  cam=None, objs=None, extents=None, models=None, state_dict=None, num_classes=None, cfg=None,
                  use_pnp=None, use_depth_refine=None, depth_refine_iter=None, depth_refine_threshold=None,
-                 depth_scale=None, vertex_scale=0.001, device="cuda", precision=None, max_batch=64, use_cuda_graph=True):
+                 depth_scale=None, vertex_scale=0.001, device="cuda", precision=None, max_batch=64, use_cuda_graph=True,
+                 pnp_type=None, use_coor_z_refine=None):
         """Reference arguments (predictor_gdrn.py:45-50):
           config_file_path   reference-style python config (configs/gdrn/**.py); None -> the YCB-V a6 defaults
           ckpt_file_path     torch checkpoint ({"model": state_dict} or a bare state_dict, "_module." prefixes stripped
@@ -42,7 +45,8 @@ class GdrnPredictor:
                              reference's args.vertex_scale): extents come from the vertex bounding boxes (_get_extents,
                              :478-498) and the meshes feed depth refine
         Keyword-only: the same pieces already loaded (cam 3x3, objs {obj_id: name}, extents {obj_id: (3,)} metres,
-        models {obj_id: (verts [V,3] metres, faces [F,3])}, state_dict).
+        models {obj_id: (verts [V,3] metres, faces [F,3])}, state_dict).  pnp_type / use_coor_z_refine override
+        TEST.PNP_TYPE (default "ransac_pnp") / TEST.USE_COOR_Z_REFINE (default False) like use_pnp overrides USE_PNP.
 
         Per-object models (the reference's configs/gdrn/*SO/**: one class-agnostic network per object): pass
         ckpt_file_path={obj_id: path} or state_dict={obj_id: state_dict}, and config_file_path as one per-object config
@@ -78,6 +82,10 @@ class GdrnPredictor:
         T.USE_DEPTH_REFINE = bool(_cfg_get(cfg, "TEST.USE_DEPTH_REFINE", False) if use_depth_refine is None else use_depth_refine)
         T.DEPTH_REFINE_ITER = depth_refine_iter or _cfg_get(cfg, "TEST.DEPTH_REFINE_ITER", 2)
         T.DEPTH_REFINE_THRESHOLD = depth_refine_threshold or _cfg_get(cfg, "TEST.DEPTH_REFINE_THRESHOLD", 0.8)
+        T.PNP_TYPE = str(_cfg_get(cfg, "TEST.PNP_TYPE", "ransac_pnp") if pnp_type is None else pnp_type)
+        T.USE_COOR_Z_REFINE = bool(_cfg_get(cfg, "TEST.USE_COOR_Z_REFINE", False) if use_coor_z_refine is None else use_coor_z_refine)
+        if T.USE_PNP:
+            self._pnp_type()   # an unknown type fails here rather than at the first postprocessing()
         self.dzi_pad_scale = float(_cfg_get(cfg, "INPUT.DZI_PAD_SCALE", 1.5))
         self.pixel_mean = tuple(_cfg_get(cfg, "MODEL.PIXEL_MEAN", (0.0, 0.0, 0.0)))
         self.pixel_std = tuple(_cfg_get(cfg, "MODEL.PIXEL_STD", (255.0, 255.0, 255.0)))
@@ -150,7 +158,7 @@ class GdrnPredictor:
         members = {}
         for oid in ids:
             mcfg = (obj_cfgs or {}).get(oid, self.cfg)
-            for k in ("USE_PNP", "USE_DEPTH_REFINE", "DEPTH_REFINE_ITER", "DEPTH_REFINE_THRESHOLD"):
+            for k in ("USE_PNP", "PNP_TYPE", "USE_DEPTH_REFINE", "USE_COOR_Z_REFINE", "DEPTH_REFINE_ITER", "DEPTH_REFINE_THRESHOLD"):
                 setattr(mcfg.TEST, k, getattr(T, k))   # the predictor's settings apply to every member
             m = GDRN_DoubleMask(mcfg, arch=_arch(mcfg), max_batch=max_batch, precision=precision)
             members[self.obj_ids.index(oid)] = self._load(m, ckpts.get(oid), state_dicts.get(oid))
@@ -270,18 +278,33 @@ class GdrnPredictor:
         return out
 
     # ---- postprocessing (predictor_gdrn.py:149-191) ---------------------------------------------
+    def _pnp_type(self):
+        """TEST.PNP_TYPE, lower-cased like the evaluator's dispatch (gdrn_evaluator.py:164-175)."""
+        from .pnp_ransac import PNP_NET_TYPES
+
+        t = str(self.cfg.TEST.PNP_TYPE).lower()
+        if t != "ransac_pnp" and t not in PNP_NET_TYPES:
+            raise NotImplementedError(f"TEST.PNP_TYPE {self.cfg.TEST.PNP_TYPE!r} (known: ransac_pnp, {', '.join(PNP_NET_TYPES)})")
+        return t
+
     def postprocessing(self, data_dict, out_dict):
         rot = out_dict["rot"]
         trans = out_dict["trans"]
         n = rot.shape[0]
         if self.cfg.TEST.USE_PNP and n > 0:
-            # get_pnp_ransac_pose for every ROI (gdrn_evaluator.py:1122-1221: EPnP RANSAC, reprojErr 3 px, 100 iters),
-            # batched on the GPU; ROIs with < 4 correspondences get the reference's -100 sentinel pose
-            from .pnp_ransac import pnp_ransac_from_maps
+            from .pnp_ransac import pnp_net_from_maps, pnp_ransac_from_maps
 
-            poses = pnp_ransac_from_maps(out_dict["coor_x"], out_dict["coor_y"], out_dict["coor_z"], out_dict["mask"],
-                                         data_dict["roi_coord_2d"], data_dict["im_H"], data_dict["im_W"], data_dict["roi_extent"],
-                                         data_dict["cam"], mask_thr=self.mask_thr)
+            pnp_type = self._pnp_type()
+            maps = (out_dict["coor_x"], out_dict["coor_y"], out_dict["coor_z"], out_dict["mask"], data_dict["roi_coord_2d"],
+                    data_dict["im_H"], data_dict["im_W"], data_dict["roi_extent"], data_dict["cam"])
+            if pnp_type == "ransac_pnp":
+                # get_pnp_ransac_pose for every ROI (gdrn_evaluator.py:1122-1221: EPnP RANSAC, reprojErr 3 px, 100 iters),
+                # batched on the GPU; ROIs with < 4 correspondences get the reference's -100 sentinel pose
+                poses = pnp_ransac_from_maps(*maps, mask_thr=self.mask_thr)
+            else:
+                # process_net_and_pnp (gdrn_evaluator.py:241-371) seeded with the network pose; ROIs with < 4
+                # correspondences keep the network pose
+                poses = pnp_net_from_maps(*maps, rot, trans, pnp_type=pnp_type, mask_thr=self.mask_thr)
             rot, trans = poses[:, :, :3].contiguous(), poses[:, :, 3].contiguous()
             out_dict = dict(out_dict, rot=rot, trans=trans)
         if self.cfg.TEST.USE_DEPTH_REFINE:
@@ -319,7 +342,7 @@ class GdrnPredictor:
         return depth_refine([m.vertices for m in self.ren_models], [m.faces for m in self.ren_models], out_dict["rot"],
                             out_dict["trans"], K_crop, xyz, out_dict["mask"], d.contiguous(),
                             iters=self.cfg.TEST.DEPTH_REFINE_ITER, thresh=self.cfg.TEST.DEPTH_REFINE_THRESHOLD,
-                            mesh_ids=inputs["roi_cls"])
+                            mesh_ids=inputs["roi_cls"], coor_z_refine=bool(self.cfg.TEST.USE_COOR_Z_REFINE))
 
 
 def _arch(cfg):

@@ -108,9 +108,10 @@ def render_meshes(mesh_ids, poses, Ks, H, W, znear=0.1, zfar=100.0, quantize_bit
 
 @_lib.on_device(2)
 def depth_refine(verts, faces, rot, trans, K_crop, xyz, mask, depth_sensor, iters=2, thresh=0.8, mesh_ids=None,
-                 znear=0.1, zfar=100.0, mask_loss_type="L1"):
+                 znear=0.1, zfar=100.0, mask_loss_type="L1", coor_z_refine=False):
     """Batched fast depth refine (gdrn_evaluator.py:515-561): `iters` x (render depth at the current pose ->
-    weighted-median depth offset along the weighted-centroid ray).
+    weighted-median depth offset along the weighted-centroid ray).  The weights are ||xyz|| * mask, or with
+    coor_z_refine (TEST.USE_COOR_Z_REFINE, :528-537) the camera-frame z of the rotated coordinates, (rot @ xyz)_z * mask.
 
     verts/faces: one mesh (tensors) or lists of meshes with `mesh_ids` [n] selecting per ROI.
     rot [n,3,3], trans [n,3], K_crop [n,3,3], xyz [n,3,h,w] (coor maps), mask [n,1,h,w] RAW visible-mask output
@@ -142,9 +143,14 @@ def depth_refine(verts, faces, rot, trans, K_crop, xyz, mask, depth_sensor, iter
     for _ in range(iters):
         poses = torch.cat([rot, t[:, :, None]], dim=2).contiguous()
         ren = render_meshes(ids, poses, K_crop, hw, hw, znear, zfar)
-        _lib.check(L.gdrn_depth_refine_step_ex(_lib.ptr(xyz), _lib.ptr(raw_mask), mask_mode, _lib.ptr(sensor), _lib.ptr(ren),
-                                               _lib.ptr(K_crop), _lib.ptr(t), n, hw, float(thresh), _lib.current_stream()),
-                   "gdrn_depth_refine_step_ex")
+        if coor_z_refine:
+            _lib.check(L.gdrn_depth_refine_step_weighted(_lib.ptr(xyz), _lib.ptr(raw_mask), mask_mode, _lib.ptr(sensor), _lib.ptr(ren),
+                                                         _lib.ptr(K_crop), _lib.ptr(rot), 1, _lib.ptr(t), n, hw, float(thresh),
+                                                         _lib.current_stream()), "gdrn_depth_refine_step_weighted")
+        else:
+            _lib.check(L.gdrn_depth_refine_step_ex(_lib.ptr(xyz), _lib.ptr(raw_mask), mask_mode, _lib.ptr(sensor), _lib.ptr(ren),
+                                                   _lib.ptr(K_crop), _lib.ptr(t), n, hw, float(thresh), _lib.current_stream()),
+                       "gdrn_depth_refine_step_ex")
     return t
 
 

@@ -246,6 +246,13 @@ int gdrn_depth_refine_step(const float* xyz, const float* mask, const float* dep
 int gdrn_depth_refine_step_ex(const float* xyz, const float* mask, int mask_mode, const float* depth_sensor,
                               const float* ren_depth, const float* K_crop, float* trans, int n, int hw, float thresh,
                               void* stream);
+/* same with the weighting selectable: weight_mode 0 = ||xyz|| (the two entries above), 1 = TEST.USE_COOR_Z_REFINE
+ * (gdrn_evaluator.py:528-537): w = (R xyz)_z * mask * (ren > 0) * (sensor > 0) with `xyz` the raw [0,1] coordinate maps
+ * and rot [n,3,3] the rotation of the pose being refined (may be NULL for mode 0).  Signed weights follow the
+ * reference's order: divide by the sum, then threshold against the max over all pixels; a zero sum leaves t unchanged. */
+int gdrn_depth_refine_step_weighted(const float* xyz, const float* mask, int mask_mode, const float* depth_sensor,
+                                    const float* ren_depth, const float* K_crop, const float* rot, int weight_mode,
+                                    float* trans, int n, int hw, float thresh, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
  * ROI crop + resize (SURVEY.md 8f rank 1) -- replaces crop_resize_by_warp_affine = cv2.warpAffine
@@ -285,6 +292,26 @@ int gdrn_pnp_ransac_maps(const float* coor_x, const float* coor_y, const float* 
 int gdrn_pnp_ransac_points(const float* pts3d, const float* pts2d, const float* Ks, const int* idxs, int n, int npts,
                            int iters, float reproj_thr, unsigned seed, float* poses, int* n_inliers,
                            unsigned char* inlier_mask, void* stream);
+
+/* ---------------------------------------------------------------------------------------------
+ * Network-initialised PnP (TEST.PNP_TYPE = net_*) -- replaces the per-ROI host loop process_net_and_pnp
+ * (core/gdrn_modeling/engine/gdrn_evaluator.py:241-371).  Same correspondences as gdrn_pnp_ransac_maps; rot_net [n,3,3]
+ * and trans_net [n,3] are the network's pose.  pnp_type:
+ *   0 net_iter_pnp       cv2.solvePnP(ITERATIVE, useExtrinsicGuess): LM over all correspondences from the network pose
+ *                        (at most 20 iterations).  The reference's 1 m translation guard never fires for this type
+ *                        (cv2 writes the result into the guess it is compared with), so none is applied.
+ *   1 net_ransac_pnp     RANSAC at `ransac_iters` (the reference passes 20); ||t - t_net|| > 1 m -> t = t_net.
+ *   2 net_ransac_pnp_rot R from the RANSAC step, t = t_net.
+ * < 4 correspondences, or no RANSAC model -> the network pose.  n_used [n] (optional): the correspondences the pose was
+ * fitted to (all selected ones for 0, the inliers for 1 / 2), 0 where the network pose is returned.  No host sync.
+ * gdrn_pnp_iterative_points: type 0 on explicit correspondences pts3d [n,npts,3], pts2d [n,npts,2] from (rot0, trans0).
+ * ------------------------------------------------------------------------------------------- */
+int gdrn_pnp_net_maps(const float* coor_x, const float* coor_y, const float* coor_z, const float* mask,
+                      const float* roi_coord_2d, const float* im_hw, const float* extents, const float* Ks,
+                      const float* rot_net, const float* trans_net, int n, int hw, int pnp_type, float mask_thr,
+                      float reproj_thr, int ransac_iters, unsigned seed, float* poses, int* n_used, void* stream);
+int gdrn_pnp_iterative_points(const float* pts3d, const float* pts2d, const float* Ks, const float* rot0,
+                              const float* trans0, int n, int npts, float* poses, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
  * Online training targets (SURVEY.md 8f rank 3) -- after rast_render_meshes, replaces the torch ops of
