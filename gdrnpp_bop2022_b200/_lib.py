@@ -92,6 +92,12 @@ _SIGNATURES = {
     "gdrn_crop_resize_u8": (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p,
                                     c_void_p]),
     "gdrn_crop_resize_f32": (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p]),
+    "gdrn_vsd_workspace_bytes": (c_size_t, [c_int, c_int]),
+    "gdrn_vsd_errors": (c_int, [c_void_p] * 3 + [c_int, c_int] + [c_void_p] * 6 + [c_int, c_void_p, c_int, c_float, c_int,
+                                                                                 c_void_p, c_size_t, c_void_p, c_void_p]),
+    "gdrn_sym_max_dist": (c_int, [c_void_p] * 9 + [c_int, c_int] + [c_void_p] * 3),
+    "gdrn_ad_workspace_bytes": (c_size_t, [c_int, c_int]),
+    "gdrn_ad_errors": (c_int, [c_void_p] * 7 + [c_int, c_int, c_void_p, c_size_t, c_void_p, c_void_p]),
 }
 
 EXPORTED_SYMBOLS = tuple(_SIGNATURES.keys())

@@ -339,6 +339,34 @@ int yolox_postprocess(const float* preds, int B, int A, int num_classes, const i
                       float conf_thre, float nms_thre, int class_agnostic, int max_out, float* dets, int* n_det,
                       void* workspace, size_t workspace_bytes, void* stream);
 
+/* ---------------------------------------------------------------------------------------------
+ * BOP pose errors over a batch of P (estimate, GT) pairs -- replaces the per-pair numpy loops of lib/pysixd/pose_error.py
+ * (vsd, mssd, mspd, add, adi) as eval_calc_errors.py drives them.  Results do not depend on the launch shape.
+ *
+ * gdrn_vsd_errors: depth_est [Ne,H,W], depth_gt [Ng,H,W] (rendered camera-space z), depth_test [Ni,H,W] (0 = missing),
+ *   all f32; pair p reads images pair_est[p], pair_gt[p], pair_img[p] (i32); Ks [P,3,3] f64, diameters [P] f64,
+ *   gate [P] u8 (0 = sphere projections do not overlap -> 1.0 for every tau); taus [T] f64 (T <= 32); delta is compared
+ *   in f32 as the reference does.  errors [P,T] f64 equal the reference's numpy vsd (bop19 visibility, step cost) bit
+ *   for bit.  counts_ws: gdrn_vsd_workspace_bytes(P, T) bytes of 64-bit pixel counts (zeroed here).
+ * gdrn_sym_max_dist: pts [sum N_o, 3] f64 with pt_offsets [O+1] i64; syms [sum S_o, 3, 4] f64 ([R|t]) with sym_offsets
+ *   [O+1] i64 (S_o >= 1); pair_obj [P] i32 indexes the objects; pose_est / pose_gt [P,3,4] f64, Ks [P,3,3] f64;
+ *   max_syms = max S_o.  mssd [P] (inf where gate_mssd[p] == 0) and mspd [P] in the units of pts / pixels.
+ * gdrn_ad_errors: use_adi [P] u8 picks ADI (1) or ADD (0); gate [P] u8 (0 -> inf); max_pts = max N_o;
+ *   ws: gdrn_ad_workspace_bytes(P, max_pts) bytes.  err [P] f64.
+ * ------------------------------------------------------------------------------------------- */
+size_t gdrn_vsd_workspace_bytes(int P, int T);
+int gdrn_vsd_errors(const float* depth_est, const float* depth_gt, const float* depth_test, int H, int W,
+                    const int* pair_est, const int* pair_gt, const int* pair_img, const double* Ks, const double* diameters,
+                    const uint8_t* gate, int P, const double* taus, int T, float delta, int normalized_by_diameter,
+                    void* counts_ws, size_t ws_bytes, double* errors, void* stream);
+int gdrn_sym_max_dist(const double* pts, const int64_t* pt_offsets, const double* syms, const int64_t* sym_offsets,
+                      const int* pair_obj, const double* pose_est, const double* pose_gt, const double* Ks,
+                      const uint8_t* gate_mssd, int P, int max_syms, double* mssd, double* mspd, void* stream);
+size_t gdrn_ad_workspace_bytes(int P, int max_pts);
+int gdrn_ad_errors(const double* pts, const int64_t* pt_offsets, const int* pair_obj, const double* pose_est,
+                   const double* pose_gt, const uint8_t* use_adi, const uint8_t* gate, int P, int max_pts, void* ws,
+                   size_t ws_bytes, double* err, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
