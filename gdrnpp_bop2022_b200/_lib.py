@@ -98,6 +98,8 @@ _SIGNATURES = {
     "gdrn_sym_max_dist": (c_int, [c_void_p] * 9 + [c_int, c_int] + [c_void_p] * 3),
     "gdrn_ad_workspace_bytes": (c_size_t, [c_int, c_int]),
     "gdrn_ad_errors": (c_int, [c_void_p] * 7 + [c_int, c_int, c_void_p, c_size_t, c_void_p, c_void_p]),
+    "gdrn_sym_proj_mean": (c_int, [c_void_p] * 9 + [c_int, c_int] + [c_void_p] * 2),
+    "gdrn_sym_rt_errors": (c_int, [c_void_p] * 6 + [c_int] + [c_void_p] * 3),
 }
 
 EXPORTED_SYMBOLS = tuple(_SIGNATURES.keys())

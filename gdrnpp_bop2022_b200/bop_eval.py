@@ -6,6 +6,8 @@ Mirrors the error functions of lib/pysixd/pose_error.py as lib/pysixd/scripts/ev
                f32 depth images (rendered estimate / GT depth, test depth in mm), K, taus and delta.
   * mssd_mspd  pose_error.mssd / mspd (:131-179) over the symmetry set of misc.get_symmetry_transformations, one pass.
   * ad         pose_error.add / adi (:256-296); ADI is a brute-force nearest-neighbour search in f64.
+  * rt_errors  pose_error.re / te or re_sym / te_sym (:359-437); proj_errors: arp_2d / arp_2d_sym (:183-193, 440-445).
+               These serve eval_pose_results_more.py, the counterpart of the reference script of that name.
 The gates of eval_calc_errors.py:360-374 are host restatements (sphere_projections_overlap, spheres_overlap) whose
 results the calls take per pair.  Units are the BOP ones: points and translations in mm, depth in mm.
 No CPU fallback: every call needs CUDA tensors and raises GdrnError otherwise.
@@ -267,6 +269,57 @@ def ad(models, obj_ids, R_est, t_est, R_gt, t_gt, use_adi, gate=None):
     return err
 
 
+def _sym_inputs(models, obj_ids, R_est, t_est, R_gt, t_gt, use_syms, what):
+    """(P, pair slots, est / GT poses [P,3,4], use_syms [P] u8, max symmetries of one pair) on the models' device."""
+    for x in (models.pts, models.syms, R_est, t_est, R_gt, t_gt, use_syms):
+        if torch.is_tensor(x) and not x.is_cuda:
+            raise GdrnError(f"{what}: needs CUDA tensors or arrays (no CPU fallback)")
+    dev = models.device
+    slots = models.slots(obj_ids)
+    P = len(slots)
+    if P == 0:
+        return 0, None, None, None, None, 0
+    po = torch.tensor(slots, dtype=torch.int32, device=dev)
+    pose_e, pose_g = _poses(R_est, t_est, P, dev, what + " est"), _poses(R_gt, t_gt, P, dev, what + " gt")
+    us = _vec(use_syms, P, torch.uint8, dev, what + " use_syms", broadcast=True)
+    max_syms = max(models.n_syms[s] if u else 1 for s, u in zip(slots, us.cpu().tolist()))
+    return P, po, pose_e, pose_g, us, max_syms
+
+
+def rt_errors(models, obj_ids, R_est, t_est, R_gt, t_gt, use_syms):
+    """Rotation error (deg) and translation error (units of t, mm) of P pairs, pose_error.re / te (use_syms False: the
+    GT pose itself) or re_sym / te_sym (True: min over the object's symmetry set, each error on its own).  use_syms is
+    one flag or [P].  Returns (re_deg [P], te [P]) f64 CUDA tensors."""
+    dev = models.device
+    P, po, pose_e, pose_g, us, _ = _sym_inputs(models, obj_ids, R_est, t_est, R_gt, t_gt, use_syms, "rt_errors")
+    with torch.cuda.device(dev):
+        re_deg = torch.empty(P, dtype=torch.float64, device=dev)
+        te = torch.empty(P, dtype=torch.float64, device=dev)
+        if P:
+            _lib.check(_lib.lib().gdrn_sym_rt_errors(_lib.ptr(models.syms), _lib.ptr(models.sym_offsets), _lib.ptr(po),
+                                                     _lib.ptr(pose_e), _lib.ptr(pose_g), _lib.ptr(us), P, _lib.ptr(re_deg),
+                                                     _lib.ptr(te), _lib.current_stream()), "gdrn_sym_rt_errors")
+    return re_deg, te
+
+
+def proj_errors(models, obj_ids, R_est, t_est, R_gt, t_gt, K, use_syms):
+    """Mean 2D projection distance (px) of P pairs, pose_error.arp_2d (use_syms False) or arp_2d_sym (True: min over the
+    object's symmetry set).  K [P,3,3] or [3,3]; use_syms one flag or [P].  Returns [P] f64."""
+    dev = models.device
+    if torch.is_tensor(K) and not K.is_cuda:
+        raise GdrnError("proj_errors: needs CUDA tensors or arrays (no CPU fallback)")
+    P, po, pose_e, pose_g, us, max_syms = _sym_inputs(models, obj_ids, R_est, t_est, R_gt, t_gt, use_syms, "proj_errors")
+    Ks = _mats(K, P, (3, 3), dev, "proj_errors K") if P else None
+    with torch.cuda.device(dev):
+        err = torch.empty(P, dtype=torch.float64, device=dev)
+        if P:
+            _lib.check(_lib.lib().gdrn_sym_proj_mean(_lib.ptr(models.pts), _lib.ptr(models.pt_offsets),
+                                                     _lib.ptr(models.syms), _lib.ptr(models.sym_offsets), _lib.ptr(po),
+                                                     _lib.ptr(pose_e), _lib.ptr(pose_g), _lib.ptr(Ks), _lib.ptr(us), P,
+                                                     max_syms, _lib.ptr(err), _lib.current_stream()), "gdrn_sym_proj_mean")
+    return err
+
+
 # ---------------------------------------------------------------------------------------------------------------------
 # Rendering for VSD: each estimate and each GT instance rendered once (float z, the egl renderer type's near / far)
 VSD_ZNEAR, VSD_ZFAR = 0.01, 10000.0
@@ -346,25 +399,10 @@ def calc_errors(error_type, dataset, ests, targets, scene_gts, scene_cameras, mo
     -> {scene_id: [{im_id, obj_id, est_id, score, errors: {gt_id: [e, ...]}}]} in the reference's order."""
     if error_type not in ERROR_TYPES:
         raise ValueError(f"error type {error_type!r} is not supported (supported: {', '.join(ERROR_TYPES)})")
-    sel = select_estimates(ests, targets, n_top, skip_missing)
-    records, pairs = {}, []   # pairs: (record, gt_id, scene_id, im_id, obj_id, est, gt)
-    for scene_id, im_id, obj_id, srt in sel:
-        scene_errs = records.setdefault(scene_id, [])
-        for est_id, est in srt:
-            rec = {"im_id": im_id, "obj_id": obj_id, "est_id": est_id, "score": est["score"], "errors": {}}
-            scene_errs.append(rec)
-            for gt_id, gt in enumerate(scene_gts[scene_id][im_id]):
-                if gt["obj_id"] == obj_id:
-                    pairs.append((rec, gt_id, scene_id, im_id, obj_id, est, gt))
+    records, pairs, arrays = error_pairs(ests, targets, scene_gts, scene_cameras, models_info, n_top, skip_missing)
     if not pairs:
         return records
-    diam = np.array([float(models_info[p[4]]["diameter"]) for p in pairs])
-    R_e = np.stack([np.asarray(p[5]["R"], np.float64).reshape(3, 3) for p in pairs])
-    t_e = np.stack([np.asarray(p[5]["t"], np.float64).reshape(3) for p in pairs])
-    R_g = np.stack([np.asarray(p[6]["cam_R_m2c"], np.float64).reshape(3, 3) for p in pairs])
-    t_g = np.stack([np.asarray(p[6]["cam_t_m2c"], np.float64).reshape(3) for p in pairs])
-    K = np.stack([np.asarray(scene_cameras[p[2]][p[3]]["cam_K"], np.float64).reshape(3, 3) for p in pairs])
-    obj = [p[4] for p in pairs]
+    diam, R_e, t_e, R_g, t_g, K, obj = arrays
     if error_type == "vsd":
         errs = _calc_vsd(pairs, obj, R_e, t_e, R_g, t_g, K, diam, meshes, load_depth, vsd_delta,
                          VSD_TAUS if vsd_taus is None else vsd_taus, vsd_normalized_by_diameter, max_bytes)
@@ -377,6 +415,36 @@ def calc_errors(error_type, dataset, ests, targets, scene_gts, scene_cameras, mo
             use_adi = [error_type == "adi" or (error_type == "ad" and is_symmetric(dataset, o, models_info[o])) for o in obj]
             e = ad(models, obj, R_e, t_e, R_g, t_g, use_adi, gate=gate).cpu().numpy()
         errs = e[:, None]
+    return fill_errors(records, pairs, errs)
+
+
+def error_pairs(ests, targets, scene_gts, scene_cameras, models_info, n_top=-1, skip_missing=True):
+    """The (estimate, GT) pairs of eval_calc_errors.py's loop: every selected estimate with every GT instance of its
+    object.  -> (records {scene_id: [{im_id, obj_id, est_id, score, errors: {}}]}, pairs [(record, gt_id, scene_id,
+    im_id, obj_id, est, gt)], (diameters [P], R_e [P,3,3], t_e [P,3], R_g, t_g, K [P,3,3], obj_ids [P])) -- the
+    arrays are None when there is no pair."""
+    records, pairs = {}, []
+    for scene_id, im_id, obj_id, srt in select_estimates(ests, targets, n_top, skip_missing):
+        scene_errs = records.setdefault(scene_id, [])
+        for est_id, est in srt:
+            rec = {"im_id": im_id, "obj_id": obj_id, "est_id": est_id, "score": est["score"], "errors": {}}
+            scene_errs.append(rec)
+            for gt_id, gt in enumerate(scene_gts[scene_id][im_id]):
+                if gt["obj_id"] == obj_id:
+                    pairs.append((rec, gt_id, scene_id, im_id, obj_id, est, gt))
+    if not pairs:
+        return records, pairs, None
+    diam = np.array([float(models_info[p[4]]["diameter"]) for p in pairs])
+    R_e = np.stack([np.asarray(p[5]["R"], np.float64).reshape(3, 3) for p in pairs])
+    t_e = np.stack([np.asarray(p[5]["t"], np.float64).reshape(3) for p in pairs])
+    R_g = np.stack([np.asarray(p[6]["cam_R_m2c"], np.float64).reshape(3, 3) for p in pairs])
+    t_g = np.stack([np.asarray(p[6]["cam_t_m2c"], np.float64).reshape(3) for p in pairs])
+    K = np.stack([np.asarray(scene_cameras[p[2]][p[3]]["cam_K"], np.float64).reshape(3, 3) for p in pairs])
+    return records, pairs, (diam, R_e, t_e, R_g, t_g, K, [p[4] for p in pairs])
+
+
+def fill_errors(records, pairs, errs):
+    """Store row p of errs [P, n] as the error list of pair p in its record.  -> records."""
     for p, e in zip(pairs, errs):
         p[0]["errors"][p[1]] = [float(v) for v in e]
     return records
@@ -583,13 +651,13 @@ def split_errors_per_tau(scene_errs, n_taus):
 
 
 def average_recalls(error_type, errors, targets, scene_gts, scene_gt_infos, models_info, im_width, n_top=-1,
-                    scene_ids=None, obj_ids=None, visib_gt_min=-1, n_taus=len(VSD_TAUS)):
-    """eval_pose_results_more.py:327-360: the recall at every threshold (and, for VSD, every tau) and their mean.
-    errors: calc_errors output.  -> (average recall, [(sign index, threshold, scores, matches)])."""
+                    scene_ids=None, obj_ids=None, visib_gt_min=-1, n_taus=len(VSD_TAUS), correct_th=CORRECT_TH):
+    """eval_pose_results_more.py:327-360: the recall at every threshold of correct_th[error_type] (and, for VSD, every
+    tau) and their mean.  errors: calc_errors output.  -> (average recall, [(sign index, threshold, scores, matches)])."""
     per_sign = split_errors_per_tau(errors, n_taus) if error_type == "vsd" else [errors]
     details = []
     for si, errs in enumerate(per_sign):
-        for th in CORRECT_TH[error_type]:
+        for th in correct_th[error_type]:
             scores, matches = calc_scores(error_type, errs, targets, scene_gts, scene_gt_infos, models_info, im_width, th,
                                           n_top, scene_ids, obj_ids, visib_gt_min)
             details.append((si, th, scores, matches))
@@ -597,16 +665,19 @@ def average_recalls(error_type, errors, targets, scene_gts, scene_gt_infos, mode
 
 
 def evaluate(error_types, dataset, ests, targets, scene_gts, scene_cameras, scene_gt_infos, models_info, im_width,
-             models=None, meshes=None, load_depth=None, n_top=-1, max_bytes=2 << 30, scene_ids=None, obj_ids=None):
+             models=None, meshes=None, load_depth=None, n_top=-1, max_bytes=2 << 30, scene_ids=None, obj_ids=None,
+             calc=calc_errors, correct_th=CORRECT_TH):
     """The BOP19 average recalls of eval_pose_results_more.py:250-380 for the given error types, computed in memory.
+    calc / correct_th: the error dispatch (calc_errors' signature) and the thresholds per error type.
     -> ({'bop19_average_recall_<type>': AR, ..., 'bop19_average_recall': mean of vsd / mssd / mspd}, {type: errors})."""
     final, all_errors = {}, {}
     for et in error_types:
-        errs = calc_errors(et, dataset, ests, targets, scene_gts, scene_cameras, models_info, models, meshes, load_depth,
+        errs = calc(et, dataset, ests, targets, scene_gts, scene_cameras, models_info, models, meshes, load_depth,
                            n_top, True, VSD_DELTAS.get(dataset, 15), VSD_TAUS, True, max_bytes)
         all_errors[et] = errs
         final["bop19_average_recall_" + et] = average_recalls(et, errs, targets, scene_gts, scene_gt_infos, models_info,
-                                                              im_width, n_top, scene_ids, obj_ids)[0]
+                                                              im_width, n_top, scene_ids, obj_ids,
+                                                              correct_th=correct_th)[0]
     if all(t in error_types for t in ("mspd", "mssd", "vsd")):
         final["bop19_average_recall"] = np.mean([final["bop19_average_recall_" + t] for t in ("mspd", "mssd", "vsd")])
     return final, all_errors
@@ -730,11 +801,17 @@ class BopSplit:
 # ---------------------------------------------------------------------------------------------------------------------
 # Command line: the arguments save_and_eval_results passes to VAL.SCRIPT_PATH, the files of eval_pose_results_more.py
 def parse_args(argv=None):
-    ap = argparse.ArgumentParser(description="BOP19 pose-error evaluation on the GPU (VSD, MSSD, MSPD, AD / ADD / ADI)")
+    return parse_eval_args(argv, "BOP19 pose-error evaluation on the GPU (VSD, MSSD, MSPD, AD / ADD / ADI)", "mspd,mssd,vsd",
+                           ERROR_TYPES)
+
+
+def parse_eval_args(argv, description, default_error_types, known_error_types):
+    """The command line of an evaluation script; error types outside known_error_types are rejected with a message."""
+    ap = argparse.ArgumentParser(description=description)
     ap.add_argument("--results_path", default="output/bop_results")
     ap.add_argument("--result_filenames", required=True, help="comma-separated result CSV names")
     ap.add_argument("--renderer_type", default="cuda", help="accepted for compatibility; renders always use the CUDA rasteriser")
-    ap.add_argument("--error_types", default="mspd,mssd,vsd")
+    ap.add_argument("--error_types", default=default_error_types)
     ap.add_argument("--eval_path", default="output/bop_eval/")
     ap.add_argument("--targets_filename", default="test_targets_bop19.json")
     ap.add_argument("--n_top", default=-1, type=int)
@@ -745,15 +822,16 @@ def parse_args(argv=None):
     args = ap.parse_args(argv)
     args.result_filenames = args.result_filenames.split(",")
     args.error_types = args.error_types.split(",")
-    bad = [t for t in args.error_types if t not in ERROR_TYPES]
+    bad = [t for t in args.error_types if t not in known_error_types]
     if bad:
-        ap.error("error types {} are not supported here (supported: {})".format(",".join(bad), ",".join(ERROR_TYPES)))
+        ap.error("error types {} are not supported here (supported: {})".format(",".join(bad), ",".join(known_error_types)))
     return args
 
 
-def run(args):
+def run(args, calc=calc_errors, correct_th=CORRECT_TH):
     """Evaluate every result file; writes errors_*.json, scores_*.json, matches_*.json and scores_bop19.json under
-    eval_path/<result name>/ with the reference's signatures.  -> {result name: final scores}."""
+    eval_path/<result name>/ with the reference's signatures.  calc / correct_th: the error dispatch and thresholds, as
+    for evaluate.  -> {result name: final scores}."""
     out = {}
     for result_filename in args.result_filenames:
         t0 = time.time()
@@ -789,7 +867,7 @@ def run(args):
                 per_sign = [{s: load_json(os.path.join(args.eval_path, result_name, sg, "errors_{:06d}.json".format(s)),
                                           keys_to_int=True) for s in scene_ids} for sg in signs]
             else:
-                errs = calc_errors(et, dataset, ests, targets, scene_gts, scene_cams, models_info, models, meshes,
+                errs = calc(et, dataset, ests, targets, scene_gts, scene_cams, models_info, models, meshes,
                                    lambda s, i: ds.depth(s, i, scene_cams[s][i].get("depth_scale", 1.0)), args.n_top, True,
                                    delta, VSD_TAUS, True, args.max_bytes)
                 per_sign = split_errors_per_tau(errs, len(VSD_TAUS)) if et == "vsd" else [errs]
@@ -800,7 +878,7 @@ def run(args):
                         save_json(os.path.join(d, "errors_{:06d}.json".format(s)), e.get(s, []))
             recalls = []
             for sg, e in zip(signs, per_sign):
-                for th in CORRECT_TH[et]:
+                for th in correct_th[et]:
                     scores, matches = calc_scores(et, e, targets, scene_gts, scene_infos, models_info, ds.im_size[0], th,
                                                   args.n_top, ds.scene_ids, obj_ids)
                     d = os.path.join(args.eval_path, result_name, sg)

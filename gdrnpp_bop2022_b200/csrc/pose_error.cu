@@ -22,6 +22,7 @@ constexpr int SYM_BLOCK = 8;       // symmetries per CTA, one per warp
 constexpr int SYM_THREADS = SYM_BLOCK * 32;
 constexpr int AD_THREADS = 256;    // also the point chunk of one CTA
 constexpr int AD_TILE = 512;       // estimate-pose points per shared-memory tile of the ADI search
+constexpr int RT_THREADS = 128;    // sym_rt_kernel: 4 pairs per CTA, one warp each
 
 __device__ __forceinline__ double warp_max_d(double v) {
 #pragma unroll
@@ -243,6 +244,143 @@ sym_max_dist_kernel(const double* __restrict__ pts, const int64_t* __restrict__ 
   }
 }
 
+__global__ void fill_inf_kernel(double* __restrict__ out, int P) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < P) out[i] = INFINITY;
+}
+
+// The pose a pair is compared against: the GT pose composed with symmetry S (R_g . R_s, R_g . t_s + t_g), or the GT
+// pose itself when S is null (proj / re / te: the identity is not always in an object's symmetry set, see
+// misc.get_symmetry_transformations).
+__device__ __forceinline__ void gt_sym_pose(const double* Pg, const double* S, double* G) {
+  if (!S) {
+    for (int j = 0; j < 12; ++j) G[j] = Pg[j];
+    return;
+  }
+  for (int r = 0; r < 3; ++r) {
+    for (int c = 0; c < 3; ++c) G[r * 4 + c] = Pg[r * 4] * S[c] + Pg[r * 4 + 1] * S[4 + c] + Pg[r * 4 + 2] * S[8 + c];
+    G[r * 4 + 3] = (Pg[r * 4] * S[3] + Pg[r * 4 + 1] * S[7] + Pg[r * 4 + 2] * S[11]) + Pg[r * 4 + 3];
+  }
+}
+
+// misc.transform_pts_Rt_2d (pose_error.py:236-253): camera-space point, then K times it, then the first two rows over
+// the third.  (misc.project_pts, used by MSPD, applies K [R|t] to the homogeneous point instead.)
+__device__ __forceinline__ void project_rt(const double* M, const double* K, double x, double y, double z, double& u,
+                                           double& v) {
+  // explicit roundings: the estimate and the GT projections are inlined at two sites, and equal poses must give equal
+  // bits (a perfect estimate has error 0, as in the reference)
+  double cx, cy, cz;
+  xform(M, x, y, z, cx, cy, cz);
+  const double a = __fma_rn(K[0], cx, __fma_rn(K[1], cy, __dmul_rn(K[2], cz)));
+  const double b = __fma_rn(K[3], cx, __fma_rn(K[4], cy, __dmul_rn(K[5], cz)));
+  const double r = __drcp_rn(__fma_rn(K[6], cx, __fma_rn(K[7], cy, __dmul_rn(K[8], cz))));   // a division per row spills
+  u = __dmul_rn(a, r);
+  v = __dmul_rn(b, r);
+}
+
+// grid (P, ceil(max_syms / SYM_BLOCK)): pose_error.arp_2d / arp_2d_sym, the mean over the object's points of the pixel
+// distance between the estimate-pose and the GT(-symmetry)-pose projections, min over the symmetries.  Warp w owns
+// symmetry w of the block and holds that symmetry's whole sum: lane l adds the distances of points l, l+32, ... in
+// order (tiles are a multiple of 32 points), then an xor tree.  So the bits depend on nothing but the pair.
+__global__ void __launch_bounds__(SYM_THREADS)
+sym_proj_mean_kernel(const double* __restrict__ pts, const int64_t* __restrict__ pt_off, const double* __restrict__ syms,
+                     const int64_t* __restrict__ sym_off, const int* __restrict__ pair_obj,
+                     const double* __restrict__ pose_est, const double* __restrict__ pose_gt,
+                     const double* __restrict__ Ks, const uint8_t* __restrict__ use_syms, double* __restrict__ err) {
+  const int p = blockIdx.x, o = pair_obj[p];
+  const bool sym = use_syms[p] != 0;
+  const int64_t s0 = sym ? sym_off[o] + (int64_t)blockIdx.y * SYM_BLOCK : 0;
+  const int ns = sym ? (int)min((int64_t)SYM_BLOCK, sym_off[o + 1] - s0) : (blockIdx.y == 0 ? 1 : 0);
+  if (ns <= 0) return;
+  __shared__ double s_est[12], s_K[9], s_gs[SYM_BLOCK][12];
+  __shared__ double s_tile[5][SYM_THREADS];   // x, y, z, estimate-pose projection u, v
+  __shared__ double s_red[SYM_BLOCK];
+  if (threadIdx.x < 12) s_est[threadIdx.x] = pose_est[(size_t)p * 12 + threadIdx.x];
+  if (threadIdx.x < 9) s_K[threadIdx.x] = Ks[(size_t)p * 9 + threadIdx.x];
+  if (threadIdx.x < ns) gt_sym_pose(pose_gt + (size_t)p * 12, sym ? syms + (size_t)(s0 + threadIdx.x) * 12 : nullptr,
+                                    s_gs[threadIdx.x]);
+  __syncthreads();
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int ws = min(warp, ns - 1);   // warps past ns idle in the point loop but keep the barriers
+  double G[12], K[9];
+#pragma unroll
+  for (int j = 0; j < 12; ++j) G[j] = s_gs[ws][j];
+#pragma unroll
+  for (int j = 0; j < 9; ++j) K[j] = s_K[j];
+  double sum = 0.0;
+  const double* X = pts + (size_t)pt_off[o] * 3;
+  const int n = (int)(pt_off[o + 1] - pt_off[o]);
+  for (int t0 = 0; t0 < n; t0 += SYM_THREADS) {
+    const int cnt = min(SYM_THREADS, n - t0);
+    __syncthreads();
+    if (threadIdx.x < cnt) {
+      const int i = t0 + threadIdx.x;
+      const double x = X[i * 3], y = X[i * 3 + 1], z = X[i * 3 + 2];
+      double eu, ev;
+      project_rt(s_est, K, x, y, z, eu, ev);
+      s_tile[0][threadIdx.x] = x; s_tile[1][threadIdx.x] = y; s_tile[2][threadIdx.x] = z;
+      s_tile[3][threadIdx.x] = eu; s_tile[4][threadIdx.x] = ev;
+    }
+    __syncthreads();
+    if (warp < ns) {
+      for (int j = lane; j < cnt; j += 32) {
+        double gu, gv;
+        project_rt(G, K, s_tile[0][j], s_tile[1][j], s_tile[2][j], gu, gv);
+        const double du = s_tile[3][j] - gu, dv = s_tile[4][j] - gv;
+        sum = __dadd_rn(sum, sqrt(du * du + dv * dv));
+      }
+    }
+  }
+  sum = warp_sum_d(sum);
+  if (lane == 0 && warp < ns) s_red[warp] = sum / (double)n;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    double best = INFINITY;
+    for (int s = 0; s < ns; ++s) best = fmin(best, s_red[s]);
+    atomicMin((unsigned long long*)(err + p), (unsigned long long)__double_as_longlong(best));
+  }
+}
+
+// pose_error.re / re_sym (:359-396): trace(R_e . R_gs^T), clamped to 3, cos = clip(0.5 (trace - 1), -1, 1), in degrees.
+__device__ __forceinline__ double rot_err_deg(const double* Pe, const double* G) {
+  double tr = 0.0;
+  for (int r = 0; r < 3; ++r) tr += Pe[r * 4] * G[r * 4] + Pe[r * 4 + 1] * G[r * 4 + 1] + Pe[r * 4 + 2] * G[r * 4 + 2];
+  tr = tr <= 3.0 ? tr : 3.0;
+  const double c = fmin(1.0, fmax(-1.0, 0.5 * (tr - 1.0)));
+  return acos(c) * (180.0 / M_PI);
+}
+
+// One warp per pair, lanes over the symmetry set (or the GT pose alone): pose_error.re(_sym) in degrees and
+// te(_sym) = |t_gs - t_e| in the units of t, each minimised over the symmetries on its own (eval_calc_errors.py
+// :574-596 calls the two functions separately).
+__global__ void __launch_bounds__(RT_THREADS)
+sym_rt_kernel(const double* __restrict__ syms, const int64_t* __restrict__ sym_off, const int* __restrict__ pair_obj,
+              const double* __restrict__ pose_est, const double* __restrict__ pose_gt,
+              const uint8_t* __restrict__ use_syms, int P, double* __restrict__ re_deg, double* __restrict__ te) {
+  const int p = blockIdx.x * (RT_THREADS / 32) + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+  if (p >= P) return;   // whole warps leave together
+  const bool sym = use_syms[p] != 0;
+  const int o = pair_obj[p];
+  const int64_t s_begin = sym ? sym_off[o] : 0, s_end = sym ? sym_off[o + 1] : 1;
+  double Pe[12], Pg[12];
+#pragma unroll
+  for (int j = 0; j < 12; ++j) { Pe[j] = pose_est[(size_t)p * 12 + j]; Pg[j] = pose_gt[(size_t)p * 12 + j]; }
+  double best_r = INFINITY, best_t = INFINITY;
+  for (int64_t s = s_begin + lane; s < s_end; s += 32) {
+    double G[12];
+    gt_sym_pose(Pg, sym ? syms + (size_t)s * 12 : nullptr, G);
+    best_r = fmin(best_r, rot_err_deg(Pe, G));
+    const double dx = G[3] - Pe[3], dy = G[7] - Pe[7], dz = G[11] - Pe[11];
+    best_t = fmin(best_t, sqrt(dx * dx + dy * dy + dz * dz));
+  }
+#pragma unroll
+  for (int off = 16; off > 0; off >>= 1) {
+    best_r = fmin(best_r, __shfl_xor_sync(0xffffffffu, best_r, off));
+    best_t = fmin(best_t, __shfl_xor_sync(0xffffffffu, best_t, off));
+  }
+  if (lane == 0) { re_deg[p] = best_r; te[p] = best_t; }
+}
+
 // Fixed-order CTA sum: xor-tree inside each warp, then the warp sums in warp order.
 __device__ __forceinline__ double block_sum_fixed(double v, double* s_red) {
   v = warp_sum_d(v);
@@ -372,6 +510,34 @@ extern "C" int gdrn_sym_max_dist(const double* pts, const int64_t* pt_offsets, c
   sym_max_dist_kernel<<<dim3(P, (max_syms + SYM_BLOCK - 1) / SYM_BLOCK), SYM_THREADS, 0, st>>>(
       pts, pt_offsets, syms, sym_offsets, pair_obj, pose_est, pose_gt, Ks, gate_mssd, mssd, mspd);
   gdrn_count_launch(2);
+  return launch_status();
+}
+
+extern "C" int gdrn_sym_proj_mean(const double* pts, const int64_t* pt_offsets, const double* syms,
+                                  const int64_t* sym_offsets, const int* pair_obj, const double* pose_est,
+                                  const double* pose_gt, const double* Ks, const uint8_t* use_syms, int P, int max_syms,
+                                  double* err, void* stream) {
+  GDRN_REQUIRE(pts && pt_offsets && syms && sym_offsets && pair_obj && pose_est && pose_gt && Ks && use_syms && err,
+               "sym_proj_mean: null argument");
+  GDRN_REQUIRE(P > 0 && max_syms > 0, "sym_proj_mean: need P > 0 and max_syms > 0");
+  cudaStream_t st = (cudaStream_t)stream;
+  fill_inf_kernel<<<(P + 255) / 256, 256, 0, st>>>(err, P);
+  sym_proj_mean_kernel<<<dim3(P, (max_syms + SYM_BLOCK - 1) / SYM_BLOCK), SYM_THREADS, 0, st>>>(
+      pts, pt_offsets, syms, sym_offsets, pair_obj, pose_est, pose_gt, Ks, use_syms, err);
+  gdrn_count_launch(2);
+  return launch_status();
+}
+
+extern "C" int gdrn_sym_rt_errors(const double* syms, const int64_t* sym_offsets, const int* pair_obj,
+                                  const double* pose_est, const double* pose_gt, const uint8_t* use_syms, int P,
+                                  double* re_deg, double* te, void* stream) {
+  GDRN_REQUIRE(syms && sym_offsets && pair_obj && pose_est && pose_gt && use_syms && re_deg && te,
+               "sym_rt_errors: null argument");
+  GDRN_REQUIRE(P > 0, "sym_rt_errors: need P > 0");
+  constexpr int pairs_per_cta = RT_THREADS / 32;
+  sym_rt_kernel<<<(P + pairs_per_cta - 1) / pairs_per_cta, RT_THREADS, 0, (cudaStream_t)stream>>>(
+      syms, sym_offsets, pair_obj, pose_est, pose_gt, use_syms, P, re_deg, te);
+  gdrn_count_launch(1);
   return launch_status();
 }
 

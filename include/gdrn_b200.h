@@ -353,6 +353,12 @@ int yolox_postprocess(const float* preds, int B, int A, int num_classes, const i
  *   max_syms = max S_o.  mssd [P] (inf where gate_mssd[p] == 0) and mspd [P] in the units of pts / pixels.
  * gdrn_ad_errors: use_adi [P] u8 picks ADI (1) or ADD (0); gate [P] u8 (0 -> inf); max_pts = max N_o;
  *   ws: gdrn_ad_workspace_bytes(P, max_pts) bytes.  err [P] f64.
+ * gdrn_sym_proj_mean: pts, syms, pair_obj, poses and Ks as gdrn_sym_max_dist; use_syms [P] u8 picks the object's
+ *   symmetry set (1, arp_2d_sym / projS) or the GT pose alone (0, arp_2d / proj; the set of an object with a continuous
+ *   symmetry holds no identity).  err [P] f64 = min over the symmetries of the mean pixel distance, points projected as
+ *   transform_pts_Rt_2d does (camera space, then K, then / z); max_syms = max over pairs of S_o (or 1).
+ * gdrn_sym_rt_errors: syms, pair_obj, poses and use_syms as above; re_deg [P] f64 = re / re_sym in degrees, te [P] f64 =
+ *   te / te_sym in the units of t, each minimised over the symmetries on its own.
  * ------------------------------------------------------------------------------------------- */
 size_t gdrn_vsd_workspace_bytes(int P, int T);
 int gdrn_vsd_errors(const float* depth_est, const float* depth_gt, const float* depth_test, int H, int W,
@@ -366,6 +372,11 @@ size_t gdrn_ad_workspace_bytes(int P, int max_pts);
 int gdrn_ad_errors(const double* pts, const int64_t* pt_offsets, const int* pair_obj, const double* pose_est,
                    const double* pose_gt, const uint8_t* use_adi, const uint8_t* gate, int P, int max_pts, void* ws,
                    size_t ws_bytes, double* err, void* stream);
+int gdrn_sym_proj_mean(const double* pts, const int64_t* pt_offsets, const double* syms, const int64_t* sym_offsets,
+                       const int* pair_obj, const double* pose_est, const double* pose_gt, const double* Ks,
+                       const uint8_t* use_syms, int P, int max_syms, double* err, void* stream);
+int gdrn_sym_rt_errors(const double* syms, const int64_t* sym_offsets, const int* pair_obj, const double* pose_est,
+                       const double* pose_gt, const uint8_t* use_syms, int P, double* re_deg, double* te, void* stream);
 
 #ifdef __cplusplus
 }
