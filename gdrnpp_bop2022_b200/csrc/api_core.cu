@@ -32,20 +32,10 @@ extern "C" int gdrn_gemm_bf16(const void* A, const void* W, const float* bias, c
                "gemm: N must be a multiple of min(block_n/2, 64) for block_n >= 64");
   GemmPlan p;
   memset(&p, 0, sizeof(p));
-  uint64_t dims_a[2] = {(uint64_t)K, (uint64_t)M};
-  uint64_t str_a[1] = {(uint64_t)K * 2};
-  uint32_t box_a[2] = {64, 128};
-  int rc = make_tmap_bf16(&p.tmap_a, A, 2, dims_a, str_a, box_a);
-  if (rc) return rc;
-  uint64_t dims_b[2] = {(uint64_t)K, (uint64_t)N};
-  uint64_t str_b[1] = {(uint64_t)K * 2};
-  uint32_t box_b[2] = {64, (uint32_t)block_n};
-  rc = make_tmap_bf16(&p.tmap_b, W, 2, dims_b, str_b, box_b);
-  if (rc) return rc;
+  p.a_ptr = A; p.a_dims[0] = K; p.a_dims[1] = M; p.a_str[0] = (uint64_t)K * 2; p.a_box[1] = 128; p.a_k = K;
   p.b_ptr = W; p.b_rows = N; p.b_ktot = K;
   p.a_rank = 2;
   p.num_taps = 1;
-  p.k_chunks = (K + 63) / 64;
   p.taps[0] = {0, 0, 0, 0, 0};
   p.m_tiles = (M + 127) / 128;
   p.n_tiles = (N + block_n - 1) / block_n;
@@ -67,7 +57,7 @@ extern "C" int gdrn_gemm_bf16(const void* A, const void* W, const float* bias, c
   if (!d_trace) GDRN_CHECK_CUDA(cudaMalloc(&d_trace, 16 * sizeof(long long)));
   GDRN_CHECK_CUDA(cudaMemsetAsync(d_trace, 0, 16 * sizeof(long long), (cudaStream_t)stream));
   p.trace = d_trace;
-  rc = gemm_tc_launch(p, block_n, (cudaStream_t)stream);
+  int rc = gemm_tc_launch(p, block_n, (cudaStream_t)stream);
   if (rc != GDRN_OK) return rc;
   long long h[16];
   GDRN_CHECK_CUDA(cudaMemcpyAsync(h, d_trace, sizeof(h), cudaMemcpyDeviceToHost, (cudaStream_t)stream));
@@ -102,20 +92,10 @@ extern "C" int gdrn_gemm_x3(const void* A, const void* W, const float* bias, con
   GDRN_REQUIRE(N % 64 == 0, "gemm_x3: N must be a multiple of 64");
   GemmPlan p;
   memset(&p, 0, sizeof(p));
-  uint64_t dims_a[2] = {(uint64_t)2 * K, (uint64_t)M};
-  uint64_t str_a[1] = {(uint64_t)2 * K * 2};
-  uint32_t box_a[2] = {64, 128};
-  int rc = make_tmap_bf16(&p.tmap_a, A, 2, dims_a, str_a, box_a);
-  if (rc) return rc;
-  uint64_t dims_b[2] = {(uint64_t)2 * K, (uint64_t)N};
-  uint64_t str_b[1] = {(uint64_t)2 * K * 2};
-  uint32_t box_b[2] = {64, (uint32_t)block_n};
-  rc = make_tmap_bf16(&p.tmap_b, W, 2, dims_b, str_b, box_b);
-  if (rc) return rc;
+  p.a_ptr = A; p.a_dims[0] = 2ULL * K; p.a_dims[1] = M; p.a_str[0] = 4ULL * K; p.a_box[1] = 128; p.a_k = K;
   p.b_ptr = W; p.b_rows = N; p.b_ktot = 2LL * K;
   p.a_rank = 2;
   p.num_taps = 1;
-  p.k_chunks = K / 64;
   p.taps[0] = {0, 0, 0, 0, 0};
   p.m_tiles = (M + 127) / 128;
   p.n_tiles = (N + block_n - 1) / block_n;
@@ -138,7 +118,7 @@ extern "C" int gdrn_gemm_x3(const void* A, const void* W, const float* bias, con
     if (!d_trace) GDRN_CHECK_CUDA(cudaMalloc(&d_trace, 16 * sizeof(long long)));
     GDRN_CHECK_CUDA(cudaMemsetAsync(d_trace, 0, 16 * sizeof(long long), (cudaStream_t)stream));
     p.trace = d_trace;
-    rc = gemm_tc_launch(p, block_n, (cudaStream_t)stream);
+    int rc = gemm_tc_launch(p, block_n, (cudaStream_t)stream);
     if (rc != GDRN_OK) return rc;
     long long h[16];
     GDRN_CHECK_CUDA(cudaMemcpyAsync(h, d_trace, sizeof(h), cudaMemcpyDeviceToHost, (cudaStream_t)stream));

@@ -285,6 +285,17 @@ __device__ __forceinline__ uint64_t make_sw128_kmajor_desc(uint32_t smem_addr) {
   return d;
 }
 
+// Same for 64-byte-swizzled tiles (rows of 32 bf16 = 64 B, 8-row atoms of 512 B, CU_TENSOR_MAP_SWIZZLE_64B): SBO = 512 B,
+// layout type 2 = SWIZZLE_64B.  Tile starts are 512-byte aligned, so the base-offset field [49,52) stays 0.
+__device__ __forceinline__ uint64_t make_sw64_kmajor_desc(uint32_t smem_addr) {
+  uint64_t d = 0;
+  d |= (uint64_t)((smem_addr & 0x3FFFF) >> 4);        // [0,14)  start address
+  d |= (uint64_t)1 << 16;                             // [16,30) leading byte offset (>>4)
+  d |= (uint64_t)(512 >> 4) << 32;                    // [32,46) stride byte offset (>>4)
+  d |= (uint64_t)2 << 62;                             // [62,64) layout type SWIZZLE_64B
+  return d;
+}
+
 }  // namespace ptx
 
 // exact-erf GELU (torch nn.GELU() default), x * Phi(x), BRANCH-FREE and short:

@@ -10,9 +10,7 @@ extern __shared__ uint8_t gemm_smem[];
 namespace {
 
 constexpr int BLOCK_M = 128;
-constexpr int BLOCK_K = 64;  // 64 bf16 = 128 B = one swizzle row
 constexpr int MMA_K = 16;
-constexpr int A_STAGE_BYTES = BLOCK_M * BLOCK_K * 2;  // 16 KB
 constexpr int NUM_THREADS = 384;              // producer warpgroup + 2 MMA / epilogue warpgroups (8 warps)
 constexpr int NUM_EPI_WARPS = 8;
 constexpr int EPI_STAGE_PITCH = 80;           // 64-byte row segment + 16 B pad (conflict-free 16-byte accesses)

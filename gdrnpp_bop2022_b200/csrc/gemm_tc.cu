@@ -1,13 +1,14 @@
 // wgmma + TMA implicit-GEMM kernel for the GDRNPP dense path (sm_90a).
 //
 // One persistent CTA per SM, warp-specialised:
-//   warp 0 lane 0   : TMA producer  (A pixel boxes + W tiles -> 128B-swizzled smem ring)
+//   warp 0 lane 0   : TMA producer  (A pixel boxes + W tiles -> swizzled smem ring)
 //   warps 4..11     : two consumer warpgroups.  Warpgroup g issues wgmma m64 x BLOCK_N x 16 (bf16 -> fp32 registers)
 //                     for rows [64g, 64g + 64) of the 128-row tile, releases each ring stage as soon as the MMAs that
 //                     read it retire, then writes its accumulators into the shared-memory accumulator tile; the same
 //                     8 warps then run the fused epilogue from there (gemm_epilogue.cuh) while the producer already
 //                     fills the ring for the next tile.
-// X3 (split-bf16, 64- / 128-wide tiles): a stage holds {A hi, A lo, W hi, W lo} and feeds all three products.
+// X3 (split-bf16, 64- / 128-wide tiles): a stage holds {A hi, A lo, W hi, W lo} of one k-chunk (32 wide for convolutions,
+// 64 for plain rows) and feeds all three products.
 // The kernel makes no function call: any call makes ptxas serialize the wgmma pipeline (C7510).
 //
 // It replaces, for the reference forward (core/gdrn_modeling/models/GDRN_double_mask.py:102-160), every
@@ -25,27 +26,39 @@ namespace {
 
 // X3: split-bf16 operands with the shared four-tile stage {A hi, A lo, W hi, W lo} of one (tap, k-chunk) feeding the three
 // products A_lo*W_hi + A_hi*W_lo + A_hi*W_hi (4 operand tiles per 3 MMA groups instead of 6 with an expanded tap list).
-template <int BLOCK_N, bool X3>
+// BK: k-chunk width (bf16 elements) of one ring stage.  64 = 128-byte rows (SWIZZLE_128B); 32 = 64-byte rows
+// (SWIZZLE_64B), X3 only: half the bytes per stage, twice the ring depth (gemm_tc_launch picks it, see there).
+template <int BLOCK_N, bool X3, int BK = 64>
 struct Cfg {
+  static_assert(BK == 64 || (X3 && BK == 32), "gemm: 32-wide k-chunks exist for the split-bf16 kernel only");
+  static constexpr int BLOCK_K = BK;
   static constexpr int NOPS = X3 ? 2 : 1;  // hi (and lo) copies of each operand per stage
+  static constexpr int A_TILE_BYTES = BLOCK_M * BLOCK_K * 2;
   static constexpr int B_TILE_BYTES = BLOCK_N * BLOCK_K * 2;
   static constexpr int B_STAGE_BYTES = NOPS * B_TILE_BYTES;
-  static constexpr int A_BYTES = NOPS * A_STAGE_BYTES;
+  static constexpr int A_BYTES = NOPS * A_TILE_BYTES;
   static constexpr int STAGE_BYTES = A_BYTES + B_STAGE_BYTES;
   static constexpr int ACC_BYTES = acc_bytes<BLOCK_N>();
   static constexpr int RING = (SMEM_BUDGET - ACC_BYTES) / STAGE_BYTES;
   static constexpr int STAGES = RING > 8 ? 8 : RING;
   static constexpr int SMEM_BYTES = ACC_BYTES + STAGES * STAGE_BYTES + 1024 /*align*/ + 256 /*barriers*/ + NUM_EPI_WARPS * EPI_STAGE_BYTES;
+  // L2 prefetch distance of A: 384 k-elements ahead of the ring, whatever the chunk width
+  static constexpr int PREFETCH_AHEAD = 384 / BLOCK_K;
   static_assert(STAGES >= 2, "gemm: shared-memory ring needs two stages");
+  // every tile start (stage, hi / lo half, warpgroup half of A) stays on a swizzle atom (1024 B / 512 B)
+  static_assert(ACC_BYTES % 1024 == 0 && STAGE_BYTES % 1024 == 0 && A_TILE_BYTES % 1024 == 0 && B_TILE_BYTES % 1024 == 0,
+                "gemm: operand tiles must keep the swizzle-atom alignment");
 };
+// the 32-wide X3 kernel consumes its stages in pairs (one 64-wide k-step): at BLOCK_N = 128 two more stages load meanwhile
+static_assert(Cfg<128, true, 32>::STAGES >= 4, "gemm: the 32-wide split-bf16 128-wide kernel needs a four-deep operand ring");
+static_assert(Cfg<64, true, 32>::STAGES >= 6, "gemm: the 32-wide split-bf16 64-wide kernel needs a six-deep operand ring");
 
-constexpr int PREFETCH_AHEAD = 6;  // k-iterations of A/B requested into L2 ahead of the shared-memory ring
 constexpr int CONSUMER_THREADS = 256;
 constexpr int BAR_ACC = 1;         // named barrier of the two consumer warpgroups (accumulator tile hand-over)
 
-template <int BLOCK_N, int EPI, bool X3>
+template <int BLOCK_N, int EPI, bool X3, int BK>
 __global__ void __launch_bounds__(NUM_THREADS, 1) gemm_tc_kernel(const __grid_constant__ GemmPlan p) {
-  using C = Cfg<BLOCK_N, X3>;
+  using C = Cfg<BLOCK_N, X3, BK>;
   // 1024-byte alignment required by SWIZZLE_128B: [accumulator tile | ring | epilogue staging | barriers]
   const uint32_t smem_base = (ptx::smem_u32(gemm_smem) + 1023u) & ~1023u;
   const uint32_t ring_base = smem_base + C::ACC_BYTES;
@@ -113,10 +126,10 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) gemm_tc_kernel(const __grid_co
           const uint32_t sa = ring_base + stage * C::STAGE_BYTES;
           const uint32_t sb = sa + C::A_BYTES;
           ptx::mbar_arrive_expect_tx(full_bar(stage), C::STAGE_BYTES);
-          const int k0 = kc * BLOCK_K;
+          const int k0 = kc * C::BLOCK_K;
 #pragma unroll
           for (int h = 0; h < C::NOPS; ++h) {   // h = 1: the lo halves, behind the hi tiles of the stage
-            const uint32_t da = sa + h * A_STAGE_BYTES;
+            const uint32_t da = sa + h * C::A_TILE_BYTES;
             const int ca = k0 + tp.c0 + h * p.x3_a_lo;
             if (p.a_rank == 2) {
               ptx::tma_load_2d(da, &p.tmap_a, full_bar(stage), ca, m_tile * BLOCK_M + tp.d1);
@@ -130,14 +143,14 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) gemm_tc_kernel(const __grid_co
           if (p.a_rank == 2) {
             // A is streamed from HBM (it was written by the previous kernel): request it into L2 several
             // k-iterations ahead so the shared-memory ring only has to cover L2 latency, not DRAM latency.
-            int pk = kc + PREFETCH_AHEAD, pm = m_tile;
+            int pk = kc + C::PREFETCH_AHEAD, pm = m_tile;
             if (pk >= p.k_chunks) {
               pk -= p.k_chunks;
               const int nt = tile + gridDim.x;
               const int nm = p.n_major ? nt % p.m_tiles : nt / p.n_tiles;
               pm = (nt < total_tiles && nm != m_tile) ? nm : -1;
             }
-            if (pm >= 0 && pk < p.k_chunks && p.num_taps == 1) ptx::tma_prefetch_2d(&p.tmap_a, pk * BLOCK_K, pm * BLOCK_M);
+            if (pm >= 0 && pk < p.k_chunks && p.num_taps == 1) ptx::tma_prefetch_2d(&p.tmap_a, pk * C::BLOCK_K, pm * BLOCK_M);
           }
           if (++stage == C::STAGES) { stage = 0; phase ^= 1; }
         }
@@ -159,30 +172,74 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) gemm_tc_kernel(const __grid_co
 #pragma unroll
       for (int i = 0; i < BLOCK_N / 2; ++i) acc[i] = 0.f;
       int prev_stage = -1;
-      for (int k = 0; k < k_iters; ++k) {
-        { const long long t0 = tr_me ? clock64() : 0; ptx::mbar_wait_nocall(full_bar(stage), phase); if (tr_me) tr_acc0 += clock64() - t0; }
-        const uint32_t sa = ring_base + stage * C::STAGE_BYTES + wg * (A_STAGE_BYTES / 2);
-        const uint32_t sb = ring_base + stage * C::STAGE_BYTES + C::A_BYTES;
-        ptx::wgmma_fence();
-        // X3: (A lo, W hi), (A hi, W lo), (A hi, W hi) -- small terms first; otherwise the single (A, W) product
-#pragma unroll
-        for (int q = 0; q < (X3 ? 3 : 1); ++q) {
-          const uint32_t a_off = (X3 && q == 0) ? A_STAGE_BYTES : 0u;
-          const uint32_t b_off = (X3 && q == 1) ? C::B_TILE_BYTES : 0u;
-          const uint64_t adesc = ptx::make_sw128_kmajor_desc(sa + a_off);
-          const uint64_t bdesc = ptx::make_sw128_kmajor_desc(sb + b_off);
-#pragma unroll
-          for (int kk = 0; kk < BLOCK_K / MMA_K; ++kk) {
-            // advance 16 bf16 = 32 B inside the 128B swizzle row: +2 in the (addr >> 4) field
-            ptx::Wgmma<BLOCK_N>::mma(acc, adesc + 2u * kk, bdesc + 2u * kk, (k | q | kk) != 0 ? 1u : 0u);
-          }
+      if constexpr (X3 && BK == 32) {
+        // Two 32-wide stages make one 64-wide k-step, issued as A_lo*W_hi, A_hi*W_lo, A_hi*W_hi over all 64 k -- small
+        // terms first, and the fp32 summation order of a 64-wide stage -- in four commit groups, so that the first stage
+        // is released as soon as its last product (hi*hi) retires, while the second one's hi*hi still runs.
+        for (int k = 0; k < k_iters; k += 2) {
+          const int s0 = stage;
+          const uint32_t ph0 = phase;
+          if (++stage == C::STAGES) { stage = 0; phase ^= 1; }
+          const int s1 = stage;
+          const uint32_t ph1 = phase;
+          if (++stage == C::STAGES) { stage = 0; phase ^= 1; }
+          const uint32_t a0 = ring_base + s0 * C::STAGE_BYTES + wg * (C::A_TILE_BYTES / 2);
+          const uint32_t b0 = ring_base + s0 * C::STAGE_BYTES + C::A_BYTES;
+          const uint32_t a1 = ring_base + s1 * C::STAGE_BYTES + wg * (C::A_TILE_BYTES / 2);
+          const uint32_t b1 = ring_base + s1 * C::STAGE_BYTES + C::A_BYTES;
+          // one product over a 32-wide stage: two k16 steps, +32 B (+2 in the (addr >> 4) field) inside the swizzle row
+          auto mma32 = [&](uint32_t a, uint32_t b, uint32_t accumulate) {
+            const uint64_t ad = ptx::make_sw64_kmajor_desc(a), bd = ptx::make_sw64_kmajor_desc(b);
+            ptx::Wgmma<BLOCK_N>::mma(acc, ad, bd, accumulate);
+            ptx::Wgmma<BLOCK_N>::mma(acc, ad + 2u, bd + 2u, 1u);
+          };
+          { const long long t0 = tr_me ? clock64() : 0; ptx::mbar_wait_nocall(full_bar(s0), ph0); if (tr_me) tr_acc0 += clock64() - t0; }
+          ptx::wgmma_fence();
+          mma32(a0 + C::A_TILE_BYTES, b0, k != 0 ? 1u : 0u);                  // lo*hi, k [0, 32)
+          ptx::wgmma_commit();
+          // the previous k-step's last group has retired: release its second stage
+          ptx::wgmma_wait<1>();
+          if (prev_stage >= 0 && wl == 0 && lane == 0) ptx::mbar_arrive(empty_bar(prev_stage));
+          { const long long t0 = tr_me ? clock64() : 0; ptx::mbar_wait_nocall(full_bar(s1), ph1); if (tr_me) tr_acc0 += clock64() - t0; }
+          ptx::wgmma_fence();
+          mma32(a1 + C::A_TILE_BYTES, b1, 1u);                                // lo*hi, k [32, 64)
+          mma32(a0, b0 + C::B_TILE_BYTES, 1u);                                // hi*lo, k [0, 32)
+          ptx::wgmma_commit();
+          mma32(a1, b1 + C::B_TILE_BYTES, 1u);                                // hi*lo, k [32, 64)
+          mma32(a0, b0, 1u);                                                  // hi*hi, k [0, 32): last read of s0
+          ptx::wgmma_commit();
+          mma32(a1, b1, 1u);                                                  // hi*hi, k [32, 64)
+          ptx::wgmma_commit();
+          ptx::wgmma_wait<1>();
+          if (wl == 0 && lane == 0) ptx::mbar_arrive(empty_bar(s0));
+          prev_stage = s1;
         }
-        ptx::wgmma_commit();
-        // the previous stage's MMAs have retired once at most this stage's group is in flight: release that slot
-        ptx::wgmma_wait<1>();
-        if (prev_stage >= 0 && wl == 0 && lane == 0) ptx::mbar_arrive(empty_bar(prev_stage));
-        prev_stage = stage;
-        if (++stage == C::STAGES) { stage = 0; phase ^= 1; }
+      } else {
+        for (int k = 0; k < k_iters; ++k) {
+          { const long long t0 = tr_me ? clock64() : 0; ptx::mbar_wait_nocall(full_bar(stage), phase); if (tr_me) tr_acc0 += clock64() - t0; }
+          const uint32_t sa = ring_base + stage * C::STAGE_BYTES + wg * (C::A_TILE_BYTES / 2);
+          const uint32_t sb = ring_base + stage * C::STAGE_BYTES + C::A_BYTES;
+          ptx::wgmma_fence();
+          // X3: (A lo, W hi), (A hi, W lo), (A hi, W hi) -- small terms first; otherwise the single (A, W) product
+#pragma unroll
+          for (int q = 0; q < (X3 ? 3 : 1); ++q) {
+            const uint32_t a_off = (X3 && q == 0) ? C::A_TILE_BYTES : 0u;
+            const uint32_t b_off = (X3 && q == 1) ? C::B_TILE_BYTES : 0u;
+            const uint64_t adesc = ptx::make_sw128_kmajor_desc(sa + a_off);
+            const uint64_t bdesc = ptx::make_sw128_kmajor_desc(sb + b_off);
+#pragma unroll
+            for (int kk = 0; kk < C::BLOCK_K / MMA_K; ++kk) {
+              // advance 16 bf16 = 32 B inside the 128B swizzle row: +2 in the (addr >> 4) field
+              ptx::Wgmma<BLOCK_N>::mma(acc, adesc + 2u * kk, bdesc + 2u * kk, (k | q | kk) != 0 ? 1u : 0u);
+            }
+          }
+          ptx::wgmma_commit();
+          // the previous stage's MMAs have retired once at most this stage's group is in flight: release that slot
+          ptx::wgmma_wait<1>();
+          if (prev_stage >= 0 && wl == 0 && lane == 0) ptx::mbar_arrive(empty_bar(prev_stage));
+          prev_stage = stage;
+          if (++stage == C::STAGES) { stage = 0; phase ^= 1; }
+        }
       }
       ptx::wgmma_wait<0>();
       if (prev_stage >= 0 && wl == 0 && lane == 0) ptx::mbar_arrive(empty_bar(prev_stage));
@@ -228,10 +285,10 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) gemm_tc_kernel(const __grid_co
   }
 }
 
-template <int BLOCK_N, int EPI, bool X3 = false>
+template <int BLOCK_N, int EPI, bool X3 = false, int BK = 64>
 int launch_inst(const GemmPlan& plan, cudaStream_t stream) {
-  using C = Cfg<BLOCK_N, X3>;
-  auto kfn = gemm_tc_kernel<BLOCK_N, EPI, X3>;
+  using C = Cfg<BLOCK_N, X3, BK>;
+  auto kfn = gemm_tc_kernel<BLOCK_N, EPI, X3, BK>;
   GDRN_OPT_IN_SMEM(kfn, C::SMEM_BYTES);
   int total = plan.m_tiles * plan.n_tiles;
   if (total <= 0) return GDRN_OK;
@@ -251,16 +308,11 @@ int gemm_tc_launch(const GemmPlan& plan_in, int block_n, cudaStream_t stream) {
     if (order >= 0) plan.n_major = order;
   }
   GDRN_REQUIRE(plan.a_rank == 2 || plan.a_rank == 4 || plan.a_rank == 5, "gemm: bad a_rank");
+  GDRN_REQUIRE(plan.a_ptr != nullptr && plan.b_ptr != nullptr && plan.a_k > 0, "gemm: plan without operands");
   plan.use_tma_store = 0;
   plan.resid_reduce = 0;
   if (block_n > 128) {
     // 128 x 256 tiles would need a 128 KB accumulator tile next to the operand ring: run them as two 128-wide tiles
-    GDRN_REQUIRE(plan.b_ptr != nullptr, "gemm: block_n 256 needs plan.b_ptr to re-tile W");
-    const uint64_t dims[2] = {(uint64_t)plan.b_ktot, (uint64_t)plan.b_rows};
-    const uint64_t str[1] = {(uint64_t)plan.b_ktot * 2};
-    const uint32_t box[2] = {64, 128};
-    int rc = make_tmap_bf16(&plan.tmap_b, plan.b_ptr, 2, dims, str, box);
-    if (rc != GDRN_OK) return rc;
     block_n = 128;
     plan.n_tiles = (plan.N + block_n - 1) / block_n;
   }
@@ -281,6 +333,22 @@ int gemm_tc_launch(const GemmPlan& plan_in, int block_n, cudaStream_t stream) {
     }
     plan.num_taps = 3 * n;
     plan.x3_expanded = 1;
+  }
+  // k-chunk width.  Split-bf16 convolutions (rank-4/5 pixel boxes, A re-read from L2 by every tap) run 32-wide chunks: the
+  // deeper ring covers their L2 round trips.  Plain rank-2 rows keep 64-wide chunks: they stream A from HBM, where 128-byte
+  // rows beat 64-byte ones (DESIGN §4.1, §7).
+  const int bk = (x3_shared && plan.a_rank != 2) ? 32 : 64;
+  {  // operand maps at that width
+    GDRN_REQUIRE(!x3_shared || plan.a_k % 64 == 0, "gemm: split-bf16 K per tap must be a multiple of 64");
+    plan.a_box[0] = (uint32_t)bk;
+    int rc = make_tmap_bf16(&plan.tmap_a, plan.a_ptr, plan.a_rank, plan.a_dims, plan.a_str, plan.a_box);
+    if (rc != GDRN_OK) return rc;
+    const uint64_t dims[2] = {(uint64_t)plan.b_ktot, (uint64_t)plan.b_rows};
+    const uint64_t str[1] = {(uint64_t)plan.b_ktot * 2};
+    const uint32_t box[2] = {(uint32_t)bk, (uint32_t)block_n};
+    rc = make_tmap_bf16(&plan.tmap_b, plan.b_ptr, 2, dims, str, box);
+    if (rc != GDRN_OK) return rc;
+    plan.k_chunks = (plan.a_k + bk - 1) / bk;
   }
   {
     static int tma_epi = -1;  // GDRN_TMA_STORE=0 falls back to the gather-store epilogue (A/B experiments)
@@ -313,7 +381,8 @@ int gemm_tc_launch(const GemmPlan& plan_in, int block_n, cudaStream_t stream) {
   }
   GDRN_REQUIRE(plan.num_taps >= 1 && plan.num_taps <= GEMM_MAX_TAPS, "gemm: bad num_taps");
 #define GDRN_GEMM_CASE_X3(BN, E) \
-  if (x3_shared && block_n == BN && plan.epi == E) return launch_inst<BN, E, true>(plan, stream);
+  if (x3_shared && block_n == BN && plan.epi == E)                                                          \
+    return bk == 32 ? launch_inst<BN, E, true, 32>(plan, stream) : launch_inst<BN, E, true, 64>(plan, stream);
   GDRN_GEMM_CASE_X3(128, EPI_GELU)
   GDRN_GEMM_CASE_X3(128, EPI_RESID)
   GDRN_GEMM_CASE_X3(128, EPI_STORE)
@@ -435,6 +504,7 @@ int make_tmap_bf16(CUtensorMap* out, const void* base, int rank, const uint64_t*
                    const uint32_t* box) {
   PFN_encodeTiled fn = get_encode_fn();
   GDRN_REQUIRE(fn != nullptr, "cuTensorMapEncodeTiled not available (no CUDA driver?)");
+  GDRN_REQUIRE(box[0] == 64 || box[0] == 32, "make_tmap_bf16: k-chunk box must be 64 or 32 elements");
   cuuint64_t gdim[5];
   cuuint64_t gstr[4];
   cuuint32_t bx[5];
@@ -446,8 +516,8 @@ int make_tmap_bf16(CUtensorMap* out, const void* base, int rank, const uint64_t*
     if (i > 0) gstr[i - 1] = strides_bytes[i - 1];
   }
   CUresult r = fn(out, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, (cuuint32_t)rank, const_cast<void*>(base), gdim, gstr, bx, es,
-                  CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                  CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+                  CU_TENSOR_MAP_INTERLEAVE_NONE, box[0] == 32 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_128B,
+                  CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) {
     char msg[160];
     snprintf(msg, sizeof(msg), "cuTensorMapEncodeTiled failed: CUresult %d (rank %d dims %llu,%llu box %u,%u)", (int)r,

@@ -3,7 +3,9 @@
 //   D[m, n] = sum_{tap} sum_{k} A_tap[m, k] * W[n, tap.b_off + k]      (bf16 x bf16 -> fp32)
 //
 // A rows are pixels of an NHWC activation tensor: a 128-row tile is a (bw x bh x bb) box of pixels
-// fetched by one TMA box load per (tap, 64-channel chunk); conv padding = TMA out-of-bounds zero fill.
+// fetched by one TMA box load per (tap, k-chunk); conv padding = TMA out-of-bounds zero fill.  The k-chunk width (32
+// for split-bf16 convolutions, 64 otherwise) is chosen by gemm_tc_launch, which encodes both operand maps from the plan's
+// a_* / b_* geometry.
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
@@ -30,17 +32,22 @@ constexpr int GEMM_MAX_TAPS = 27;  // 9 spatial taps x 3 split-bf16 products
 
 struct GemmPlan {
   // ---- A operand ----
-  CUtensorMap tmap_a;
+  CUtensorMap tmap_a;   // set by gemm_tc_launch from a_ptr / a_dims / a_str / a_box
   int a_rank;           // 2: plain [M,K] rows; 4: (C,W,H,B); 5: (2C, W/2, 2, H/2, B) stride-2 view
+  const void* a_ptr;    // A base
+  uint64_t a_dims[5];   // tensor dims, innermost (channels) first
+  uint64_t a_str[4];    // byte strides of dims 1..a_rank-1
+  uint32_t a_box[5];    // pixel box of dims 1..a_rank-1 (a_box[0], the k-chunk width, is set by gemm_tc_launch)
+  int a_k;              // K per tap (elements)
   int lg_bw, lg_bh, lg_bb;  // log2 of the pixel box (bw*bh*bb == 128); rank 2 ignores them
   int tiles_x, tiles_y;     // tiles per image along x / y (rank 4/5)
   int num_taps;
   GemmTap taps[GEMM_MAX_TAPS];
-  int k_chunks;         // ceil(K_per_tap / 64)
+  int k_chunks;         // set by gemm_tc_launch: ceil(a_k / k-chunk width)
   // ---- B operand ----
-  CUtensorMap tmap_b;   // 2D [rows][K_total] bf16, K-major
+  CUtensorMap tmap_b;   // 2D [rows][K_total] bf16, K-major; set by gemm_tc_launch from b_ptr / b_rows / b_ktot
   int b_rows_per_class; // EPI_OUTCONV: row offset multiplier for the ROI class (0 otherwise)
-  const void* b_ptr;    // W base / rows / row length (elements): lets gemm_tc_launch re-tile W for 128-wide tiles
+  const void* b_ptr;    // W base / rows / row length (elements)
   long long b_rows, b_ktot;
   // ---- problem ----
   int m_tiles, n_tiles;
@@ -106,5 +113,6 @@ int make_tmap_store(CUtensorMap* out, const void* base, int is_f32, const uint64
 // row-wise STS.128), anything else SWIZZLE_NONE (dense [rows][box0] shared-memory tile)
 int make_tmap_store_plain(CUtensorMap* out, const void* base, int is_f32, const uint64_t* dims,
                           const uint64_t* strides_bytes, const uint32_t* box);
+// K-major operand tiles: box[0] of 64 elements (128-byte rows) uses SWIZZLE_128B, of 32 elements (64-byte rows) SWIZZLE_64B
 int make_tmap_bf16(CUtensorMap* out, const void* base, int rank, const uint64_t* dims, const uint64_t* strides_bytes,
                    const uint32_t* box);

@@ -23,6 +23,8 @@
 
 namespace {
 
+constexpr int BLOCK_K = 64;                       // 64 bf16 = 128 B = one swizzle row
+constexpr int A_STAGE_BYTES = BLOCK_M * BLOCK_K * 2;  // 16 KB
 constexpr int MF_C = 128;
 constexpr int MF_HC = 64;                         // hidden columns per chunk
 constexpr int MF_CHUNKS = 4 * MF_C / MF_HC;       // 8

@@ -344,27 +344,35 @@ int ilog2(int v) { int l = 0; while ((1 << l) < v) ++l; return l; }
 
 // A = plain [M,K] rows
 // S = 2: rows are [hi K | lo K] (split-bf16); the tap list is expanded by expand_x3() afterwards
+// A operand geometry; gemm_tc_launch encodes the tensor map with the k-chunk width of the kernel it picks
+void set_a(GemmPlan& p, const void* A, int rank, const uint64_t* dims, const uint64_t* str, const uint32_t* box, int K) {
+  p.a_rank = rank;
+  p.a_ptr = A;
+  for (int i = 0; i < rank; ++i) {
+    p.a_dims[i] = dims[i];
+    p.a_box[i] = box[i];
+    if (i > 0) p.a_str[i - 1] = str[i - 1];
+  }
+  p.a_k = K;
+}
+
 int plan_a2d(GemmPlan& p, const void* A, long long M, int K, int S = 1) {
   uint64_t dims[2] = {(uint64_t)S * K, (uint64_t)M};
   uint64_t str[1] = {(uint64_t)S * K * 2};
-  uint32_t box[2] = {64, 128};
-  p.a_rank = 2;
+  uint32_t box[2] = {0, 128};
+  set_a(p, A, 2, dims, str, box, K);
   p.num_taps = 1;
   p.taps[0] = {0, 0, 0, 0, 0};
-  p.k_chunks = (K + 63) / 64;
   p.m_tiles = (int)((M + 127) / 128);
   p.M = (int)M;
-  return make_tmap_bf16(&p.tmap_a, A, 2, dims, str, box);
+  return GDRN_OK;
 }
 
 int plan_b(GemmPlan& p, const void* W, long long rows, long long Ktot, int block_n, int N, int S = 1) {
-  uint64_t dims[2] = {(uint64_t)S * Ktot, (uint64_t)rows};
-  uint64_t str[1] = {(uint64_t)S * Ktot * 2};
-  uint32_t box[2] = {64, (uint32_t)block_n};
   p.N = N;
   p.n_tiles = (N + block_n - 1) / block_n;
   p.b_ptr = W; p.b_rows = rows; p.b_ktot = (long long)S * Ktot;
-  return make_tmap_bf16(&p.tmap_b, W, 2, dims, str, box);
+  return GDRN_OK;
 }
 
 // A = NHWC [B,H,W,C] pixel boxes; output grid OHxOW = (H*osy, W*osx) handled by the caller's mapping fields
@@ -375,14 +383,13 @@ int plan_a4d(GemmPlan& p, const void* act, int B, int H, int W, int C, int S = 1
   const uint64_t RC_ = (uint64_t)S * C;  // row (pixel) width in elements
   uint64_t dims[4] = {RC_, (uint64_t)W, (uint64_t)H, (uint64_t)B};
   uint64_t str[3] = {RC_ * 2, (uint64_t)W * RC_ * 2, (uint64_t)H * W * RC_ * 2};
-  uint32_t box[4] = {64, (uint32_t)bw, (uint32_t)bh, (uint32_t)bb};
-  p.a_rank = 4;
+  uint32_t box[4] = {0, (uint32_t)bw, (uint32_t)bh, (uint32_t)bb};
+  set_a(p, act, 4, dims, str, box, C);
   p.lg_bw = ilog2(bw); p.lg_bh = ilog2(bh); p.lg_bb = ilog2(bb);
   p.tiles_x = W / bw; p.tiles_y = H / bh;
-  p.k_chunks = (C + 63) / 64;
   p.m_tiles = p.tiles_x * p.tiles_y * ((B + bb - 1) / bb);
   p.M = B;
-  return make_tmap_bf16(&p.tmap_a, act, 4, dims, str, box);
+  return GDRN_OK;
 }
 
 // stride-2 view of NHWC [B,H,W,C]: (2C, W/2, 2, H/2, B); output grid (H/2 x W/2)
@@ -394,14 +401,13 @@ int plan_a5d_s2(GemmPlan& p, const void* act, int B, int H, int W, int C, int S 
   const uint64_t RC_ = (uint64_t)S * C;
   uint64_t dims[5] = {2 * RC_, (uint64_t)OW, 2, (uint64_t)OH, (uint64_t)B};
   uint64_t str[4] = {2 * RC_ * 2, (uint64_t)W * RC_ * 2, (uint64_t)2 * W * RC_ * 2, (uint64_t)H * W * RC_ * 2};
-  uint32_t box[5] = {64, (uint32_t)bw, 1, (uint32_t)bh, (uint32_t)bb};
-  p.a_rank = 5;
+  uint32_t box[5] = {0, (uint32_t)bw, 1, (uint32_t)bh, (uint32_t)bb};
+  set_a(p, act, 5, dims, str, box, C);
   p.lg_bw = ilog2(bw); p.lg_bh = ilog2(bh); p.lg_bb = ilog2(bb);
   p.tiles_x = OW / bw; p.tiles_y = OH / bh;
-  p.k_chunks = (C + 63) / 64;
   p.m_tiles = p.tiles_x * p.tiles_y * ((B + bb - 1) / bb);
   p.M = B;
-  return make_tmap_bf16(&p.tmap_a, act, 5, dims, str, box);
+  return GDRN_OK;
 }
 
 // split-bf16: taps[] keeps listing the hi operands; gemm_tc_launch expands them to the three products
