@@ -1,5 +1,5 @@
 // Internal header of the wgmma GEMM kernel (gemm_tc.cu): tile constants, output-row mapping and the epilogues
-// (shared-memory accumulator tile -> registers -> fused math -> global / shared memory).
+// (shared-memory accumulator tile or wgmma fragments -> fused math -> global / shared memory).
 #pragma once
 #include "common.cuh"
 #include "gemm_tc.h"
@@ -14,8 +14,9 @@ constexpr int MMA_K = 16;
 constexpr int NUM_THREADS = 384;              // producer warpgroup + 2 MMA / epilogue warpgroups (8 warps)
 constexpr int NUM_EPI_WARPS = 8;
 constexpr int EPI_STAGE_PITCH = 80;           // 64-byte row segment + 16 B pad (conflict-free 16-byte accesses)
-// per epilogue warp: either the TMA-store staging tile (32 rows x 128 B, 128B-swizzled, 1024-aligned) or, for the
-// gather-store path, 32 rows x 80 B + 32 x int64 row map + bias/gamma (2 x 128 f32) = 3840 B
+// per epilogue warp: either the TMA-store staging tile (32 rows x 128 B, 128B-swizzled, 1024-aligned), two pairs of
+// 16 x 64 B hi / lo tiles (register GELU epilogue) or, for the gather-store path, 32 rows x 80 B + 32 x int64 row map +
+// bias/gamma (2 x 128 f32) = 3840 B
 constexpr int EPI_STAGE_BYTES = 4096;
 constexpr int SMEM_BUDGET = 227 * 1024 - NUM_EPI_WARPS * EPI_STAGE_BYTES - 1024 - 256;
 
@@ -760,55 +761,67 @@ __device__ __forceinline__ void epilogue_tile_tma(const GemmPlan& p, int m_tile,
   if (trc && lane == 0) { p.trace[8] += tq_tmem; p.trace[9] += tq_comp; p.trace[10] += tq_flush; }
 }
 
-// Split-bf16 (x3) outputs with TMA stores (EPI_STORE / EPI_GELU, bf16 [M, 2N] = [hi N | lo N] rows).
-// A thread owns one accumulator row.  Per 32-column chunk it computes hi = bf16(v) and
-// lo = bf16(v - hi) in registers (the long part: exact-erf GELU), THEN waits for the previous chunk's TMA stores to
-// have read the staging buffer (long finished by then), writes hi / lo into two 32-row x 64-byte tiles and one
-// lane issues two stores: hi at column `col`, lo at column N + col.  Rows beyond M are clipped by the tensor map
-// (SWIZZLE_64B, box {32, 32}: gemm_tc_launch builds it with make_tmap_store_plain).
-template <int BLOCK_N, int EPI, int NEW>
-__device__ __forceinline__ void epilogue_tile_tma_split(const GemmPlan& p, int m_tile, int n_tile, uint32_t tmem_acc, int ew,
-                                                        int lane, uint8_t* stg) {
-  static_assert(EPI == EPI_STORE || EPI == EPI_GELU, "split TMA epilogue: STORE / GELU only");
-  constexpr int CPW = BLOCK_N / (NEW / 4);
-  constexpr int CH = 32;
-  static_assert(CPW % CH == 0, "a warp owns whole 32-column chunks");
-  const int q = ew & 3, half = ew >> 2;
-  const int n0 = n_tile * BLOCK_N + half * CPW;
-  const uint32_t tmem_row = tmem_acc + ((uint32_t)(q * 32) << 16) + half * CPW;
-  const uint32_t stg_u32 = ptx::smem_u32(stg);
-  uint4* my_hi = reinterpret_cast<uint4*>(stg + lane * 64);
-  uint4* my_lo = reinterpret_cast<uint4*>(stg + 2048 + lane * 64);
-  const int row0 = m_tile * BLOCK_M + q * 32;
-  const bool trc = (p.trace != nullptr) && blockIdx.x == 0 && ew == 0;   // GDRN_GEMM_TRACE: phase cycles of one warp
-  long long tq_tmem = 0, tq_comp = 0, tq_flush = 0;
-#pragma unroll 1
-  for (int c = 0; c < CPW; c += CH) {
-    const int col = n0 + c;
-    if (col >= p.N) break;  // warp-uniform
-    float v[CH];
-    long long tq0 = trc ? clock64() : 0;
-    acc_load_chunk<BLOCK_N, CH>(tmem_row + c, v);
-    if (trc) { const long long t = clock64(); tq_tmem += t - tq0; tq0 = t; }
-    // element PAIRS (f2_*): this epilogue is FMA-pipe bound, see gelu_erf2
-    f32x2_t v2[CH / 2];
+// Epilogues straight from the wgmma accumulator fragments: split-bf16 rank-2 GEMMs with EPI_STORE (fp32 out), EPI_GELU
+// ([hi N | lo N] bf16 out) and EPI_RESID, i.e. the ConvNeXt MLPs and downsamples (gemm_tc_launch picks them).  Warp wl of
+// consumer warpgroup wg holds tile rows w = 64 wg + 16 wl + (lane >> 2) and w + 8 (`wrow` = 64 wg + 16 wl) and, of every
+// 8-column group j, the columns 8 j + 2 (lane & 3) + {0, 1}: acc[4 j], acc[4 j + 1] on row w, acc[4 j + 2], acc[4 j + 3] on
+// row w + 8.  The arithmetic per element is that of the accumulator-tile epilogues, operation for operation.
+// Rows >= M and columns >= N are neither read nor written.
+
+// EPI_RESID: this thread's residual pairs x[2 j + h] (row w + 8 h, group j), loaded before the last MMAs retire
+template <int BLOCK_N>
+__device__ __forceinline__ void frag_resid_load(const GemmPlan& p, int m_tile, int n_tile, int wrow, int lane,
+                                                float2 (&x)[BLOCK_N / 4]) {
+  const long long r0 = (long long)m_tile * BLOCK_M + wrow + (lane >> 2);
+  const int c0 = n_tile * BLOCK_N + (lane & 3) * 2;
+  // two row pointers and immediate column offsets: no per-element address registers next to the accumulators
+  const float* xr[2] = {p.resid + r0 * p.ldo + c0, p.resid + (r0 + 8) * p.ldo + c0};
 #pragma unroll
-    for (int j = 0; j < CH / 2; ++j) v2[j] = f2_pack(v[2 * j], v[2 * j + 1]);
-    if (p.bias) {
+  for (int j = 0; j < BLOCK_N / 8; ++j) {
 #pragma unroll
-      for (int j = 0; j < CH; j += 4) {
-        const float4 b4 = __ldg(reinterpret_cast<const float4*>(p.bias + col + j));
-        v2[j / 2] = f2_add(v2[j / 2], f2_pack(b4.x, b4.y));
-        v2[j / 2 + 1] = f2_add(v2[j / 2 + 1], f2_pack(b4.z, b4.w));
+    for (int h = 0; h < 2; ++h)
+      x[2 * j + h] = (r0 + 8 * h < p.M && c0 + 8 * j < p.N) ? *reinterpret_cast<const float2*>(xr[h] + 8 * j) : make_float2(0.f, 0.f);
+  }
+}
+
+// EPI_GELU: per 32-column chunk, bias + exact-erf GELU + hi / lo split as element pairs, then hi and lo go into two
+// 16-row x 64-byte tiles of the warp's staging slot (SWIZZLE_64B: 16-byte piece c of row r at c ^ ((r >> 1) & 3), so the
+// 4-byte stores of a warp hit 32 distinct banks) and one lane issues two TMA stores (map box {32, 16}): hi at column
+// `col`, lo at N + col; the map clips rows >= M.  The slot holds two such pairs, used in turn (`sbuf` counts the chunks
+// this warp has stored), so a chunk's stores may still be reading while the next chunk is written.
+template <int BLOCK_N, int EPI>
+__device__ __forceinline__ void epilogue_regs(const GemmPlan& p, int m_tile, int n_tile, int wrow, int lane,
+                                              const float (&acc)[BLOCK_N / 2], const float2 (&x)[EPI == EPI_RESID ? BLOCK_N / 4 : 1],
+                                              uint8_t* stg, uint32_t& sbuf) {
+  static_assert(EPI == EPI_STORE || EPI == EPI_GELU || EPI == EPI_RESID, "register epilogue: STORE / GELU / RESID only");
+  const long long r0 = (long long)m_tile * BLOCK_M + wrow + (lane >> 2);
+  const int c0 = n_tile * BLOCK_N + (lane & 3) * 2;
+  if constexpr (EPI == EPI_GELU) {
+    const int sw = (lane >> 3) & 3;   // ((lane >> 2) >> 1) & 3; the same for row + 8
+#pragma unroll
+    for (int ch = 0; ch < BLOCK_N / 32; ++ch) {
+      const int col = n_tile * BLOCK_N + ch * 32;
+      if (col >= p.N) break;   // warp-uniform
+      f32x2_t v2[8];           // [2 jj + h]: group 4 ch + jj, row w + 8 h
+#pragma unroll
+      for (int jj = 0; jj < 4; ++jj) {
+#pragma unroll
+        for (int h = 0; h < 2; ++h) v2[2 * jj + h] = f2_pack(acc[4 * (4 * ch + jj) + 2 * h], acc[4 * (4 * ch + jj) + 2 * h + 1]);
       }
-    }
-    if constexpr (EPI == EPI_GELU) {
+      if (p.bias) {
+#pragma unroll
+        for (int jj = 0; jj < 4; ++jj) {
+          const float2 b = __ldg(reinterpret_cast<const float2*>(p.bias + c0 + ch * 32 + 8 * jj));
+          v2[2 * jj] = f2_add(v2[2 * jj], f2_pack(b.x, b.y));
+          v2[2 * jj + 1] = f2_add(v2[2 * jj + 1], f2_pack(b.x, b.y));
+        }
+      }
       if (p.gelu_mode == 3) {
 #pragma unroll
-        for (int j = 0; j < CH / 2; ++j) v2[j] = gelu_erf2(v2[j]);
+        for (int j = 0; j < 8; ++j) v2[j] = gelu_erf2(v2[j]);
       } else {                         // A/B knobs: 5 = scalar A&S form, 4 = libm erff, else the bf16-mode fit
 #pragma unroll
-        for (int j = 0; j < CH / 2; ++j) {
+        for (int j = 0; j < 8; ++j) {
           float2 f = f2_unpack(v2[j]);
           if (p.gelu_mode == 5) { f.x = gelu_erf(f.x); f.y = gelu_erf(f.y); }
           else if (p.gelu_mode == 4) {
@@ -818,47 +831,62 @@ __device__ __forceinline__ void epilogue_tile_tma_split(const GemmPlan& p, int m
           v2[j] = f2_pack(f.x, f.y);
         }
       }
-    }
-    uint32_t hi[CH / 2], lo[CH / 2];
+      uint32_t hi[8], lo[8];
 #pragma unroll
-    for (int j = 0; j < CH / 2; ++j) {
-      const float2 f = f2_unpack(v2[j]);
-      const uint32_t hb = pack_bf16(f.x, f.y);
-      hi[j] = hb;
-      const float2 d = f2_unpack(f2_sub(v2[j], f2_pack(__uint_as_float(hb << 16), __uint_as_float(hb & 0xffff0000u))));
-      lo[j] = pack_bf16(d.x, d.y);
-    }
-    if (trc) { const long long t = clock64(); tq_comp += t - tq0; tq0 = t; }
-    if (lane == 0) ptx::bulk_wait_read0();   // the previous chunk's stores have read the staging tiles
-    __syncwarp();
-    // 64-byte rows, SWIZZLE_64B: chunk c of row r lives at c ^ ((r >> 1) & 3) -- eight consecutive lanes cover all 32 banks
-    const int sw = (lane >> 1) & 3;
+      for (int j = 0; j < 8; ++j) {
+        const float2 f = f2_unpack(v2[j]);
+        const uint32_t hb = pack_bf16(f.x, f.y);
+        hi[j] = hb;
+        const float2 d = f2_unpack(f2_sub(v2[j], f2_pack(__uint_as_float(hb << 16), __uint_as_float(hb & 0xffff0000u))));
+        lo[j] = pack_bf16(d.x, d.y);
+      }
+      if (lane == 0) ptx::bulk_wait_read1();   // the stores issued from this half of the slot two chunks ago have read it
+      __syncwarp();
+      uint8_t* buf = stg + (sbuf & 1u) * 2048u;   // [hi 16 x 64 B | lo 16 x 64 B]
 #pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      my_hi[j ^ sw] = make_uint4(hi[4 * j], hi[4 * j + 1], hi[4 * j + 2], hi[4 * j + 3]);
-      my_lo[j ^ sw] = make_uint4(lo[4 * j], lo[4 * j + 1], lo[4 * j + 2], lo[4 * j + 3]);
+      for (int jj = 0; jj < 4; ++jj) {
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const int off = ((lane >> 2) + 8 * h) * 64 + ((jj ^ sw) << 4) + (lane & 3) * 4;
+          *reinterpret_cast<uint32_t*>(buf + off) = hi[2 * jj + h];
+          *reinterpret_cast<uint32_t*>(buf + 1024 + off) = lo[2 * jj + h];
+        }
+      }
+      ptx::fence_proxy_async();
+      __syncwarp();
+      if (lane == 0) {
+        const uint32_t src = ptx::smem_u32(buf);
+        const int row0 = m_tile * BLOCK_M + wrow;
+        ptx::tma_store_2d(&p.tmap_out, src, col, row0);
+        ptx::tma_store_2d(&p.tmap_out, src + 1024, p.N + col, row0);
+        ptx::bulk_commit();
+      }
+      ++sbuf;
     }
-    ptx::fence_proxy_async();
-    __syncwarp();
-    if (lane == 0) {
-      ptx::tma_store_2d(&p.tmap_out, stg_u32, col, row0);
-      ptx::tma_store_2d(&p.tmap_out, stg_u32 + 2048, p.N + col, row0);
-      ptx::bulk_commit();
+  } else {
+    // fp32 out: 8-byte stores, four lanes fill one 32-byte sector of a row
+    float* orow[2] = {reinterpret_cast<float*>(p.out) + r0 * p.ldo + c0, reinterpret_cast<float*>(p.out) + (r0 + 8) * p.ldo + c0};
+    const bool rv[2] = {r0 < p.M, r0 + 8 < p.M};
+#pragma unroll
+    for (int j = 0; j < BLOCK_N / 8; ++j) {
+      const int c = c0 + 8 * j;
+      if (c >= p.N) continue;
+      const float2 b = p.bias ? __ldg(reinterpret_cast<const float2*>(p.bias + c)) : make_float2(0.f, 0.f);
+      const float2 g = EPI == EPI_RESID ? __ldg(reinterpret_cast<const float2*>(p.gamma + c)) : make_float2(0.f, 0.f);
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        if (!rv[h]) continue;
+        float2 v = make_float2(acc[4 * j + 2 * h] + b.x, acc[4 * j + 2 * h + 1] + b.y);
+        if constexpr (EPI == EPI_RESID) v = make_float2(fmaf(g.x, v.x, x[2 * j + h].x), fmaf(g.y, v.y, x[2 * j + h].y));
+        *reinterpret_cast<float2*>(orow[h] + 8 * j) = v;
+      }
     }
-    if (trc) tq_flush += clock64() - tq0;
   }
-  if (trc && lane == 0) { p.trace[8] += tq_tmem; p.trace[9] += tq_comp; p.trace[10] += tq_flush; }
 }
 
 template <int BLOCK_N, int EPI>
 __device__ __forceinline__ void epilogue_tile_staged(const GemmPlan& p, int m_tile, int n_tile, uint32_t tmem_acc,
                                                      int ew, int lane, uint8_t* stg) {
-  if constexpr (EPI == EPI_GELU) {
-    if (p.use_tma_store && p.split) {  // launch-uniform: split-bf16 output through TMA tile stores
-      epilogue_tile_tma_split<BLOCK_N, EPI, NUM_EPI_WARPS>(p, m_tile, n_tile, tmem_acc, ew, lane, stg);
-      return;
-    }
-  }
   if constexpr (BLOCK_N >= 128 && (EPI == EPI_STORE || EPI == EPI_GELU || EPI == EPI_RESID)) {
     if (p.use_tma_store) {  // launch-uniform
       if constexpr (EPI == EPI_RESID) {

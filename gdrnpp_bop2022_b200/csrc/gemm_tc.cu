@@ -6,7 +6,8 @@
 //                     for rows [64g, 64g + 64) of the 128-row tile, releases each ring stage as soon as the MMAs that
 //                     read it retire, then writes its accumulators into the shared-memory accumulator tile; the same
 //                     8 warps then run the fused epilogue from there (gemm_epilogue.cuh) while the producer already
-//                     fills the ring for the next tile.
+//                     fills the ring for the next tile.  Split-bf16 plain-row GELU / RESID / fp32 STORE GEMMs (REG) skip
+//                     the tile: every warp runs the epilogue on its own fragments, and the ring takes the tile's bytes.
 // X3 (split-bf16, 64- / 128-wide tiles): a stage holds {A hi, A lo, W hi, W lo} of one k-chunk (32 wide for convolutions,
 // 64 for plain rows) and feeds all three products.
 // The kernel makes no function call: any call makes ptxas serialize the wgmma pipeline (C7510).
@@ -28,9 +29,12 @@ namespace {
 // products A_lo*W_hi + A_hi*W_lo + A_hi*W_hi (4 operand tiles per 3 MMA groups instead of 6 with an expanded tap list).
 // BK: k-chunk width (bf16 elements) of one ring stage.  64 = 128-byte rows (SWIZZLE_128B); 32 = 64-byte rows
 // (SWIZZLE_64B), X3 only: half the bytes per stage, twice the ring depth (gemm_tc_launch picks it, see there).
-template <int BLOCK_N, bool X3, int BK = 64>
+// REG: the epilogue runs straight from the wgmma registers (epilogue_regs), so there is no shared-memory accumulator tile
+// and its bytes go to the ring (split-bf16 plain rows with 64-wide chunks only).
+template <int BLOCK_N, bool X3, int BK = 64, bool REG = false>
 struct Cfg {
   static_assert(BK == 64 || (X3 && BK == 32), "gemm: 32-wide k-chunks exist for the split-bf16 kernel only");
+  static_assert(!REG || (X3 && BK == 64), "gemm: the register epilogue exists for the 64-wide split-bf16 kernel only");
   static constexpr int BLOCK_K = BK;
   static constexpr int NOPS = X3 ? 2 : 1;  // hi (and lo) copies of each operand per stage
   static constexpr int A_TILE_BYTES = BLOCK_M * BLOCK_K * 2;
@@ -38,7 +42,7 @@ struct Cfg {
   static constexpr int B_STAGE_BYTES = NOPS * B_TILE_BYTES;
   static constexpr int A_BYTES = NOPS * A_TILE_BYTES;
   static constexpr int STAGE_BYTES = A_BYTES + B_STAGE_BYTES;
-  static constexpr int ACC_BYTES = acc_bytes<BLOCK_N>();
+  static constexpr int ACC_BYTES = REG ? 0 : acc_bytes<BLOCK_N>();
   static constexpr int RING = (SMEM_BUDGET - ACC_BYTES) / STAGE_BYTES;
   static constexpr int STAGES = RING > 8 ? 8 : RING;
   static constexpr int SMEM_BYTES = ACC_BYTES + STAGES * STAGE_BYTES + 1024 /*align*/ + 256 /*barriers*/ + NUM_EPI_WARPS * EPI_STAGE_BYTES;
@@ -52,13 +56,16 @@ struct Cfg {
 // the 32-wide X3 kernel consumes its stages in pairs (one 64-wide k-step): at BLOCK_N = 128 two more stages load meanwhile
 static_assert(Cfg<128, true, 32>::STAGES >= 4, "gemm: the 32-wide split-bf16 128-wide kernel needs a four-deep operand ring");
 static_assert(Cfg<64, true, 32>::STAGES >= 6, "gemm: the 32-wide split-bf16 64-wide kernel needs a six-deep operand ring");
+// without the accumulator tile the 64-wide split-bf16 ring gains a stage: 3 x 64 KB at BLOCK_N = 128, 4 x 48 KB at 64
+static_assert(Cfg<128, true, 64, true>::STAGES >= 3, "gemm: the register-epilogue split-bf16 128-wide kernel needs a three-deep operand ring");
+static_assert(Cfg<64, true, 64, true>::STAGES >= 4, "gemm: the register-epilogue split-bf16 64-wide kernel needs a four-deep operand ring");
 
 constexpr int CONSUMER_THREADS = 256;
 constexpr int BAR_ACC = 1;         // named barrier of the two consumer warpgroups (accumulator tile hand-over)
 
-template <int BLOCK_N, int EPI, bool X3, int BK>
+template <int BLOCK_N, int EPI, bool X3, int BK, bool REG>
 __global__ void __launch_bounds__(NUM_THREADS, 1) gemm_tc_kernel(const __grid_constant__ GemmPlan p) {
-  using C = Cfg<BLOCK_N, X3, BK>;
+  using C = Cfg<BLOCK_N, X3, BK, REG>;
   // 1024-byte alignment required by SWIZZLE_128B: [accumulator tile | ring | epilogue staging | barriers]
   const uint32_t smem_base = (ptx::smem_u32(gemm_smem) + 1023u) & ~1023u;
   const uint32_t ring_base = smem_base + C::ACC_BYTES;
@@ -93,71 +100,77 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) gemm_tc_kernel(const __grid_co
   const int k_iters = p.num_taps * p.k_chunks;
   // optional cycle accounting of CTA 0 (GDRN_GEMM_TRACE, api_core.cu): who waits for whom
   const bool tr = (p.trace != nullptr) && blockIdx.x == 0;
-  long long tr_acc0 = 0, tr_acc1 = 0;
+  long long tr_acc0 = 0, tr_acc1 = 0, tr_epi = 0;
   const long long tr_start = tr ? clock64() : 0;
 
-  if (warp == 0 && lane == 0) {
-    // ================= TMA producer =================
-    int stage = 0;
-    uint32_t phase = 0;
-    for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
-      const int n_tile = p.n_major ? tile / p.m_tiles : tile % p.n_tiles;
-      const int m_tile = p.n_major ? tile % p.m_tiles : tile / p.n_tiles;
-      int x0 = 0, y0 = 0, b0 = 0;
-      if (p.a_rank != 2) {
-        int tx = m_tile % p.tiles_x;
-        int t2 = m_tile / p.tiles_x;
-        x0 = tx << p.lg_bw;
-        y0 = (t2 % p.tiles_y) << p.lg_bh;
-        b0 = (t2 / p.tiles_y) << p.lg_bb;
-      }
-      int brow = n_tile * BLOCK_N;
-      if (EPI == EPI_OUTCONV) {
-        long long grow = (long long)m_tile * BLOCK_M;
-        int b = (int)(grow / p.rows_per_roi);
-        int cls = p.roi_classes ? (int)p.roi_classes[b] : 0;   // NULL: class-agnostic head (one slab)
-        cls = cls < 0 ? 0 : (cls >= p.num_classes ? p.num_classes - 1 : cls);  // never index outside the weights
-        brow += cls * p.b_rows_per_class;
-      }
-      for (int tap = 0; tap < p.num_taps; ++tap) {
-        const GemmTap tp = p.taps[tap];
-        for (int kc = 0; kc < p.k_chunks; ++kc) {
-          { const long long t0 = tr ? clock64() : 0; ptx::mbar_wait_nocall(empty_bar(stage), phase ^ 1); if (tr) tr_acc0 += clock64() - t0; }
-          const uint32_t sa = ring_base + stage * C::STAGE_BYTES;
-          const uint32_t sb = sa + C::A_BYTES;
-          ptx::mbar_arrive_expect_tx(full_bar(stage), C::STAGE_BYTES);
-          const int k0 = kc * C::BLOCK_K;
+  // REG: the consumers keep their accumulators live through the epilogue, so they take the registers the producer
+  // warpgroup does not use (setmaxnreg is per warpgroup: warps 1..3 and lanes 1..31 of warp 0 lower theirs too)
+  if (warp < 4) {
+    if constexpr (REG) ptx::setmaxnreg_dec<40>();
+    if (warp == 0 && lane == 0) {
+      // ================= TMA producer =================
+      int stage = 0;
+      uint32_t phase = 0;
+      for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
+        const int n_tile = p.n_major ? tile / p.m_tiles : tile % p.n_tiles;
+        const int m_tile = p.n_major ? tile % p.m_tiles : tile / p.n_tiles;
+        int x0 = 0, y0 = 0, b0 = 0;
+        if (p.a_rank != 2) {
+          int tx = m_tile % p.tiles_x;
+          int t2 = m_tile / p.tiles_x;
+          x0 = tx << p.lg_bw;
+          y0 = (t2 % p.tiles_y) << p.lg_bh;
+          b0 = (t2 / p.tiles_y) << p.lg_bb;
+        }
+        int brow = n_tile * BLOCK_N;
+        if (EPI == EPI_OUTCONV) {
+          long long grow = (long long)m_tile * BLOCK_M;
+          int b = (int)(grow / p.rows_per_roi);
+          int cls = p.roi_classes ? (int)p.roi_classes[b] : 0;   // NULL: class-agnostic head (one slab)
+          cls = cls < 0 ? 0 : (cls >= p.num_classes ? p.num_classes - 1 : cls);  // never index outside the weights
+          brow += cls * p.b_rows_per_class;
+        }
+        for (int tap = 0; tap < p.num_taps; ++tap) {
+          const GemmTap tp = p.taps[tap];
+          for (int kc = 0; kc < p.k_chunks; ++kc) {
+            { const long long t0 = tr ? clock64() : 0; ptx::mbar_wait_nocall(empty_bar(stage), phase ^ 1); if (tr) tr_acc0 += clock64() - t0; }
+            const uint32_t sa = ring_base + stage * C::STAGE_BYTES;
+            const uint32_t sb = sa + C::A_BYTES;
+            ptx::mbar_arrive_expect_tx(full_bar(stage), C::STAGE_BYTES);
+            const int k0 = kc * C::BLOCK_K;
 #pragma unroll
-          for (int h = 0; h < C::NOPS; ++h) {   // h = 1: the lo halves, behind the hi tiles of the stage
-            const uint32_t da = sa + h * C::A_TILE_BYTES;
-            const int ca = k0 + tp.c0 + h * p.x3_a_lo;
+            for (int h = 0; h < C::NOPS; ++h) {   // h = 1: the lo halves, behind the hi tiles of the stage
+              const uint32_t da = sa + h * C::A_TILE_BYTES;
+              const int ca = k0 + tp.c0 + h * p.x3_a_lo;
+              if (p.a_rank == 2) {
+                ptx::tma_load_2d(da, &p.tmap_a, full_bar(stage), ca, m_tile * BLOCK_M + tp.d1);
+              } else if (p.a_rank == 4) {
+                ptx::tma_load_4d(da, &p.tmap_a, full_bar(stage), ca, x0 + tp.d1, y0 + tp.d2, b0);
+              } else {
+                ptx::tma_load_5d(da, &p.tmap_a, full_bar(stage), ca, x0 + tp.d1, tp.d2, y0 + tp.d3, b0);
+              }
+              ptx::tma_load_2d(sb + h * C::B_TILE_BYTES, &p.tmap_b, full_bar(stage), tp.b_off + k0 + h * p.x3_b_lo, brow);
+            }
             if (p.a_rank == 2) {
-              ptx::tma_load_2d(da, &p.tmap_a, full_bar(stage), ca, m_tile * BLOCK_M + tp.d1);
-            } else if (p.a_rank == 4) {
-              ptx::tma_load_4d(da, &p.tmap_a, full_bar(stage), ca, x0 + tp.d1, y0 + tp.d2, b0);
-            } else {
-              ptx::tma_load_5d(da, &p.tmap_a, full_bar(stage), ca, x0 + tp.d1, tp.d2, y0 + tp.d3, b0);
+              // A is streamed from HBM (it was written by the previous kernel): request it into L2 several
+              // k-iterations ahead so the shared-memory ring only has to cover L2 latency, not DRAM latency.
+              int pk = kc + C::PREFETCH_AHEAD, pm = m_tile;
+              if (pk >= p.k_chunks) {
+                pk -= p.k_chunks;
+                const int nt = tile + gridDim.x;
+                const int nm = p.n_major ? nt % p.m_tiles : nt / p.n_tiles;
+                pm = (nt < total_tiles && nm != m_tile) ? nm : -1;
+              }
+              if (pm >= 0 && pk < p.k_chunks && p.num_taps == 1) ptx::tma_prefetch_2d(&p.tmap_a, pk * C::BLOCK_K, pm * BLOCK_M);
             }
-            ptx::tma_load_2d(sb + h * C::B_TILE_BYTES, &p.tmap_b, full_bar(stage), tp.b_off + k0 + h * p.x3_b_lo, brow);
+            if (++stage == C::STAGES) { stage = 0; phase ^= 1; }
           }
-          if (p.a_rank == 2) {
-            // A is streamed from HBM (it was written by the previous kernel): request it into L2 several
-            // k-iterations ahead so the shared-memory ring only has to cover L2 latency, not DRAM latency.
-            int pk = kc + C::PREFETCH_AHEAD, pm = m_tile;
-            if (pk >= p.k_chunks) {
-              pk -= p.k_chunks;
-              const int nt = tile + gridDim.x;
-              const int nm = p.n_major ? nt % p.m_tiles : nt / p.n_tiles;
-              pm = (nt < total_tiles && nm != m_tile) ? nm : -1;
-            }
-            if (pm >= 0 && pk < p.k_chunks && p.num_taps == 1) ptx::tma_prefetch_2d(&p.tmap_a, pk * C::BLOCK_K, pm * BLOCK_M);
-          }
-          if (++stage == C::STAGES) { stage = 0; phase ^= 1; }
         }
       }
+      if (tr) { p.trace[0] = tr_acc0; p.trace[6] = clock64() - tr_start; p.trace[7] = (total_tiles - 1 - (int)blockIdx.x) / (int)gridDim.x + 1; }
     }
-    if (tr) { p.trace[0] = tr_acc0; p.trace[6] = clock64() - tr_start; p.trace[7] = (total_tiles - 1 - (int)blockIdx.x) / (int)gridDim.x + 1; }
-  } else if (warp >= 4) {
+  } else {
+    if constexpr (REG) ptx::setmaxnreg_inc<232>();
     // ================= consumers: wgmma mainloop, accumulator hand-over, epilogue =================
     const int ew = warp - 4;
     const int wg = ew >> 2;             // rows [64 wg, 64 wg + 64) of the tile
@@ -165,6 +178,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) gemm_tc_kernel(const __grid_co
     const bool tr_me = tr && ew == 0 && lane == 0;
     int stage = 0;
     uint32_t phase = 0;
+    uint32_t sbuf = 0;  // REG, EPI_GELU: chunks this warp has TMA-stored (picks the half of its staging slot)
     for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
       const int n_tile = p.n_major ? tile / p.m_tiles : tile % p.n_tiles;
       const int m_tile = p.n_major ? tile % p.m_tiles : tile / p.n_tiles;
@@ -241,8 +255,17 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) gemm_tc_kernel(const __grid_co
           if (++stage == C::STAGES) { stage = 0; phase ^= 1; }
         }
       }
+      float2 xres[REG && EPI == EPI_RESID ? BLOCK_N / 4 : 1];
+      if constexpr (REG && EPI == EPI_RESID) frag_resid_load<BLOCK_N>(p, m_tile, n_tile, wg * 64 + wl * 16, lane, xres);
       ptx::wgmma_wait<0>();
       if (prev_stage >= 0 && wl == 0 && lane == 0) ptx::mbar_arrive(empty_bar(prev_stage));
+      if constexpr (REG) {
+        const long long t0 = tr_me ? clock64() : 0;
+        epilogue_regs<BLOCK_N, EPI>(p, m_tile, n_tile, wg * 64 + wl * 16, lane, acc, xres, stage_base + ew * EPI_STAGE_BYTES,
+                                    sbuf);
+        if (tr_me) tr_epi += clock64() - t0;
+        continue;
+      }
 
       if (kStaged && EPI != EPI_GNSTATS && !p.use_tma_store) {
         // this warp's bias (and layer-scale gamma) segment -> its shared-memory slot
@@ -280,15 +303,15 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) gemm_tc_kernel(const __grid_co
         epilogue_tile<BLOCK_N, EPI>(p, m_tile, n_tile, acc_row, lane, stage_base + ew * EPI_STAGE_BYTES);
       }
     }
-    if (tr_me) { p.trace[1] = tr_acc0; p.trace[3] = tr_acc1; }
+    if (tr_me) { p.trace[1] = tr_acc0; p.trace[3] = tr_acc1; if (REG) p.trace[9] = tr_epi; }
     if (lane == 0) ptx::bulk_wait0();  // outstanding TMA stores (no-op when none were issued)
   }
 }
 
-template <int BLOCK_N, int EPI, bool X3 = false, int BK = 64>
+template <int BLOCK_N, int EPI, bool X3 = false, int BK = 64, bool REG = false>
 int launch_inst(const GemmPlan& plan, cudaStream_t stream) {
-  using C = Cfg<BLOCK_N, X3, BK>;
-  auto kfn = gemm_tc_kernel<BLOCK_N, EPI, X3, BK>;
+  using C = Cfg<BLOCK_N, X3, BK, REG>;
+  auto kfn = gemm_tc_kernel<BLOCK_N, EPI, X3, BK, REG>;
   GDRN_OPT_IN_SMEM(kfn, C::SMEM_BYTES);
   int total = plan.m_tiles * plan.n_tiles;
   if (total <= 0) return GDRN_OK;
@@ -369,17 +392,31 @@ int gemm_tc_launch(const GemmPlan& plan_in, int block_n, cudaStream_t stream) {
       plan.resid_reduce = (red && plan.epi == EPI_RESID && plan.resid == plan.out) ? 1 : 0;
     }
   }
-  if (x3_shared && plan.epi == EPI_GELU && plan.a_rank == 2 && plan.N % 64 == 0 && ((uintptr_t)plan.out % 16 == 0) &&
-      ((plan.ldo * 2) % 16 == 0)) {
-    // split-bf16 GELU output [hi N | lo N]: two dense 32 x 64-byte tiles per 32-column chunk, TMA-stored
+  // Split-bf16 plain rows with an element-wise epilogue (the ConvNeXt MLPs and downsamples) run it straight from the wgmma
+  // registers: without the accumulator tile the operand ring is one stage deeper (DESIGN §4.1).  The split GELU output
+  // [hi N | lo N] leaves through TMA stores of 16-row x 64-byte tiles; without the alignment those need, the GELU keeps the
+  // accumulator-tile path.
+  const bool gelu_tma = plan.N % 64 == 0 && ((uintptr_t)plan.out % 16 == 0) && ((plan.ldo * 2) % 16 == 0);
+  const bool reg_epi = x3_shared && plan.a_rank == 2 &&
+                       (plan.epi == EPI_RESID || (plan.epi == EPI_STORE && plan.out_f32) || (plan.epi == EPI_GELU && gelu_tma));
+  if (reg_epi && plan.epi == EPI_GELU) {
     const uint64_t dims[2] = {(uint64_t)plan.ldo, (uint64_t)plan.M};
     const uint64_t str[1] = {(uint64_t)plan.ldo * 2};
-    const uint32_t box[2] = {32u, 32u};
+    const uint32_t box[2] = {32u, 16u};
     int rc = make_tmap_store_plain(&plan.tmap_out, plan.out, 0, dims, str, box);
     if (rc != GDRN_OK) return rc;
     plan.use_tma_store = 1;
   }
   GDRN_REQUIRE(plan.num_taps >= 1 && plan.num_taps <= GEMM_MAX_TAPS, "gemm: bad num_taps");
+#define GDRN_GEMM_CASE_REG(BN, E) \
+  if (reg_epi && block_n == BN && plan.epi == E) return launch_inst<BN, E, true, 64, true>(plan, stream);
+  GDRN_GEMM_CASE_REG(128, EPI_GELU)
+  GDRN_GEMM_CASE_REG(128, EPI_RESID)
+  GDRN_GEMM_CASE_REG(128, EPI_STORE)
+  GDRN_GEMM_CASE_REG(64, EPI_GELU)
+  GDRN_GEMM_CASE_REG(64, EPI_RESID)
+  GDRN_GEMM_CASE_REG(64, EPI_STORE)
+#undef GDRN_GEMM_CASE_REG
 #define GDRN_GEMM_CASE_X3(BN, E) \
   if (x3_shared && block_n == BN && plan.epi == E)                                                          \
     return bk == 32 ? launch_inst<BN, E, true, 32>(plan, stream) : launch_inst<BN, E, true, 64>(plan, stream);

@@ -85,7 +85,8 @@ struct GemmPlan {
   const float* roi_coord_2d;     // [B,2,64,64] fp32 NCHW
   void* pnp_in;                  // bf16 [B*4096, 128]
   // debug: CTA 0 writes [0] producer empty-wait, [1] consumer full-wait, [3] accumulator hand-over, [6] CTA cycles,
-  // [7] tiles of CTA 0, [8..10] epilogue warp 0 accumulator loads / compute / flush (clock64 cycles)
+  // [7] tiles of CTA 0, [8..10] epilogue warp 0 accumulator loads / compute / flush (clock64 cycles; the register
+  // epilogue has no hand-over and books its whole epilogue as compute)
   long long* trace;
   float* map_mask; float* map_full; float* map_x; float* map_y; float* map_z; float* map_region;  // NCHW or null
 };
