@@ -89,6 +89,15 @@ _SIGNATURES = {
     "yolox_postprocess_workspace_bytes": (c_size_t, [c_int, c_int]),
     "yolox_postprocess": (c_int, [c_void_p] + [c_int] * 3 + [c_void_p, c_void_p, c_int, c_float, c_float, c_int, c_int, c_void_p, c_void_p,
                                   c_void_p, c_size_t, c_void_p]),
+    "yolox_model_create": (c_int, [POINTER(c_void_p), c_double, c_double] + [c_int] * 5),
+    "yolox_model_destroy": (None, [c_void_p]),
+    "yolox_model_load_tensor": (c_int, [c_void_p, c_char_p, c_void_p, c_int64, c_void_p]),
+    "yolox_model_missing": (c_int, [c_void_p]),
+    "yolox_model_num_anchors": (c_int, [c_void_p]),
+    "yolox_model_workspace_bytes": (c_size_t, [c_void_p, c_int]),
+    "yolox_model_forward": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_size_t, c_void_p]),
+    "yolox_postprocess_single_workspace_bytes": (c_size_t, [c_int] * 3),
+    "yolox_postprocess_single": (c_int, [c_void_p] + [c_int] * 3 + [c_float, c_float] + [c_void_p] * 3 + [c_size_t, c_void_p]),
     "gdrn_crop_resize_u8": (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p,
                                     c_void_p]),
     "gdrn_crop_resize_f32": (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p]),

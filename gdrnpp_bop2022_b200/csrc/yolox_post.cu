@@ -12,7 +12,7 @@
 //   3. yolox_nms_mask_kernel: 64 x 64 IoU tiles -> suppression bit masks (torchvision's devIoU arithmetic; different
 //      classes never suppress each other unless class_agnostic -- batched_nms' coordinate-offset trick without the offsets)
 //   4. yolox_nms_reduce_kernel: one warp walks the sorted candidates, ORs the masks of the kept ones, writes the kept rows
-// The YOLOX network itself (backbone / PAFPN / head convolutions) is out of scope (SURVEY.md 8: a different model).
+// The YOLOX network itself (backbone / PAFPN / head convolutions) runs in yolox_net.cu.
 #include "common.cuh"
 
 namespace {

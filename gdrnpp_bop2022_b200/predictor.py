@@ -166,12 +166,17 @@ class GdrnPredictor:
 
     # ---- preprocessing (predictor_gdrn.py:301-476) ---------------------------------------------
     def preprocessing(self, outputs, image, depth_img=None):
-        """outputs: [n,7] detections (x1,y1,x2,y2,score,cls_score,cls) like the YOLOX stage; image: HxWx3 BGR uint8;
+        """outputs: [n,7] detections (x1,y1,x2,y2,score,cls_score,cls) like the YOLOX stage, or the detector's list
+        ``[dets or None]`` as YoloPredictor.inference returns it (element 0 is used; None = no ROIs); image: HxWx3 BGR uint8;
         depth_img: HxW (scaled by depth_scale like the reference).  Per-ROI bookkeeping follows predictor_gdrn.py:396-415
         (centre, bw/bh >= 1, scale = min(max(bw,bh)*DZI_PAD_SCALE, max(H,W)), resize_ratio = out_res/scale); the crops
         -- the reference's per-ROI cv2.warpAffine loop (:417-438) -- are three batched GPU launches with OpenCV's exact
         arithmetic (csrc/crop_resize.cu)."""
         dev = self.device
+        if isinstance(outputs, (list, tuple)) and len(outputs) <= 1 and (
+                len(outputs) == 0 or outputs[0] is None or (torch.is_tensor(outputs[0]) and outputs[0].dim() == 2)):
+            # the detector's list form (YoloPredictor.inference, predictor_gdrn.py:320): element 0, None = no ROIs
+            outputs = outputs[0] if len(outputs) and outputs[0] is not None else np.zeros((0, 7), np.float32)
         det = np.asarray(outputs.detach().cpu() if torch.is_tensor(outputs) else outputs, np.float32).reshape(-1, 7)
         n = det.shape[0]
         image = np.ascontiguousarray(image.detach().cpu().numpy() if torch.is_tensor(image) else image, np.uint8)

@@ -208,3 +208,73 @@ def make_icosphere_mesh(subdiv=3, extent=(0.1, 0.1, 0.1)):
         f = nf
     verts = np.array(v, dtype=np.float64) * (np.array(extent, dtype=np.float64) / 2.0)
     return verts.astype(np.float32), np.array(f, dtype=np.int32)
+
+
+def make_yolox_state_dict(forward, depth=0.33, width=0.25, num_classes=8, seed=0, calib_hw=(640, 640), calib_batch=2,
+                          device="cpu", target_conf=0.5, keep_frac=0.03, bn_gain=(0.4, 0.6), var_floor=1.0, bn_bias_std=1.0):
+    """Seeded YOLOX weights with the reference's state-dict keys (unfused, BatchNorm buffers included).
+
+    Random weights through a hundred folded conv layers would explode or vanish, so every BatchNorm's running mean and
+    variance are set from the statistics of its own input on a seeded calibration batch (``calib_batch`` images of ``calib_hw``; calibrate at the input size that will be
+    run: the SPP pools and the zero-padded borders make the statistics depend on the map size),
+    passed through ``forward`` (a float64 functional restatement of the network, ``forward(sd, x, depth,
+    num_classes, on_conv=...)`` calling ``on_conv(prefix, conv_out)`` before each BatchNorm, as the test oracle does)
+    layer by layer: activations stay O(1) as in a trained
+    network.  Each variance is floored at its layer's mean variance, so that channels that are nearly constant over the
+    calibration images do not amplify other inputs.  Conv weights N(0, 1/fan_in) (box predictions x 0.25), BatchNorm
+    weight U(0.4, 0.6) and bias N(0, 1): with the biases large against the weights the random network sits in the
+    ordered regime, where a rounding error shrinks from layer to layer instead of growing (with weight U(0.8, 1.2) and
+    bias N(0, 0.2) the fp32 forward of YOLOX-X already misses the fp64 one by pixels).  The prediction biases
+    start from the head's prior_prob = 0.01 init and are then shifted so that on the calibration batch the median class
+    logit reaches sigmoid 0.9 and about ``keep_frac`` of the anchors score at least ``target_conf``: a few hundred of
+    the 8400 anchors of a 640 x 640 image clear such a threshold."""
+    from .yolox_model import YOLOX
+
+    shapes = {k: tuple(v.shape) for k, v in YOLOX(depth, width, num_classes, max_batch=1).state_dict().items()}
+    g = torch.Generator().manual_seed(seed)
+    sd = {}
+    for k, s in shapes.items():
+        if k.endswith("num_batches_tracked"):
+            sd[k] = torch.zeros((), dtype=torch.int64)
+        elif len(s) == 4:
+            sd[k] = torch.randn(s, generator=g, dtype=torch.float64) * math.sqrt(1.0 / (s[1] * s[2] * s[3]))
+            if ".reg_preds." in k:
+                sd[k] *= 0.25
+        elif k.endswith("bn.weight"):
+            sd[k] = torch.rand(s, generator=g, dtype=torch.float64) * (bn_gain[1] - bn_gain[0]) + bn_gain[0]
+        elif k.endswith("running_var"):
+            sd[k] = torch.ones(s, dtype=torch.float64)
+        elif k.endswith("running_mean"):
+            sd[k] = torch.zeros(s, dtype=torch.float64)
+        elif ".obj_preds." in k or ".cls_preds." in k:
+            sd[k] = torch.full(s, -math.log((1 - 0.01) / 0.01), dtype=torch.float64)
+        elif ".reg_preds." in k:
+            sd[k] = torch.zeros(s, dtype=torch.float64)
+        else:
+            sd[k] = torch.randn(s, generator=g, dtype=torch.float64) * bn_bias_std
+    dev = torch.device(device)
+    sd = {k: v.to(dev) for k, v in sd.items()}
+    x = torch.rand((calib_batch, 3) + tuple(calib_hw), generator=g, dtype=torch.float64).to(dev) * 255
+
+    def calibrate(prefix, y):
+        sd[prefix + ".bn.running_mean"] = y.mean((0, 2, 3))
+        v = y.var((0, 2, 3), unbiased=False)
+        # floor: a channel that is nearly constant over noise images must not amplify another image's offsets
+        sd[prefix + ".bn.running_var"] = v + var_floor * v.mean()
+
+    with torch.no_grad():
+        forward(sd, x, depth, num_classes, on_conv=calibrate)
+        for k in range(3):   # logits without the prior
+            sd[f"head.obj_preds.{k}.bias"].zero_()
+            sd[f"head.cls_preds.{k}.bias"].zero_()
+        d = forward(sd, x, depth, num_classes)
+        logit = lambda p: torch.log(p) - torch.log1p(-p)  # noqa: E731
+        zc = logit(d[..., 5:].clamp(1e-12, 1 - 1e-12)).flatten()
+        zo = logit(d[..., 4].clamp(1e-12, 1 - 1e-12)).flatten()
+        b_c = math.log(9.0) - torch.quantile(zc, 0.5).item()
+        q = min(target_conf / 0.9, 0.999)
+        b_o = math.log(q / (1 - q)) - torch.quantile(zo, 1 - keep_frac).item()
+        for k in range(3):
+            sd[f"head.obj_preds.{k}.bias"].fill_(b_o)
+            sd[f"head.cls_preds.{k}.bias"].fill_(b_c)
+    return {k: (v.float() if v.is_floating_point() else v).cpu() for k, v in sd.items()}

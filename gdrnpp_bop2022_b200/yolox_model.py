@@ -1,0 +1,417 @@
+"""The YOLOX detector network (det/yolox/models: YOLOX(YOLOPAFPN(depth, width), YOLOXHead(num_classes, width))) on the
+CUDA kernels of csrc/yolox_net.cu, and a reader of the reference's YOLOX LazyConfig files.
+
+``YOLOX`` carries the reference's state-dict keys (``backbone.backbone.stem.conv.conv.weight``, ``...bn.running_var``,
+``num_batches_tracked``, ``head.cls_preds.0.bias``, ...), unfused or fused (conv bias, no ``bn``: what fuse_model saves).
+Its forward returns ``{"det_preds": [B, A, 5 + nc]}`` decoded like ``YOLOXHead`` with ``decode_in_inference=True``.
+
+At the first forward for an input size the state dict goes to the C ABI engine of csrc/yolox_net.cu (yolox_model_*),
+which folds the BatchNorms into the conv weights in float64 (fuse_conv_and_bn, det/yolox/utils/model_utils.py:33-58,
+eps 1e-3 as YOLOX.init_yolo sets it), packs them for the implicit-GEMM conv kernel and lays the layer plan out over fp32
+NHWC activation buffers in a workspace the module owns (the C caller owns it).  Concatenations are channel slices of
+those buffers: every producer writes its slice directly, so torch.cat costs nothing.  The two first head 3x3 convs of a
+level (cls_convs[k][0], reg_convs[k][0]) read the same stem output and run as one conv with doubled N; reg + obj
+predictions are one conv over reg_feat and the class predictions one over cls_feat, both into one raw buffer per level.
+A forward is 156 launches at YOLOX-X; ``capture_graph`` replays them as one CUDA graph.  No CPU fallback.
+"""
+import ast
+import ctypes
+import os
+from types import SimpleNamespace
+
+import torch
+import torch.nn as nn
+
+from . import _lib
+
+BN_EPS = 1e-3
+STRIDES = (8, 16, 32)
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# module tree with the reference's names (det/yolox/models/network_blocks.py, darknet.py, yolo_pafpn.py, yolo_head.py)
+# ---------------------------------------------------------------------------------------------------------------------
+class BaseConv(nn.Module):
+    def __init__(self, cin, cout, ksize, stride=1):
+        super().__init__()
+        self.stride = stride
+        self.conv = nn.Conv2d(cin, cout, ksize, stride, (ksize - 1) // 2, bias=False)
+        self.bn = nn.BatchNorm2d(cout, eps=BN_EPS, momentum=0.03)
+
+    def to_fused_layout(self):
+        if self.bn is not None:
+            self.conv.bias = nn.Parameter(torch.zeros(self.conv.out_channels, device=self.conv.weight.device))
+            self.bn = None
+
+    def folded(self):
+        """(W [Cout, Cin, k, k], b [Cout]) float64 with the BatchNorm folded in (fuse_conv_and_bn)."""
+        w = self.conv.weight.detach().double().cpu()
+        cb = None if self.conv.bias is None else self.conv.bias.detach().double().cpu()
+        if self.bn is None:
+            return w, (torch.zeros(w.shape[0], dtype=torch.float64) if cb is None else cb)
+        return fold_bn(w, self.bn.weight.detach().double().cpu(), self.bn.bias.detach().double().cpu(),
+                       self.bn.running_mean.double().cpu(), self.bn.running_var.double().cpu(), cb, self.bn.eps)
+
+
+def fold_bn(w, bn_w, bn_b, mean, var, conv_bias=None, eps=BN_EPS):
+    """fuse_conv_and_bn (det/yolox/utils/model_utils.py:33-58) in the dtype of the inputs."""
+    w_bn = torch.diag(bn_w.div(torch.sqrt(eps + var)))
+    fw = torch.mm(w_bn, w.reshape(w.shape[0], -1)).view(w.shape)
+    b_conv = torch.zeros(w.shape[0], dtype=w.dtype) if conv_bias is None else conv_bias
+    b_bn = bn_b - bn_w.mul(mean).div(torch.sqrt(var + eps))
+    return fw, torch.mm(w_bn, b_conv.reshape(-1, 1)).reshape(-1) + b_bn
+
+
+class Bottleneck(nn.Module):
+    def __init__(self, c, shortcut):
+        super().__init__()
+        self.conv1 = BaseConv(c, c, 1)
+        self.conv2 = BaseConv(c, c, 3)
+        self.use_add = shortcut
+
+
+class CSPLayer(nn.Module):
+    def __init__(self, cin, cout, n, shortcut=True):
+        super().__init__()
+        h = int(cout * 0.5)
+        self.hidden = h
+        self.conv1 = BaseConv(cin, h, 1)
+        self.conv2 = BaseConv(cin, h, 1)
+        self.conv3 = BaseConv(2 * h, cout, 1)
+        self.m = nn.Sequential(*[Bottleneck(h, shortcut) for _ in range(n)])
+
+
+class Focus(nn.Module):
+    def __init__(self, cout):
+        super().__init__()
+        self.conv = BaseConv(12, cout, 3)
+
+
+class SPPBottleneck(nn.Module):
+    def __init__(self, cin, cout):
+        super().__init__()
+        h = cin // 2
+        self.conv1 = BaseConv(cin, h, 1)
+        self.conv2 = BaseConv(4 * h, cout, 1)
+
+
+class CSPDarknet(nn.Module):
+    def __init__(self, depth, width):
+        super().__init__()
+        b = int(width * 64)
+        bd = max(round(depth * 3), 1)
+        self.stem = Focus(b)
+        self.dark2 = nn.Sequential(BaseConv(b, 2 * b, 3, 2), CSPLayer(2 * b, 2 * b, bd))
+        self.dark3 = nn.Sequential(BaseConv(2 * b, 4 * b, 3, 2), CSPLayer(4 * b, 4 * b, 3 * bd))
+        self.dark4 = nn.Sequential(BaseConv(4 * b, 8 * b, 3, 2), CSPLayer(8 * b, 8 * b, 3 * bd))
+        self.dark5 = nn.Sequential(BaseConv(8 * b, 16 * b, 3, 2), SPPBottleneck(16 * b, 16 * b),
+                                   CSPLayer(16 * b, 16 * b, bd, shortcut=False))
+
+
+class YOLOPAFPN(nn.Module):
+    def __init__(self, depth, width, in_channels=(256, 512, 1024)):
+        super().__init__()
+        c0, c1, c2 = (int(c * width) for c in in_channels)
+        n = round(3 * depth)
+        self.backbone = CSPDarknet(depth, width)
+        self.lateral_conv0 = BaseConv(c2, c1, 1)
+        self.C3_p4 = CSPLayer(2 * c1, c1, n, False)
+        self.reduce_conv1 = BaseConv(c1, c0, 1)
+        self.C3_p3 = CSPLayer(2 * c0, c0, n, False)
+        self.bu_conv2 = BaseConv(c0, c0, 3, 2)
+        self.C3_n3 = CSPLayer(2 * c0, c1, n, False)
+        self.bu_conv1 = BaseConv(c1, c1, 3, 2)
+        self.C3_n4 = CSPLayer(2 * c1, c2, n, False)
+
+
+class YOLOXHead(nn.Module):
+    def __init__(self, num_classes, width, in_channels=(256, 512, 1024)):
+        super().__init__()
+        ch = int(256 * width)
+        self.num_classes = num_classes
+        # registration order of the reference (state-dict key order)
+        self.cls_convs = nn.ModuleList(nn.Sequential(BaseConv(ch, ch, 3), BaseConv(ch, ch, 3)) for _ in in_channels)
+        self.reg_convs = nn.ModuleList(nn.Sequential(BaseConv(ch, ch, 3), BaseConv(ch, ch, 3)) for _ in in_channels)
+        self.cls_preds = nn.ModuleList(nn.Conv2d(ch, num_classes, 1) for _ in in_channels)
+        self.reg_preds = nn.ModuleList(nn.Conv2d(ch, 4, 1) for _ in in_channels)
+        self.obj_preds = nn.ModuleList(nn.Conv2d(ch, 1, 1) for _ in in_channels)
+        self.stems = nn.ModuleList(BaseConv(int(c * width), ch, 1) for c in in_channels)
+
+
+def _base_convs(module):
+    return [m for m in module.modules() if isinstance(m, BaseConv)]
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# engine: the C ABI model of csrc/yolox_net.cu for one (device, max_batch, H, W, precision)
+# ---------------------------------------------------------------------------------------------------------------------
+class _Engine:
+    def __init__(self, model, device, H, W):
+        L = _lib.lib()
+        self.device = device
+        h = ctypes.c_void_p()
+        _lib.check(L.yolox_model_create(ctypes.byref(h), model.depth, model.width, model.num_classes, model.max_batch, H, W,
+                                         1 if model.precision == "bf16x3" else 0), "yolox_model_create")
+        self.handle = h
+        self.A = L.yolox_model_num_anchors(h)
+        self.workspace = None
+        st = _lib.current_stream()
+        for k, v in model.state_dict().items():
+            if k.endswith("num_batches_tracked"):
+                continue
+            t = v.detach().to(device=device, dtype=torch.float32).contiguous()
+            _lib.check(L.yolox_model_load_tensor(h, k.encode(), _lib.ptr(t), t.numel(), st), f"yolox_model_load_tensor({k})")
+        missing = L.yolox_model_missing(h)
+        if missing != 0:
+            raise _lib.GdrnError(f"yolox_model_missing: {missing} convs lack a tensor ({_lib.last_error()})")
+
+    def new_workspace(self, B):
+        return torch.empty(_lib.lib().yolox_model_workspace_bytes(self.handle, B), dtype=torch.uint8, device=self.device)
+
+    def run(self, x, det, ws):
+        _lib.check(_lib.lib().yolox_model_forward(self.handle, _lib.ptr(x), x.shape[0], _lib.ptr(det), _lib.ptr(ws), ws.numel(),
+                                                  _lib.current_stream()), "yolox_model_forward")
+
+    def __del__(self):
+        try:
+            if self.handle:
+                _lib.lib().yolox_model_destroy(self.handle)
+        except Exception:  # noqa: BLE001 -- interpreter shutdown
+            pass
+
+
+class YOLOX(nn.Module):
+    """YOLOX(YOLOPAFPN(depth, width), YOLOXHead(num_classes, width)) for inference on the GPU.  precision "bf16x3"
+    (split-bf16 operands, the default) or "bf16"; batches larger than ``max_batch`` run in chunks."""
+
+    def __init__(self, depth=1.33, width=1.25, num_classes=80, max_batch=8, precision="bf16x3"):
+        super().__init__()
+        if precision not in ("bf16x3", "bf16"):
+            raise ValueError(f"precision must be 'bf16x3' or 'bf16', got {precision!r}")
+        self.depth, self.width, self.num_classes = float(depth), float(width), int(num_classes)
+        self.max_batch, self.precision = int(max_batch), precision
+        self.c_in = tuple(int(c * width) for c in (256, 512, 1024))
+        self.backbone = YOLOPAFPN(depth, width)
+        self.head = YOLOXHead(num_classes, width)
+        self._engines = {}
+        self._param_version = 0
+        self._graph_pinned = False
+
+    def fuse(self):
+        """Replace every conv + BatchNorm by the folded conv (fuse_model): the state dict then has conv biases and no bn."""
+        with torch.no_grad():
+            for m in _base_convs(self):
+                if m.bn is not None:
+                    w, b = m.folded()
+                    m.conv.weight.copy_(w.to(m.conv.weight))
+                    m.to_fused_layout()
+                    m.conv.bias.copy_(b.to(m.conv.bias))
+        self._param_version += 1
+        return self
+
+    def load_state_dict(self, state_dict, strict=True, **kw):
+        fused = not any(".bn." in k for k in state_dict) and any(k.endswith("stem.conv.conv.bias") for k in state_dict)
+        if fused:
+            for m in _base_convs(self):
+                m.to_fused_layout()
+        self._param_version += 1
+        return super().load_state_dict(state_dict, strict=strict, **kw)
+
+    def _engine(self, device, H, W):
+        if self._engines and next(iter(self._engines.values())).device != device:
+            raise _lib.GdrnError("this YOLOX's engine lives on another device; build one model per device")
+        key = (H, W)
+        eng = self._engines.get(key)
+        if eng is not None and eng.version != self._param_version:
+            if self._graph_pinned:
+                raise _lib.GdrnError("weights changed after capture_graph(): re-capture before reloading weights")
+            eng = None
+        if eng is None:
+            eng = _Engine(self, device, H, W)
+            eng.version = self._param_version
+            self._engines[key] = eng
+        return eng
+
+    def forward(self, x, targets=None, augment=False, cfg=None, _workspace=None):
+        """x [B,3,H,W] float (BGR, 0..255), H and W multiples of 32, on CUDA -> {"det_preds": [B, A, 5 + nc]}."""
+        if augment:
+            raise NotImplementedError("multi-scale test-time augmentation (test.augment) is not implemented")
+        if self.training:
+            raise NotImplementedError("YOLOX here is inference only (no training losses)")
+        if not torch.is_tensor(x) or not x.is_cuda:
+            raise _lib.GdrnError("YOLOX.forward needs a CUDA tensor (no CPU fallback)")
+        if x.dim() != 4 or x.shape[1] != 3:
+            raise ValueError(f"YOLOX.forward expects [B,3,H,W], got {tuple(x.shape)}")
+        B, _, H, W = x.shape
+        if H % 32 or W % 32 or H < 32 or W < 32:
+            raise ValueError(f"YOLOX input size must be a positive multiple of 32, got {H}x{W}")
+        x = x.detach().to(torch.float32).contiguous()
+        with torch.cuda.device(x.device):
+            eng = self._engine(x.device, H, W)
+            det = torch.empty((B, eng.A, 5 + self.num_classes), dtype=torch.float32, device=x.device)
+            ws = _workspace if _workspace is not None else eng.workspace
+            need = _lib.lib().yolox_model_workspace_bytes(eng.handle, B)
+            if ws is None or ws.numel() < need:
+                ws = eng.workspace = eng.new_workspace(B)
+            eng.run(x, det, ws)   # batches above max_batch run in chunks inside the engine
+        return {"det_preds": det}
+
+    def capture_graph(self, x, warmup=2):
+        """Capture one forward over the static input ``x`` into a CUDA graph -> ``(replay, out_dict)``: ``replay()``
+        re-runs the forward as one graph launch on the current stream; refill ``x`` in place between replays."""
+        if not (torch.is_tensor(x) and x.is_cuda and x.is_contiguous() and x.dtype == torch.float32):
+            raise _lib.GdrnError("capture_graph: x must be a contiguous float32 CUDA tensor")
+        if x.shape[0] > self.max_batch:
+            raise _lib.GdrnError(f"capture_graph: batch {x.shape[0]} above max_batch={self.max_batch}")
+        with torch.cuda.device(x.device):
+            self.forward(x)   # builds the engine and loads the weights outside the capture
+            # the graph bakes the workspace pointer in: it gets a workspace of its own, kept alive by replay()
+            ws = self._engines[(x.shape[2], x.shape[3])].new_workspace(x.shape[0])
+            side = torch.cuda.Stream(device=x.device)
+            side.wait_stream(torch.cuda.current_stream())
+            with torch.cuda.stream(side):
+                for _ in range(warmup):
+                    self.forward(x, _workspace=ws)
+            torch.cuda.current_stream().wait_stream(side)
+            torch.cuda.synchronize()
+            graph = torch.cuda.CUDAGraph()
+            with torch.cuda.graph(graph):
+                out = self.forward(x, _workspace=ws)
+        self._graph_pinned = True
+
+        def replay(_graph=graph, _ws=ws):
+            _graph.replay()
+
+        return replay, out
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# LazyConfig reader
+# ---------------------------------------------------------------------------------------------------------------------
+_MODEL_DEFAULTS = {"backbone.depth": 1.0, "backbone.width": 1.0, "backbone.in_channels": [256, 512, 1024],
+                   "backbone.depthwise": False, "backbone.act": "silu", "head.num_classes": 80,
+                   "head.width": "${..backbone.width}", "head.in_channels": "${..backbone.in_channels}",
+                   "head.depthwise": False, "head.act": "silu", "head.strides": [8, 16, 32]}
+_TEST_KEYS = ("test_size", "conf_thr", "nms_thr")
+
+
+def _literal(node, path):
+    try:
+        return ast.literal_eval(node)
+    except ValueError:
+        raise ValueError(f"{path}: {ast.unparse(node)!r} is not a literal the config reader can evaluate") from None
+
+
+def _dotted(node):
+    parts = []
+    while isinstance(node, ast.Attribute):
+        parts.append(node.attr)
+        node = node.value
+    if isinstance(node, ast.Name):
+        parts.append(node.id)
+        return ".".join(reversed(parts))
+    return None
+
+
+def _read_config(path, seen):
+    path = os.path.abspath(path)
+    if path in seen:
+        raise ValueError(f"{path}: import cycle")
+    seen = seen | {path}
+    tree = ast.parse(open(path).read(), path)
+    model, test = {}, {}
+    for node in tree.body:
+        if isinstance(node, ast.ImportFrom) and node.level == 1 and node.module:
+            names = {a.name for a in node.names}
+            if names & {"model", "test"}:
+                base = os.path.join(os.path.dirname(path), *node.module.split(".")) + ".py"
+                bm, bt = _read_config(base, seen)
+                model.update(bm)
+                test.update(bt)
+            continue
+        if isinstance(node, ast.Assign) and len(node.targets) == 1:
+            tgt, val = _dotted(node.targets[0]), node.value
+        elif isinstance(node, ast.AnnAssign):
+            tgt, val = _dotted(node.target), node.value
+        elif isinstance(node, ast.Expr) and isinstance(node.value, ast.Call) and _dotted(node.value.func) in (
+                "model.update", "test.update", "model.backbone.update", "model.head.update"):
+            obj = _dotted(node.value.func)[:-len(".update")]
+            for kw in node.value.keywords:
+                _set(model, test, f"{obj}.{kw.arg}", kw.value, path)
+            continue
+        else:
+            continue
+        if tgt is None:
+            continue
+        if tgt == "model":
+            model = {}
+            _read_lazy_call(val, "", model, path)
+        elif tgt == "test":
+            if isinstance(val, ast.Call) and _dotted(val.func) == "dict":
+                test = {}
+                for kw in val.keywords:
+                    if kw.arg in _TEST_KEYS:
+                        test[kw.arg] = _literal(kw.value, f"{path}: test.{kw.arg}")
+            # test = OmegaConf.create(test) and similar wrappers keep the values
+        elif tgt.startswith(("model.", "test.")):
+            _set(model, test, tgt, val, path)
+    return model, test
+
+
+def _set(model, test, tgt, val, path):
+    if tgt.startswith("model."):
+        key = tgt[len("model."):]
+        if isinstance(val, ast.Call):
+            _read_lazy_call(val, key + ".", model, path)
+        else:
+            model[key] = _literal(val, f"{path}: {tgt}")
+    elif tgt.startswith("test.") and tgt[len("test."):] in _TEST_KEYS:
+        test[tgt[len("test."):]] = _literal(val, f"{path}: {tgt}")
+
+
+def _read_lazy_call(node, prefix, out, path):
+    """model = L(YOLOX)(backbone=L(YOLOPAFPN)(depth=..., ...), head=L(YOLOXHead)(...)): keyword arguments by path."""
+    if not isinstance(node, ast.Call):
+        raise ValueError(f"{path}: model{('.' + prefix[:-1]) if prefix else ''} is not a LazyCall")
+    for kw in node.keywords:
+        if isinstance(kw.value, ast.Call) and isinstance(kw.value.func, ast.Call):
+            _read_lazy_call(kw.value, prefix + kw.arg + ".", out, path)
+        else:
+            out[prefix + kw.arg] = _literal(kw.value, f"{path}: model.{prefix}{kw.arg}")
+
+
+def load_yolox_config(path):
+    """Read a reference YOLOX LazyConfig (configs/yolox/**.py) without executing it: the literal assignments to
+    model.backbone.depth / width, model.head.num_classes and test.test_size / conf_thr / nms_thr, following the
+    ``from .yolox_base import ...`` chain.  A model setting the engine cannot honour (depthwise convs, an activation
+    other than silu, other strides or channel lists, a head width other than the backbone's) raises ValueError.
+    -> SimpleNamespace(depth, width, num_classes, test_size (h, w), conf_thr, nms_thr)."""
+    model, test = _read_config(path, frozenset())
+    cfg = dict(_MODEL_DEFAULTS)
+    for k, v in model.items():
+        if k not in cfg:
+            raise ValueError(f"{path}: model.{k} = {v!r} is not supported by the YOLOX engine")
+        cfg[k] = v
+    bad = []
+    for k in ("backbone.depthwise", "head.depthwise"):
+        if cfg[k]:
+            bad.append(f"model.{k} = {cfg[k]!r} (depthwise YOLOX is not supported)")
+    for k in ("backbone.act", "head.act"):
+        if cfg[k] != "silu":
+            bad.append(f"model.{k} = {cfg[k]!r} (only silu)")
+    if list(cfg["backbone.in_channels"]) != [256, 512, 1024]:
+        bad.append(f"model.backbone.in_channels = {cfg['backbone.in_channels']!r}")
+    if cfg["head.in_channels"] not in ("${..backbone.in_channels}", [256, 512, 1024]):
+        bad.append(f"model.head.in_channels = {cfg['head.in_channels']!r}")
+    if cfg["head.width"] not in ("${..backbone.width}", cfg["backbone.width"]):
+        bad.append(f"model.head.width = {cfg['head.width']!r} differs from the backbone width")
+    if list(cfg["head.strides"]) != [8, 16, 32]:
+        bad.append(f"model.head.strides = {cfg['head.strides']!r}")
+    if bad:
+        raise ValueError(f"{path}: " + "; ".join(bad))
+    missing = [k for k in _TEST_KEYS if k not in test]
+    if missing:
+        raise ValueError(f"{path}: test.{', test.'.join(missing)} not found")
+    return SimpleNamespace(depth=float(cfg["backbone.depth"]), width=float(cfg["backbone.width"]),
+                           num_classes=int(cfg["head.num_classes"]), test_size=tuple(int(v) for v in test["test_size"]),
+                           conf_thr=float(test["conf_thr"]), nms_thr=float(test["nms_thr"]))

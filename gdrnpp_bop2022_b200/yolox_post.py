@@ -3,7 +3,7 @@
 Mirrors ``postprocess(det_preds, num_classes, conf_thre, nms_thre, class_agnostic)`` (det/yolox/utils/boxes.py:34-80) and
 ``YOLOXHead.decode_outputs`` (det/yolox/models/yolo_head.py:239-255) with one call of libgdrn_b200.so per batch
 (csrc/yolox_post.cu): decode, filter, class-aware NMS, rows ``(x1, y1, x2, y2, obj_conf, class_conf, class_pred)`` in
-descending score order.  The YOLOX network itself is out of scope.  No CPU fallback.
+descending score order.  The YOLOX network itself is yolox_model.py.  No CPU fallback.
 """
 import torch
 

@@ -340,6 +340,35 @@ int yolox_postprocess(const float* preds, int B, int A, int num_classes, const i
                       void* workspace, size_t workspace_bytes, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
+ * YOLOX detector network (det/yolox/models: CSPDarknet + YOLOPAFPN + YOLOXHead, inference), csrc/yolox_net.cu.
+ *   yolox_model_create: one engine per (depth, width, num_classes, max_batch, H, W, precision); H, W multiples of 32;
+ *     precision 1 = bf16x3 (split-bf16 operands), 0 = bf16.  Channel counts must be multiples of 8.
+ *   yolox_model_load_tensor: one tensor of a reference state dict by name (device f32, numel elements): unfused
+ *     (conv.weight + bn.weight / bias / running_mean / running_var, BatchNorm eps 1e-3) or fused (conv.weight +
+ *     conv.bias); prediction convs as head.{cls,reg,obj}_preds.k.{weight,bias}.  Synchronises the stream (load time).
+ *   yolox_model_missing: folds BatchNorm in float64 and packs every conv whose tensors are all present; returns how
+ *     many convs still lack a tensor (0 = ready).
+ *   yolox_model_workspace_bytes(B): caller-owned activation workspace for a forward of B images (chunks of max_batch).
+ *   yolox_model_forward: img [B,3,H,W] f32 (BGR, 0..255) -> det_preds [B, A, 5 + num_classes] f32 (decoded boxes
+ *     cx, cy, w, h; sigmoid obj; sigmoid classes), A = yolox_model_num_anchors.  No allocation, no synchronisation.
+ *   yolox_postprocess_single: keep-single-instance post-process of the reference predictor (predictor_yolo.py:84-140):
+ *     per class the highest-scoring anchor with obj * cls_conf >= conf_thre, class-agnostic NMS, rows in ascending
+ *     class order; dets [B, num_classes, 7], n_det [B] i32.  Classes without such an anchor are left out.
+ * ------------------------------------------------------------------------------------------- */
+typedef struct YoloxModel YoloxModel;
+int yolox_model_create(YoloxModel** out, double depth, double width, int num_classes, int max_batch, int H, int W, int precision);
+void yolox_model_destroy(YoloxModel* m);
+int yolox_model_load_tensor(YoloxModel* m, const char* key, const float* data, int64_t numel, void* stream);
+int yolox_model_missing(YoloxModel* m);
+int yolox_model_num_anchors(const YoloxModel* m);
+size_t yolox_model_workspace_bytes(YoloxModel* m, int B);
+int yolox_model_forward(YoloxModel* m, const float* img, int B, float* det_preds, void* workspace, size_t workspace_bytes,
+                        void* stream);
+size_t yolox_postprocess_single_workspace_bytes(int B, int A, int num_classes);
+int yolox_postprocess_single(const float* preds, int B, int A, int num_classes, float conf_thre, float nms_thre, float* dets,
+                             int* n_det, void* workspace, size_t workspace_bytes, void* stream);
+
+/* ---------------------------------------------------------------------------------------------
  * BOP pose errors over a batch of P (estimate, GT) pairs -- replaces the per-pair numpy loops of lib/pysixd/pose_error.py
  * (vsd, mssd, mspd, add, adi) as eval_calc_errors.py drives them.  Results do not depend on the launch shape.
  *

@@ -1,0 +1,348 @@
+"""YOLOX detector network: oracle vs the reference fixture, state-dict layout, BN folding, config reader and the
+keep-single-instance semantics on the host; the CUDA forward, post-process and predictor chain on the GPU."""
+import math
+import os
+import sys
+
+import numpy as np
+import pytest
+import torch
+
+from conftest import ROOT
+
+sys.path.insert(0, os.path.join(ROOT, "tools"))
+from make_golden_ref_yolox import draw_state_dict  # noqa: E402
+
+from gdrnpp_bop2022_b200.yolox_model import YOLOX, fold_bn, load_yolox_config  # noqa: E402
+from oracle import yolox_oracle as O  # noqa: E402
+
+GOLD = os.path.join(ROOT, "tests", "golden", "ref_yolox.npz")
+
+
+def _gold():
+    z = np.load(GOLD)
+    sd = draw_state_dict(list(z["names"]), list(z["shapes"]))
+    return z, sd
+
+
+def _f64(sd, device="cpu"):
+    return {k: (v.double() if v.is_floating_point() else v).to(device) for k, v in sd.items()}
+
+
+def test_oracle_reproduces_reference_fixture():
+    z, sd = _gold()
+    out = O.yolox_forward(_f64(sd), torch.from_numpy(z["x"]).double(), float(z["depth"]), int(z["num_classes"]))
+    ref = torch.from_numpy(z["det_preds"]).double()
+    assert out.shape == ref.shape
+    # the fixture is the reference's fp32 forward: agreement to fp32 round-off of values up to ~90
+    assert torch.allclose(out, ref, rtol=1e-5, atol=2e-5), (out - ref).abs().max()
+
+
+def test_state_dict_layout_matches_reference_unfused_and_fused():
+    z, sd = _gold()
+    m = YOLOX(float(z["depth"]), float(z["width"]), int(z["num_classes"]))
+    names = list(z["names"])
+    shapes = [tuple(int(d) for d in s.split(",")) if s else () for s in z["shapes"]]
+    assert list(m.state_dict().keys()) == names
+    assert [tuple(v.shape) for v in m.state_dict().values()] == shapes
+    m.load_state_dict(sd)
+    m.fuse()
+    fused = m.state_dict()
+    assert not any(".bn." in k for k in fused) and "backbone.backbone.stem.conv.conv.bias" in fused
+    m2 = YOLOX(float(z["depth"]), float(z["width"]), int(z["num_classes"]))
+    m2.load_state_dict(fused)   # a fuse_model checkpoint loads into a fresh module
+    assert list(m2.state_dict().keys()) == list(fused.keys())
+    # the fused weights run through the oracle give the same detections
+    out = O.yolox_forward(_f64(fused), torch.from_numpy(z["x"]).double(), float(z["depth"]), int(z["num_classes"]))
+    assert torch.allclose(out, torch.from_numpy(z["det_preds"]).double(), rtol=1e-4, atol=1e-4)
+
+
+def test_bn_folding_matches_fuse_conv_and_bn():
+    g = torch.Generator().manual_seed(3)
+    conv = torch.nn.Conv2d(16, 24, 3, padding=1, bias=False).double()
+    bn = torch.nn.BatchNorm2d(24, eps=1e-3).double().eval()
+    with torch.no_grad():
+        conv.weight.copy_(torch.randn(conv.weight.shape, generator=g, dtype=torch.float64))
+        bn.weight.copy_(torch.rand(24, generator=g, dtype=torch.float64) + 0.5)
+        bn.bias.copy_(torch.randn(24, generator=g, dtype=torch.float64))
+        bn.running_mean.copy_(torch.randn(24, generator=g, dtype=torch.float64))
+        bn.running_var.copy_(torch.rand(24, generator=g, dtype=torch.float64) + 0.1)
+    w, b = fold_bn(conv.weight.detach(), bn.weight.detach(), bn.bias.detach(), bn.running_mean, bn.running_var)
+    x = torch.randn(2, 16, 8, 8, generator=g, dtype=torch.float64)
+    with torch.no_grad():
+        ref = bn(conv(x))
+    assert torch.allclose(torch.nn.functional.conv2d(x, w, b, padding=1), ref, atol=1e-12)
+
+
+BASE_CFG = '''
+from detectron2.config import LazyCall as L
+from omegaconf import OmegaConf
+from det.yolox.models import YOLOX, YOLOPAFPN, YOLOXHead
+model = L(YOLOX)(
+    backbone=L(YOLOPAFPN)(
+        depth=1.0,
+        width=1.0,
+        in_channels=[256, 512, 1024],
+    ),
+    head=L(YOLOXHead)(
+        num_classes=1,
+        width="${..backbone.width}",
+        in_channels="${..backbone.in_channels}",
+    ),
+)
+test = dict(
+    test_dataset_names=DATASETS.TEST,
+    test_size=(640, 640),  # (height, width)
+    conf_thr=0.01,
+    nms_thr=0.65,
+    num_classes="${model.head.num_classes}",
+    half_test=True,
+)
+test = OmegaConf.create(test)
+'''
+
+DERIVED_CFG = '''
+import os.path as osp
+from .yolox_base import train, val, test, model, dataloader, optimizer, lr_config, DATASETS  # noqa
+train.update(exp_name="x")
+model.backbone.depth = 1.33
+model.backbone.width = 1.25
+model.head.num_classes = 8
+test.test_dataset_names = DATASETS.TEST
+test.augment = True
+test.scales = (1, 0.75, 0.83, 1.12, 1.25)
+test.conf_thr = 0.001
+'''
+
+
+def test_load_yolox_config(tmp_path):
+    (tmp_path / "yolox_base.py").write_text(BASE_CFG)
+    (tmp_path / "yolox_x_lmo.py").write_text(DERIVED_CFG)
+    c = load_yolox_config(str(tmp_path / "yolox_x_lmo.py"))
+    assert (c.depth, c.width, c.num_classes, c.test_size, c.conf_thr, c.nms_thr) == (1.33, 1.25, 8, (640, 640), 0.001, 0.65)
+    c = load_yolox_config(str(tmp_path / "yolox_base.py"))
+    assert (c.depth, c.width, c.num_classes, c.conf_thr) == (1.0, 1.0, 1, 0.01)
+    for bad in ("model.backbone.depthwise = True\n", 'model.head.act = "relu"\n', "model.head.width = 0.5\n"):
+        (tmp_path / "bad.py").write_text(DERIVED_CFG + bad)
+        with pytest.raises(ValueError):
+            load_yolox_config(str(tmp_path / "bad.py"))
+
+
+@pytest.mark.skipif(not os.environ.get("GDRN_REFERENCE_SRC"), reason="GDRN_REFERENCE_SRC not set")
+def test_load_shipped_yolox_configs():
+    import glob
+
+    files = sorted(glob.glob(os.path.join(os.environ["GDRN_REFERENCE_SRC"], "configs", "yolox", "bop_pbr", "yolox_x_*.py")))
+    assert files
+    for f in files:
+        c = load_yolox_config(f)
+        assert (c.depth, c.width, c.test_size) == (1.33, 1.25, (640, 640)) and c.num_classes >= 1
+
+
+def test_keep_single_instance_semantics_on_host():
+    # 3 classes; class 0 has two candidates (the higher wins), class 1 overlaps class 0's winner and scores lower
+    # (suppressed), class 2 has none above the threshold (dropped, not a random row)
+    def row(cx, cy, w, h, obj, cls):
+        return [cx, cy, w, h, obj] + cls
+
+    det = np.array([
+        row(50, 50, 20, 20, 0.9, [0.8, 0.1, 0.1]),
+        row(52, 50, 20, 20, 0.95, [0.9, 0.1, 0.1]),
+        row(51, 50, 20, 20, 0.9, [0.1, 0.7, 0.1]),
+        row(150, 150, 10, 10, 0.9, [0.1, 0.2, 0.3]),
+        row(250, 250, 10, 10, 0.9, [0.1, 0.6, 0.1]),
+    ])
+    out = O.keep_single_instance(det, 3, conf_thre=0.5, nms_thre=0.45)
+    assert out.shape == (1, 7)
+    assert out[0, 6] == 0 and math.isclose(out[0, 4], 0.95) and math.isclose(out[0, 0], 42.0)
+    # without the overlap, one row per class in ascending class order
+    det[2, :2] = [300, 300]
+    out = O.keep_single_instance(det, 3, conf_thre=0.5, nms_thre=0.45)
+    assert list(out[:, 6]) == [0, 1] and math.isclose(out[1, 5], 0.7)
+    assert O.keep_single_instance(det, 3, conf_thre=0.99, nms_thre=0.45) is None
+
+
+# ------------------------------------------------------------------------------------------------------------- GPU
+def _run(depth, width, nc, sd, x, precision, max_batch=8):
+    m = YOLOX(depth, width, nc, max_batch=max_batch, precision=precision).eval()
+    m.load_state_dict(sd)
+    return m.to("cuda"), m(x.cuda())["det_preds"]
+
+
+def _errs(out, ref):
+    d = (out.double().cpu() - ref.cpu()).abs()
+    return d[..., :4].max().item(), d[..., 4:].max().item()
+
+
+def _fp32_errs(sd, x, depth, nc, ref):
+    """Error of the same forward in fp32 (cuDNN, TF32 off) against fp64, printed beside the CUDA errors: it shows how
+    much of the bars the synthetic network's own conditioning uses up."""
+    tf32 = torch.backends.cudnn.allow_tf32
+    torch.backends.cudnn.allow_tf32 = False
+    try:
+        r32 = O.yolox_forward({k: v.float().cuda() if v.is_floating_point() else v for k, v in sd.items()},
+                              x.float().cuda(), depth, nc)
+    finally:
+        torch.backends.cudnn.allow_tf32 = tf32
+    return _errs(r32, ref)
+
+
+BARS = {"bf16x3": (0.05, 1e-4), "bf16": (2.0, 2e-2)}   # max box-coordinate error (px), max score error
+
+
+_SD = {}
+
+
+def _synthetic(depth, width, nc, hw, calib_batch):
+    from gdrnpp_bop2022_b200.synthetic import make_yolox_state_dict
+
+    key = (depth, width, nc, hw, calib_batch)
+    if key not in _SD:
+        _SD[key] = make_yolox_state_dict(O.yolox_forward, depth, width, nc, seed=0, calib_hw=hw, calib_batch=calib_batch, device="cuda")
+    return _SD[key]
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("B", [1, 3])
+def test_yolox_x_640_against_fp64_oracle(B):
+    sd = _synthetic(1.33, 1.25, 8, (640, 640), 2)
+    x = torch.rand((B, 3, 640, 640), generator=torch.Generator().manual_seed(7)) * 255
+    ref = O.yolox_forward(_f64(sd, "cuda"), x.double().cuda(), 1.33, 8)
+    fb, fs = _fp32_errs(sd, x, 1.33, 8, ref)
+    print(f"YOLOX-X 640x640 B={B} fp32 cuDNN: max box err {fb:.3g} px, max score err {fs:.3g}")
+    for precision, (box_tol, score_tol) in BARS.items():
+        _, out = _run(1.33, 1.25, 8, sd, x, precision)
+        eb, es = _errs(out, ref)
+        print(f"YOLOX-X 640x640 B={B} {precision}: max box err {eb:.3g} px, max score err {es:.3g}")
+        assert eb < box_tol and es < score_tol, (precision, eb, es)
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("width,hw,B", [(0.25, (64, 96), 1), (0.25, (64, 96), 5), (0.5, (64, 96), 2),
+                                        (0.25, (480, 640), 2), (0.5, (480, 640), 1)])
+def test_small_and_odd_shapes(width, hw, B):
+    sd = _synthetic(0.33, width, 8, hw, 32 if hw[0] < 100 else 2)
+    x = torch.rand((B, 3) + hw, generator=torch.Generator().manual_seed(8)) * 255
+    ref = O.yolox_forward(_f64(sd, "cuda"), x.double().cuda(), 0.33, 8)
+    fb, fs = _fp32_errs(sd, x, 0.33, 8, ref)
+    for precision, (box_tol, score_tol) in BARS.items():
+        _, out = _run(0.33, width, 8, sd, x, precision, max_batch=2)   # B = 5 runs in chunks of 2
+        eb, es = _errs(out, ref)
+        print(f"width {width} {hw} B={B} {precision}: box {eb:.3g} px score {es:.3g}; fp32 cuDNN {fb:.3g} px {fs:.3g}")
+        assert eb < box_tol and es < score_tol, (precision, eb, es)
+
+
+@pytest.mark.gpu
+def test_reference_fixture_on_gpu():
+    z, sd = _gold()
+    ref = O.yolox_forward(_f64(sd), torch.from_numpy(z["x"]).double(), float(z["depth"]), int(z["num_classes"]))
+    for precision, (box_tol, score_tol) in BARS.items():
+        _, out = _run(float(z["depth"]), float(z["width"]), int(z["num_classes"]), sd, torch.from_numpy(z["x"]), precision)
+        eb, es = _errs(out, ref)
+        print(f"reference fixture {precision}: box {eb:.3g} px score {es:.3g}")
+        assert eb < box_tol and es < score_tol, (precision, eb, es)
+    # the engine folds BatchNorm itself: a fuse_model state dict gives the same detections
+    m = YOLOX(float(z["depth"]), float(z["width"]), int(z["num_classes"]))
+    m.load_state_dict(sd)
+    m.fuse()
+    _, out = _run(float(z["depth"]), float(z["width"]), int(z["num_classes"]), m.state_dict(), torch.from_numpy(z["x"]), "bf16x3")
+    eb, es = _errs(out, ref)
+    assert eb < 0.05 and es < 1e-4, ("fused", eb, es)
+
+
+@pytest.mark.gpu
+def test_determinism_batch_independence_and_graph():
+    sd = _synthetic(0.33, 0.25, 8, (480, 640), 2)
+    x = (torch.rand((5, 3, 480, 640), generator=torch.Generator().manual_seed(9)) * 255).cuda()
+    m = YOLOX(0.33, 0.25, 8, max_batch=5).eval()
+    m.load_state_dict(sd)
+    m.cuda()
+    a = m(x)["det_preds"]
+    b = m(x)["det_preds"]
+    assert torch.equal(a, b)
+    for i in (0, 3):
+        assert torch.equal(m(x[i:i + 1].contiguous())["det_preds"][0], a[i])
+    xs = x[:1].clone()
+    replay, out = m.capture_graph(xs)
+    xs.copy_(x[3:4])
+    replay()
+    torch.cuda.synchronize()
+    assert torch.equal(out["det_preds"][0], a[3])
+
+
+@pytest.mark.gpu
+def test_invalid_input():
+    from gdrnpp_bop2022_b200._lib import GdrnError
+
+    m = YOLOX(0.33, 0.25, 3).eval()
+    with pytest.raises((GdrnError, ValueError)):
+        m(torch.zeros(1, 3, 64, 96))            # CPU tensor
+    m.cuda()
+    with pytest.raises((GdrnError, ValueError)):
+        m(torch.zeros(1, 3, 64, 90, device="cuda"))
+    with pytest.raises(NotImplementedError):
+        m(torch.zeros(1, 3, 64, 96, device="cuda"), augment=True)
+
+
+def _scene(seed=0, H=480, W=640):
+    rng = np.random.RandomState(seed)
+    img = (rng.rand(H, W, 3) * 255).astype(np.uint8)
+    return img
+
+
+@pytest.mark.gpu
+def test_predictor_matches_oracle_pipeline():
+    from types import SimpleNamespace
+
+    from gdrnpp_bop2022_b200.predictor_yolo import YoloPredictor, preproc
+
+    sd = _synthetic(0.33, 0.5, 8, (640, 640), 2)
+    cfg = SimpleNamespace(depth=0.33, width=0.5, num_classes=8, test_size=(640, 640), conf_thr=0.5, nms_thr=0.45)
+    img = _scene(1, 480, 640)
+    x, r = preproc(img, cfg.test_size)
+    d = O.yolox_forward(_f64(sd, "cuda"), torch.from_numpy(x)[None].double().cuda(), 0.33, 8)[0].cpu().numpy()
+    score = np.sort(d[:, 4] * d[:, 5:].max(1))
+    # a threshold near 0.5 in a gap of the oracle scores, so that the comparison is well-posed
+    gaps = [(abs(0.5 * (a + b) - 0.5), 0.5 * (a + b)) for a, b in zip(score[:-1], score[1:]) if b - a > 2e-3]
+    cfg.conf_thr = float(min(gaps)[1])
+    assert np.abs(score - cfg.conf_thr).min() > 1e-3, "an oracle score sits on the threshold"
+    pred = YoloPredictor(cfg=cfg, state_dict={"_module." + k: v for k, v in sd.items()})
+    out = pred.inference(img)
+    ious = []
+    ref = O.keep_single_instance(d, 8, cfg.conf_thr, cfg.nms_thr, ious=ious)
+    assert all(abs(v - cfg.nms_thr) > 1e-3 for v in ious), "a compared IoU sits on the NMS threshold"
+    assert ref is not None and out[0] is not None
+    got = out[0].cpu().numpy()
+    assert got.shape == ref.shape, (got, ref)
+    assert (got[:, 6] == ref[:, 6]).all()
+    print("predictor vs oracle pipeline: box err", np.abs(got[:, :4] - ref[:, :4] / r).max(), "score err",
+          np.abs(got[:, 4:6] - ref[:, 4:6]).max())
+    assert np.abs(got[:, :4] - ref[:, :4] / r).max() < 0.05 and np.abs(got[:, 4:6] - ref[:, 4:6]).max() < 1e-4
+
+
+@pytest.mark.gpu
+def test_predictor_chains_into_gdrn_predictor():
+    from types import SimpleNamespace
+
+    from gdrnpp_bop2022_b200.predictor import GdrnPredictor
+    from gdrnpp_bop2022_b200.predictor_yolo import YoloPredictor
+    from gdrnpp_bop2022_b200.synthetic import YCBV_K, make_state_dict
+
+    sd = _synthetic(0.33, 0.25, 3, (640, 640), 2)
+    cfg = SimpleNamespace(depth=0.33, width=0.25, num_classes=3, test_size=(640, 640), conf_thr=0.3, nms_thr=0.65)
+    yolo = YoloPredictor(cfg=cfg, state_dict=sd)
+    objs = {i: "obj_%06d" % i for i in range(1, 22)}
+    gdrn = GdrnPredictor(cam=YCBV_K, objs=objs, extents={i: (0.1, 0.1, 0.1) for i in objs}, state_dict=make_state_dict())
+    img = _scene(2)
+    outputs = yolo.inference(img)
+    assert isinstance(outputs, list) and len(outputs) == 1 and outputs[0] is not None
+    data = gdrn.preprocessing(outputs=outputs, image=img)
+    assert data["roi_img"].shape[0] == outputs[0].shape[0]
+    poses = gdrn.postprocessing(data, gdrn.inference(data))
+    assert len(poses) >= 1
+    # no detections: zero ROIs, no exception
+    yolo.cfg.conf_thr = 1.01
+    outputs = yolo.inference(img)
+    assert outputs == [None]
+    data = gdrn.preprocessing(outputs=outputs, image=img)
+    assert data["roi_img"].shape[0] == 0
