@@ -213,6 +213,65 @@ __global__ void yolox_focus_kernel(const float* __restrict__ img, int B, int H, 
   for (int q = 0; q < 4; ++q) o[q] = make_float4(v[4 * q], v[4 * q + 1], v[4 * q + 2], v[4 * q + 3]);
 }
 
+// one axis of torch's upsample_bilinear2d (align_corners=False, output size given): source row / column i0, the step to
+// the next one (0 at the last) and the weight of the next one; scale = (float)in / out
+struct YSample { int i0, step; float lam; };
+__device__ __forceinline__ YSample yolox_bilinear_axis(int dst, float scale, int in) {
+  float src = scale * (dst + 0.5f) - 0.5f;
+  src = src < 0.f ? 0.f : src;
+  YSample s;
+  s.i0 = (int)src;
+  s.step = s.i0 < in - 1 ? 1 : 0;
+  s.lam = src - (float)s.i0;
+  return s;
+}
+
+// Focus of the multi-scale test input (model_utils.scale_img: bilinear resize of [B,3,H,W] to the content size sh x sw,
+// then padding right / bottom with 0.447 * 255 up to PH x PW) without materialising the scaled image: every pixel Focus
+// reads is sampled from the original input.  Output as yolox_focus_kernel: NHWC [B,PH/2,PW/2,16], (TL, BL, TR, BR) x 3.
+__global__ void yolox_focus_resample_kernel(const float* __restrict__ img, int B, int H, int W, int PH, int PW, int sh, int sw,
+                                            float scale_h, float scale_w, float* __restrict__ out) {
+  ptx::griddep_launch();
+  ptx::griddep_wait();   // PDL: the producer kernel's writes are visible from here on
+  const int h2 = PH / 2, w2 = PW / 2;
+  const long long n = (long long)B * h2 * w2;
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const int x = (int)(i % w2);
+  const long long tt = i / w2;
+  const int y = (int)(tt % h2), b = (int)(tt / h2);
+  const float pad = (float)(0.447 * 255);
+  YSample ry[2], rx[2];
+#pragma unroll
+  for (int d = 0; d < 2; ++d) {
+    ry[d] = yolox_bilinear_axis(2 * y + d, scale_h, H);
+    rx[d] = yolox_bilinear_axis(2 * x + d, scale_w, W);
+  }
+  float v[16];
+  const int dy[4] = {0, 1, 0, 1}, dx[4] = {0, 0, 1, 1};
+#pragma unroll
+  for (int q = 0; q < 4; ++q) {
+    const YSample& sy = ry[dy[q]];
+    const YSample& sx = rx[dx[q]];
+    const bool inside = 2 * y + dy[q] < sh && 2 * x + dx[q] < sw;
+    const float h1l = sy.lam, h0l = 1.f - h1l, w1l = sx.lam, w0l = 1.f - w1l;
+#pragma unroll
+    for (int c = 0; c < 3; ++c) {
+      float r = pad;
+      if (inside) {
+        const float* p0 = img + (((long long)b * 3 + c) * H + sy.i0) * W + sx.i0;
+        const float* p1 = p0 + (long long)sy.step * W;
+        r = h0l * (w0l * __ldg(p0) + w1l * __ldg(p0 + sx.step)) + h1l * (w0l * __ldg(p1) + w1l * __ldg(p1 + sx.step));
+      }
+      v[q * 3 + c] = r;
+    }
+  }
+  v[12] = v[13] = v[14] = v[15] = 0.f;
+  float4* o = reinterpret_cast<float4*>(out + i * 16);
+#pragma unroll
+  for (int q = 0; q < 4; ++q) o[q] = make_float4(v[4 * q], v[4 * q + 1], v[4 * q + 2], v[4 * q + 3]);
+}
+
 // SPPBottleneck (network_blocks.py:118-133): max-pools 5 / 9 / 13, stride 1, padding k/2 (-inf, like nn.MaxPool2d) of the
 // C channels at slice 0 of buf, written to slices C, 2C, 3C of the same buffer
 __global__ void yolox_spp_kernel(float* __restrict__ buf, int B, int H, int W, int ld, int C) {
@@ -263,9 +322,11 @@ __global__ void yolox_upsample2x_kernel(const float* __restrict__ src, int lds, 
 }
 
 // head output of one level (yolo_head.py:191-254): raw [B, h*w, 5 + nc] (reg 4 | obj | cls) -> det_preds rows
-// [a_off, a_off + h*w) of [B, A, 5 + nc]: xy = (xy + grid) * stride, wh = exp(wh) * stride, sigmoid(obj), sigmoid(cls)
+// [a_off, a_off + h*w) of [B, A, 5 + nc]: xy = (xy + grid) * stride, wh = exp(wh) * stride, sigmoid(obj), sigmoid(cls).
+// The four box columns are then multiplied by inv_scale: the test-time-augmentation de-scale det[..., :4] /= s, which
+// torch evaluates on CUDA for a Python-scalar divisor as x * (1.0f / (float)s).  inv_scale = 1 leaves them exact.
 __global__ void yolox_head_out_kernel(const float* __restrict__ raw, int B, int h, int w, int nc, int stride, int A, int a_off,
-                                      float* __restrict__ det) {
+                                      float inv_scale, float* __restrict__ det) {
   ptx::griddep_launch();
   ptx::griddep_wait();   // PDL: the producer kernel's writes are visible from here on
   const int C = 5 + nc;
@@ -282,6 +343,7 @@ __global__ void yolox_head_out_kernel(const float* __restrict__ raw, int B, int 
   else if (c == 1) o = __fmul_rn(__fadd_rn(v, (float)(loc / w)), st);
   else if (c < 4) o = __fmul_rn(expf(v), st);
   else o = __frcp_rn(__fadd_rn(1.f, expf(-v)));
+  if (c < 4) o = __fmul_rn(o, inv_scale);
   det[((long long)b * A + a_off + loc) * C + c] = o;
 }
 
@@ -394,6 +456,8 @@ inline int blocks_for(long long n, int t) { return (int)((n + t - 1) / t); }
 // BatchNorm, or fused conv + bias); BatchNorm is folded on the host in float64 once every tensor of a conv is present.
 // Activations live in the caller's workspace as fp32 NHWC buffers; a concatenation is one buffer whose producers write
 // their own channel slices.  The forward allocates nothing, does not synchronise and launches with PDL.
+// Multi-scale test-time augmentation adds one layer plan per scale over the same packed weights (yolox_model_set_scales);
+// a scaled plan's Focus step resamples the original input and its head outputs land at the scale's anchor base.
 // ---------------------------------------------------------------------------------------------------------------------
 #include <algorithm>
 #include <cmath>
@@ -420,149 +484,166 @@ struct YStep {
 };
 struct YBuf { long long pix; int ld; };   // pixels per image, channels
 
+// the layer plan of one network input size.  Plan 0 runs the create-time H x W input as it is; a test-time-augmentation
+// plan runs the input resampled to sh x sw and padded to H x W (model_utils.scale_img) and de-scales its boxes.
+struct YPlan {
+  int H = 0, W = 0;          // network input size (multiples of 32)
+  int sh = 0, sw = 0;        // content size of the resampled image
+  bool resample = false;
+  float inv_scale = 1.f;     // box de-scale factor 1.0f / (float)s
+  int A = 0;                 // anchors
+  std::vector<YBuf> bufs;
+  std::vector<YStep> steps;
+  std::vector<size_t> offs;  // per-buffer workspace offsets (recomputed per chunk size)
+};
+
 }  // namespace
 
 struct YoloxModel {
-  int nc, max_batch, H, W, split, A;
+  int nc, max_batch, H, W, split;
+  double depth, width;
   std::map<std::string, std::vector<double>> host;   // loaded tensors (float64)
-  std::map<std::string, YConv> convs;                  // packed GEMM operands by plan name
-  std::map<std::string, std::vector<std::string>> sources;   // plan name -> the base convs / pred convs it packs from
-  std::vector<YBuf> bufs;
-  std::vector<YStep> steps;
-  std::vector<size_t> offs;                            // per-buffer workspace offsets (recomputed per chunk size)
+  std::map<std::string, YConv> convs;                  // packed GEMM operands by conv name, shared by every plan
+  std::map<std::string, std::vector<std::string>> sources;   // conv name -> the base convs / pred convs it packs from
+  std::vector<YPlan> plans;                            // [0]: the create-time size; then one per non-unit TTA scale
+  std::vector<int> tta_plan;                           // yolox_model_set_scales: plan index per scale, in scale order
+  int A_tta = 0;                                       // anchors summed over the scales
 };
 
 namespace {
 
 size_t yx_align(size_t v) { return (v + 255) & ~(size_t)255; }
 
-int yx_buf(YoloxModel* m, int h, int w, int c) { m->bufs.push_back({(long long)h * w, c}); return (int)m->bufs.size() - 1; }
+int yx_buf(YPlan* pl, int h, int w, int c) { pl->bufs.push_back({(long long)h * w, c}); return (int)pl->bufs.size() - 1; }
 
+// conv shapes do not depend on the input size: the first plan declares them, later plans find them declared
 void yx_conv_decl(YoloxModel* m, const std::string& name, int cin, int cout, int k, const std::vector<std::string>& src) {
+  if (m->convs.count(name)) return;
   YConv c; c.cin = cin; c.cout = cout; c.k = k;
   m->convs[name] = c;
   m->sources[name] = src;
 }
 
-void yx_conv(YoloxModel* m, const std::string& name, int src, int s_off, int s_c, int dst, int d_off, int d_c, int h, int w,
+void yx_conv(YPlan* pl, const std::string& name, int src, int s_off, int s_c, int dst, int d_off, int d_c, int h, int w,
              int ks, int stride = 1, int res = -1, int r_off = 0, int act = 1) {
   YStep s; s.kind = YS_CONV; s.w = name; s.src = src; s.s_off = s_off; s.s_c = s_c; s.dst = dst; s.d_off = d_off; s.d_c = d_c;
   s.h = h; s.wd = w; s.ks = ks; s.stride = stride; s.res = res; s.r_off = r_off; s.act = act;
-  m->steps.push_back(s);
+  pl->steps.push_back(s);
 }
 
 void yx_base(YoloxModel* m, const std::string& p, int cin, int cout, int k) { yx_conv_decl(m, p, cin, cout, k, {p}); }
 
 // CSPLayer: conv1 / conv2 into the two halves of one concat buffer, bottlenecks in place over the first half (the shortcut
 // add after the activation reads and writes each element in the same thread), conv3 from the whole buffer
-void yx_csp(YoloxModel* m, const std::string& p, int cin, int cout, int n, bool shortcut, int src, int s_off, int dst, int d_off,
+void yx_csp(YoloxModel* m, YPlan* pl, const std::string& p, int cin, int cout, int n, bool shortcut, int src, int s_off, int dst, int d_off,
             int h, int w) {
   const int hd = cout / 2;
   yx_base(m, p + ".conv1", cin, hd, 1);
   yx_base(m, p + ".conv2", cin, hd, 1);
   yx_base(m, p + ".conv3", 2 * hd, cout, 1);
-  const int cat = yx_buf(m, h, w, 2 * hd);
-  yx_conv(m, p + ".conv1", src, s_off, cin, cat, 0, hd, h, w, 1);
-  yx_conv(m, p + ".conv2", src, s_off, cin, cat, hd, hd, h, w, 1);
-  const int tmp = n ? yx_buf(m, h, w, hd) : -1;
+  const int cat = yx_buf(pl, h, w, 2 * hd);
+  yx_conv(pl, p + ".conv1", src, s_off, cin, cat, 0, hd, h, w, 1);
+  yx_conv(pl, p + ".conv2", src, s_off, cin, cat, hd, hd, h, w, 1);
+  const int tmp = n ? yx_buf(pl, h, w, hd) : -1;
   for (int i = 0; i < n; ++i) {
     const std::string q = p + ".m." + std::to_string(i);
     yx_base(m, q + ".conv1", hd, hd, 1);
     yx_base(m, q + ".conv2", hd, hd, 3);
-    yx_conv(m, q + ".conv1", cat, 0, hd, tmp, 0, hd, h, w, 1);
-    yx_conv(m, q + ".conv2", tmp, 0, hd, cat, 0, hd, h, w, 3, 1, shortcut ? cat : -1, 0);
+    yx_conv(pl, q + ".conv1", cat, 0, hd, tmp, 0, hd, h, w, 1);
+    yx_conv(pl, q + ".conv2", tmp, 0, hd, cat, 0, hd, h, w, 3, 1, shortcut ? cat : -1, 0);
   }
-  yx_conv(m, p + ".conv3", cat, 0, 2 * hd, dst, d_off, cout, h, w, 1);
+  yx_conv(pl, p + ".conv3", cat, 0, 2 * hd, dst, d_off, cout, h, w, 1);
 }
 
-void yx_build(YoloxModel* m, double depth, double width) {
+void yx_build(YoloxModel* m, YPlan* pl) {
+  const double depth = m->depth, width = m->width;
   const int b = (int)(width * 64), bd = std::max((int)std::lround(depth * 3), 1), nf = (int)std::lround(3 * depth);
   const int c0 = (int)(256 * width), c1 = (int)(512 * width), c2 = (int)(1024 * width), ch = (int)(256 * width);
   int sh[6], sw[6];
-  for (int i = 0; i < 6; ++i) { sh[i] = m->H >> i; sw[i] = m->W >> i; }
+  for (int i = 0; i < 6; ++i) { sh[i] = pl->H >> i; sw[i] = pl->W >> i; }
   const std::string p = "backbone.backbone.";
   YStep f; f.kind = YS_FOCUS;
-  f.dst = yx_buf(m, sh[1], sw[1], 16);
-  m->steps.push_back(f);
+  f.dst = yx_buf(pl, sh[1], sw[1], 16);
+  pl->steps.push_back(f);
   yx_conv_decl(m, p + "stem.conv", 16, b, 3, {p + "stem.conv"});   // 12 Focus channels, padded to 16 with zero weights
-  const int x = yx_buf(m, sh[1], sw[1], b);
-  yx_conv(m, p + "stem.conv", f.dst, 0, 16, x, 0, b, sh[1], sw[1], 3);
-  int t = yx_buf(m, sh[2], sw[2], 2 * b);
+  const int x = yx_buf(pl, sh[1], sw[1], b);
+  yx_conv(pl, p + "stem.conv", f.dst, 0, 16, x, 0, b, sh[1], sw[1], 3);
+  int t = yx_buf(pl, sh[2], sw[2], 2 * b);
   yx_base(m, p + "dark2.0", b, 2 * b, 3);
-  yx_conv(m, p + "dark2.0", x, 0, b, t, 0, 2 * b, sh[1], sw[1], 3, 2);
-  const int d2 = yx_buf(m, sh[2], sw[2], 2 * b);
-  yx_csp(m, p + "dark2.1", 2 * b, 2 * b, bd, true, t, 0, d2, 0, sh[2], sw[2]);
-  const int cat_p3 = yx_buf(m, sh[3], sw[3], 2 * c0), cat_p4 = yx_buf(m, sh[4], sw[4], 2 * c1);
-  t = yx_buf(m, sh[3], sw[3], 4 * b);
+  yx_conv(pl, p + "dark2.0", x, 0, b, t, 0, 2 * b, sh[1], sw[1], 3, 2);
+  const int d2 = yx_buf(pl, sh[2], sw[2], 2 * b);
+  yx_csp(m, pl, p + "dark2.1", 2 * b, 2 * b, bd, true, t, 0, d2, 0, sh[2], sw[2]);
+  const int cat_p3 = yx_buf(pl, sh[3], sw[3], 2 * c0), cat_p4 = yx_buf(pl, sh[4], sw[4], 2 * c1);
+  t = yx_buf(pl, sh[3], sw[3], 4 * b);
   yx_base(m, p + "dark3.0", 2 * b, 4 * b, 3);
-  yx_conv(m, p + "dark3.0", d2, 0, 2 * b, t, 0, 4 * b, sh[2], sw[2], 3, 2);
-  yx_csp(m, p + "dark3.1", 4 * b, 4 * b, 3 * bd, true, t, 0, cat_p3, c0, sh[3], sw[3]);     // dark3 -> cat_p3[c0:]
-  t = yx_buf(m, sh[4], sw[4], 8 * b);
+  yx_conv(pl, p + "dark3.0", d2, 0, 2 * b, t, 0, 4 * b, sh[2], sw[2], 3, 2);
+  yx_csp(m, pl, p + "dark3.1", 4 * b, 4 * b, 3 * bd, true, t, 0, cat_p3, c0, sh[3], sw[3]);     // dark3 -> cat_p3[c0:]
+  t = yx_buf(pl, sh[4], sw[4], 8 * b);
   yx_base(m, p + "dark4.0", 4 * b, 8 * b, 3);
-  yx_conv(m, p + "dark4.0", cat_p3, c0, c0, t, 0, 8 * b, sh[3], sw[3], 3, 2);
-  yx_csp(m, p + "dark4.1", 8 * b, 8 * b, 3 * bd, true, t, 0, cat_p4, c1, sh[4], sw[4]);     // dark4 -> cat_p4[c1:]
-  t = yx_buf(m, sh[5], sw[5], 16 * b);
+  yx_conv(pl, p + "dark4.0", cat_p3, c0, c0, t, 0, 8 * b, sh[3], sw[3], 3, 2);
+  yx_csp(m, pl, p + "dark4.1", 8 * b, 8 * b, 3 * bd, true, t, 0, cat_p4, c1, sh[4], sw[4]);     // dark4 -> cat_p4[c1:]
+  t = yx_buf(pl, sh[5], sw[5], 16 * b);
   yx_base(m, p + "dark5.0", 8 * b, 16 * b, 3);
-  yx_conv(m, p + "dark5.0", cat_p4, c1, c1, t, 0, 16 * b, sh[4], sw[4], 3, 2);
-  const int hs = 8 * b, spp = yx_buf(m, sh[5], sw[5], 4 * hs);
+  yx_conv(pl, p + "dark5.0", cat_p4, c1, c1, t, 0, 16 * b, sh[4], sw[4], 3, 2);
+  const int hs = 8 * b, spp = yx_buf(pl, sh[5], sw[5], 4 * hs);
   yx_base(m, p + "dark5.1.conv1", 16 * b, hs, 1);
-  yx_conv(m, p + "dark5.1.conv1", t, 0, 16 * b, spp, 0, hs, sh[5], sw[5], 1);
+  yx_conv(pl, p + "dark5.1.conv1", t, 0, 16 * b, spp, 0, hs, sh[5], sw[5], 1);
   YStep sp; sp.kind = YS_SPP; sp.dst = spp; sp.d_c = hs; sp.h = sh[5]; sp.wd = sw[5];
-  m->steps.push_back(sp);
-  const int t2 = yx_buf(m, sh[5], sw[5], 16 * b);
+  pl->steps.push_back(sp);
+  const int t2 = yx_buf(pl, sh[5], sw[5], 16 * b);
   yx_base(m, p + "dark5.1.conv2", 4 * hs, 16 * b, 1);
-  yx_conv(m, p + "dark5.1.conv2", spp, 0, 4 * hs, t2, 0, 16 * b, sh[5], sw[5], 1);
-  const int d5 = yx_buf(m, sh[5], sw[5], 16 * b);
-  yx_csp(m, p + "dark5.2", 16 * b, 16 * b, bd, false, t2, 0, d5, 0, sh[5], sw[5]);
+  yx_conv(pl, p + "dark5.1.conv2", spp, 0, 4 * hs, t2, 0, 16 * b, sh[5], sw[5], 1);
+  const int d5 = yx_buf(pl, sh[5], sw[5], 16 * b);
+  yx_csp(m, pl, p + "dark5.2", 16 * b, 16 * b, bd, false, t2, 0, d5, 0, sh[5], sw[5]);
   // PAFPN (yolo_pafpn.py:82-115)
   const std::string q = "backbone.";
-  const int cat_n4 = yx_buf(m, sh[5], sw[5], 2 * c1), cat_n3 = yx_buf(m, sh[4], sw[4], 2 * c0);
+  const int cat_n4 = yx_buf(pl, sh[5], sw[5], 2 * c1), cat_n3 = yx_buf(pl, sh[4], sw[4], 2 * c0);
   yx_base(m, q + "lateral_conv0", c2, c1, 1);
-  yx_conv(m, q + "lateral_conv0", d5, 0, c2, cat_n4, c1, c1, sh[5], sw[5], 1);              // fpn_out0 -> cat_n4[c1:]
+  yx_conv(pl, q + "lateral_conv0", d5, 0, c2, cat_n4, c1, c1, sh[5], sw[5], 1);              // fpn_out0 -> cat_n4[c1:]
   YStep u; u.kind = YS_UP; u.src = cat_n4; u.s_off = c1; u.d_c = c1; u.dst = cat_p4; u.d_off = 0; u.h = sh[5]; u.wd = sw[5];
-  m->steps.push_back(u);
-  const int f_out0 = yx_buf(m, sh[4], sw[4], c1);
-  yx_csp(m, q + "C3_p4", 2 * c1, c1, nf, false, cat_p4, 0, f_out0, 0, sh[4], sw[4]);
+  pl->steps.push_back(u);
+  const int f_out0 = yx_buf(pl, sh[4], sw[4], c1);
+  yx_csp(m, pl, q + "C3_p4", 2 * c1, c1, nf, false, cat_p4, 0, f_out0, 0, sh[4], sw[4]);
   yx_base(m, q + "reduce_conv1", c1, c0, 1);
-  yx_conv(m, q + "reduce_conv1", f_out0, 0, c1, cat_n3, c0, c0, sh[4], sw[4], 1);           // fpn_out1 -> cat_n3[c0:]
+  yx_conv(pl, q + "reduce_conv1", f_out0, 0, c1, cat_n3, c0, c0, sh[4], sw[4], 1);           // fpn_out1 -> cat_n3[c0:]
   u.src = cat_n3; u.s_off = c0; u.d_c = c0; u.dst = cat_p3; u.h = sh[4]; u.wd = sw[4];
-  m->steps.push_back(u);
-  const int pan2 = yx_buf(m, sh[3], sw[3], c0);
-  yx_csp(m, q + "C3_p3", 2 * c0, c0, nf, false, cat_p3, 0, pan2, 0, sh[3], sw[3]);
+  pl->steps.push_back(u);
+  const int pan2 = yx_buf(pl, sh[3], sw[3], c0);
+  yx_csp(m, pl, q + "C3_p3", 2 * c0, c0, nf, false, cat_p3, 0, pan2, 0, sh[3], sw[3]);
   yx_base(m, q + "bu_conv2", c0, c0, 3);
-  yx_conv(m, q + "bu_conv2", pan2, 0, c0, cat_n3, 0, c0, sh[3], sw[3], 3, 2);
-  const int pan1 = yx_buf(m, sh[4], sw[4], c1);
-  yx_csp(m, q + "C3_n3", 2 * c0, c1, nf, false, cat_n3, 0, pan1, 0, sh[4], sw[4]);
+  yx_conv(pl, q + "bu_conv2", pan2, 0, c0, cat_n3, 0, c0, sh[3], sw[3], 3, 2);
+  const int pan1 = yx_buf(pl, sh[4], sw[4], c1);
+  yx_csp(m, pl, q + "C3_n3", 2 * c0, c1, nf, false, cat_n3, 0, pan1, 0, sh[4], sw[4]);
   yx_base(m, q + "bu_conv1", c1, c1, 3);
-  yx_conv(m, q + "bu_conv1", pan1, 0, c1, cat_n4, 0, c1, sh[4], sw[4], 3, 2);
-  const int pan0 = yx_buf(m, sh[5], sw[5], c2);
-  yx_csp(m, q + "C3_n4", 2 * c1, c2, nf, false, cat_n4, 0, pan0, 0, sh[5], sw[5]);
+  yx_conv(pl, q + "bu_conv1", pan1, 0, c1, cat_n4, 0, c1, sh[4], sw[4], 3, 2);
+  const int pan0 = yx_buf(pl, sh[5], sw[5], c2);
+  yx_csp(m, pl, q + "C3_n4", 2 * c1, c2, nf, false, cat_n4, 0, pan0, 0, sh[5], sw[5]);
   // head (yolo_head.py:191-254): cls_convs[k][0] and reg_convs[k][0] as one conv with doubled N; reg + obj as one conv
   const int feats[3] = {pan2, pan1, pan0}, fch[3] = {c0, c1, c2}, strides[3] = {8, 16, 32};
   int a_off = 0;
   for (int k = 0; k < 3; ++k) {
     const int lv = k + 3, h = sh[lv], w = sw[lv];
     const std::string hk = "head.", ks = std::to_string(k);
-    const int stem = yx_buf(m, h, w, ch), both = yx_buf(m, h, w, 2 * ch), cf = yx_buf(m, h, w, ch), rf = yx_buf(m, h, w, ch);
-    const int raw = yx_buf(m, h, w, 5 + m->nc);
+    const int stem = yx_buf(pl, h, w, ch), both = yx_buf(pl, h, w, 2 * ch), cf = yx_buf(pl, h, w, ch), rf = yx_buf(pl, h, w, ch);
+    const int raw = yx_buf(pl, h, w, 5 + m->nc);
     yx_base(m, hk + "stems." + ks, fch[k], ch, 1);
-    yx_conv(m, hk + "stems." + ks, feats[k], 0, fch[k], stem, 0, ch, h, w, 1);
+    yx_conv(pl, hk + "stems." + ks, feats[k], 0, fch[k], stem, 0, ch, h, w, 1);
     yx_conv_decl(m, hk + "conv0." + ks, ch, 2 * ch, 3, {hk + "cls_convs." + ks + ".0", hk + "reg_convs." + ks + ".0"});
-    yx_conv(m, hk + "conv0." + ks, stem, 0, ch, both, 0, 2 * ch, h, w, 3);
+    yx_conv(pl, hk + "conv0." + ks, stem, 0, ch, both, 0, 2 * ch, h, w, 3);
     yx_base(m, hk + "cls_convs." + ks + ".1", ch, ch, 3);
     yx_base(m, hk + "reg_convs." + ks + ".1", ch, ch, 3);
-    yx_conv(m, hk + "cls_convs." + ks + ".1", both, 0, ch, cf, 0, ch, h, w, 3);
-    yx_conv(m, hk + "reg_convs." + ks + ".1", both, ch, ch, rf, 0, ch, h, w, 3);
+    yx_conv(pl, hk + "cls_convs." + ks + ".1", both, 0, ch, cf, 0, ch, h, w, 3);
+    yx_conv(pl, hk + "reg_convs." + ks + ".1", both, ch, ch, rf, 0, ch, h, w, 3);
     yx_conv_decl(m, hk + "regobj." + ks, ch, 5, 1, {hk + "reg_preds." + ks, hk + "obj_preds." + ks});
     yx_conv_decl(m, hk + "cls." + ks, ch, m->nc, 1, {hk + "cls_preds." + ks});
-    yx_conv(m, hk + "regobj." + ks, rf, 0, ch, raw, 0, 5, h, w, 1, 1, -1, 0, 0);
-    yx_conv(m, hk + "cls." + ks, cf, 0, ch, raw, 5, m->nc, h, w, 1, 1, -1, 0, 0);
+    yx_conv(pl, hk + "regobj." + ks, rf, 0, ch, raw, 0, 5, h, w, 1, 1, -1, 0, 0);
+    yx_conv(pl, hk + "cls." + ks, cf, 0, ch, raw, 5, m->nc, h, w, 1, 1, -1, 0, 0);
     YStep hd; hd.kind = YS_HEAD; hd.src = raw; hd.h = h; hd.wd = w; hd.extra = strides[k]; hd.d_off = a_off;
-    m->steps.push_back(hd);
+    pl->steps.push_back(hd);
     a_off += h * w;
   }
-  m->A = a_off;
-  m->offs.resize(m->bufs.size());
+  pl->A = a_off;
+  pl->offs.resize(pl->bufs.size());
 }
 
 // folded float64 weights [cout][cin][k][k] and bias of one source: a BaseConv prefix (conv + bn or fused conv + bias) or a
@@ -644,9 +725,9 @@ int yx_pack(YoloxModel* m, const std::string& name, YConv& c, bool& ok) {
   return GDRN_OK;
 }
 
-int yx_launch_conv(const YoloxModel* m, const YStep& s, const YConv& c, float* const* bp, int B, cudaStream_t st) {
+int yx_launch_conv(const YoloxModel* m, const YPlan& pl, const YStep& s, const YConv& c, float* const* bp, int B, cudaStream_t st) {
   ConvArgs p;
-  p.x = bp[s.src]; p.ldx = m->bufs[s.src].ld; p.cx_off = s.s_off; p.Cin = s.s_c; p.H = s.h; p.W = s.wd;
+  p.x = bp[s.src]; p.ldx = pl.bufs[s.src].ld; p.cx_off = s.s_off; p.Cin = s.s_c; p.H = s.h; p.W = s.wd;
   p.w_hi = c.hi; p.w_lo = m->split ? c.lo : nullptr;
   p.K = c.k * c.k * c.cin;
   p.bias = c.bias; p.Cout = c.cout;
@@ -654,8 +735,8 @@ int yx_launch_conv(const YoloxModel* m, const YStep& s, const YConv& c, float* c
   p.OH = (s.h + 2 * p.pad - c.k) / s.stride + 1;
   p.OW = (s.wd + 2 * p.pad - c.k) / s.stride + 1;
   p.M = (long long)B * p.OH * p.OW;
-  p.out = bp[s.dst]; p.ldo = m->bufs[s.dst].ld; p.co_off = s.d_off;
-  p.resid = s.res >= 0 ? bp[s.res] : nullptr; p.ldr = s.res >= 0 ? m->bufs[s.res].ld : 0; p.cr_off = s.r_off;
+  p.out = bp[s.dst]; p.ldo = pl.bufs[s.dst].ld; p.co_off = s.d_off;
+  p.resid = s.res >= 0 ? bp[s.res] : nullptr; p.ldr = s.res >= 0 ? pl.bufs[s.res].ld : 0; p.cr_off = s.r_off;
   p.act = s.act;
   const dim3 grid((unsigned)((p.M + CV_BM - 1) / CV_BM), (unsigned)((c.cout + CV_BN - 1) / CV_BN));
   if (m->split) GDRN_CHECK_CUDA(gdrn_launch_dep(yolox_conv_kernel<true>, grid, dim3(CV_THREADS), 0, st, p));
@@ -663,13 +744,73 @@ int yx_launch_conv(const YoloxModel* m, const YStep& s, const YConv& c, float* c
   return GDRN_OK;
 }
 
-size_t yx_layout(YoloxModel* m, int nb) {
+size_t yx_layout(YPlan& pl, int nb) {
   size_t off = 0;
-  for (size_t i = 0; i < m->bufs.size(); ++i) {
-    m->offs[i] = off;
-    off += yx_align((size_t)m->bufs[i].pix * nb * m->bufs[i].ld * 4);
+  for (size_t i = 0; i < pl.bufs.size(); ++i) {
+    pl.offs[i] = off;
+    off += yx_align((size_t)pl.bufs[i].pix * nb * pl.bufs[i].ld * 4);
   }
   return off;
+}
+
+// workspace of a forward of B images over the given plans: the largest plan at the first chunk's size
+size_t yx_workspace(YoloxModel* m, const std::vector<int>& plans, int B) {
+  size_t need = 0;
+  for (int k : plans) need = std::max(need, yx_layout(m->plans[k], std::min(B, m->max_batch)));
+  return need + 256;
+}
+
+bool yx_ready(const YoloxModel* m) {
+  for (auto& kv : m->convs)
+    if (!kv.second.packed) return false;
+  return true;
+}
+
+// one plan over nb images of the original [nb,3,H,W] input x: det rows [a_base, a_base + pl.A) of [nb, A_row, 5 + nc]
+int yx_run_plan(YoloxModel* m, YPlan& pl, const float* x, int nb, float* det, int A_row, int a_base, uint8_t* base, cudaStream_t st,
+                int& launches) {
+  float* bp[512];
+  GDRN_REQUIRE(pl.bufs.size() <= 512, "yolox_model_forward: too many buffers");
+  yx_layout(pl, nb);
+  for (size_t i = 0; i < pl.bufs.size(); ++i) bp[i] = reinterpret_cast<float*>(base + pl.offs[i]);
+  const int C = 5 + m->nc;
+  for (const YStep& s : pl.steps) {
+    if (s.kind == YS_CONV) {
+      const int rc = yx_launch_conv(m, pl, s, m->convs.at(s.w), bp, nb, st);
+      if (rc != GDRN_OK) return rc;
+    } else if (s.kind == YS_FOCUS) {
+      const long long n = (long long)nb * (pl.H / 2) * (pl.W / 2);
+      if (pl.resample)
+        GDRN_CHECK_CUDA(gdrn_launch_dep(yolox_focus_resample_kernel, dim3(blocks_for(n, 256)), dim3(256), 0, st, x, nb, m->H, m->W,
+                                        pl.H, pl.W, pl.sh, pl.sw, (float)m->H / (float)pl.sh, (float)m->W / (float)pl.sw, bp[s.dst]));
+      else
+        GDRN_CHECK_CUDA(gdrn_launch_dep(yolox_focus_kernel, dim3(blocks_for(n, 256)), dim3(256), 0, st, x, nb, pl.H, pl.W, bp[s.dst]));
+    } else if (s.kind == YS_SPP) {
+      const long long n = (long long)nb * s.h * s.wd * s.d_c;
+      GDRN_CHECK_CUDA(gdrn_launch_dep(yolox_spp_kernel, dim3(blocks_for(n, 256)), dim3(256), 0, st, bp[s.dst], nb, s.h, s.wd,
+                                      pl.bufs[s.dst].ld, s.d_c));
+    } else if (s.kind == YS_UP) {
+      const long long n = (long long)nb * 4 * s.h * s.wd * s.d_c;
+      GDRN_CHECK_CUDA(gdrn_launch_dep(yolox_upsample2x_kernel, dim3(blocks_for(n, 256)), dim3(256), 0, st,
+                                      (const float*)bp[s.src], pl.bufs[s.src].ld, s.s_off, bp[s.dst], pl.bufs[s.dst].ld, s.d_off,
+                                      nb, s.h, s.wd, s.d_c));
+    } else {
+      const long long n = (long long)nb * s.h * s.wd * C;
+      GDRN_CHECK_CUDA(gdrn_launch_dep(yolox_head_out_kernel, dim3(blocks_for(n, 256)), dim3(256), 0, st, (const float*)bp[s.src],
+                                      nb, s.h, s.wd, m->nc, s.extra, A_row, a_base + s.d_off, pl.inv_scale, det));
+    }
+    ++launches;
+  }
+  return GDRN_OK;
+}
+
+// the plan of one scale: model_utils.scale_img sizes in double arithmetic from the create-time H x W
+int yx_scale_sizes(int H, int W, double s, int* ph, int* pw, int* sh, int* sw) {
+  *sh = (int)(H * s);
+  *sw = (int)(W * s);
+  *ph = (int)(std::ceil(H * s / 32) * 32);
+  *pw = (int)(std::ceil(W * s / 32) * 32);
+  return *sh >= 1 && *sw >= 1;
 }
 
 }  // namespace
@@ -687,7 +828,11 @@ extern "C" int yolox_model_create(YoloxModel** out, double depth, double width, 
                "yolox_model_create: the width must give channel counts that are multiples of 8 (every standard YOLOX width does)");
   YoloxModel* m = new YoloxModel();
   m->nc = num_classes; m->max_batch = max_batch; m->H = H; m->W = W; m->split = precision;
-  yx_build(m, depth, width);
+  m->depth = depth; m->width = width;
+  m->plans.resize(1);
+  YPlan& p0 = m->plans[0];
+  p0.H = p0.sh = H; p0.W = p0.sw = W;
+  yx_build(m, &p0);
   *out = m;
   return GDRN_OK;
 }
@@ -723,53 +868,89 @@ extern "C" int yolox_model_missing(YoloxModel* m) {
   return missing;
 }
 
-extern "C" int yolox_model_num_anchors(const YoloxModel* m) { return m ? m->A : 0; }
+extern "C" int yolox_model_num_anchors(const YoloxModel* m) { return m ? m->plans[0].A : 0; }
 
 extern "C" size_t yolox_model_workspace_bytes(YoloxModel* m, int B) {
   if (!m || B <= 0) return 0;
-  return yx_layout(m, std::min(B, m->max_batch)) + 256;
+  return yx_workspace(m, {0}, B);
 }
 
 extern "C" int yolox_model_forward(YoloxModel* m, const float* img, int B, float* det_preds, void* workspace, size_t workspace_bytes,
                                    void* stream) {
   GDRN_REQUIRE(m && img && det_preds && workspace && B > 0, "yolox_model_forward: bad arguments");
-  for (auto& kv : m->convs) GDRN_REQUIRE(kv.second.packed, "yolox_model_forward: weights missing (load every tensor, then yolox_model_missing)");
-  const int nb0 = std::min(B, m->max_batch);
-  GDRN_REQUIRE(workspace_bytes >= yx_layout(m, nb0) + 256, "yolox_model_forward: workspace too small");
+  GDRN_REQUIRE(yx_ready(m), "yolox_model_forward: weights missing (load every tensor, then yolox_model_missing)");
+  GDRN_REQUIRE(workspace_bytes >= yx_workspace(m, {0}, B), "yolox_model_forward: workspace too small");
   cudaStream_t st = (cudaStream_t)stream;
   uint8_t* base = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(workspace) + 255) & ~(uintptr_t)255);
-  float* bp[512];
-  GDRN_REQUIRE(m->bufs.size() <= 512, "yolox_model_forward: too many buffers");
+  YPlan& pl = m->plans[0];
   const int C = 5 + m->nc;
   int launches = 0;
   for (int i0 = 0; i0 < B; i0 += m->max_batch) {
     const int nb = std::min(m->max_batch, B - i0);
-    yx_layout(m, nb);
-    for (size_t i = 0; i < m->bufs.size(); ++i) bp[i] = reinterpret_cast<float*>(base + m->offs[i]);
+    const int rc = yx_run_plan(m, pl, img + (size_t)i0 * 3 * m->H * m->W, nb, det_preds + (size_t)i0 * pl.A * C, pl.A, 0, base, st,
+                               launches);
+    if (rc != GDRN_OK) return rc;
+  }
+  gdrn_count_launch(launches);
+  return GDRN_OK;
+}
+
+// Multi-scale test-time augmentation (YOLOX.forward(augment=True)).  Host only: plans are layer lists over the shared
+// packed weights, so nothing is allocated on the device and no weight is re-packed.  A scale of exactly 1.0 reuses plan 0.
+extern "C" int yolox_model_set_scales(YoloxModel* m, const double* scales, int n_scales) {
+  GDRN_REQUIRE(m && scales && n_scales > 0, "yolox_model_set_scales: bad arguments");
+  for (int i = 0; i < n_scales; ++i) {
+    int ph, pw, sh, sw;
+    GDRN_REQUIRE(std::isfinite(scales[i]) && scales[i] > 0 && yx_scale_sizes(m->H, m->W, scales[i], &ph, &pw, &sh, &sw),
+                 "yolox_model_set_scales: a scale gives an empty resampled image (int(H * s) or int(W * s) is 0)");
+  }
+  m->plans.resize(1);
+  m->tta_plan.clear();
+  m->A_tta = 0;
+  for (int i = 0; i < n_scales; ++i) {
+    const double s = scales[i];
+    if (s == 1.0) {
+      m->tta_plan.push_back(0);
+    } else {
+      YPlan pl;
+      yx_scale_sizes(m->H, m->W, s, &pl.H, &pl.W, &pl.sh, &pl.sw);
+      pl.resample = true;
+      pl.inv_scale = 1.0f / (float)s;
+      yx_build(m, &pl);
+      m->plans.push_back(std::move(pl));
+      m->tta_plan.push_back((int)m->plans.size() - 1);
+    }
+    m->A_tta += m->plans[m->tta_plan.back()].A;
+  }
+  return GDRN_OK;
+}
+
+extern "C" int yolox_model_num_anchors_tta(const YoloxModel* m) { return m ? m->A_tta : 0; }
+
+extern "C" size_t yolox_model_workspace_bytes_tta(YoloxModel* m, int B) {
+  if (!m || B <= 0 || m->tta_plan.empty()) return 0;
+  return yx_workspace(m, m->tta_plan, B);
+}
+
+extern "C" int yolox_model_forward_tta(YoloxModel* m, const float* img, int B, float* det_preds, void* workspace, size_t workspace_bytes,
+                                       void* stream) {
+  GDRN_REQUIRE(m && img && det_preds && workspace && B > 0, "yolox_model_forward_tta: bad arguments");
+  GDRN_REQUIRE(!m->tta_plan.empty(), "yolox_model_forward_tta: no scales (call yolox_model_set_scales first)");
+  GDRN_REQUIRE(yx_ready(m), "yolox_model_forward_tta: weights missing (load every tensor, then yolox_model_missing)");
+  GDRN_REQUIRE(workspace_bytes >= yx_workspace(m, m->tta_plan, B), "yolox_model_forward_tta: workspace too small");
+  cudaStream_t st = (cudaStream_t)stream;
+  uint8_t* base = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(workspace) + 255) & ~(uintptr_t)255);
+  const int C = 5 + m->nc;
+  int launches = 0;
+  for (int i0 = 0; i0 < B; i0 += m->max_batch) {
+    const int nb = std::min(m->max_batch, B - i0);
     const float* x = img + (size_t)i0 * 3 * m->H * m->W;
-    float* det = det_preds + (size_t)i0 * m->A * C;
-    for (const YStep& s : m->steps) {
-      if (s.kind == YS_CONV) {
-        const int rc = yx_launch_conv(m, s, m->convs.at(s.w), bp, nb, st);
-        if (rc != GDRN_OK) return rc;
-      } else if (s.kind == YS_FOCUS) {
-        const long long n = (long long)nb * (m->H / 2) * (m->W / 2);
-        GDRN_CHECK_CUDA(gdrn_launch_dep(yolox_focus_kernel, dim3(blocks_for(n, 256)), dim3(256), 0, st, x, nb, m->H, m->W, bp[s.dst]));
-      } else if (s.kind == YS_SPP) {
-        const long long n = (long long)nb * s.h * s.wd * s.d_c;
-        GDRN_CHECK_CUDA(gdrn_launch_dep(yolox_spp_kernel, dim3(blocks_for(n, 256)), dim3(256), 0, st, bp[s.dst], nb, s.h, s.wd,
-                                        m->bufs[s.dst].ld, s.d_c));
-      } else if (s.kind == YS_UP) {
-        const long long n = (long long)nb * 4 * s.h * s.wd * s.d_c;
-        GDRN_CHECK_CUDA(gdrn_launch_dep(yolox_upsample2x_kernel, dim3(blocks_for(n, 256)), dim3(256), 0, st,
-                                        (const float*)bp[s.src], m->bufs[s.src].ld, s.s_off, bp[s.dst], m->bufs[s.dst].ld, s.d_off,
-                                        nb, s.h, s.wd, s.d_c));
-      } else {
-        const long long n = (long long)nb * s.h * s.wd * C;
-        GDRN_CHECK_CUDA(gdrn_launch_dep(yolox_head_out_kernel, dim3(blocks_for(n, 256)), dim3(256), 0, st, (const float*)bp[s.src],
-                                        nb, s.h, s.wd, m->nc, s.extra, m->A, s.d_off, det));
-      }
-      ++launches;
+    float* det = det_preds + (size_t)i0 * m->A_tta * C;
+    int a_base = 0;
+    for (int k : m->tta_plan) {   // the scales in order, one after the other in the same workspace
+      const int rc = yx_run_plan(m, m->plans[k], x, nb, det, m->A_tta, a_base, base, st, launches);
+      if (rc != GDRN_OK) return rc;
+      a_base += m->plans[k].A;
     }
   }
   gdrn_count_launch(launches);

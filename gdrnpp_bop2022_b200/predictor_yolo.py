@@ -16,7 +16,7 @@ import numpy as np
 import torch
 
 from . import _lib
-from .yolox_model import YOLOX, load_yolox_config
+from .yolox_model import YOLOX, load_yolox_config, tta_scales
 
 
 def preproc(img, input_size):
@@ -57,12 +57,14 @@ def postprocess_single_instance(det_preds, num_classes, conf_thre, nms_thre):
 
 class YoloPredictor:
     def __init__(self, exp_name="yolox-x", config_file_path=None, ckpt_file_path=None, fuse=True, fp16=False, *,
-                 state_dict=None, precision=None, device="cuda", cfg=None, max_batch=1, use_cuda_graph=True):
+                 state_dict=None, precision=None, device="cuda", cfg=None, max_batch=1, use_cuda_graph=True, augment=False):
         """Reference arguments (predictor_yolo.py:29-34).  ``exp_name`` is accepted and unused: the config file names
         the model.  ``fuse`` is accepted: the BatchNorms are always folded.  ``fp16=True`` selects the bf16 mode (the
         nearest here to the reference's half regime); an explicit ``precision`` wins.  Keyword-only: ``state_dict``
-        instead of a checkpoint, ``cfg`` (the namespace load_yolox_config returns) instead of a config file."""
-        self.exp_name, self.fuse = exp_name, fuse
+        instead of a checkpoint, ``cfg`` (the namespace load_yolox_config returns) instead of a config file, and
+        ``augment=True`` to run the multi-scale test-time augmentation over ``cfg.scales`` (the reference predictor
+        never passes augment, hence the default)."""
+        self.exp_name, self.fuse, self.augment = exp_name, fuse, bool(augment)
         if cfg is None:
             if config_file_path is None:
                 raise ValueError("YoloPredictor needs config_file_path or cfg=")
@@ -80,16 +82,18 @@ class YoloPredictor:
         self.model.load_state_dict(state_dict)
         self.model.to(self.device)
         self.use_cuda_graph = bool(use_cuda_graph)
-        self._graph = None   # (replay, static input, static det_preds)
+        self._graph = None   # (replay, static input, static det_preds, scales)
 
     def _forward(self, img):
+        kw = {"augment": True, "cfg": self.cfg} if self.augment else {}
         if not self.use_cuda_graph:
-            return self.model(img)["det_preds"]
-        if self._graph is None or self._graph[1].shape != img.shape:
+            return self.model(img, **kw)["det_preds"]
+        scales = tta_scales(self.cfg) if self.augment else None
+        if self._graph is None or self._graph[1].shape != img.shape or self._graph[3] != scales:
             static = img.clone()
-            replay, out = self.model.capture_graph(static)
-            self._graph = (replay, static, out["det_preds"])
-        replay, static, det = self._graph
+            replay, out = self.model.capture_graph(static, **kw)
+            self._graph = (replay, static, out["det_preds"], scales)
+        replay, static, det, _ = self._graph
         static.copy_(img)
         replay()
         return det

@@ -13,10 +13,18 @@ those buffers: every producer writes its slice directly, so torch.cat costs noth
 level (cls_convs[k][0], reg_convs[k][0]) read the same stem output and run as one conv with doubled N; reg + obj
 predictions are one conv over reg_feat and the class predictions one over cls_feat, both into one raw buffer per level.
 A forward is 156 launches at YOLOX-X; ``capture_graph`` replays them as one CUDA graph.  No CPU fallback.
+
+``forward(x, augment=True, cfg=cfg)`` is the reference's multi-scale test-time augmentation (det/yolox/models/yolox.py:53-86,
+what ``test.augment = True`` / ``test.scales`` select): for each scale s of ``cfg.scales`` the input is resampled like
+model_utils.scale_img (bilinear to int(H*s) x int(W*s), padded with 0.447*255 to a multiple of 32), run through the
+network, its boxes divided by s, and the outputs concatenated along the anchor axis in scale order.  The same engine
+serves every scale: one layer plan per input size over one set of packed weights.  The resampling happens inside the
+Focus kernel of each scaled plan, so the scaled images are never stored.
 """
 import ast
 import ctypes
 import os
+from collections.abc import Mapping
 from types import SimpleNamespace
 
 import torch
@@ -154,6 +162,7 @@ class _Engine:
                                          1 if model.precision == "bf16x3" else 0), "yolox_model_create")
         self.handle = h
         self.A = L.yolox_model_num_anchors(h)
+        self.scales, self.A_tta = None, 0   # the test-time-augmentation scale set (yolox_model_set_scales)
         self.workspace = None
         st = _lib.current_stream()
         for k, v in model.state_dict().items():
@@ -165,12 +174,25 @@ class _Engine:
         if missing != 0:
             raise _lib.GdrnError(f"yolox_model_missing: {missing} convs lack a tensor ({_lib.last_error()})")
 
-    def new_workspace(self, B):
-        return torch.empty(_lib.lib().yolox_model_workspace_bytes(self.handle, B), dtype=torch.uint8, device=self.device)
+    def set_scales(self, scales):
+        """Lay out one plan per scale (host only); a no-op when the set is unchanged."""
+        if scales != self.scales:
+            L = _lib.lib()
+            _lib.check(L.yolox_model_set_scales(self.handle, (ctypes.c_double * len(scales))(*scales), len(scales)),
+                       "yolox_model_set_scales")
+            self.scales, self.A_tta = scales, L.yolox_model_num_anchors_tta(self.handle)
 
-    def run(self, x, det, ws):
-        _lib.check(_lib.lib().yolox_model_forward(self.handle, _lib.ptr(x), x.shape[0], _lib.ptr(det), _lib.ptr(ws), ws.numel(),
-                                                  _lib.current_stream()), "yolox_model_forward")
+    def workspace_bytes(self, B, tta=False):
+        L = _lib.lib()
+        return (L.yolox_model_workspace_bytes_tta if tta else L.yolox_model_workspace_bytes)(self.handle, B)
+
+    def new_workspace(self, B, tta=False):
+        return torch.empty(self.workspace_bytes(B, tta), dtype=torch.uint8, device=self.device)
+
+    def run(self, x, det, ws, tta=False):
+        fn, name = (_lib.lib().yolox_model_forward_tta, "yolox_model_forward_tta") if tta else (_lib.lib().yolox_model_forward,
+                                                                                              "yolox_model_forward")
+        _lib.check(fn(self.handle, _lib.ptr(x), x.shape[0], _lib.ptr(det), _lib.ptr(ws), ws.numel(), _lib.current_stream()), name)
 
     def __del__(self):
         try:
@@ -233,9 +255,13 @@ class YOLOX(nn.Module):
         return eng
 
     def forward(self, x, targets=None, augment=False, cfg=None, _workspace=None):
-        """x [B,3,H,W] float (BGR, 0..255), H and W multiples of 32, on CUDA -> {"det_preds": [B, A, 5 + nc]}."""
-        if augment:
-            raise NotImplementedError("multi-scale test-time augmentation (test.augment) is not implemented")
+        """x [B,3,H,W] float (BGR, 0..255), H and W multiples of 32, on CUDA -> {"det_preds": [B, A, 5 + nc]}.
+        ``augment=True`` runs the multi-scale test-time augmentation over ``cfg.scales`` (an attribute or a mapping key,
+        as the reference's OmegaConf test config carries it) -> {"det_preds": [B, A_tta, 5 + nc]}, the scales' anchors
+        in scale order.  Without scales there is nothing to run: the reference defines no default set."""
+        scales = tta_scales(cfg) if augment else None
+        if augment and scales is None:
+            raise NotImplementedError("augment=True needs cfg.scales (the reference's test.scales); there is no default")
         if self.training:
             raise NotImplementedError("YOLOX here is inference only (no training losses)")
         if not torch.is_tensor(x) or not x.is_cuda:
@@ -248,41 +274,58 @@ class YOLOX(nn.Module):
         x = x.detach().to(torch.float32).contiguous()
         with torch.cuda.device(x.device):
             eng = self._engine(x.device, H, W)
-            det = torch.empty((B, eng.A, 5 + self.num_classes), dtype=torch.float32, device=x.device)
+            tta = scales is not None
+            if tta:
+                eng.set_scales(scales)
+            det = torch.empty((B, eng.A_tta if tta else eng.A, 5 + self.num_classes), dtype=torch.float32, device=x.device)
             ws = _workspace if _workspace is not None else eng.workspace
-            need = _lib.lib().yolox_model_workspace_bytes(eng.handle, B)
-            if ws is None or ws.numel() < need:
-                ws = eng.workspace = eng.new_workspace(B)
-            eng.run(x, det, ws)   # batches above max_batch run in chunks inside the engine
+            if ws is None or ws.numel() < eng.workspace_bytes(B, tta):
+                ws = eng.workspace = eng.new_workspace(B, tta)
+            eng.run(x, det, ws, tta)   # batches above max_batch run in chunks inside the engine
         return {"det_preds": det}
 
-    def capture_graph(self, x, warmup=2):
+    def capture_graph(self, x, warmup=2, augment=False, cfg=None):
         """Capture one forward over the static input ``x`` into a CUDA graph -> ``(replay, out_dict)``: ``replay()``
-        re-runs the forward as one graph launch on the current stream; refill ``x`` in place between replays."""
+        re-runs the forward as one graph launch on the current stream; refill ``x`` in place between replays.
+        ``augment`` / ``cfg`` as in ``forward``: the multi-scale forward replays as one graph too."""
         if not (torch.is_tensor(x) and x.is_cuda and x.is_contiguous() and x.dtype == torch.float32):
             raise _lib.GdrnError("capture_graph: x must be a contiguous float32 CUDA tensor")
         if x.shape[0] > self.max_batch:
             raise _lib.GdrnError(f"capture_graph: batch {x.shape[0]} above max_batch={self.max_batch}")
         with torch.cuda.device(x.device):
-            self.forward(x)   # builds the engine and loads the weights outside the capture
+            self.forward(x, augment=augment, cfg=cfg)   # builds the engine and its plans outside the capture
             # the graph bakes the workspace pointer in: it gets a workspace of its own, kept alive by replay()
-            ws = self._engines[(x.shape[2], x.shape[3])].new_workspace(x.shape[0])
+            ws = self._engines[(x.shape[2], x.shape[3])].new_workspace(x.shape[0], tta=bool(augment))
             side = torch.cuda.Stream(device=x.device)
             side.wait_stream(torch.cuda.current_stream())
             with torch.cuda.stream(side):
                 for _ in range(warmup):
-                    self.forward(x, _workspace=ws)
+                    self.forward(x, augment=augment, cfg=cfg, _workspace=ws)
             torch.cuda.current_stream().wait_stream(side)
             torch.cuda.synchronize()
             graph = torch.cuda.CUDAGraph()
             with torch.cuda.graph(graph):
-                out = self.forward(x, _workspace=ws)
+                out = self.forward(x, augment=augment, cfg=cfg, _workspace=ws)
         self._graph_pinned = True
 
         def replay(_graph=graph, _ws=ws):
             _graph.replay()
 
         return replay, out
+
+
+def tta_scales(cfg):
+    """The test-time-augmentation scales of a test config (``cfg.scales`` or ``cfg["scales"]``) as a tuple of Python
+    floats, or None when there are none."""
+    if cfg is None:
+        return None
+    scales = cfg.get("scales") if isinstance(cfg, Mapping) else getattr(cfg, "scales", None)
+    if scales is None:
+        return None
+    scales = tuple(float(s) for s in scales)
+    if not scales:
+        raise ValueError("cfg.scales is empty")
+    return scales
 
 
 # ---------------------------------------------------------------------------------------------------------------------
@@ -293,6 +336,7 @@ _MODEL_DEFAULTS = {"backbone.depth": 1.0, "backbone.width": 1.0, "backbone.in_ch
                    "head.width": "${..backbone.width}", "head.in_channels": "${..backbone.in_channels}",
                    "head.depthwise": False, "head.act": "silu", "head.strides": [8, 16, 32]}
 _TEST_KEYS = ("test_size", "conf_thr", "nms_thr")
+_TEST_OPTIONAL = {"augment": False, "scales": None}   # test-time augmentation, off unless the config sets it
 
 
 def _literal(node, path):
@@ -350,7 +394,7 @@ def _read_config(path, seen):
             if isinstance(val, ast.Call) and _dotted(val.func) == "dict":
                 test = {}
                 for kw in val.keywords:
-                    if kw.arg in _TEST_KEYS:
+                    if kw.arg in _TEST_KEYS or kw.arg in _TEST_OPTIONAL:
                         test[kw.arg] = _literal(kw.value, f"{path}: test.{kw.arg}")
             # test = OmegaConf.create(test) and similar wrappers keep the values
         elif tgt.startswith(("model.", "test.")):
@@ -365,7 +409,7 @@ def _set(model, test, tgt, val, path):
             _read_lazy_call(val, key + ".", model, path)
         else:
             model[key] = _literal(val, f"{path}: {tgt}")
-    elif tgt.startswith("test.") and tgt[len("test."):] in _TEST_KEYS:
+    elif tgt.startswith("test.") and (tgt[len("test."):] in _TEST_KEYS or tgt[len("test."):] in _TEST_OPTIONAL):
         test[tgt[len("test."):]] = _literal(val, f"{path}: {tgt}")
 
 
@@ -382,10 +426,11 @@ def _read_lazy_call(node, prefix, out, path):
 
 def load_yolox_config(path):
     """Read a reference YOLOX LazyConfig (configs/yolox/**.py) without executing it: the literal assignments to
-    model.backbone.depth / width, model.head.num_classes and test.test_size / conf_thr / nms_thr, following the
+    model.backbone.depth / width, model.head.num_classes and test.test_size / conf_thr / nms_thr / augment / scales, following the
     ``from .yolox_base import ...`` chain.  A model setting the engine cannot honour (depthwise convs, an activation
     other than silu, other strides or channel lists, a head width other than the backbone's) raises ValueError.
-    -> SimpleNamespace(depth, width, num_classes, test_size (h, w), conf_thr, nms_thr)."""
+    -> SimpleNamespace(depth, width, num_classes, test_size (h, w), conf_thr, nms_thr, augment (default False),
+    scales (a tuple, default None)).  The namespace is also the ``cfg`` of ``YOLOX.forward(augment=True, cfg=cfg)``."""
     model, test = _read_config(path, frozenset())
     cfg = dict(_MODEL_DEFAULTS)
     for k, v in model.items():
@@ -414,4 +459,6 @@ def load_yolox_config(path):
         raise ValueError(f"{path}: test.{', test.'.join(missing)} not found")
     return SimpleNamespace(depth=float(cfg["backbone.depth"]), width=float(cfg["backbone.width"]),
                            num_classes=int(cfg["head.num_classes"]), test_size=tuple(int(v) for v in test["test_size"]),
-                           conf_thr=float(test["conf_thr"]), nms_thr=float(test["nms_thr"]))
+                           conf_thr=float(test["conf_thr"]), nms_thr=float(test["nms_thr"]),
+                           augment=bool(test.get("augment", _TEST_OPTIONAL["augment"])),
+                           scales=None if test.get("scales") is None else tuple(test["scales"]))

@@ -351,6 +351,16 @@ int yolox_postprocess(const float* preds, int B, int A, int num_classes, const i
  *   yolox_model_workspace_bytes(B): caller-owned activation workspace for a forward of B images (chunks of max_batch).
  *   yolox_model_forward: img [B,3,H,W] f32 (BGR, 0..255) -> det_preds [B, A, 5 + num_classes] f32 (decoded boxes
  *     cx, cy, w, h; sigmoid obj; sigmoid classes), A = yolox_model_num_anchors.  No allocation, no synchronisation.
+ *   yolox_model_set_scales: multi-scale test-time augmentation (YOLOX.forward(augment=True), model_utils.scale_img):
+ *     one layer plan per scale s over the same packed weights, for the create-time H x W resampled (bilinear,
+ *     align_corners=False) to (int)(H*s) x (int)(W*s) and padded with 0.447*255 to ceil(H*s/32)*32 x ceil(W*s/32)*32;
+ *     s == 1.0 is the plain plan.  Replaces the previous set.  Host only, no CUDA call; a scale with an empty resampled
+ *     image is an error.
+ *   yolox_model_num_anchors_tta: A_tta, the anchors summed over the scales.
+ *   yolox_model_workspace_bytes_tta(B): workspace of yolox_model_forward_tta (the largest plan's).
+ *   yolox_model_forward_tta: img [B,3,H,W] -> det_preds [B, A_tta, 5 + num_classes], the scales' outputs in scale order
+ *     along the anchor axis, boxes of scale s multiplied by 1.0f / (float)s (torch's det[..., :4] /= s on CUDA).  Scales
+ *     run one after the other per max_batch chunk in one workspace.  No allocation, no synchronisation.
  *   yolox_postprocess_single: keep-single-instance post-process of the reference predictor (predictor_yolo.py:84-140):
  *     per class the highest-scoring anchor with obj * cls_conf >= conf_thre, class-agnostic NMS, rows in ascending
  *     class order; dets [B, num_classes, 7], n_det [B] i32.  Classes without such an anchor are left out.
@@ -364,6 +374,11 @@ int yolox_model_num_anchors(const YoloxModel* m);
 size_t yolox_model_workspace_bytes(YoloxModel* m, int B);
 int yolox_model_forward(YoloxModel* m, const float* img, int B, float* det_preds, void* workspace, size_t workspace_bytes,
                         void* stream);
+int yolox_model_set_scales(YoloxModel* m, const double* scales, int n_scales);
+int yolox_model_num_anchors_tta(const YoloxModel* m);
+size_t yolox_model_workspace_bytes_tta(YoloxModel* m, int B);
+int yolox_model_forward_tta(YoloxModel* m, const float* img, int B, float* det_preds, void* workspace, size_t workspace_bytes,
+                            void* stream);
 size_t yolox_postprocess_single_workspace_bytes(int B, int A, int num_classes);
 int yolox_postprocess_single(const float* preds, int B, int A, int num_classes, float conf_thre, float nms_thre, float* dets,
                              int* n_det, void* workspace, size_t workspace_bytes, void* stream);
