@@ -45,6 +45,8 @@ _SIGNATURES = {
         [c_void_p] + [c_void_p] * 8 + [c_int] + [c_void_p] * 3 + [POINTER(GdrnMaps), c_void_p, c_size_t, c_void_p],
     ),
     "gdrn_model_debug_read": (c_int64, [c_void_p, c_char_p, c_int, c_void_p, c_void_p, c_void_p]),
+    "gdrn_model_run_stage": (c_int, [c_void_p, c_char_p, c_int] + [c_void_p] * 7 + [POINTER(GdrnMaps), c_void_p, c_size_t,
+                                                                                  c_void_p]),
     "gdrn_gemm_bf16": (c_int, [c_void_p] * 6 + [c_int] * 6 + [c_void_p]),
     "gdrn_mlp_fused_x3": (c_int, [c_void_p] * 7 + [ctypes.c_longlong, c_int, c_void_p]),
     "gdrn_dwconv_ln": (c_int, [c_void_p] * 6 + [c_int] * 4 + [c_float, c_int, c_int, c_void_p]),

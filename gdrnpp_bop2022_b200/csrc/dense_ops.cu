@@ -590,6 +590,16 @@ __global__ void bf16_to_f32_kernel(const __nv_bfloat16* __restrict__ src, float*
     dst[i] = __bfloat162float(src[i]);
 }
 
+// split bf16 [rows, 2C] = [hi C | lo C] -> fp32 [rows, C] = hi + lo
+__global__ void split_to_f32_kernel(const __nv_bfloat16* __restrict__ src, float* __restrict__ dst, long long rows, int C) {
+  ptx::griddep_launch();
+  ptx::griddep_wait();
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < rows * C; i += (long long)gridDim.x * blockDim.x) {
+    const long long r = i / C, c = i % C;
+    dst[i] = __bfloat162float(src[r * 2 * C + c]) + __bfloat162float(src[r * 2 * C + C + c]);
+  }
+}
+
 // ------------------------------------------------------------------------------------------------
 // GroupNorm apply + exact-erf GELU (+ bilinear x2, align_corners=True).  One thread per (output pixel, 8 channels).
 // per-(image, group) mean / rstd from the double sums accumulated by the conv epilogue
@@ -1117,6 +1127,15 @@ int launch_bf16_to_f32(const __nv_bfloat16* src, float* dst, long long n, cudaSt
   long long blocks = (n + 255) / 256;
   if (blocks > 8192) blocks = 8192;
   GDRN_CHECK_CUDA(gdrn_launch_dep(bf16_to_f32_kernel, dim3((int)blocks), dim3(256), 0, st, src, dst, n));
+  GDRN_CHECK_CUDA(cudaGetLastError());
+  gdrn_count_launch(1);
+  return GDRN_OK;
+}
+
+int launch_split_to_f32(const __nv_bfloat16* src, float* dst, long long rows, int C, cudaStream_t st) {
+  long long blocks = (rows * C + 255) / 256;
+  if (blocks > 8192) blocks = 8192;
+  GDRN_CHECK_CUDA(gdrn_launch_dep(split_to_f32_kernel, dim3((int)blocks), dim3(256), 0, st, src, dst, rows, C));
   GDRN_CHECK_CUDA(cudaGetLastError());
   gdrn_count_launch(1);
   return GDRN_OK;

@@ -60,3 +60,5 @@ int launch_pose_lift(const float* raw, int ld, const float* cams, const float* c
 
 // debug: bf16 -> fp32 copy
 int launch_bf16_to_f32(const __nv_bfloat16* src, float* dst, long long n, cudaStream_t st);
+// debug: split bf16 [rows, 2C] ([hi C | lo C]) -> fp32 [rows, C] = hi + lo
+int launch_split_to_f32(const __nv_bfloat16* src, float* dst, long long rows, int C, cudaStream_t st);

@@ -435,6 +435,172 @@ void prof_end(GdrnModel* m, cudaStream_t st) {
   m->prof_used += 2;
 }
 
+// tile width: the largest one the N dimension divides into (the CTA-pair kernels need N % block_n == 0) that still yields
+// at least half a wave of CTAs; small batches (the per-image case: 5 ROIs, BASELINE configs[4]) otherwise run their long-K
+// GEMMs on a dozen SMs (stage-2 fc2 at B = 5: 20 CTAs of 96 k-iterations, 51 us -> 80 CTAs at width 64)
+int pick_bn(int N, long long M) {
+  const int half_wave = gdrn_num_sms() / 2;
+  const long long m_tiles = (M + 127) / 128;
+  int bn = N % 256 == 0 ? 256 : (N % 128 == 0 ? 128 : 64);
+  while (bn > 64 && m_tiles * (N / bn) < half_wave) bn >>= 1;
+  return bn;
+}
+
+void reset_plan(GemmPlan& p) { memset(&p, 0, sizeof(p)); }
+
+// GroupNorm sums of head layer i (0: deconv, 1..6: head convs, 7..9: Patch-PnP convs)
+double* stat_slot(const Workspace& w, int B, int i) { return w.gn_stats + (size_t)i * B * 32 * 2; }
+
+// ---------------- geometry head and Patch-PnP, one function per stage ----------------
+// gdrn_model_forward runs them in this order; gdrn_model_run_stage runs one of them on its own.
+
+// deconv 3x3 s2 (8x8 -> 16x16) as four parity GEMMs into w.R + GN + GELU into `out` [B,16,16,256]
+int stage_deconv(GdrnModel* m, const Workspace& w, int B, const __nv_bfloat16* feat, __nv_bfloat16* out, cudaStream_t st) {
+  const int PR = m->precise, S = PR ? 2 : 1;
+  const int C3 = m->arch.cp[3];
+  GemmPlan p;
+  for (int py = 0; py < 2; ++py)
+    for (int px = 0; px < 2; ++px) {
+      reset_plan(p);
+      RC(plan_a4d(p, feat, B, 8, 8, C3, S));
+      int nt = 0;
+      for (int jy = 0; jy < (py ? 2 : 1); ++jy)
+        for (int jx = 0; jx < (px ? 2 : 1); ++jx) {
+          // ky = py ? 2*jy : 1 -> iy = a + (ky == 0 ? 1 : 0)
+          const int dy = (py && jy == 0) ? 1 : 0, dx = (px && jx == 0) ? 1 : 0;
+          p.taps[nt] = {0, dx, dy, 0, nt * C3};
+          ++nt;
+        }
+      p.num_taps = nt;
+      // only B/2 row tiles (8x8 inputs): narrow N tiles so that the launch still covers the SMs
+      const int dbn = p.m_tiles >= 96 ? 256 : 64;
+      RC(plan_b(p, m->deconv_w[py * 2 + px], 256, (long long)nt * C3, dbn, 256, S));
+      if (PR) set_x3(p, C3, nt * C3);
+      p.epi = EPI_GNSTATS; p.out_f32 = PR; p.out = w.R; p.ldo = 256;
+      p.OH = 16; p.OW = 16; p.osy = 2; p.osx = 2; p.ooy = py; p.oox = px;
+      p.gn_stats = stat_slot(w, B, 0); p.gn_groups = 32; p.gn_cpg = 8;
+      RCP(0, gemm_tc_launch(p, dbn, st));
+    }
+  RCP(2, launch_gn_gelu(w.R, PR, stat_slot(w, B, 0), w.gn_mr, m->gn_w[0], m->gn_b[0], out, B, 16, 16, 256, 32, 1e-5f, PR, st));
+  return GDRN_OK;
+}
+
+// head conv li (0..5, at 16, 16, 32, 32, 64, 64 pixels): 3x3 conv into w.R + GN + GELU into `out`; after convs 1 and 3 the
+// GN + GELU result goes to `in` (the conv's input, dead by then) and the bilinear x2 of it to `out`
+int stage_head_conv(GdrnModel* m, const Workspace& w, int B, int li, __nv_bfloat16* in, __nv_bfloat16* out, cudaStream_t st) {
+  const int PR = m->precise, S = PR ? 2 : 1;
+  const int hres = 16 << (li / 2);
+  GemmPlan p;
+  reset_plan(p);
+  RC(plan_a4d(p, in, B, hres, hres, 256, S));
+  for (int t = 0; t < 9; ++t) p.taps[t] = {0, t % 3 - 1, t / 3 - 1, 0, t * 256};
+  p.num_taps = 9;
+  const int hbn = pick_bn(256, (long long)B * hres * hres);   // narrower tiles when a small batch leaves most SMs without one
+  RC(plan_b(p, m->hconv_w[li], 256, 9 * 256, hbn, 256, S));
+  if (PR) set_x3(p, 256, 9 * 256);
+  p.epi = EPI_GNSTATS; p.out_f32 = PR; p.out = w.R; p.ldo = 256;
+  p.OH = hres; p.OW = hres; p.osy = 1; p.osx = 1; p.ooy = 0; p.oox = 0;
+  p.gn_stats = stat_slot(w, B, li + 1); p.gn_groups = 32; p.gn_cpg = 8;
+  RCP(0, gemm_tc_launch(p, hbn, st));
+  if (li % 2 == 0 || li == 5) {
+    RCP(2, launch_gn_gelu(w.R, PR, stat_slot(w, B, li + 1), w.gn_mr, m->gn_w[li + 1], m->gn_b[li + 1], out, B, hres, hres, 256, 32,
+                          1e-5f, PR, st));
+  } else {
+    RCP(2, launch_gn_gelu(w.R, PR, stat_slot(w, B, li + 1), w.gn_mr, m->gn_w[li + 1], m->gn_b[li + 1], in, B, hres, hres, 256, 32,
+                          1e-5f, PR, st));
+    RCP(2, launch_upsample2x(in, out, B, hres, hres, 256, PR, st));
+  }
+  return GDRN_OK;
+}
+
+// out conv (class gathered) + Patch-PnP input assembly into w.pnp_in (+ the optional NCHW maps)
+int stage_out_conv(GdrnModel* m, const Workspace& w, int B, const __nv_bfloat16* in, const int64_t* roi_classes,
+                   const float* roi_extents, const float* roi_coord_2d, const GdrnMaps* maps, cudaStream_t st) {
+  const int PR = m->precise, S = PR ? 2 : 1;
+  GemmPlan p;
+  reset_plan(p);
+  RC(plan_a2d(p, in, (long long)B * 64 * 64, 256, S));
+  RC(plan_b(p, m->out_w, (long long)m->num_classes * 80, 256, 80, 80, S));
+  if (PR) set_x3(p, 256, 256);
+  p.n_tiles = 1;
+  p.b_rows_per_class = 80;
+  p.epi = EPI_OUTCONV;
+  p.roi_classes = reinterpret_cast<const long long*>(roi_classes);
+  p.num_classes = m->num_classes;
+  p.rows_per_roi = 4096;
+  p.oc_bias = m->out_b;
+  p.roi_extents = roi_extents;
+  p.roi_coord_2d = roi_coord_2d;
+  p.pnp_in = w.pnp_in;
+  if (maps && maps->mask) {
+    GDRN_REQUIRE(maps->full_mask && maps->coor_x && maps->coor_y && maps->coor_z && maps->region,
+                 "forward: GdrnMaps must be all set or all NULL");
+    p.map_mask = maps->mask; p.map_full = maps->full_mask; p.map_x = maps->coor_x; p.map_y = maps->coor_y;
+    p.map_z = maps->coor_z; p.map_region = maps->region;
+  }
+  RCP(0, gemm_tc_launch(p, 80, st));
+  return GDRN_OK;
+}
+
+// Patch-PnP conv i (0..2): 3x3 s2 conv of `in` [B,2r,2r,128] into w.pR + GN + GELU into w.pP [B,r,r,128] (split-bf16 mode,
+// i = 2: fp32 into w.pF, the input of the fp32 FC stack)
+int stage_pnp_conv(GdrnModel* m, const Workspace& w, int B, int i, const __nv_bfloat16* in, cudaStream_t st) {
+  const int PR = m->precise, S = PR ? 2 : 1;
+  const int ires = 64 >> i, ores = ires / 2;
+  GemmPlan p;
+  reset_plan(p);
+  RC(plan_a5d_s2(p, in, B, ires, ires, 128, S));
+  // input (2*o + k - 1): k=0 -> parity 1, half index o-1; k=1 -> parity 0, o; k=2 -> parity 1, o
+  for (int t = 0; t < 9; ++t) {
+    const int ky = t / 3, kx = t % 3;
+    const int pyy = (ky == 1) ? 0 : 1, dyy = (ky == 0) ? -1 : 0;
+    const int pxx = (kx == 1) ? 0 : 1, dxx = (kx == 0) ? -1 : 0;
+    p.taps[t] = {pxx * S * 128, dxx, pyy, dyy, t * 128};
+  }
+  p.num_taps = 9;
+  RC(plan_b(p, m->pconv_w[i], 128, 9 * 128, 128, 128, S));
+  if (PR) set_x3(p, 128, 9 * 128);
+  p.epi = EPI_GNSTATS; p.out_f32 = PR; p.out = w.pR; p.ldo = 128;
+  p.OH = ores; p.OW = ores; p.osy = 1; p.osx = 1;
+  p.gn_stats = stat_slot(w, B, 7 + i); p.gn_groups = 32; p.gn_cpg = 4;
+  RCP(0, gemm_tc_launch(p, 128, st));
+  if (PR && i == 2) {  // last feature map feeds the fp32 FC stack
+    RCP(2, launch_gn_gelu_f32(reinterpret_cast<const float*>(w.pR), stat_slot(w, B, 7 + i), w.gn_mr, m->pgn_w[i], m->pgn_b[i], w.pF, B,
+                              ores, ores, 128, 32, 1e-5f, st));
+  } else {
+    // the conv has read its input (pnp_in or pP) by now: GN + GELU may overwrite pP
+    RCP(2, launch_gn_gelu(w.pR, PR, stat_slot(w, B, 7 + i), w.gn_mr, m->pgn_w[i], m->pgn_b[i], w.pP, B, ores, ores, 128, 32, 1e-5f, PR, st));
+  }
+  return GDRN_OK;
+}
+
+// FC stack: Patch-PnP feature [B,8192] (w.pF fp32 in split-bf16 mode, w.pP bf16 otherwise) -> 1024 -> 256 -> 9 into w.fout [B,16]
+int stage_pnp_fc(GdrnModel* m, const Workspace& w, int B, cudaStream_t st) {
+  if (m->precise) {
+    RCP(2, launch_fc_f32(w.pF, m->pfc1_wf, m->pfc1_b, w.f1f, w.fc_part, B, 1024, 8192, 1024, 1, st));
+    RCP(2, launch_fc_f32(w.f1f, m->pfc2_wf, m->pfc2_b, w.f2f, w.fc_part, B, 256, 1024, 256, 1, st));
+    RCP(2, launch_fc_f32(w.f2f, m->pfcrt_wf, m->pfcrt_b, w.fout, w.fc_part, B, 16, 256, 16, 0, st));
+    return GDRN_OK;
+  }
+  GemmPlan p;
+  reset_plan(p);
+  RC(plan_a2d(p, w.pP, B, 8192));
+  RC(plan_b(p, m->pfc1_w, 1024, 8192, 64, 1024));
+  p.epi = EPI_GELU; p.gelu_mode = 0; p.out = w.f1; p.ldo = 1024; p.bias = m->pfc1_b;
+  RCP(0, gemm_tc_launch(p, 64, st));
+  reset_plan(p);
+  RC(plan_a2d(p, w.f1, B, 1024));
+  RC(plan_b(p, m->pfc2_w, 256, 1024, 64, 256));
+  p.epi = EPI_GELU; p.gelu_mode = 0; p.out = w.f2; p.ldo = 256; p.bias = m->pfc2_b;
+  RCP(0, gemm_tc_launch(p, 64, st));
+  reset_plan(p);
+  RC(plan_a2d(p, w.f2, B, 256));
+  RC(plan_b(p, m->pfcrt_w, 16, 256, 16, 16));
+  p.epi = EPI_STORE; p.out_f32 = 1; p.out = w.fout; p.ldo = 16; p.bias = m->pfcrt_b;
+  RCP(0, gemm_tc_launch(p, 16, st));
+  return GDRN_OK;
+}
+
 }  // namespace
 
 // ================================================================================================
@@ -563,16 +729,6 @@ extern "C" int gdrn_model_forward(GdrnModel* m, const float* roi_img, const int6
       return GDRN_ERR_INVALID;
     }
   }
-  // tile width: the largest one the N dimension divides into (the CTA-pair kernels need N % block_n == 0) that still yields
-  // at least half a wave of CTAs; small batches (the per-image case: 5 ROIs, BASELINE configs[4]) otherwise run their long-K
-  // GEMMs on a dozen SMs (stage-2 fc2 at B = 5: 20 CTAs of 96 k-iterations, 51 us -> 80 CTAs at width 64)
-  const int half_wave = gdrn_num_sms() / 2;
-  auto pick_bn = [half_wave](int N, long long M) {
-    const long long m_tiles = (M + 127) / 128;
-    int bn = N % 256 == 0 ? 256 : (N % 128 == 0 ? 128 : 64);
-    while (bn > 64 && m_tiles * (N / bn) < half_wave) bn >>= 1;
-    return bn;
-  };
   // ---------------- stages ----------------
   int res = 64;
   for (int s = 0; s < 4; ++s) {
@@ -626,141 +782,18 @@ extern "C" int gdrn_model_forward(GdrnModel* m, const float* roi_img, const int6
   else RCP(2, launch_cast_bf16(w.X, w.feat, (long long)B * 64 * C3, st));
 
   // ---------------- geometry head ----------------
-  double* stats = w.gn_stats;
-  auto stat_slot = [&](int i) { return stats + (size_t)i * B * 32 * 2; };
-  // deconv 3x3 s2 (8x8 -> 16x16) as four parity GEMMs
-  for (int py = 0; py < 2; ++py)
-    for (int px = 0; px < 2; ++px) {
-      reset();
-      RC(plan_a4d(p, w.feat, B, 8, 8, C3, S));
-      int nt = 0;
-      for (int jy = 0; jy < (py ? 2 : 1); ++jy)
-        for (int jx = 0; jx < (px ? 2 : 1); ++jx) {
-          // ky = py ? 2*jy : 1 -> iy = a + (ky == 0 ? 1 : 0)
-          const int dy = (py && jy == 0) ? 1 : 0, dx = (px && jx == 0) ? 1 : 0;
-          p.taps[nt] = {0, dx, dy, 0, nt * C3};
-          ++nt;
-        }
-      p.num_taps = nt;
-      // only B/2 row tiles (8x8 inputs): narrow N tiles so that the launch still covers the SMs
-      const int dbn = p.m_tiles >= 96 ? 256 : 64;
-      RC(plan_b(p, m->deconv_w[py * 2 + px], 256, (long long)nt * C3, dbn, 256, S));
-      if (PR) set_x3(p, C3, nt * C3);
-      p.epi = EPI_GNSTATS; p.out_f32 = PR; p.out = w.R; p.ldo = 256;
-      p.OH = 16; p.OW = 16; p.osy = 2; p.osx = 2; p.ooy = py; p.oox = px;
-      p.gn_stats = stat_slot(0); p.gn_groups = 32; p.gn_cpg = 8;
-      RCP(0, gemm_tc_launch(p, dbn, st));
-    }
-  RCP(2, launch_gn_gelu(w.R, PR, stat_slot(0), w.gn_mr, m->gn_w[0], m->gn_b[0], w.P, B, 16, 16, 256, 32, 1e-5f, PR, st));
+  RC(stage_deconv(m, w, B, w.feat, w.P, st));
   __nv_bfloat16* cur = w.P;
   __nv_bfloat16* nxt = w.Q;
-  int hres = 16;
-  for (int blk = 0; blk < 3; ++blk) {
-    for (int j = 0; j < 2; ++j) {
-      const int li = blk * 2 + j;  // conv index 0..5, gn index li+1
-      reset();
-      RC(plan_a4d(p, cur, B, hres, hres, 256, S));
-      for (int t = 0; t < 9; ++t) p.taps[t] = {0, t % 3 - 1, t / 3 - 1, 0, t * 256};
-      p.num_taps = 9;
-      const int hbn = pick_bn(256, (long long)B * hres * hres);   // narrower tiles when a small batch leaves most SMs without one
-      RC(plan_b(p, m->hconv_w[li], 256, 9 * 256, hbn, 256, S));
-      if (PR) set_x3(p, 256, 9 * 256);
-      p.epi = EPI_GNSTATS; p.out_f32 = PR; p.out = w.R; p.ldo = 256;
-      p.OH = hres; p.OW = hres; p.osy = 1; p.osx = 1; p.ooy = 0; p.oox = 0;
-      p.gn_stats = stat_slot(li + 1); p.gn_groups = 32; p.gn_cpg = 8;
-      RCP(0, gemm_tc_launch(p, hbn, st));
-      const int up = (j == 1 && blk < 2) ? 2 : 1;
-      if (up == 1) {
-        RCP(2, launch_gn_gelu(w.R, PR, stat_slot(li + 1), w.gn_mr, m->gn_w[li + 1], m->gn_b[li + 1], nxt, B, hres, hres, 256, 32,
-                              1e-5f, PR, st));
-      } else {
-        // GN + GELU at the low resolution into `cur` (the conv's input, dead now), then bilinear x2 into `nxt`
-        RCP(2, launch_gn_gelu(w.R, PR, stat_slot(li + 1), w.gn_mr, m->gn_w[li + 1], m->gn_b[li + 1], cur, B, hres, hres, 256, 32,
-                              1e-5f, PR, st));
-        RCP(2, launch_upsample2x(cur, nxt, B, hres, hres, 256, PR, st));
-      }
-      std::swap(cur, nxt);
-      hres *= up;
-    }
+  for (int li = 0; li < 6; ++li) {
+    RC(stage_head_conv(m, w, B, li, cur, nxt, st));
+    std::swap(cur, nxt);
   }
-  // out conv (class gathered) + Patch-PnP input assembly
-  reset();
-  RC(plan_a2d(p, cur, M0, 256, S));
-  RC(plan_b(p, m->out_w, (long long)m->num_classes * 80, 256, 80, 80, S));
-  if (PR) set_x3(p, 256, 256);
-  p.n_tiles = 1;
-  p.b_rows_per_class = 80;
-  p.epi = EPI_OUTCONV;
-  p.roi_classes = reinterpret_cast<const long long*>(roi_classes);
-  p.num_classes = m->num_classes;
-  p.rows_per_roi = 4096;
-  p.oc_bias = m->out_b;
-  p.roi_extents = roi_extents;
-  p.roi_coord_2d = roi_coord_2d;
-  p.pnp_in = w.pnp_in;
-  if (maps && maps->mask) {
-    GDRN_REQUIRE(maps->full_mask && maps->coor_x && maps->coor_y && maps->coor_z && maps->region,
-                 "forward: GdrnMaps must be all set or all NULL");
-    p.map_mask = maps->mask; p.map_full = maps->full_mask; p.map_x = maps->coor_x; p.map_y = maps->coor_y;
-    p.map_z = maps->coor_z; p.map_region = maps->region;
-  }
-  RCP(0, gemm_tc_launch(p, 80, st));
+  RC(stage_out_conv(m, w, B, cur, roi_classes, roi_extents, roi_coord_2d, maps, st));
 
   // ---------------- Patch-PnP ----------------
-  {
-    const __nv_bfloat16* in = w.pnp_in;
-    int ires = 64;
-    for (int i = 0; i < 3; ++i) {
-      const int ores = ires / 2;
-      reset();
-      RC(plan_a5d_s2(p, in, B, ires, ires, 128, S));
-      // input (2*o + k - 1): k=0 -> parity 1, half index o-1; k=1 -> parity 0, o; k=2 -> parity 1, o
-      for (int t = 0; t < 9; ++t) {
-        const int ky = t / 3, kx = t % 3;
-        const int pyy = (ky == 1) ? 0 : 1, dyy = (ky == 0) ? -1 : 0;
-        const int pxx = (kx == 1) ? 0 : 1, dxx = (kx == 0) ? -1 : 0;
-        p.taps[t] = {pxx * S * 128, dxx, pyy, dyy, t * 128};
-      }
-      p.num_taps = 9;
-      RC(plan_b(p, m->pconv_w[i], 128, 9 * 128, 128, 128, S));
-      if (PR) set_x3(p, 128, 9 * 128);
-      p.epi = EPI_GNSTATS; p.out_f32 = PR; p.out = w.pR; p.ldo = 128;
-      p.OH = ores; p.OW = ores; p.osy = 1; p.osx = 1;
-      p.gn_stats = stat_slot(7 + i); p.gn_groups = 32; p.gn_cpg = 4;
-      RCP(0, gemm_tc_launch(p, 128, st));
-      if (PR && i == 2) {  // last feature map feeds the fp32 FC stack
-        RCP(2, launch_gn_gelu_f32(reinterpret_cast<const float*>(w.pR), stat_slot(7 + i), w.gn_mr, m->pgn_w[i], m->pgn_b[i], w.pF, B,
-                                  ores, ores, 128, 32, 1e-5f, st));
-      } else {
-        RCP(2, launch_gn_gelu(w.pR, PR, stat_slot(7 + i), w.gn_mr, m->pgn_w[i], m->pgn_b[i], w.pP, B, ores, ores, 128, 32, 1e-5f, PR, st));
-      }
-      // ping-pong between pP and a second buffer is unnecessary: the conv reads pP (or pnp_in) and writes pR
-      in = w.pP;
-      ires = ores;
-    }
-    // FC stack: [B,8192] -> 1024 -> 256 -> 9
-    if (PR) {
-      RCP(2, launch_fc_f32(w.pF, m->pfc1_wf, m->pfc1_b, w.f1f, w.fc_part, B, 1024, 8192, 1024, 1, st));
-      RCP(2, launch_fc_f32(w.f1f, m->pfc2_wf, m->pfc2_b, w.f2f, w.fc_part, B, 256, 1024, 256, 1, st));
-      RCP(2, launch_fc_f32(w.f2f, m->pfcrt_wf, m->pfcrt_b, w.fout, w.fc_part, B, 16, 256, 16, 0, st));
-    } else {
-    reset();
-    RC(plan_a2d(p, w.pP, B, 8192));
-    RC(plan_b(p, m->pfc1_w, 1024, 8192, 64, 1024));
-    p.epi = EPI_GELU; p.gelu_mode = 0; p.out = w.f1; p.ldo = 1024; p.bias = m->pfc1_b;
-    RCP(0, gemm_tc_launch(p, 64, st));
-    reset();
-    RC(plan_a2d(p, w.f1, B, 1024));
-    RC(plan_b(p, m->pfc2_w, 256, 1024, 64, 256));
-    p.epi = EPI_GELU; p.gelu_mode = 0; p.out = w.f2; p.ldo = 256; p.bias = m->pfc2_b;
-    RCP(0, gemm_tc_launch(p, 64, st));
-    reset();
-    RC(plan_a2d(p, w.f2, B, 256));
-    RC(plan_b(p, m->pfcrt_w, 16, 256, 16, 16));
-    p.epi = EPI_STORE; p.out_f32 = 1; p.out = w.fout; p.ldo = 16; p.bias = m->pfcrt_b;
-    RCP(0, gemm_tc_launch(p, 16, st));
-    }
-  }
+  for (int i = 0; i < 3; ++i) RC(stage_pnp_conv(m, w, B, i, i == 0 ? w.pnp_in : w.pP, st));
+  RC(stage_pnp_fc(m, w, B, st));
   RCP(2, launch_pose_lift(w.fout, 16, roi_cams, roi_centers, roi_whs, resize_ratios, out_rot, out_trans, out_raw, B, st));
   return GDRN_OK;
 }
@@ -823,4 +856,89 @@ extern "C" int64_t gdrn_model_debug_read(GdrnModel* m, const char* name, int bat
     return GDRN_ERR_INVALID;
   }
   return n;
+}
+
+extern "C" int gdrn_model_run_stage(GdrnModel* m, const char* stage, int batch, const float* in, float* out, float* raw_out,
+                                    double* gn_stats_out, const int64_t* roi_classes, const float* roi_extents,
+                                    const float* roi_coord_2d, const GdrnMaps* maps, void* workspace, size_t workspace_bytes,
+                                    void* stream) {
+  GDRN_REQUIRE(m && stage && in && out && workspace, "run_stage: null argument");
+  if (m->missing != 0) {
+    gdrn_set_last_error(__FILE__, __LINE__, "run_stage: model weights not fully loaded");
+    return GDRN_ERR_STATE;
+  }
+  GDRN_REQUIRE(batch >= 1 && batch <= m->max_batch, "run_stage: batch out of range");
+  if (workspace_bytes < gdrn_model_workspace_bytes(m, batch)) {
+    gdrn_set_last_error(__FILE__, __LINE__, "run_stage: workspace too small");
+    return GDRN_ERR_STATE;
+  }
+  // stage index: "head_conv0".."head_conv5" / "pnp_conv0".."pnp_conv2"
+  auto indexed = [stage](const char* prefix, int n) {
+    const size_t l = strlen(prefix);
+    return (!strncmp(stage, prefix, l) && stage[l] >= '0' && stage[l] < '0' + n && stage[l + 1] == 0) ? stage[l] - '0' : -1;
+  };
+  const int li = indexed("head_conv", 6), pi = indexed("pnp_conv", 3);
+  const bool deconv = !strcmp(stage, "deconv"), out_conv = !strcmp(stage, "out_conv"), pnp_fc = !strcmp(stage, "pnp_fc");
+  GDRN_REQUIRE(deconv || li >= 0 || out_conv || pi >= 0 || pnp_fc, "run_stage: unknown stage");
+  GDRN_REQUIRE(!(out_conv || pnp_fc) || (!raw_out && !gn_stats_out), "run_stage: this stage has no conv output / GroupNorm sums");
+  if (out_conv) {
+    GDRN_REQUIRE(roi_extents && roi_coord_2d, "run_stage: out_conv needs roi_extents and roi_coord_2d");
+    GDRN_REQUIRE(roi_classes || m->num_classes == 1, "run_stage: roi_classes is NULL but the head is class-aware");
+  }
+  cudaStream_t st = (cudaStream_t)stream;
+  const int B = batch, PR = m->precise;
+  void* wbase = reinterpret_cast<void*>((reinterpret_cast<uintptr_t>(workspace) + 1023) & ~(uintptr_t)1023);
+  Workspace w = carve(m, B, wbase);
+  m->prof_used = 0;
+  m->prof_cat.clear();
+  GDRN_CHECK_CUDA(cudaMemsetAsync(w.gn_stats, 0, w.zero_bytes, st));
+  // fp32 -> the stage's operand format (bf16 or [hi | lo] split rows) and back
+  auto encode = [&](__nv_bfloat16* dst, long long rows, int C) {
+    return PR ? launch_cast_split(in, dst, rows, C, st) : launch_cast_bf16(in, dst, rows * C, st);
+  };
+  auto decode = [&](const __nv_bfloat16* src, long long rows, int C) {
+    return PR ? launch_split_to_f32(src, out, rows, C, st) : launch_bf16_to_f32(src, out, rows * C, st);
+  };
+  auto copy_f32 = [&](float* dst, const void* src, long long n) {
+    GDRN_CHECK_CUDA(cudaMemcpyAsync(dst, src, n * 4, cudaMemcpyDeviceToDevice, st));
+    return GDRN_OK;
+  };
+  const void* raw = nullptr;   // pre-GroupNorm conv output (fp32 in split-bf16 mode, bf16 otherwise) and its element count
+  long long raw_n = 0;
+  if (deconv) {
+    const int C3 = m->arch.cp[3];
+    RC(encode(w.feat, (long long)B * 64, C3));
+    RC(stage_deconv(m, w, B, w.feat, w.P, st));
+    RC(decode(w.P, (long long)B * 256, 256));
+    raw = w.R; raw_n = (long long)B * 256 * 256;
+  } else if (li >= 0) {
+    const int h = 16 << (li / 2), ho = (li == 1 || li == 3) ? 2 * h : h;
+    RC(encode(w.P, (long long)B * h * h, 256));
+    RC(stage_head_conv(m, w, B, li, w.P, w.Q, st));
+    RC(decode(w.Q, (long long)B * ho * ho, 256));
+    raw = w.R; raw_n = (long long)B * h * h * 256;
+  } else if (out_conv) {
+    RC(encode(w.P, (long long)B * 4096, 256));
+    RC(stage_out_conv(m, w, B, w.P, roi_classes, roi_extents, roi_coord_2d, maps, st));
+    RC(decode(w.pnp_in, (long long)B * 4096, 128));
+  } else if (pi >= 0) {
+    const int ires = 64 >> pi, ores = ires / 2;
+    __nv_bfloat16* src = pi == 0 ? w.pnp_in : w.pP;
+    RC(encode(src, (long long)B * ires * ires, 128));
+    RC(stage_pnp_conv(m, w, B, pi, src, st));
+    if (PR && pi == 2) RC(copy_f32(out, w.pF, (long long)B * ores * ores * 128));
+    else RC(decode(w.pP, (long long)B * ores * ores, 128));
+    raw = w.pR; raw_n = (long long)B * ores * ores * 128;
+  } else {
+    if (PR) RC(copy_f32(w.pF, in, (long long)B * 8192));
+    else RC(launch_cast_bf16(in, w.pP, (long long)B * 8192, st));
+    RC(stage_pnp_fc(m, w, B, st));
+    RC(copy_f32(out, w.fout, (long long)B * 16));
+  }
+  if (raw_out) {
+    if (PR) RC(copy_f32(raw_out, raw, raw_n));
+    else RC(launch_bf16_to_f32(reinterpret_cast<const __nv_bfloat16*>(raw), raw_out, raw_n, st));
+  }
+  if (gn_stats_out) GDRN_CHECK_CUDA(cudaMemcpyAsync(gn_stats_out, w.gn_stats, w.zero_bytes, cudaMemcpyDeviceToDevice, st));
+  return GDRN_OK;
 }

@@ -343,6 +343,52 @@ class GDRN_DoubleMask(nn.Module):
             raise _lib.GdrnError(f"debug_read({name}) failed: {_lib.last_error()}")
         return dst[:n]
 
+    def run_stage(self, stage, x, roi_classes=None, roi_extents=None, roi_coord_2d=None, want_raw=False, want_maps=False):
+        """One geometry-head / Patch-PnP stage of the forward on the fp32 NHWC CUDA tensor ``x`` (gdrn_model_run_stage in
+        include/gdrn_b200.h lists the stages and shapes).  Returns ``{"out"}`` plus, when ``want_raw``, ``"raw"`` (the conv
+        output before GroupNorm) and ``"gn_stats"`` (float64 [10,B,32,2]), and, when ``want_maps``, the six NCHW maps of
+        "out_conv"."""
+        dev = x.device
+        B = x.shape[0]
+        x = x.detach().to(dtype=torch.float32).contiguous()
+        if stage == "deconv":
+            out_shape, raw_shape = (B, 16, 16, 256), (B, 16, 16, 256)
+        elif stage.startswith("head_conv"):
+            li = int(stage[len("head_conv"):])
+            h = 16 << (li // 2)
+            ho = 2 * h if li in (1, 3) else h
+            out_shape, raw_shape = (B, ho, ho, 256), (B, h, h, 256)
+        elif stage == "out_conv":
+            out_shape, raw_shape = (B, 64, 64, 128), None
+        elif stage.startswith("pnp_conv"):
+            r = 32 >> int(stage[len("pnp_conv"):])
+            out_shape, raw_shape = (B, r, r, 128), (B, r, r, 128)
+        elif stage == "pnp_fc":
+            out_shape, raw_shape = (B, 16), None
+        else:
+            raise ValueError(f"unknown stage {stage!r}")
+        res = {"out": torch.empty(out_shape, dtype=torch.float32, device=dev)}
+        if want_raw:
+            res["raw"] = torch.empty(raw_shape, dtype=torch.float32, device=dev)
+            res["gn_stats"] = torch.empty((10, B, 32, 2), dtype=torch.float64, device=dev)
+        maps = None
+        if want_maps:
+            for name, ch in (("mask", 1), ("full_mask", 1), ("coor_x", 1), ("coor_y", 1), ("coor_z", 1), ("region", 65)):
+                res[name] = torch.empty((B, ch, 64, 64), dtype=torch.float32, device=dev)
+            maps = _lib.GdrnMaps(*[res[k].data_ptr() for k in ("mask", "full_mask", "coor_x", "coor_y", "coor_z", "region")])
+        f32 = lambda t: None if t is None else t.detach().to(device=dev, dtype=torch.float32).contiguous()
+        cls = None if roi_classes is None else roi_classes.detach().to(device=dev, dtype=torch.int64).contiguous()
+        ext, c2d = f32(roi_extents), f32(roi_coord_2d)
+        with torch.cuda.device(dev):
+            self._ensure_engine(dev)
+            ws = self._get_workspace(B, dev)
+            rc = _lib.lib().gdrn_model_run_stage(
+                self._handle, stage.encode(), B, _lib.ptr(x), _lib.ptr(res["out"]), _lib.ptr(res.get("raw")),
+                _lib.ptr(res.get("gn_stats")), _lib.ptr(cls), _lib.ptr(ext), _lib.ptr(c2d),
+                ctypes.byref(maps) if maps is not None else None, _lib.ptr(ws), ws.numel(), _lib.current_stream())
+            _lib.check(rc, f"gdrn_model_run_stage({stage})")
+        return res
+
 
 def build_model_optimizer(cfg, is_test=True):
     """Reference entry point (GDRN_double_mask.py:539-615).  Only the test-time build is in scope."""

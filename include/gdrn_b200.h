@@ -96,6 +96,28 @@ int gdrn_model_get_profile(GdrnModel* m, float* ms_out, int* launches_out);
  * ([B,h,w,256] NHWC, post GN+GELU) | "pnp_in" ([B,64,64,128]) . Returns element count or <0. */
 int64_t gdrn_model_debug_read(GdrnModel* m, const char* name, int batch, float* dst, void* workspace, void* stream);
 
+/* Test / measurement entry: runs ONE geometry-head or Patch-PnP stage of gdrn_model_forward -- the same host function,
+ * plans and kernels the forward launches -- on the model's packed weights, in a gdrn_model_workspace_bytes(m, batch)
+ * workspace.  The fp32 input is first cast to the stage's operand format (bf16, or [hi | lo] split rows in split-bf16 mode);
+ * the outputs are decoded to fp32 (hi + lo).  All tensors NHWC unless noted.
+ *   stage          in                       out
+ *   "deconv"       [B,8,8,C3]               [B,16,16,256]      3x3 s2 transposed conv + GroupNorm + GELU
+ *   "head_conv<i>" [B,h,h,256], i = 0..5,   [B,h',h',256]      3x3 conv + GroupNorm + GELU (+ bilinear x2 after i = 1, 3)
+ *                  h = 16,16,32,32,64,64
+ *   "out_conv"     [B,64,64,256]            [B,64,64,128]      class-gathered 1x1 conv -> Patch-PnP input (69 channels +
+ *                                                              zero pad); maps (optional, NCHW) as in gdrn_model_forward
+ *   "pnp_conv<i>"  [B,2r,2r,128], r = 32>>i [B,r,r,128]        3x3 s2 conv + GroupNorm + GELU
+ *   "pnp_fc"       [B,8,8,128]              [B,16]             fc1 -> fc2 -> fc_r | fc_t (rows 0-5 rot6d, 6-8 t_, rest 0)
+ * C3 is the stored backbone width (1024 for convnext_base).  For the conv stages, raw_out (optional) receives the conv
+ * output before GroupNorm (at the conv's resolution) and gn_stats_out (optional) the whole table of GroupNorm sums
+ * [10][B][32][2] (layer: 0 deconv, 1-6 head convs, 7-9 Patch-PnP convs; per (image, group): sum, sum of squares), cleared
+ * before the stage runs.  roi_classes / roi_extents / roi_coord_2d as in gdrn_model_forward, read by "out_conv" only.
+ * No allocation, no synchronisation. */
+int gdrn_model_run_stage(GdrnModel* m, const char* stage, int batch, const float* in, float* out, float* raw_out,
+                         double* gn_stats_out, const int64_t* roi_classes, const float* roi_extents,
+                         const float* roi_coord_2d, const GdrnMaps* maps, void* workspace, size_t workspace_bytes,
+                         void* stream);
+
 /* Plain GEMM through the same wgmma kernel, exported for tests and roofline measurement:
  * out[M,N] = epi(A[M,K] @ W[N,K]^T + bias); A, W bf16 row-major (K contiguous, lda/ldw = K).
  * epi: 0 = store (out bf16 or fp32 by out_f32), 1 = GELU -> bf16, 2 = resid + gamma*(.) -> fp32. */
