@@ -107,6 +107,11 @@ _SIGNATURES = {
     "gdrn_crop_resize_u8": (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p,
                                     c_void_p]),
     "gdrn_crop_resize_f32": (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p]),
+    "gdrn_roi_setup": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_double, c_int, c_int]
+                       + [c_void_p] * 12 + [c_void_p]),
+    "gdrn_roi_crop_multi": (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int,
+                                    c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
+                                    c_void_p]),
     "gdrn_vsd_workspace_bytes": (c_size_t, [c_int, c_int]),
     "gdrn_vsd_errors": (c_int, [c_void_p] * 3 + [c_int, c_int] + [c_void_p] * 6 + [c_int, c_void_p, c_int, c_float, c_int,
                                                                                  c_void_p, c_size_t, c_void_p, c_void_p]),

@@ -7,37 +7,11 @@
 // built from cvRound()ed per-column / per-row terms, 5 fractional bits, 15-bit integer bilinear weights with the
 // (32767, 0, 0, 1) quirk at integer positions, (sum + 2^14) >> 15, zero border.  One thread per output pixel; the
 // uint8 path writes the normalised NCHW fp32 crop the stem kernel consumes.  Memory-bound: 12 B written per pixel.
-#include "common.cuh"
+#include "crop_common.cuh"
 
 namespace {
 
-struct SrcCoord { int X, Y; };
-
-// every double operation with explicit rounding: nvcc must not contract a*b+c into an FMA (the host code does not)
-__device__ __forceinline__ void invert_affine(const double* __restrict__ M, double (&iM)[6]) {
-  double D = __dsub_rn(__dmul_rn(M[0], M[4]), __dmul_rn(M[1], M[3]));
-  D = D != 0 ? __ddiv_rn(1.0, D) : 0.0;
-  const double A11 = __dmul_rn(M[4], D), A22 = __dmul_rn(M[0], D);
-  iM[0] = A11; iM[1] = __dmul_rn(M[1], -D); iM[3] = __dmul_rn(M[3], -D); iM[4] = A22;
-  iM[2] = __dsub_rn(__dmul_rn(-iM[0], M[2]), __dmul_rn(iM[1], M[5]));
-  iM[5] = __dsub_rn(__dmul_rn(-iM[3], M[2]), __dmul_rn(iM[4], M[5]));
-}
-
-__device__ __forceinline__ SrcCoord src_coord(const double (&iM)[6], int x, int y, bool nearest) {
-  constexpr int AB_BITS = 10, AB_SCALE = 1 << 10, INTER_BITS = 5;
-  const int round_delta = nearest ? AB_SCALE / 2 : AB_SCALE / 32 / 2;
-  const int adelta = __double2int_rn(__dmul_rn(__dmul_rn(iM[0], (double)x), (double)AB_SCALE));
-  const int bdelta = __double2int_rn(__dmul_rn(__dmul_rn(iM[3], (double)x), (double)AB_SCALE));
-  const int X0 = __double2int_rn(__dmul_rn(__dadd_rn(__dmul_rn(iM[1], (double)y), iM[2]), (double)AB_SCALE)) + round_delta;
-  const int Y0 = __double2int_rn(__dmul_rn(__dadd_rn(__dmul_rn(iM[4], (double)y), iM[5]), (double)AB_SCALE)) + round_delta;
-  SrcCoord c;
-  const int sh = nearest ? AB_BITS : AB_BITS - INTER_BITS;
-  c.X = (X0 + adelta) >> sh;
-  c.Y = (Y0 + bdelta) >> sh;
-  return c;
-}
-
-__device__ __forceinline__ int sat_short(int v) { return v > 32767 ? 32767 : (v < -32768 ? -32768 : v); }
+using crop::SrcCoord;
 
 __global__ void __launch_bounds__(256)
 crop_resize_u8_kernel(const uint8_t* __restrict__ img, int H, int W, int C, const double* __restrict__ Ms, int n, int oh,
@@ -48,25 +22,17 @@ crop_resize_u8_kernel(const uint8_t* __restrict__ img, int H, int W, int C, cons
   const int b = (int)(idx / per);
   const int y = (int)((idx % per) / ow), x = (int)(idx % ow);
   double iM[6];
-  invert_affine(Ms + 6 * b, iM);
-  const SrcCoord sc = src_coord(iM, x, y, false);
-  const int sx = sat_short(sc.X >> 5), sy = sat_short(sc.Y >> 5);
-  const int fx = sc.X & 31, fy = sc.Y & 31;
-  // 15-bit weights: exact products of the 1/32 fractions; saturate_cast<short>(32768) = 32767, deficit to weight 3
-  int w[4] = {(32 - fy) * (32 - fx) * 32, (32 - fy) * fx * 32, fy * (32 - fx) * 32, fy * fx * 32};
-  if (w[0] > 32767) { w[0] = 32767; w[3] += 1; }
-  const bool in00 = sx >= 0 && sx < W && sy >= 0 && sy < H, in01 = sx + 1 >= 0 && sx + 1 < W && sy >= 0 && sy < H;
-  const bool in10 = sx >= 0 && sx < W && sy + 1 >= 0 && sy + 1 < H, in11 = sx + 1 >= 0 && sx + 1 < W && sy + 1 >= 0 && sy + 1 < H;
-  const uint8_t* p00 = img + ((long long)sy * W + sx) * C;
+  crop::invert_affine(Ms + 6 * b, iM);
+  const crop::U8Tap t = crop::u8_tap(crop::src_coord(iM, x, y, false), H, W);
+  const uint8_t* p00 = img + ((long long)t.sy * W + t.sx) * C;
   const double mean[3] = {m0, m1, m2}, stdv[3] = {s0, s1, s2};
   for (int c = 0; c < C; ++c) {
     int v = 0;
-    if (in00) v += p00[c] * w[0];
-    if (in01) v += p00[C + c] * w[1];
-    if (in10) v += p00[(long long)W * C + c] * w[2];
-    if (in11) v += p00[(long long)W * C + C + c] * w[3];
-    v = (v + (1 << 14)) >> 15;
-    v = v < 0 ? 0 : (v > 255 ? 255 : v);
+    if (t.in[0]) v += p00[c] * t.w[0];
+    if (t.in[1]) v += p00[C + c] * t.w[1];
+    if (t.in[2]) v += p00[(long long)W * C + c] * t.w[2];
+    if (t.in[3]) v += p00[(long long)W * C + C + c] * t.w[3];
+    v = crop::u8_round(v);
     // normalize_image: (uint8 - mean) / std in float64, then astype(float32) (predictor_gdrn.py normalize_image)
     const int cc = c < 3 ? c : 2;
     out[((long long)b * C + c) * per + (long long)y * ow + x] = __double2float_rn(__ddiv_rn(__dsub_rn((double)v, mean[cc]), stdv[cc]));
@@ -82,25 +48,20 @@ crop_resize_f32_kernel(const float* __restrict__ src, int H, int W, int C, const
   const int b = (int)(idx / per);
   const int y = (int)((idx % per) / ow), x = (int)(idx % ow);
   double iM[6];
-  invert_affine(Ms + 6 * b, iM);
-  const SrcCoord sc = src_coord(iM, x, y, nearest != 0);
+  crop::invert_affine(Ms + 6 * b, iM);
+  const SrcCoord sc = crop::src_coord(iM, x, y, nearest != 0);
   float* o = out + (long long)b * C * per + (long long)y * ow + x;
   if (nearest) {
     const bool in = sc.X >= 0 && sc.X < W && sc.Y >= 0 && sc.Y < H;
     for (int c = 0; c < C; ++c) o[c * per] = in ? src[((long long)sc.Y * W + sc.X) * C + c] : 0.f;
     return;
   }
-  const int sx = sc.X >> 5, sy = sc.Y >> 5;
-  const float ax = (float)(sc.X & 31) * (1.f / 32), ay = (float)(sc.Y & 31) * (1.f / 32);
-  const float w0 = __fmul_rn(1.f - ay, 1.f - ax), w1 = __fmul_rn(1.f - ay, ax), w2 = __fmul_rn(ay, 1.f - ax), w3 = __fmul_rn(ay, ax);
-  const bool in00 = sx >= 0 && sx < W && sy >= 0 && sy < H, in01 = sx + 1 >= 0 && sx + 1 < W && sy >= 0 && sy < H;
-  const bool in10 = sx >= 0 && sx < W && sy + 1 >= 0 && sy + 1 < H, in11 = sx + 1 >= 0 && sx + 1 < W && sy + 1 >= 0 && sy + 1 < H;
-  const float* p00 = src + ((long long)sy * W + sx) * C;
+  const crop::F32Tap t = crop::f32_tap(sc, H, W);
+  const float* p00 = src + ((long long)t.sy * W + t.sx) * C;
   for (int c = 0; c < C; ++c) {
-    const float a = in00 ? p00[c] : 0.f, bq = in01 ? p00[C + c] : 0.f;
-    const float cq = in10 ? p00[(long long)W * C + c] : 0.f, d = in11 ? p00[(long long)W * C + C + c] : 0.f;
-    // same association as OpenCV's scalar remapBilinear: ((a*w0 + b*w1) + c*w2) + d*w3, no FMA
-    o[c * per] = __fadd_rn(__fadd_rn(__fadd_rn(__fmul_rn(a, w0), __fmul_rn(bq, w1)), __fmul_rn(cq, w2)), __fmul_rn(d, w3));
+    const float a = t.in[0] ? p00[c] : 0.f, bq = t.in[1] ? p00[C + c] : 0.f;
+    const float cq = t.in[2] ? p00[(long long)W * C + c] : 0.f, d = t.in[3] ? p00[(long long)W * C + C + c] : 0.f;
+    o[c * per] = crop::f32_blend(t, a, bq, cq, d);
   }
 }
 

@@ -498,3 +498,81 @@ def crop_resize_float(src, M, output_size, nearest=False, out=None):
     _lib.check(_lib.lib().gdrn_crop_resize_f32(_lib.ptr(src), H, W, C, _lib.ptr(Md), n, int(oh), int(ow), int(bool(nearest)),
                                                _lib.ptr(out), _lib.current_stream()), "gdrn_crop_resize_f32")
     return out
+
+
+# ---------------------------------------------------------------------------------------------------------------
+# Model inputs for the ROIs of many images (read_data_test + batch_data_test, datasets/data_loader.py:751-797,
+# engine/engine_utils.py:213-241) in two launches: csrc/roi_batch.cu
+# ---------------------------------------------------------------------------------------------------------------
+ROI_BATCH_KEYS = (("roi_center", (2,), torch.float32), ("roi_wh", (2,), torch.float32), ("scale", (), torch.float32),
+                  ("resize_ratio", (), torch.float32), ("roi_extent", (3,), torch.float32), ("roi_cam", (3, 3), torch.float32),
+                  ("roi_cls", (), torch.int64), ("im_H", (), torch.float32), ("im_W", (), torch.float32),
+                  ("bbox_est", (4,), torch.float32), ("M_in", (6,), torch.float64), ("M_out", (6,), torch.float64))
+
+
+def roi_batch_buffers(n, device, input_res=256, output_res=64, with_depth=False):
+    """Preallocated outputs of roi_batch_inputs for n ROIs (static buffers a CUDA graph can be captured over)."""
+    z = lambda shape, dtype=torch.float32: torch.zeros((n,) + tuple(shape), dtype=dtype, device=device)
+    out = {k: z(shape, dtype) for k, shape, dtype in ROI_BATCH_KEYS}
+    out["roi_img"] = z((3, input_res, input_res))
+    out["roi_coord_2d"] = z((2, output_res, output_res))
+    if with_depth:
+        out["roi_depth"] = z((1, input_res, input_res))
+        out["depth_sensor"] = z((output_res, output_res))
+    return out
+
+
+@_lib.on_device(0)
+def roi_batch_inputs(images, dets, Ks, extents, dzi_pad_scale=1.5, input_res=256, output_res=64,
+                     pixel_mean=(0.0, 0.0, 0.0), pixel_std=(255.0, 255.0, 255.0), depth=None, depth_factor=None, out=None):
+    """The model inputs of a batch of images, as batch_data_test returns them, from two kernels (gdrn_roi_setup +
+    gdrn_roi_crop_multi) on the current stream; no allocation when ``out`` is given, no synchronisation.
+
+    images [N,H,W,C] uint8 CUDA (BGR, C = 1 or 3; one call per image size); dets: mapping with "det_meta" [n,2] int32
+    (image index, label) and "bbox_est" [n,4] float32 XYWH_ABS (CUDA), plus optional "score" / "time" [n] passed
+    through; Ks [N,3,3] float32 CUDA; extents [nc,3] float32 CUDA (per label); depth [N,H,W] uint16 CUDA with
+    depth_factor [N] float64 CUDA (1000 / depth_scale) adds roi_depth [n,1,in,in] and the 64x64 depth-refine sensor crop
+    ("depth_sensor" [n,out,out]).  Returns a dict: roi_img, roi_coord_2d, roi_center, roi_wh, scale, resize_ratio,
+    roi_extent, roi_cam, roi_cls (int64), im_H, im_W, bbox_est (XYXY), M_in / M_out [n,6] float64 and the pass-through
+    keys.  Image indices and labels are validated by the caller (they come from host data)."""
+    _check_cuda_contig(images, "images")
+    if images.dtype != torch.uint8 or images.dim() != 4 or images.shape[3] not in (1, 3):
+        raise ValueError(f"images must be [N,H,W,1|3] uint8, got {tuple(images.shape)} {images.dtype}")
+    N, H, W, C = images.shape
+    meta, xywh = dets["det_meta"], dets["bbox_est"]
+    for t, name, dt in ((meta, "det_meta", torch.int32), (xywh, "bbox_est", torch.float32), (Ks, "Ks", torch.float32),
+                        (extents, "extents", torch.float32)):
+        _check_cuda_contig(t, name)
+        if t.dtype != dt:
+            raise ValueError(f"{name} must be {dt}")
+    n = meta.shape[0]
+    if tuple(Ks.shape) != (N, 3, 3):
+        raise ValueError(f"Ks must be [{N},3,3], got {tuple(Ks.shape)}")
+    with_depth = depth is not None
+    if with_depth:
+        _check_cuda_contig(depth, "depth")
+        _check_cuda_contig(depth_factor, "depth_factor")
+        if depth.dtype != torch.uint16 or tuple(depth.shape) != (N, H, W) or depth_factor.dtype != torch.float64:
+            raise ValueError("depth must be [N,H,W] uint16 with depth_factor [N] float64")
+    if out is None:
+        out = roi_batch_buffers(n, images.device, input_res, output_res, with_depth)
+    im_hw = torch.full((max(N, 1), 2), H, dtype=torch.int32, device=images.device)   # device fills: no host copy
+    im_hw[:, 1].fill_(W)
+    p = _lib.ptr
+    L = _lib.lib()
+    _lib.check(L.gdrn_roi_setup(p(meta), p(xywh), n, p(Ks), p(im_hw), p(extents), float(dzi_pad_scale), int(input_res),
+                                int(output_res), *[p(out[k]) for k, _, _ in ROI_BATCH_KEYS], _lib.current_stream()),
+               "gdrn_roi_setup")
+    mean = (ctypes.c_double * 3)(*[float(v) for v in pixel_mean])
+    std = (ctypes.c_double * 3)(*[float(v) for v in pixel_std])
+    _lib.check(L.gdrn_roi_crop_multi(p(images), H, W, C, p(meta), p(out["M_in"]), p(out["M_out"]), n, int(input_res),
+                                     int(output_res), mean, std, p(depth) if with_depth else None,
+                                     p(depth_factor) if with_depth else None, p(out["roi_img"]), p(out["roi_coord_2d"]),
+                                     p(out.get("roi_depth")) if with_depth else None,
+                                     p(out.get("depth_sensor")) if with_depth else None, _lib.current_stream()),
+               "gdrn_roi_crop_multi")
+    res = dict(out)
+    for k in ("score", "time"):
+        if k in dets:
+            res[k] = dets[k]
+    return res

@@ -278,3 +278,85 @@ def make_yolox_state_dict(forward, depth=0.33, width=0.25, num_classes=8, seed=0
             sd[f"head.obj_preds.{k}.bias"].fill_(b_o)
             sd[f"head.cls_preds.{k}.bias"].fill_(b_c)
     return {k: (v.float() if v.is_floating_point() else v).cpu() for k, v in sd.items()}
+
+
+def write_bop_tree(root, dataset="ycbv", num_images=12, num_scenes=2, H=480, W=640, dets_per_image=6, seed=0, gray=False,
+                   obj_ids=None, with_depth=True):
+    """A small BOP test split under ``root`` (the reference's ``datasets/`` directory): BOP_DATASETS/<dataset>/ with
+    test_targets_bop19.json, test/<scene>/{rgb|gray, depth, scene_camera.json, scene_gt.json, scene_gt_info.json},
+    models_eval/ (box meshes in mm + models_info.json) and test/test_bboxes/dets.json (detections, XYWH boxes around the
+    ground-truth objects, some partly outside the image).  Colour images are random BGR PNGs (``gray``: 8-bit TIFs in
+    gray/, as ITODD), depth 16-bit PNGs of a tilted plane.  -> path of the detection file relative to ``root``, as "datasets/..."."""
+    import json
+    import os
+
+    import cv2
+
+    from .ply import save_ply
+
+    rng = np.random.RandomState(seed)
+    base = os.path.join(root, "BOP_DATASETS", dataset)
+    split = os.path.join(base, "test_primesense" if dataset in ("tless", "hb") else "test")
+    models = os.path.join(base, "models_eval")
+    os.makedirs(models, exist_ok=True)
+    obj_ids = list(obj_ids or range(1, 22))
+    info = {}
+    faces = np.array([[0, 1, 3], [0, 3, 2], [4, 6, 7], [4, 7, 5], [0, 4, 5], [0, 5, 1], [2, 3, 7], [2, 7, 6],
+                      [0, 2, 6], [0, 6, 4], [1, 5, 7], [1, 7, 3]], np.int32)
+    for o in obj_ids:
+        half = rng.uniform(20, 60, 3)
+        pts = np.array([[sx, sy, sz] for sx in (-1, 1) for sy in (-1, 1) for sz in (-1, 1)], np.float32) * half
+        save_ply(os.path.join(models, "obj_{:06d}.ply".format(o)), pts, faces)
+        info[str(o)] = {"diameter": float(2 * np.linalg.norm(half)), "min_x": float(-half[0]), "min_y": float(-half[1]),
+                        "min_z": float(-half[2]), "size_x": float(2 * half[0]), "size_y": float(2 * half[1]),
+                        "size_z": float(2 * half[2])}
+    with open(os.path.join(models, "models_info.json"), "w") as f:
+        json.dump(info, f)
+    targets, dets = [], {}
+    color_dir, ext = ("gray", ".tif") if gray else ("rgb", ".png")
+    per_scene = -(-num_images // num_scenes)
+    for s in range(num_scenes):
+        scene_id = s + 1
+        sdir = os.path.join(split, "{:06d}".format(scene_id))
+        os.makedirs(os.path.join(sdir, color_dir), exist_ok=True)
+        os.makedirs(os.path.join(sdir, "depth"), exist_ok=True)
+        cams, gts, gt_infos = {}, {}, {}
+        for k in range(min(per_scene, num_images - s * per_scene)):
+            im_id = 3 * k + 1
+            f = W * rng.uniform(0.9, 1.1)
+            K = [f, 0.0, W / 2 + rng.uniform(-5, 5), 0.0, f, H / 2 + rng.uniform(-5, 5), 0.0, 0.0, 1.0]
+            depth_scale = float(rng.choice([0.1, 1.0]))
+            cams[str(im_id)] = {"cam_K": K, "depth_scale": depth_scale}
+            im = rng.randint(0, 256, (H, W) if gray else (H, W, 3)).astype(np.uint8)
+            cv2.imwrite(os.path.join(sdir, color_dir, "{:06d}{}".format(im_id, ext)), im)
+            yy, xx = np.mgrid[0:H, 0:W]   # a tilted plane 0.8-1.2 m away with a few mm of noise, in depth_scale units
+            depth_mm = 800 + 300 * xx / W + 100 * yy / H + rng.uniform(0, 5, (H, W))
+            cv2.imwrite(os.path.join(sdir, "depth", "{:06d}{}".format(im_id, ext)),
+                        np.round(depth_mm / depth_scale).astype(np.uint16))
+            gts[str(im_id)], gt_infos[str(im_id)], cur = [], [], []
+            for j, o in enumerate(rng.choice(obj_ids, min(dets_per_image, len(obj_ids)), replace=False)):
+                o = int(o)
+                R = cv2.Rodrigues(rng.uniform(-1, 1, 3))[0]
+                t = np.array([rng.uniform(-150, 150), rng.uniform(-100, 100), rng.uniform(600, 1200)])
+                gts[str(im_id)].append({"obj_id": o, "cam_R_m2c": R.reshape(-1).tolist(), "cam_t_m2c": t.tolist()})
+                u, v = f * t[0] / t[2] + K[2], f * t[1] / t[2] + K[5]
+                bw, bh = rng.uniform(0.3, 200), rng.uniform(0.3, 200)
+                x, y = u - bw / 2 + rng.uniform(-100, 100) * (j == 0), v - bh / 2
+                gt_infos[str(im_id)].append({"bbox_obj": [int(x), int(y), int(bw), int(bh)],
+                                             "bbox_visib": [int(x), int(y), int(bw), int(bh)], "px_count_all": 1000,
+                                             "px_count_valid": 1000, "px_count_visib": 900, "visib_fract": 0.9})
+                cur.append({"obj_id": o, "bbox_est": [float(x), float(y), float(bw), float(bh)],
+                            "score": float(np.round(rng.uniform(0.05, 1.0), 2)), "time": 0.01})
+            dets["{}/{}".format(scene_id, im_id)] = cur
+            for o in sorted({g["obj_id"] for g in gts[str(im_id)]}):
+                targets.append({"scene_id": scene_id, "im_id": im_id, "obj_id": o,
+                                "inst_count": sum(g["obj_id"] == o for g in gts[str(im_id)])})
+        for name, content in (("scene_camera.json", cams), ("scene_gt.json", gts), ("scene_gt_info.json", gt_infos)):
+            with open(os.path.join(sdir, name), "w") as f:
+                json.dump(content, f)
+    with open(os.path.join(base, "test_targets_bop19.json"), "w") as f:
+        json.dump(targets, f)
+    os.makedirs(os.path.join(split, "test_bboxes"), exist_ok=True)
+    with open(os.path.join(split, "test_bboxes", "dets.json"), "w") as f:
+        json.dump(dets, f)
+    return "datasets/" + os.path.relpath(os.path.join(split, "test_bboxes", "dets.json"), root)

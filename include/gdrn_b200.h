@@ -295,6 +295,37 @@ int gdrn_crop_resize_f32(const float* src, int H, int W, int C, const double* M,
                          int nearest, float* out, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
+ * Model inputs for the ROIs of many images in one forward -- replaces the per-image read_data_test
+ * (core/gdrn_modeling/datasets/data_loader.py:751-797) + batch_data_test (engine/engine_utils.py:213-241) of the
+ * reference's test loop (build_gdrn_test_loader, batch_size = 1).
+ *
+ * gdrn_roi_setup: one thread per ROI, the loader's dtype path step for step (see csrc/roi_batch.cu).
+ *   det_meta [n,2] i32 (image index, label), det_xywh [n,4] f32 (bbox_est, XYWH_ABS); per image K [N,3,3] f32 and
+ *   im_hw [N,2] i32 (H, W); extents [nc,3] f32 per label.  Outputs with batch_data_test's dtypes: roi_center [n,2],
+ *   roi_wh [n,2], scale [n], resize_ratio [n], roi_extent [n,3], roi_cam [n,3,3], im_H [n], im_W [n], bbox_xyxy [n,4]
+ *   (f32), roi_cls [n] (i64), and the forward affine matrices M_in / M_out [n,6] f64 of get_affine_transform for
+ *   in_res / out_res.  Indices are not range-checked on the device: the caller validates them.
+ * gdrn_roi_crop_multi: every crop of the batch in one launch, with crop_resize.cu's exact warpAffine arithmetic;
+ *   ROI i reads image det_meta[i].image.
+ *   images [N,H,W,C] u8 BGR, C = 1 (replicated to three channels, as cv2.imread(..., IMREAD_COLOR)) or 3;
+ *   pixel_mean / pixel_std: host arrays [3].
+ *   -> roi_img [n,3,in_res,in_res] f32 (bilinear + normalize_image);
+ *      roi_coord_2d [n,2,out_res,out_res] f32: bilinear crop of get_2d_coord_np's grid, computed in the kernel;
+ *   optional (NULL to skip; they need depth [N,H,W] u16 and depth_factor [N] f64, device):
+ *      roi_depth [n,1,in_res,in_res] f32: nearest crop of f32((double)depth / depth_factor) metres;
+ *      depth_sensor [n,out_res,out_res] f32: ((a+b)+(c+d))*0.25 of the centre 2x2 of every 4x4 cell of roi_depth
+ *      (in_res = 4 * out_res), the sensor crop depth refine reads.
+ * ------------------------------------------------------------------------------------------- */
+int gdrn_roi_setup(const int* det_meta, const float* det_xywh, int n, const float* K, const int* im_hw,
+                   const float* extents, double dzi_pad_scale, int in_res, int out_res, float* roi_center, float* roi_wh,
+                   float* scale, float* resize_ratio, float* roi_extent, float* roi_cam, long long* roi_cls, float* im_H,
+                   float* im_W, float* bbox_xyxy, double* M_in, double* M_out, void* stream);
+int gdrn_roi_crop_multi(const uint8_t* images, int H, int W, int C, const int* det_meta, const double* M_in,
+                        const double* M_out, int n, int in_res, int out_res, const double* pixel_mean,
+                        const double* pixel_std, const uint16_t* depth, const double* depth_factor, float* roi_img,
+                        float* roi_coord_2d, float* roi_depth, float* depth_sensor, void* stream);
+
+/* ---------------------------------------------------------------------------------------------
  * Batched RANSAC-PnP (SURVEY.md 8f rank 2) -- replaces the per-ROI host loop get_pnp_ransac_pose
  * (core/gdrn_modeling/engine/gdrn_evaluator.py:1122-1221) + misc.pnp_v2 (lib/pysixd/misc.py:153-208) =
  * cv2.solvePnPRansac(EPNP, reprojectionError 3, 100 iterations), the reference predictor's default TEST.USE_PNP path.
