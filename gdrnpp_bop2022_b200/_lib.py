@@ -120,6 +120,12 @@ _SIGNATURES = {
     "gdrn_ad_errors": (c_int, [c_void_p] * 7 + [c_int, c_int, c_void_p, c_size_t, c_void_p, c_void_p]),
     "gdrn_sym_proj_mean": (c_int, [c_void_p] * 9 + [c_int, c_int] + [c_void_p] * 2),
     "gdrn_sym_rt_errors": (c_int, [c_void_p] * 6 + [c_int] + [c_void_p] * 3),
+    "yolox_letterbox_workspace_bytes": (c_size_t, [c_int] * 5),
+    "yolox_letterbox": (c_int, [c_void_p] + [c_int] * 6 + [c_void_p, c_void_p, c_size_t, c_void_p]),
+    "coco_eval_match": (c_int, [c_void_p] * 9 + [c_int] * 3 + [c_void_p, c_int, c_void_p, c_int, c_int] + [c_void_p] * 9),
+    "coco_eval_accumulate_workspace_bytes": (c_size_t, [c_int]),
+    "coco_eval_accumulate": (c_int, [c_void_p] * 8 + [c_int] * 6 + [c_void_p, c_int, c_void_p, c_int, c_void_p, c_size_t,
+                                                                     c_void_p, c_void_p, c_void_p]),
 }
 
 EXPORTED_SYMBOLS = tuple(_SIGNATURES.keys())

@@ -576,3 +576,40 @@ def roi_batch_inputs(images, dets, Ks, extents, dzi_pad_scale=1.5, input_res=256
         if k in dets:
             res[k] = dets[k]
     return res
+
+
+# ---------------------------------------------------------------------------------------------------------------
+# YOLOX test-time letterbox (base_data_from_list.load_resized_img + ValTransform preproc): csrc/yolox_letterbox.cu
+# ---------------------------------------------------------------------------------------------------------------
+def letterbox_ratio(h, w, test_size):
+    """preproc's ratio r = min(th / h, tw / w) and resized size (int(h r), int(w r))."""
+    r = min(test_size[0] / h, test_size[1] / w)
+    return r, (int(h * r), int(w * r))
+
+
+def letterbox_workspace(N, H, W, test_size, device):
+    """The u8 workspace yolox_letterbox needs for this size (an empty tensor when one resize suffices)."""
+    nb = _lib.lib().yolox_letterbox_workspace_bytes(N, H, W, int(test_size[0]), int(test_size[1]))
+    return torch.empty(nb, dtype=torch.uint8, device=device)
+
+
+@_lib.on_device(0)
+def yolox_letterbox(images, test_size, out=None, workspace=None):
+    """images [N,H,W,C] uint8 CUDA (BGR, C = 1 is replicated to three channels) -> [N,3,th,tw] float32: the network
+    input of the reference's test loop, bit-exact to cv2.resize(INTER_LINEAR) + 114 padding + HWC->CHW.  A size whose
+    second ValTransform resize is not the identity is resized twice, as the reference does (two launches); every
+    shipped split takes one.  No synchronisation."""
+    _check_cuda_contig(images, "images")
+    if images.dtype != torch.uint8 or images.dim() != 4 or images.shape[3] not in (1, 3):
+        raise ValueError(f"images must be [N,H,W,1|3] uint8, got {tuple(images.shape)} {images.dtype}")
+    N, H, W, C = images.shape
+    th, tw = int(test_size[0]), int(test_size[1])
+    if out is None:
+        out = torch.empty((N, 3, th, tw), dtype=torch.float32, device=images.device)
+    elif tuple(out.shape) != (N, 3, th, tw) or out.dtype != torch.float32 or not out.is_contiguous():
+        raise ValueError(f"out must be a contiguous [{N},3,{th},{tw}] float32 tensor")
+    if workspace is None:
+        workspace = letterbox_workspace(N, H, W, test_size, images.device)
+    _lib.check(_lib.lib().yolox_letterbox(_lib.ptr(images), N, H, W, C, th, tw, _lib.ptr(out), _lib.ptr(workspace),
+                                          workspace.numel(), _lib.current_stream()), "yolox_letterbox")
+    return out

@@ -457,8 +457,78 @@ def load_yolox_config(path):
     missing = [k for k in _TEST_KEYS if k not in test]
     if missing:
         raise ValueError(f"{path}: test.{', test.'.join(missing)} not found")
+    ex = _read_test_loop_settings(path, frozenset())
+    output_dir = ex.get("output_dir")
+    if output_dir is None:   # train.output_dir = osp.abspath(__file__).replace("configs", "output", 1)[0:-3]
+        output_dir = os.path.abspath(path).replace("configs", "output", 1)[0:-3]
     return SimpleNamespace(depth=float(cfg["backbone.depth"]), width=float(cfg["backbone.width"]),
                            num_classes=int(cfg["head.num_classes"]), test_size=tuple(int(v) for v in test["test_size"]),
                            conf_thr=float(test["conf_thr"]), nms_thr=float(test["nms_thr"]),
                            augment=bool(test.get("augment", _TEST_OPTIONAL["augment"])),
-                           scales=None if test.get("scales") is None else tuple(test["scales"]))
+                           scales=None if test.get("scales") is None else tuple(test["scales"]),
+                           test_dataset_names=tuple(ex.get("test_dataset_names", ())),
+                           half_test=bool(ex.get("half_test", False)), amp_test=bool(ex.get("amp_test", False)),
+                           output_dir=output_dir, eval_cached=bool(ex.get("eval_cached", False)),
+                           legacy=bool(ex.get("legacy", False)), filter_scene=bool(ex.get("filter_scene", False)))
+
+
+def _read_test_loop_settings(path, seen):
+    """The settings of the dataset test loop (main_yolox.py --eval-only) along the import chain: DATASETS.TEST /
+    test.test_dataset_names, test.half_test / amp_test, val.eval_cached, a literal train.output_dir, and the
+    ValTransform(legacy=...) / YOLOX_COCOEvaluator(filter_scene=...) arguments of the test loaders."""
+    path = os.path.abspath(path)
+    if path in seen:
+        raise ValueError(f"{path}: import cycle")
+    tree = ast.parse(open(path).read(), path)
+    out = {}
+
+    def lit(node, default=None):
+        try:
+            return ast.literal_eval(node)
+        except ValueError:
+            return default
+
+    for node in tree.body:
+        if isinstance(node, ast.ImportFrom) and node.level == 1 and node.module:
+            base = os.path.join(os.path.dirname(path), *node.module.split(".")) + ".py"
+            if os.path.exists(base) and {a.name for a in node.names} & {"test", "DATASETS", "train", "val"}:
+                out.update(_read_test_loop_settings(base, seen | {path}))
+            continue
+        if isinstance(node, ast.Assign) and len(node.targets) == 1:
+            tgt, val = _dotted(node.targets[0]), node.value
+            if tgt in ("test", "val", "train", "DATASETS") and isinstance(val, ast.Call) and _dotted(val.func) == "dict":
+                for kw in val.keywords:
+                    _test_loop_key(out, f"{tgt}.{kw.arg}", kw.value, lit)
+            elif tgt:
+                _test_loop_key(out, tgt, val, lit)
+        elif isinstance(node, ast.Expr) and isinstance(node.value, ast.Call) and _dotted(node.value.func) in (
+                "train.update", "test.update", "val.update"):
+            obj = _dotted(node.value.func)[:-len(".update")]
+            for kw in node.value.keywords:
+                _test_loop_key(out, f"{obj}.{kw.arg}", kw.value, lit)
+        for sub in ast.walk(node):
+            if isinstance(sub, ast.Call) and isinstance(sub.func, ast.Call) and sub.func.args:
+                name = _dotted(sub.func.args[0])   # L(ValTransform)(legacy=...)
+                for kw in sub.keywords:
+                    if name == "ValTransform" and kw.arg == "legacy":
+                        out["legacy"] = bool(lit(kw.value, True))
+                    elif name == "YOLOX_COCOEvaluator" and kw.arg == "filter_scene":
+                        out["filter_scene"] = bool(lit(kw.value, True))
+    return out
+
+
+def _test_loop_key(out, tgt, val, lit):
+    if tgt == "DATASETS.TEST":
+        names = lit(val)
+        if names is not None:
+            out["datasets_test"] = tuple(names)
+            out["test_dataset_names"] = tuple(names)
+    elif tgt == "test.test_dataset_names":
+        names = out.get("datasets_test", ()) if _dotted(val) == "DATASETS.TEST" else lit(val)
+        if names is not None:
+            out["test_dataset_names"] = tuple(names)
+    elif tgt in ("test.half_test", "test.amp_test", "val.eval_cached"):
+        out[tgt.split(".")[1]] = bool(lit(val, True))
+    elif tgt == "train.output_dir":
+        v = lit(val)
+        out["output_dir"] = v if isinstance(v, str) else None

@@ -12,10 +12,11 @@ from . import _lib
 
 @_lib.on_device(0)
 def postprocess_padded(det_preds, num_classes, conf_thre=0.7, nms_thre=0.45, class_agnostic=False, hw=None, strides=None,
-                       max_out=None):
+                       max_out=None, workspace=None):
     """-> (dets [B, max_out, 7], n_det [B] int32), both on the device, no synchronisation.  ``hw`` (list of (rows, cols)
     per pyramid level) + ``strides``: det_preds are RAW head outputs and are decoded here; otherwise they are decoded
-    (cx, cy, w, h) boxes, as YOLOXHead returns them with decode_in_inference."""
+    (cx, cy, w, h) boxes, as YOLOXHead returns them with decode_in_inference.  ``workspace``: a one-element list that
+    holds the NMS workspace across calls (grown when a call needs more), so a loop does not allocate it per batch."""
     if not det_preds.is_cuda:
         raise _lib.GdrnError("yolox postprocess needs CUDA tensors (no CPU fallback)")
     dev = det_preds.device
@@ -33,7 +34,13 @@ def postprocess_padded(det_preds, num_classes, conf_thre=0.7, nms_thre=0.45, cla
         hw_t = torch.tensor([[int(h), int(w)] for h, w in hw], dtype=torch.int32, device=dev)
         st_t = torch.tensor([int(s) for s in strides], dtype=torch.int32, device=dev)
     L = _lib.lib()
-    ws = torch.empty(L.yolox_postprocess_workspace_bytes(B, A), dtype=torch.uint8, device=dev)
+    nb = L.yolox_postprocess_workspace_bytes(B, A)
+    if workspace is None:
+        ws = torch.empty(nb, dtype=torch.uint8, device=dev)
+    else:
+        if workspace[0] is None or workspace[0].numel() < nb or workspace[0].device != dev:
+            workspace[0] = torch.empty(nb, dtype=torch.uint8, device=dev)
+        ws = workspace[0]
     _lib.check(L.yolox_postprocess(_lib.ptr(p), B, A, int(num_classes), _lib.ptr(hw_t), _lib.ptr(st_t), n_levels, float(conf_thre),
                                    float(nms_thre), int(bool(class_agnostic)), max_out, _lib.ptr(dets), _lib.ptr(n_det), _lib.ptr(ws),
                                    ws.numel(), _lib.current_stream()), "yolox_postprocess")

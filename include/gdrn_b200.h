@@ -475,6 +475,38 @@ int gdrn_sym_proj_mean(const double* pts, const int64_t* pt_offsets, const doubl
 int gdrn_sym_rt_errors(const double* syms, const int64_t* sym_offsets, const int* pair_obj, const double* pose_est,
                        const double* pose_gt, const uint8_t* use_syms, int P, double* re_deg, double* te, void* stream);
 
+/* ---------------------------------------------------------------------------------------------
+ * YOLOX test-time letterbox (csrc/yolox_letterbox.cu): N uint8 HWC images of one size (C = 1 is replicated to BGR)
+ * -> out [N,3,th,tw] f32, the image resized to (int(h r), int(w r)) with r = min(th/h, tw/w), bit-exact to
+ * cv2.resize(INTER_LINEAR), placed top-left on a 114 canvas.  When ValTransform's second resize is not the identity for
+ * that size the image is resized twice through a u8 workspace of yolox_letterbox_workspace_bytes (0 otherwise).
+ * ------------------------------------------------------------------------------------------- */
+size_t yolox_letterbox_workspace_bytes(int N, int H, int W, int th, int tw);
+int yolox_letterbox(const uint8_t* images, int N, int H, int W, int C, int th, int tw, float* out, void* workspace,
+                    size_t workspace_bytes, void* stream);
+
+/* ---------------------------------------------------------------------------------------------
+ * COCO bbox evaluation (csrc/coco_eval.cu), pycocotools COCOeval evaluate + accumulate.  P (image, category) pairs in
+ * (category, image) order; GT and detections grouped by pair (input order kept inside a pair), offsets [P+1].
+ *   coco_eval_match: per pair the kept detections (stable descending score, at most max_det; kept offsets
+ *     pair_kept_off [P+1], Dkept in all) -> dt_order (input index), kept_score, kept_rank; ious at pair_iou_off
+ *     (kept x G per pair); gt_ignore [A,Gtot]; dt_match [A,T,Dkept] (matched GT index + 1, 0 = none);
+ *     dt_ignore [A,T,Dkept]; gt_match [A,T,Gtot] (kept position + 1 of the matching detection, 0 = none).
+ *   coco_eval_accumulate: per category (cat_off [K+1] over kept detections, cat_gt_off [K+1] over GT, cat_pairs [K])
+ *     precision [T,R,K,A,M] and recall [T,K,A,M], both pre-filled with -1 by the caller.
+ * ------------------------------------------------------------------------------------------- */
+int coco_eval_match(const double* gt_box, const double* gt_area, const uint8_t* gt_crowd, const double* dt_box,
+                    const double* dt_score, const int* pair_gt_off, const int* pair_dt_off, const int* pair_kept_off,
+                    const long long* pair_iou_off, int P, int Gtot, int Dkept, const double* iou_thrs, int T,
+                    const double* area_rng, int A, int max_det, int* dt_order, double* kept_score, int* kept_rank,
+                    double* ious, uint8_t* gt_ignore, int* dt_match, uint8_t* dt_ignore, int* gt_match, void* stream);
+size_t coco_eval_accumulate_workspace_bytes(int Dkept);
+int coco_eval_accumulate(const double* kept_score, const int* kept_rank, const int* dt_match, const uint8_t* dt_ignore,
+                         const uint8_t* gt_ignore, const int* cat_off, const int* cat_gt_off, const int* cat_pairs,
+                         int max_cat_dets, int K, int Dkept, int Gtot, int T, int A, const double* rec_thrs, int R,
+                         const int* max_dets, int M, void* workspace, size_t workspace_bytes, double* precision,
+                         double* recall, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
