@@ -341,18 +341,21 @@ dwconv_ln_cluster_kernel(const __grid_constant__ CUtensorMap tmap_x, const __gri
   // shuffles only, PUSHES that partial into every CTA of the cluster (distributed shared memory stores), and after
   // ONE cluster barrier each warp combines the C/64 partials with Chan's parallel-variance formula.  No block-level
   // barrier, no remote loads, and nothing remote is touched after the barrier (so no exit barrier is needed).
-  constexpr float INV_W = 1.0f / 64.0f;  // channels per warp = 64
+  // Zero pad channels (c >= c_real, all in the last 64-channel group) are left out of the group's mean and M2.
   const int pix = row0 * TW + lane / LPP;   // the thread's R rows are contiguous in the row-major tile
   float s_loc, m2_loc;
   {
+    const int cw = c0 + wc * 64;             // first channel of this warp's group
+    const float inv_n = 1.0f / (float)min(64, c_real - cw);
+    const bool real_x = c0 + cl < c_real, real_y = c0 + cl + 1 < c_real;
     float a[NV];
 #pragma unroll
     for (int i = 0; i < NV; ++i) a[i] = ax[i] + ay[i];
     s_loc = lane_transpose_reduce<NV>(a, lane);           // lane L: pixel L / LPP of this thread-row
 #pragma unroll
     for (int i = 0; i < NV; ++i) {
-      const float m = __shfl_sync(0xffffffffu, s_loc, i * LPP) * INV_W;
-      const float dx = ax[i] - m, dy = ay[i] - m;
+      const float m = __shfl_sync(0xffffffffu, s_loc, i * LPP) * inv_n;
+      const float dx = real_x ? ax[i] - m : 0.f, dy = real_y ? ay[i] - m : 0.f;
       a[i] = fmaf(dx, dx, dy * dy);
     }
     m2_loc = lane_transpose_reduce<NV>(a, lane);
@@ -377,13 +380,14 @@ dwconv_ln_cluster_kernel(const __grid_constant__ CUtensorMap tmap_x, const __gri
     float tot = 0.f;
     for (int k = 0; k < nparts; ++k) tot += s_parts[k * NPIX + pix].x;
     mean_p = tot / (float)c_real;
+    // Chan combine over the real channels: group k holds n_k = min(64, c_real - 64 k) of them
     float m2 = 0.f;
     for (int k = 0; k < nparts; ++k) {
       const float2 v = s_parts[k * NPIX + pix];
-      const float d = v.x * INV_W - mean_p;
-      m2 += fmaf(64.0f * d, d, v.y);
+      const float n_k = (float)min(64, c_real - 64 * k);
+      const float d = v.x / n_k - mean_p;
+      m2 += fmaf(n_k * d, d, v.y);
     }
-    m2 = fmaf(-(float)(C - c_real) * mean_p, mean_p, m2);   // zero pad channels each added mean^2 (exact no-op when c_real == C)
     rstd_p = rsqrtf(m2 / (float)c_real + eps);
   }
   // ---- normalise + affine, bf16x2 out (a warp writes 128 contiguous bytes per pixel) ----
@@ -462,17 +466,22 @@ ln_patchify2_kernel(const float* __restrict__ x, const float* __restrict__ ln_w,
   for (int o = 16; o > 0; o >>= 1)
 #pragma unroll
     for (int p = 0; p < 4; ++p) s[p] += __shfl_xor_sync(0xffffffffu, s[p], o);
+  // centred sum of squares over the c_real real channels only: the zero pad channels are masked out of the pass
+  // (subtracting their (C - c_real) * mean^2 afterwards cancels catastrophically when |mean| >> std)
+  auto centred = [c_real](float x, float mean, int c) { return c < c_real ? x - mean : 0.f; };
 #pragma unroll
   for (int p = 0; p < 4; ++p) {
     s[p] = s[p] / (float)c_real;   // mean (zero pad channels do not contribute to the sum)
     q[p] = 0.f;
 #pragma unroll
     for (int k = 0; k < NV; ++k) {
+      const int c = (k * 32 + lane) * VW;
       if constexpr (VW == 4) {
-        const float dx = v[p][k][0] - s[p], dy = v[p][k][1] - s[p], dz = v[p][k][2] - s[p], dw = v[p][k][3] - s[p];
+        const float dx = centred(v[p][k][0], s[p], c), dy = centred(v[p][k][1], s[p], c + 1);
+        const float dz = centred(v[p][k][2], s[p], c + 2), dw = centred(v[p][k][3], s[p], c + 3);
         q[p] += (dx * dx + dy * dy) + (dz * dz + dw * dw);
       } else {
-        const float dx = v[p][k][0] - s[p], dy = v[p][k][1] - s[p];
+        const float dx = centred(v[p][k][0], s[p], c), dy = centred(v[p][k][1], s[p], c + 1);
         q[p] += dx * dx + dy * dy;
       }
     }
@@ -495,8 +504,7 @@ ln_patchify2_kernel(const float* __restrict__ x, const float* __restrict__ ln_w,
     }
 #pragma unroll
     for (int p = 0; p < 4; ++p) {
-      // each zero pad channel added mean^2 to q (exact no-op when c_real == C)
-      const float r = rsqrtf(fmaf(-(float)(C - c_real) * s[p], s[p], q[p]) / (float)c_real + eps);
+      const float r = rsqrtf(q[p] / (float)c_real + eps);
       float o[VW];
 #pragma unroll
       for (int e = 0; e < VW; ++e) o[e] = fmaf((v[p][k][e] - s[p]) * r, gw[e], gb[e]);

@@ -210,21 +210,23 @@ dwconv_ln_pp_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_con
     }
     PP_MARK(3);
     // ---- LayerNorm statistics of this warp's 64 channels (shuffles only) ----
-    constexpr float INV_W = 1.0f / 64.0f;
+    // Zero pad channels (c >= c_real, all in the last slice) are left out of the slice's mean and M2.
     // pixel (tile-local index) of value q of this thread: R2 maps q -> (row rp2 + q / 8, column xh8 + q % 8)
     const int vi = lane / LPP;
     const int pix = R2 ? (rp2 + (vi >> 3)) * TW + xh8 + (vi & 7) : row0 * TW + vi;
     float s_loc, m2_loc;
     {
+      const float inv_n = 1.0f / (float)min(CPC, c_real - c0);
+      const bool real_x = c0 + cl < c_real, real_y = c0 + cl + 1 < c_real;
       float a[NV];
 #pragma unroll
       for (int q = 0; q < NV; ++q) { const float2 t = f2_unpack(acc[q]); a[q] = t.x + t.y; }
       s_loc = lane_transpose_reduce<NV>(a, lane);
 #pragma unroll
       for (int q = 0; q < NV; ++q) {
-        const float m = __shfl_sync(0xffffffffu, s_loc, q * LPP) * INV_W;
+        const float m = __shfl_sync(0xffffffffu, s_loc, q * LPP) * inv_n;
         const float2 t = f2_unpack(acc[q]);
-        const float dx = t.x - m, dy = t.y - m;
+        const float dx = real_x ? t.x - m : 0.f, dy = real_y ? t.y - m : 0.f;
         a[q] = fmaf(dx, dx, dy * dy);
       }
       m2_loc = lane_transpose_reduce<NV>(a, lane);
@@ -252,13 +254,14 @@ dwconv_ln_pp_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_con
 #pragma unroll
       for (int r = 0; r < NR; ++r) tot += pv[r].x;
       const float mean_p = tot / (float)c_real;
+      // Chan combine over the real channels: slice r holds n_r = min(64, c_real - 64 r) of them
       float m2 = 0.f;
 #pragma unroll
       for (int r = 0; r < NR; ++r) {
-        const float d = pv[r].x * INV_W - mean_p;
-        m2 += fmaf(64.0f * d, d, pv[r].y);
+        const float n_r = (float)min(CPC, c_real - CPC * r);
+        const float d = pv[r].x / n_r - mean_p;
+        m2 += fmaf(n_r * d, d, pv[r].y);
       }
-      m2 = fmaf(-(float)(C - c_real) * mean_p, mean_p, m2);   // zero pad channels each added mean^2 (exact no-op when c_real == C)
       my_stats[pix] = make_float2(mean_p, rsqrtf(m2 / (float)c_real + eps));
     }
     PP_MARK(7);

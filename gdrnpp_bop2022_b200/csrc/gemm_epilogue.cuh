@@ -235,6 +235,8 @@ __device__ __forceinline__ void epilogue_tile(const GemmPlan& p, int m_tile, int
     }
     const int ln_n = p.ln_n > 0 ? p.ln_n : p.N;
     const float mean = sum / (float)ln_n;
+    // centred sum of squares over the ln_n real columns only: the zero pad columns are masked out of the pass (subtracting
+    // their (N - ln_n) * mean^2 afterwards cancels catastrophically when |mean| >> std)
     float sq = 0.f;
 #pragma unroll 1
     for (int c = 0; c < p.N; c += CH) {
@@ -242,9 +244,8 @@ __device__ __forceinline__ void epilogue_tile(const GemmPlan& p, int m_tile, int
       acc_load_chunk<BLOCK_N, CH>(tmem_row + c, v);
       load_vec<CH>(p.bias, c, p.N, bias);
 #pragma unroll
-      for (int j = 0; j < CH; ++j) { float d = v[j] + bias[j] - mean; sq = fmaf(d, d, sq); }
+      for (int j = 0; j < CH; ++j) { const float d = c + j < ln_n ? v[j] + bias[j] - mean : 0.f; sq = fmaf(d, d, sq); }
     }
-    sq = fmaf(-(float)(p.N - ln_n) * mean, mean, sq);   // each zero pad column added mean^2 (exact no-op without padding)
     const float rstd = rsqrtf(sq / (float)ln_n + p.ln_eps);
 #pragma unroll 1
     for (int c = 0; c < p.N; c += CH) {

@@ -448,8 +448,114 @@ int pick_bn(int N, long long M) {
 
 void reset_plan(GemmPlan& p) { memset(&p, 0, sizeof(p)); }
 
+// run_stage names: true when `name` is `prefix` followed by a decimal index (and, with j, "_" and a second one); no sign,
+// no leading zeros
+bool stage_index(const char* name, const char* prefix, int* i, int* j = nullptr) {
+  const size_t l = strlen(prefix);
+  if (strncmp(name, prefix, l)) return false;
+  const char* p = name + l;
+  auto number = [&p](int* v) {
+    if (*p < '0' || *p > '9' || (p[0] == '0' && p[1] >= '0' && p[1] <= '9')) return false;
+    int x = 0;
+    for (int n = 0; *p >= '0' && *p <= '9'; ++n, ++p) {
+      if (n == 6) return false;
+      x = 10 * x + (*p - '0');
+    }
+    *v = x;
+    return true;
+  };
+  if (!number(i)) return false;
+  if (j && (*p++ != '_' || !number(j))) return false;
+  return *p == 0;
+}
+
 // GroupNorm sums of head layer i (0: deconv, 1..6: head convs, 7..9: Patch-PnP convs)
 double* stat_slot(const Workspace& w, int B, int i) { return w.gn_stats + (size_t)i * B * 32 * 2; }
+
+// ---------------- ConvNeXt backbone, one function per stage ----------------
+// The residual stream lives in w.X (fp32 NHWC, stored width cp[s]); each stage updates it in place.  gdrn_model_forward
+// runs them in order; gdrn_model_run_stage runs one of them on its own.
+
+// stem: roi_img [B,3,256,256] -> 4x4/s4 conv as GEMM (K=48 padded to 64) + bias + LayerNorm2d in the epilogue -> w.X [B,64,64,cp0]
+int stage_stem(GdrnModel* m, const Workspace& w, int B, const float* roi_img, cudaStream_t st) {
+  const int PR = m->precise, S = PR ? 2 : 1;
+  const int C0 = m->arch.dims[0], C0p = m->arch.cp[0];
+  const long long M0 = (long long)B * 64 * 64;
+  RCP(2, launch_stem_patchify(roi_img, w.A, B, 256, 256, PR, st));
+  if (C0p != 128) {   // convnext_base (128) and tiny / small (96 stored 128 wide: pad rows of stem_w are zero)
+    gdrn_set_last_error(__FILE__, __LINE__, "forward: the fused stem epilogue needs a 128-wide (padded) first stage");
+    return GDRN_ERR_INVALID;
+  }
+  GemmPlan p;
+  reset_plan(p);
+  RC(plan_a2d(p, w.A, M0, 64, S));
+  RC(plan_b(p, m->stem_w, C0p, 64, 128, C0p, S));
+  if (PR) set_x3(p, 64, 64);
+  p.epi = EPI_BIAS_LN; p.out = w.X; p.ldo = C0p; p.bias = m->stem_b;
+  p.ln_w = m->stem_ln_w; p.ln_b = m->stem_ln_b; p.ln_eps = 1e-6f; p.ln_n = C0;
+  RCP(0, gemm_tc_launch(p, 128, st));
+  return GDRN_OK;
+}
+
+// downsample in front of stage s (1..3): LayerNorm2d + 2x2 patchify of w.X [B,2r,2r,cp[s-1]] into the operand w.A
+// [B*r*r, 4*cp[s-1]], then the 2x2/s2 conv as GEMM + bias into w.X [B,r,r,cp[s]], r = 64 >> s
+int stage_downsample(GdrnModel* m, const Workspace& w, int B, int s, cudaStream_t st) {
+  const Arch& a = m->arch;
+  const int PR = m->precise, S = PR ? 2 : 1;
+  const int C = a.cp[s], Ci = a.cp[s - 1];
+  const int res = 64 >> s;
+  RCP(2, launch_ln_patchify2(w.X, m->down[s].ln_w, m->down[s].ln_b, w.A, B, 2 * res, 2 * res, Ci, 1e-6f, PR, st, a.dims[s - 1]));
+  const long long M = (long long)B * res * res;
+  GemmPlan p;
+  reset_plan(p);
+  RC(plan_a2d(p, w.A, M, 4 * Ci, S));
+  const int bn = pick_bn(C, M);
+  RC(plan_b(p, m->down[s].w, C, 4 * Ci, bn, C, S));
+  if (PR) set_x3(p, 4 * Ci, 4 * Ci);
+  p.epi = EPI_STORE; p.out_f32 = 1; p.out = w.X; p.ldo = C; p.bias = m->down[s].b;
+  RCP(0, gemm_tc_launch(p, bn, st));
+  return GDRN_OK;
+}
+
+// block i of stage s on w.X [B,r,r,cp[s]], r = 64 >> s: depthwise 7x7 + LayerNorm into the operand w.A [B*r*r, cp[s]], then
+// the MLP fc1 -> GELU -> fc2 -> *gamma -> +residual back into w.X (one fused kernel where supported, else two GEMMs via w.Hb)
+int stage_block(GdrnModel* m, const Workspace& w, int B, int s, int i, cudaStream_t st) {
+  const Arch& a = m->arch;
+  const int PR = m->precise, S = PR ? 2 : 1;
+  const int gelu_mode = PR ? 3 : m->gelu_mode;
+  const int res = 64 >> s;
+  const int Cr = a.dims[s];   // channels of the reference model
+  const int C = a.cp[s];      // stored width (pad channels are zero)
+  const int H4 = 4 * Cr;      // hidden width of the MLP
+  const long long M = (long long)B * res * res;
+  const BlockW& bw = m->blocks[s][i];
+  RCP(1, launch_dwconv_ln(w.X, bw.dw_w, bw.dw_b, bw.ln_w, bw.ln_b, w.A, B, res, res, C, 1e-6f, PR, st, Cr));
+  if (!PR && m->fuse_mlp && m->gelu_mode == 1 && Cr == C && mlp_fused_supported(C, M)) {
+    // stage 0: fc1 -> GELU -> fc2 -> residual in one kernel (no 4C-wide Hb round trip through HBM)
+    RCP(0, mlp_fused_launch(w.A, bw.fc1_w, bw.fc1_b, bw.fc2_w, bw.fc2_b, bw.gamma, w.X, M, C, st));
+    return GDRN_OK;
+  }
+  if (PR && m->fuse_mlp_x3 && Cr == C && mlp_fused_x3_supported(C, M)) {
+    RCP(0, mlp_fused_x3_launch(w.A, bw.fc1_w, bw.fc1_b, bw.fc2_w, bw.fc2_b, bw.gamma, w.X, M, C, st));
+    return GDRN_OK;
+  }
+  GemmPlan p;
+  reset_plan(p);
+  RC(plan_a2d(p, w.A, M, C, S));
+  const int bn1 = pick_bn(H4, M);
+  RC(plan_b(p, bw.fc1_w, H4, C, bn1, H4, S));
+  if (PR) set_x3(p, C, C);
+  p.epi = EPI_GELU; p.gelu_mode = gelu_mode; p.out = w.Hb; p.ldo = S * H4; p.bias = bw.fc1_b;
+  RCP(0, gemm_tc_launch(p, bn1, st));
+  reset_plan(p);
+  RC(plan_a2d(p, w.Hb, M, H4, S));
+  const int bn2 = pick_bn(C, M);
+  RC(plan_b(p, bw.fc2_w, C, H4, bn2, C, S));
+  if (PR) set_x3(p, H4, H4);
+  p.epi = EPI_RESID; p.out_f32 = 1; p.out = w.X; p.resid = w.X; p.ldo = C; p.bias = bw.fc2_b; p.gamma = bw.gamma;
+  RCP(0, gemm_tc_launch(p, bn2, st));
+  return GDRN_OK;
+}
 
 // ---------------- geometry head and Patch-PnP, one function per stage ----------------
 // gdrn_model_forward runs them in this order; gdrn_model_run_stage runs one of them on its own.
@@ -705,77 +811,13 @@ extern "C" int gdrn_model_forward(GdrnModel* m, const float* roi_img, const int6
   m->prof_cat.clear();
   GDRN_CHECK_CUDA(cudaMemsetAsync(w.gn_stats, 0, w.zero_bytes, st));   // GroupNorm sums
 
-  GemmPlan p;
-  auto reset = [&]() { memset(&p, 0, sizeof(p)); p.ldo = 0; };
   const int PR = m->precise;
-  const int S = PR ? 2 : 1;
-  const int gelu_mode = PR ? 3 : m->gelu_mode;
 
-  // ---------------- stem: 4x4/s4 conv as GEMM (K=48 padded to 64) + bias + LayerNorm2d in the epilogue ----------------
-  const long long M0 = (long long)B * 64 * 64;
-  RCP(2, launch_stem_patchify(roi_img, w.A, B, 256, 256, PR, st));
-  {
-    const int C0 = a.dims[0], C0p = a.cp[0];
-    reset();
-    RC(plan_a2d(p, w.A, M0, 64, S));
-    if (C0p == 128) {   // convnext_base (128) and tiny / small (96 stored 128 wide: pad rows of stem_w are zero)
-      RC(plan_b(p, m->stem_w, C0p, 64, 128, C0p, S));
-      if (PR) set_x3(p, 64, 64);
-      p.epi = EPI_BIAS_LN; p.out = w.X; p.ldo = C0p; p.bias = m->stem_b;
-      p.ln_w = m->stem_ln_w; p.ln_b = m->stem_ln_b; p.ln_eps = 1e-6f; p.ln_n = C0;
-      RCP(0, gemm_tc_launch(p, 128, st));
-    } else {
-      gdrn_set_last_error(__FILE__, __LINE__, "forward: the fused stem epilogue needs a 128-wide (padded) first stage");
-      return GDRN_ERR_INVALID;
-    }
-  }
-  // ---------------- stages ----------------
-  int res = 64;
+  // ---------------- ConvNeXt backbone ----------------
+  RC(stage_stem(m, w, B, roi_img, st));
   for (int s = 0; s < 4; ++s) {
-    const int Cr = a.dims[s];   // channels of the reference model
-    const int C = a.cp[s];      // stored width (pad channels are zero)
-    if (s > 0) {
-      const int Ci = a.cp[s - 1];
-      RCP(2, launch_ln_patchify2(w.X, m->down[s].ln_w, m->down[s].ln_b, w.A, B, res, res, Ci, 1e-6f, PR, st, a.dims[s - 1]));
-      res /= 2;
-      const long long M = (long long)B * res * res;
-      reset();
-      RC(plan_a2d(p, w.A, M, 4 * Ci, S));
-      const int bn = pick_bn(C, M);
-      RC(plan_b(p, m->down[s].w, C, 4 * Ci, bn, C, S));
-      if (PR) set_x3(p, 4 * Ci, 4 * Ci);
-      p.epi = EPI_STORE; p.out_f32 = 1; p.out = w.X; p.ldo = C; p.bias = m->down[s].b;
-      RCP(0, gemm_tc_launch(p, bn, st));
-    }
-    const int H4 = 4 * Cr;      // hidden width of the MLP
-    const long long M = (long long)B * res * res;
-    for (int i = 0; i < a.depths[s]; ++i) {
-      const BlockW& bw = m->blocks[s][i];
-      RCP(1, launch_dwconv_ln(w.X, bw.dw_w, bw.dw_b, bw.ln_w, bw.ln_b, w.A, B, res, res, C, 1e-6f, PR, st, Cr));
-      if (!PR && m->fuse_mlp && m->gelu_mode == 1 && Cr == C && mlp_fused_supported(C, M)) {
-        // stage 0: fc1 -> GELU -> fc2 -> residual in one kernel (no 4C-wide Hb round trip through HBM)
-        RCP(0, mlp_fused_launch(w.A, bw.fc1_w, bw.fc1_b, bw.fc2_w, bw.fc2_b, bw.gamma, w.X, M, C, st));
-        continue;
-      }
-      if (PR && m->fuse_mlp_x3 && Cr == C && mlp_fused_x3_supported(C, M)) {
-        RCP(0, mlp_fused_x3_launch(w.A, bw.fc1_w, bw.fc1_b, bw.fc2_w, bw.fc2_b, bw.gamma, w.X, M, C, st));
-        continue;
-      }
-      reset();
-      RC(plan_a2d(p, w.A, M, C, S));
-      const int bn1 = pick_bn(H4, M);
-      RC(plan_b(p, bw.fc1_w, H4, C, bn1, H4, S));
-      if (PR) set_x3(p, C, C);
-      p.epi = EPI_GELU; p.gelu_mode = gelu_mode; p.out = w.Hb; p.ldo = S * H4; p.bias = bw.fc1_b;
-      RCP(0, gemm_tc_launch(p, bn1, st));
-      reset();
-      RC(plan_a2d(p, w.Hb, M, H4, S));
-      const int bn2 = pick_bn(C, M);
-      RC(plan_b(p, bw.fc2_w, C, H4, bn2, C, S));
-      if (PR) set_x3(p, H4, H4);
-      p.epi = EPI_RESID; p.out_f32 = 1; p.out = w.X; p.resid = w.X; p.ldo = C; p.bias = bw.fc2_b; p.gamma = bw.gamma;
-      RCP(0, gemm_tc_launch(p, bn2, st));
-    }
+    if (s > 0) RC(stage_downsample(m, w, B, s, st));
+    for (int i = 0; i < a.depths[s]; ++i) RC(stage_block(m, w, B, s, i, st));
   }
   const int C3 = a.cp[3];
   if (PR) RCP(2, launch_cast_split(w.X, w.feat, (long long)B * 64, C3, st));
@@ -872,15 +914,21 @@ extern "C" int gdrn_model_run_stage(GdrnModel* m, const char* stage, int batch, 
     gdrn_set_last_error(__FILE__, __LINE__, "run_stage: workspace too small");
     return GDRN_ERR_STATE;
   }
-  // stage index: "head_conv0".."head_conv5" / "pnp_conv0".."pnp_conv2"
-  auto indexed = [stage](const char* prefix, int n) {
-    const size_t l = strlen(prefix);
-    return (!strncmp(stage, prefix, l) && stage[l] >= '0' && stage[l] < '0' + n && stage[l + 1] == 0) ? stage[l] - '0' : -1;
-  };
-  const int li = indexed("head_conv", 6), pi = indexed("pnp_conv", 3);
+  const Arch& a = m->arch;
+  // indexed stages: "head_conv<i>", "pnp_conv<i>", "down<s>", "block<s>_<i>"
+  int li = -1, pi = -1, ds = -1, bs = -1, bi = -1;
+  const bool stem = !strcmp(stage, "stem");
+  const bool down = stage_index(stage, "down", &ds), block = stage_index(stage, "block", &bs, &bi);
+  const bool head_conv = stage_index(stage, "head_conv", &li), pnp_conv = stage_index(stage, "pnp_conv", &pi);
   const bool deconv = !strcmp(stage, "deconv"), out_conv = !strcmp(stage, "out_conv"), pnp_fc = !strcmp(stage, "pnp_fc");
-  GDRN_REQUIRE(deconv || li >= 0 || out_conv || pi >= 0 || pnp_fc, "run_stage: unknown stage");
-  GDRN_REQUIRE(!(out_conv || pnp_fc) || (!raw_out && !gn_stats_out), "run_stage: this stage has no conv output / GroupNorm sums");
+  GDRN_REQUIRE(stem || down || block || deconv || head_conv || out_conv || pnp_conv || pnp_fc, "run_stage: unknown stage");
+  GDRN_REQUIRE(!head_conv || li < 6, "run_stage: head_conv index out of range (0..5)");
+  GDRN_REQUIRE(!pnp_conv || pi < 3, "run_stage: pnp_conv index out of range (0..2)");
+  GDRN_REQUIRE(!down || (ds >= 1 && ds <= 3), "run_stage: down index out of range (1..3)");
+  GDRN_REQUIRE(!block || (bs <= 3 && bi < a.depths[bs]), "run_stage: block index out of range for this arch");
+  const bool backbone = stem || down || block;
+  GDRN_REQUIRE(!(stem || out_conv || pnp_fc) || !raw_out, "run_stage: this stage has no conv output / operand");
+  GDRN_REQUIRE(!(backbone || out_conv || pnp_fc) || !gn_stats_out, "run_stage: this stage has no GroupNorm sums");
   if (out_conv) {
     GDRN_REQUIRE(roi_extents && roi_coord_2d, "run_stage: out_conv needs roi_extents and roi_coord_2d");
     GDRN_REQUIRE(roi_classes || m->num_classes == 1, "run_stage: roi_classes is NULL but the head is class-aware");
@@ -896,22 +944,40 @@ extern "C" int gdrn_model_run_stage(GdrnModel* m, const char* stage, int batch, 
   auto encode = [&](__nv_bfloat16* dst, long long rows, int C) {
     return PR ? launch_cast_split(in, dst, rows, C, st) : launch_cast_bf16(in, dst, rows * C, st);
   };
-  auto decode = [&](const __nv_bfloat16* src, long long rows, int C) {
-    return PR ? launch_split_to_f32(src, out, rows, C, st) : launch_bf16_to_f32(src, out, rows * C, st);
+  auto decode_to = [&](float* dst, const __nv_bfloat16* src, long long rows, int C) {
+    return PR ? launch_split_to_f32(src, dst, rows, C, st) : launch_bf16_to_f32(src, dst, rows * C, st);
   };
+  auto decode = [&](const __nv_bfloat16* src, long long rows, int C) { return decode_to(out, src, rows, C); };
   auto copy_f32 = [&](float* dst, const void* src, long long n) {
     GDRN_CHECK_CUDA(cudaMemcpyAsync(dst, src, n * 4, cudaMemcpyDeviceToDevice, st));
     return GDRN_OK;
   };
   const void* raw = nullptr;   // pre-GroupNorm conv output (fp32 in split-bf16 mode, bf16 otherwise) and its element count
   long long raw_n = 0;
-  if (deconv) {
+  // backbone: the fp32 residual stream w.X is the stage's input and output in both modes; raw_out is the GEMM A operand
+  // the LayerNorm kernel wrote (w.A)
+  if (stem) {
+    RC(stage_stem(m, w, B, in, st));
+    RC(copy_f32(out, w.X, (long long)B * 64 * 64 * a.cp[0]));
+  } else if (down) {
+    const int r = 64 >> ds, Ci = a.cp[ds - 1];
+    RC(copy_f32(w.X, in, (long long)B * 4 * r * r * Ci));
+    RC(stage_downsample(m, w, B, ds, st));
+    RC(copy_f32(out, w.X, (long long)B * r * r * a.cp[ds]));
+    if (raw_out) RC(decode_to(raw_out, w.A, (long long)B * r * r, 4 * Ci));
+  } else if (block) {
+    const int r = 64 >> bs, C = a.cp[bs];
+    RC(copy_f32(w.X, in, (long long)B * r * r * C));
+    RC(stage_block(m, w, B, bs, bi, st));
+    RC(copy_f32(out, w.X, (long long)B * r * r * C));
+    if (raw_out) RC(decode_to(raw_out, w.A, (long long)B * r * r, C));
+  } else if (deconv) {
     const int C3 = m->arch.cp[3];
     RC(encode(w.feat, (long long)B * 64, C3));
     RC(stage_deconv(m, w, B, w.feat, w.P, st));
     RC(decode(w.P, (long long)B * 256, 256));
     raw = w.R; raw_n = (long long)B * 256 * 256;
-  } else if (li >= 0) {
+  } else if (head_conv) {
     const int h = 16 << (li / 2), ho = (li == 1 || li == 3) ? 2 * h : h;
     RC(encode(w.P, (long long)B * h * h, 256));
     RC(stage_head_conv(m, w, B, li, w.P, w.Q, st));
@@ -921,7 +987,7 @@ extern "C" int gdrn_model_run_stage(GdrnModel* m, const char* stage, int batch, 
     RC(encode(w.P, (long long)B * 4096, 256));
     RC(stage_out_conv(m, w, B, w.P, roi_classes, roi_extents, roi_coord_2d, maps, st));
     RC(decode(w.pnp_in, (long long)B * 4096, 128));
-  } else if (pi >= 0) {
+  } else if (pnp_conv) {
     const int ires = 64 >> pi, ores = ires / 2;
     __nv_bfloat16* src = pi == 0 ? w.pnp_in : w.pP;
     RC(encode(src, (long long)B * ires * ires, 128));
@@ -935,7 +1001,7 @@ extern "C" int gdrn_model_run_stage(GdrnModel* m, const char* stage, int batch, 
     RC(stage_pnp_fc(m, w, B, st));
     RC(copy_f32(out, w.fout, (long long)B * 16));
   }
-  if (raw_out) {
+  if (raw_out && raw) {
     if (PR) RC(copy_f32(raw_out, raw, raw_n));
     else RC(launch_bf16_to_f32(reinterpret_cast<const __nv_bfloat16*>(raw), raw_out, raw_n, st));
   }

@@ -15,6 +15,7 @@ forward raises.
 """
 import ctypes
 import os
+import re
 from types import SimpleNamespace
 
 import torch
@@ -344,33 +345,52 @@ class GDRN_DoubleMask(nn.Module):
         return dst[:n]
 
     def run_stage(self, stage, x, roi_classes=None, roi_extents=None, roi_coord_2d=None, want_raw=False, want_maps=False):
-        """One geometry-head / Patch-PnP stage of the forward on the fp32 NHWC CUDA tensor ``x`` (gdrn_model_run_stage in
-        include/gdrn_b200.h lists the stages and shapes).  Returns ``{"out"}`` plus, when ``want_raw``, ``"raw"`` (the conv
-        output before GroupNorm) and ``"gn_stats"`` (float64 [10,B,32,2]), and, when ``want_maps``, the six NCHW maps of
-        "out_conv"."""
+        """One backbone / geometry-head / Patch-PnP stage of the forward on the fp32 CUDA tensor ``x`` (NCHW roi_img for
+        "stem", NHWC otherwise; gdrn_model_run_stage in include/gdrn_b200.h lists the stages and shapes).  Returns
+        ``{"out"}`` plus, when ``want_raw``, ``"raw"`` (head stages: the conv output before GroupNorm; "down<s>" /
+        "block<s>_<i>": the GEMM operand written by the LayerNorm kernel) and, for the head stages, ``"gn_stats"`` (float64
+        [10,B,32,2]), and, when ``want_maps``, the six NCHW maps of "out_conv"."""
         dev = x.device
         B = x.shape[0]
         x = x.detach().to(dtype=torch.float32).contiguous()
-        if stage == "deconv":
-            out_shape, raw_shape = (B, 16, 16, 256), (B, 16, 16, 256)
-        elif stage.startswith("head_conv"):
+        depths, dims = CONVNEXT_ARCH[self.arch]
+        cp = [(d + 63) // 64 * 64 for d in dims]   # stored stage widths (zero pad channels)
+        m_down = re.fullmatch(r"down([1-3])", stage)
+        m_block = re.fullmatch(r"block([0-3])_(0|[1-9][0-9]*)", stage)
+        gn = False
+        if stage == "stem":
+            out_shape, raw_shape = (B, 64, 64, cp[0]), None
+        elif m_down:
+            s = int(m_down.group(1))
+            r = 64 >> s
+            out_shape, raw_shape = (B, r, r, cp[s]), (B, r, r, 4 * cp[s - 1])
+        elif m_block and int(m_block.group(2)) < depths[int(m_block.group(1))]:
+            s = int(m_block.group(1))
+            r = 64 >> s
+            out_shape = raw_shape = (B, r, r, cp[s])
+        elif stage == "deconv":
+            out_shape, raw_shape, gn = (B, 16, 16, 256), (B, 16, 16, 256), True
+        elif re.fullmatch(r"head_conv[0-5]", stage):
             li = int(stage[len("head_conv"):])
             h = 16 << (li // 2)
             ho = 2 * h if li in (1, 3) else h
-            out_shape, raw_shape = (B, ho, ho, 256), (B, h, h, 256)
+            out_shape, raw_shape, gn = (B, ho, ho, 256), (B, h, h, 256), True
         elif stage == "out_conv":
             out_shape, raw_shape = (B, 64, 64, 128), None
-        elif stage.startswith("pnp_conv"):
+        elif re.fullmatch(r"pnp_conv[0-2]", stage):
             r = 32 >> int(stage[len("pnp_conv"):])
-            out_shape, raw_shape = (B, r, r, 128), (B, r, r, 128)
+            out_shape, raw_shape, gn = (B, r, r, 128), (B, r, r, 128), True
         elif stage == "pnp_fc":
             out_shape, raw_shape = (B, 16), None
         else:
-            raise ValueError(f"unknown stage {stage!r}")
+            raise ValueError(f"unknown stage {stage!r} for {self.arch}")
         res = {"out": torch.empty(out_shape, dtype=torch.float32, device=dev)}
         if want_raw:
+            if raw_shape is None:
+                raise ValueError(f"stage {stage!r} has no conv output / operand to return")
             res["raw"] = torch.empty(raw_shape, dtype=torch.float32, device=dev)
-            res["gn_stats"] = torch.empty((10, B, 32, 2), dtype=torch.float64, device=dev)
+            if gn:
+                res["gn_stats"] = torch.empty((10, B, 32, 2), dtype=torch.float64, device=dev)
         maps = None
         if want_maps:
             for name, ch in (("mask", 1), ("full_mask", 1), ("coor_x", 1), ("coor_y", 1), ("coor_z", 1), ("region", 65)):

@@ -92,15 +92,23 @@ int gdrn_model_set_profiling(GdrnModel* m, int enable);
 int gdrn_model_get_profile(GdrnModel* m, float* ms_out, int* launches_out);
 
 /* debugging / parity hooks: copy an internal activation (after the last forward on the same workspace)
- * as fp32 into dst.  name: "conv_feat" ([B,8,8,C3] NHWC) | "stage0".."stage3" | "head16"|"head32"|"head64"
- * ([B,h,w,256] NHWC, post GN+GELU) | "pnp_in" ([B,64,64,128]) . Returns element count or <0. */
+ * as fp32 into dst.  name: "stage3_x" ([B,8,8,C3] NHWC, the fp32 backbone output) | "fc_out" ([B,16], rows 0-5 rot6d,
+ * 6-8 t_) | "conv_feat" ([B,8,8,C3], the bf16 backbone output) | "head64" ([B,64,64,256], last head conv after GN+GELU) |
+ * "pnp_in" ([B,64,64,128]) | "pnp_feat" ([B,8192]).  Split-bf16 mode reads "stage3_x" and "fc_out" only.
+ * C3 as in gdrn_model_run_stage.  Returns element count or <0. */
 int64_t gdrn_model_debug_read(GdrnModel* m, const char* name, int batch, float* dst, void* workspace, void* stream);
 
-/* Test / measurement entry: runs ONE geometry-head or Patch-PnP stage of gdrn_model_forward -- the same host function,
- * plans and kernels the forward launches -- on the model's packed weights, in a gdrn_model_workspace_bytes(m, batch)
- * workspace.  The fp32 input is first cast to the stage's operand format (bf16, or [hi | lo] split rows in split-bf16 mode);
- * the outputs are decoded to fp32 (hi + lo).  All tensors NHWC unless noted.
+/* Test / measurement entry: runs ONE backbone, geometry-head or Patch-PnP stage of gdrn_model_forward -- the same host
+ * function, plans and kernels the forward launches -- on the model's packed weights, in a gdrn_model_workspace_bytes(m, batch)
+ * workspace.  Head / Patch-PnP stages: the fp32 input is first cast to the stage's operand format (bf16, or [hi | lo] split
+ * rows in split-bf16 mode); the outputs are decoded to fp32 (hi + lo).  Backbone stages: the residual stream is fp32 in both
+ * modes, so input and output are copied unchanged.  All tensors NHWC unless noted.
  *   stage          in                       out
+ *   "stem"         [B,3,256,256] NCHW       [B,64,64,cp0]      4x4 s4 conv + LayerNorm2d
+ *   "down<s>"      [B,2r,2r,cp[s-1]],       [B,r,r,cp[s]]      LayerNorm2d + 2x2 s2 conv; raw_out: the GEMM operand
+ *                  s = 1..3, r = 64>>s                         [B,r,r,4*cp[s-1]] (LayerNorm output, 2x2 patch rows)
+ *   "block<s>_<i>" [B,r,r,cp[s]], r = 64>>s [B,r,r,cp[s]]      ConvNeXt block i of stage s (i < depth, e.g. "block2_26");
+ *                                                              raw_out: the GEMM operand [B,r,r,cp[s]] (dwconv + LayerNorm)
  *   "deconv"       [B,8,8,C3]               [B,16,16,256]      3x3 s2 transposed conv + GroupNorm + GELU
  *   "head_conv<i>" [B,h,h,256], i = 0..5,   [B,h',h',256]      3x3 conv + GroupNorm + GELU (+ bilinear x2 after i = 1, 3)
  *                  h = 16,16,32,32,64,64
@@ -108,7 +116,9 @@ int64_t gdrn_model_debug_read(GdrnModel* m, const char* name, int batch, float* 
  *                                                              zero pad); maps (optional, NCHW) as in gdrn_model_forward
  *   "pnp_conv<i>"  [B,2r,2r,128], r = 32>>i [B,r,r,128]        3x3 s2 conv + GroupNorm + GELU
  *   "pnp_fc"       [B,8,8,128]              [B,16]             fc1 -> fc2 -> fc_r | fc_t (rows 0-5 rot6d, 6-8 t_, rest 0)
- * C3 is the stored backbone width (1024 for convnext_base).  For the conv stages, raw_out (optional) receives the conv
+ * cp[s] is the stored width of backbone stage s: its channel count rounded up to a multiple of 64 (convnext_tiny / small:
+ * 128, 192, 384, 768 for 96, 192, 384, 768 channels); the pad channels are zero.  C3 = cp[3] (1024 for convnext_base).
+ * Backbone stages take no gn_stats_out.  For the head conv stages, raw_out (optional) receives the conv
  * output before GroupNorm (at the conv's resolution) and gn_stats_out (optional) the whole table of GroupNorm sums
  * [10][B][32][2] (layer: 0 deconv, 1-6 head convs, 7-9 Patch-PnP convs; per (image, group): sum, sum of squares), cleared
  * before the stage runs.  roi_classes / roi_extents / roi_coord_2d as in gdrn_model_forward, read by "out_conv" only.
