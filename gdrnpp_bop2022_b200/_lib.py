@@ -126,6 +126,12 @@ _SIGNATURES = {
     "coco_eval_accumulate_workspace_bytes": (c_size_t, [c_int]),
     "coco_eval_accumulate": (c_int, [c_void_p] * 8 + [c_int] * 6 + [c_void_p, c_int, c_void_p, c_int, c_void_p, c_size_t,
                                                                      c_void_p, c_void_p, c_void_p]),
+    "gdrn_mask_paste": (c_int, [c_void_p] + [c_int] * 4 + [c_void_p, c_int, c_int, c_float, c_void_p, c_void_p]),
+    "gdrn_mask_rle_max_chars": (c_size_t, [c_int, c_int]),
+    "gdrn_mask_rle_workspace_bytes": (c_size_t, [c_int] * 3),
+    "gdrn_mask_paste_rle": (c_int, [c_void_p, c_void_p] + [c_int] * 4 + [c_void_p, c_void_p, c_int, c_int, c_float, c_void_p,
+                                                                       c_size_t, c_void_p, c_size_t, c_void_p, c_void_p]),
+    "gdrn_rle_confusion": (c_int, [c_void_p, c_size_t, c_void_p, c_int, c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p]),
 }
 
 EXPORTED_SYMBOLS = tuple(_SIGNATURES.keys())

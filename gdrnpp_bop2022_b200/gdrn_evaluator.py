@@ -355,17 +355,55 @@ def gdrn_inference_on_dataset(cfg, model, datasets_root, *, train_obj_ids=None, 
     events), wall, and the batch count."""
     device = torch.device(device)
     ts = test_set or TestSet(cfg, datasets_root, train_obj_ids)
+    with_depth = bool(cfg_get(cfg, "TEST.USE_DEPTH_REFINE", False)) and not cfg_get(cfg, "TEST.USE_PNP", False)
+    meshes = ts.meshes(device) if with_depth else None
+    mask_thr = float(cfg_get(cfg, "MODEL.POSE_NET.GEO_HEAD.MASK_THR_TEST", 0.5))
+    return _run_batches(cfg, model, ts, _PoseRows(cfg, ts, meshes, mask_thr), with_depth, max_batch, num_workers,
+                        use_cuda_graph, device, stats)
+
+
+class _PoseRows:
+    """Output step of the test loop: GDRN_Evaluator.process's post-processing dispatch, one D2H copy of the poses, one
+    result row per ROI."""
+
+    def __init__(self, cfg, ts, meshes, mask_thr):
+        self.cfg, self.ts, self.meshes, self.mask_thr = cfg, ts, meshes, mask_thr
+        self.pose_dev = {}
+
+    def post(self, inp, out, n, slot, hw):
+        rot, trans = postprocess(self.cfg, inp, out, self.meshes, self.mask_thr)
+        pose = self.pose_dev.get(n)
+        if pose is None:
+            pose = self.pose_dev[n] = torch.empty((n, 3, 4), dtype=torch.float32, device=rot.device)
+        pose[:, :, :3].copy_(rot)
+        pose[:, :, 3].copy_(trans)
+        return pose
+
+    def d2h(self, pose):
+        host_pose = torch.empty(tuple(pose.shape), dtype=torch.float32, pin_memory=True)
+        host_pose.copy_(pose, non_blocking=True)
+        return host_pose
+
+    def empty(self):
+        return torch.empty((0, 3, 4))
+
+    def rows(self, imgs, host_pose, batch_seconds):
+        return batch_rows(self.ts.images, imgs, host_pose.numpy(), batch_seconds)
+
+
+def _run_batches(cfg, model, ts, output, with_depth, max_batch, num_workers, use_cuda_graph, device, stats):
+    """The batched loop shared by the test and save-results loops; ``output`` is the per-batch output step:
+    post(inp, out, n, slot, (H, W)) enqueues its device work after the forward (slot: the batch's double-buffer index),
+    d2h(state) enqueues the copies to the host, and rows(imgs, payload, batch_seconds) turns them into results once the
+    batch's copies are done (empty() is the payload of a batch without ROIs)."""
     if not isinstance(model, PerObjectGDRN) and model.class_aware and model.num_classes != len(ts.obj_ids):
         raise ValueError(f"MODEL.POSE_NET.NUM_CLASSES={model.num_classes} but dataset {ts.dataset!r} has "
                          f"{len(ts.obj_ids)} objects")
     if max_batch is None:
         max_batch = max(m.max_batch for m in model.members.values()) if isinstance(model, PerObjectGDRN) else model.max_batch
-    with_depth = bool(cfg_get(cfg, "TEST.USE_DEPTH_REFINE", False)) and not cfg_get(cfg, "TEST.USE_PNP", False)
-    meshes = ts.meshes(device) if with_depth else None
     in_res, out_res = cfg_get(cfg, "MODEL.POSE_NET.INPUT_RES", 256), cfg_get(cfg, "MODEL.POSE_NET.OUTPUT_RES", 64)
     pix_mean, pix_std = cfg_get(cfg, "MODEL.PIXEL_MEAN", (0.0, 0.0, 0.0)), cfg_get(cfg, "MODEL.PIXEL_STD", (255.0, 255.0, 255.0))
     dzi = float(cfg_get(cfg, "INPUT.DZI_PAD_SCALE", 1.5))
-    mask_thr = float(cfg_get(cfg, "MODEL.POSE_NET.GEO_HEAD.MASK_THR_TEST", 0.5))
     records = ts.records
     if not records:
         return []
@@ -414,7 +452,7 @@ def gdrn_inference_on_dataset(cfg, model, datasets_root, *, train_obj_ids=None, 
         return imgs, n
 
     out_rows = []
-    pending = None   # the previous batch: (imgs, n, pinned poses, event after their D2H copy)
+    pending = None   # the previous batch: (imgs, payload of its D2H copies, event after them)
     tstat = {"h2d": [], "roi_build": [], "forward": [], "post": [], "d2h": []}
     pool = ThreadPoolExecutor(num_workers)
     feeder = ThreadPoolExecutor(1)
@@ -422,10 +460,10 @@ def gdrn_inference_on_dataset(cfg, model, datasets_root, *, train_obj_ids=None, 
     t_last = [t_start]
 
     def finish(p):
-        imgs, n, host_pose, done = p
+        imgs, payload, done = p
         done.synchronize()
         now = time.perf_counter()
-        out_rows.extend(batch_rows(ts.images, imgs, host_pose.numpy(), now - t_last[0]))
+        out_rows.extend(output.rows(imgs, payload, now - t_last[0]))
         t_last[0] = now
 
     try:
@@ -447,14 +485,13 @@ def gdrn_inference_on_dataset(cfg, model, datasets_root, *, train_obj_ids=None, 
             if timing:
                 e[1].record(stream)
             if n == 0:
-                host_pose = torch.empty((0, 3, 4))
+                payload = output.empty()
                 done = torch.cuda.Event()
                 done.record(stream)
             else:
                 st = static.get((n, with_depth))
                 if st is None:
                     st = static[(n, with_depth)] = roi_batch_buffers(n, device, in_res, out_res, with_depth)
-                    st["pose_dev"] = torch.empty((n, 3, 4), dtype=torch.float32, device=device)
                 d = stage.d
                 inp = roi_batch_inputs(d["images"], {"det_meta": d["det_meta"], "bbox_est": d["bbox_est"]}, d["K"],
                                        ts.extents(device), dzi, in_res, out_res, pix_mean, pix_std,
@@ -465,13 +502,10 @@ def gdrn_inference_on_dataset(cfg, model, datasets_root, *, train_obj_ids=None, 
                 out = _forward(model, inp, graphs, use_cuda_graph)
                 if timing:
                     e[3].record(stream)
-                rot, trans = postprocess(cfg, inp, out, meshes, mask_thr)
-                st["pose_dev"][:, :, :3].copy_(rot)
-                st["pose_dev"][:, :, 3].copy_(trans)
+                state = output.post(inp, out, n, bi % 2, keys[batches[bi][0]][:2])
                 if timing:
                     e[4].record(stream)
-                host_pose = torch.empty((n, 3, 4), dtype=torch.float32, pin_memory=True)
-                host_pose.copy_(st["pose_dev"], non_blocking=True)
+                payload = output.d2h(state)
                 done = torch.cuda.Event()
                 done.record(stream)
                 if timing:
@@ -480,7 +514,7 @@ def gdrn_inference_on_dataset(cfg, model, datasets_root, *, train_obj_ids=None, 
                         tstat[k].append((a, b))
             if pending is not None:
                 finish(pending)
-            pending = (imgs, n, host_pose, done)
+            pending = (imgs, payload, done)
         if pending is not None:
             finish(pending)
     finally:
@@ -493,7 +527,7 @@ def gdrn_inference_on_dataset(cfg, model, datasets_root, *, train_obj_ids=None, 
         stats["wall"] = time.perf_counter() - t_start
         stats["batches"] = len(batches)
         stats["images"] = len(records)
-        stats["rois"] = len(out_rows)
+        stats["rois"] = sum(len(a) for _, a in records)
     return out_rows
 
 
@@ -510,6 +544,145 @@ def batch_rows(images, imgs, poses, batch_seconds):
                          "R": poses[k, :, :3].astype(np.float64), "t": poses[k, :, 3].astype(np.float64), "time": t_img})
             k += 1
     return rows
+
+
+# ------------------------------------------------------------------------------------------------ save results
+def save_record(det, pose, mask_rle, full_mask_rle, use_pnp):
+    """One ROI's entry of results.pkl (gdrn_save_result_of_dataset, gdrn_evaluator.py:957-976): bbox_est is the
+    loader's float32 XYXY box; R / t are the network's float32 pose, or with TEST.USE_PNP misc.pnp_v2's float64 pose
+    (the float32 -100 sentinel where fewer than 4 points were selected)."""
+    x, y, w, h = np.asarray(det["bbox_est"], np.float32)
+    pose = np.asarray(pose, np.float32)
+    if use_pnp and not (pose == -100).all():
+        pose = pose.astype(np.float64)
+    return {"obj_id": det["obj_id"], "score": float(np.float32(det["score"])),
+            "bbox_est": np.array([x, y, x + w, y + h], np.float32), "mask": mask_rle, "full_mask": full_mask_rle,
+            "R": pose[:, :3].copy(), "t": pose[:, 3].copy()}
+
+
+class _SaveRecords:
+    """Output step of the save-results loop: the pose (TEST.USE_PNP: get_pnp_ransac_pose, i.e. pnp_ransac_from_maps;
+    else the network's; never depth refine) and both masks pasted and RLE-encoded on the device (gdrn_mask_paste_rle).
+    The [2n,2] string table travels with the poses; the string bytes follow in rows(), after the batch's event, from
+    this slot's device buffer (two slots: batch k + 1 is already running when batch k's strings are copied)."""
+
+    def __init__(self, cfg, ts, mask_thr, device):
+        from .native_ops import MaskRleBuffers, mask_prob_mode
+
+        self.ts, self.mask_thr = ts, mask_thr
+        self.use_pnp = bool(cfg_get(cfg, "TEST.USE_PNP", False))
+        # both masks use MASK_LOSS_TYPE, as get_out_mask(cfg, ...) does for the full mask too
+        self.loss_type = str(cfg_get(cfg, "MODEL.POSE_NET.LOSS_CFG.MASK_LOSS_TYPE", "L1"))
+        mask_prob_mode(self.loss_type)
+        self.bufs = [MaskRleBuffers(device), MaskRleBuffers(device)]
+        self.pose_dev = {}
+        self.side = torch.cuda.Stream(device)
+        self.host_chars = torch.empty(0, dtype=torch.uint8).pin_memory()
+
+    def post(self, inp, out, n, slot, hw):
+        from .native_ops import paste_masks_rle_launch
+
+        pose = self.pose_dev.get(n)
+        if pose is None:
+            pose = self.pose_dev[n] = torch.empty((n, 3, 4), dtype=torch.float32, device=out["rot"].device)
+        if self.use_pnp:
+            from .pnp_ransac import pnp_ransac_from_maps
+
+            pose.copy_(pnp_ransac_from_maps(out["coor_x"], out["coor_y"], out["coor_z"], out["mask"], inp["roi_coord_2d"],
+                                            inp["im_H"], inp["im_W"], inp["roi_extent"], inp["roi_cam"],
+                                            mask_thr=self.mask_thr))
+        else:
+            pose[:, :, :3].copy_(out["rot"])
+            pose[:, :, 3].copy_(out["trans"])
+        bufs = paste_masks_rle_launch(out["mask"], out["full_mask"], inp["roi_center"], inp["scale"], hw, self.mask_thr,
+                                      self.loss_type, self.bufs[slot])
+        return pose, bufs, n, hw
+
+    def d2h(self, state):
+        pose, bufs, n, hw = state
+        host_pose = torch.empty((n, 3, 4), dtype=torch.float32, pin_memory=True)
+        host_pose.copy_(pose, non_blocking=True)
+        host_table = torch.empty((2 * n, 2), dtype=torch.int64, pin_memory=True)
+        host_table.copy_(bufs.table[:2 * n], non_blocking=True)
+        return host_pose, host_table, bufs, hw
+
+    def empty(self):
+        return None
+
+    def rows(self, imgs, payload, batch_seconds):
+        if payload is None:
+            return []
+        from .native_ops import rle_dicts
+
+        host_pose, host_table, bufs, (H, W) = payload
+        table = host_table.numpy()
+        total = int(table[-1].sum())
+        if self.host_chars.numel() < total:
+            self.host_chars = torch.empty(total, dtype=torch.uint8).pin_memory()
+        with torch.cuda.stream(self.side):   # the batch's kernels are done (its event was waited on)
+            self.host_chars[:total].copy_(bufs.chars[:total], non_blocking=True)
+        self.side.synchronize()
+        rles = rle_dicts(table, self.host_chars[:total].numpy(), H, W)
+        n = len(rles) // 2
+        poses = host_pose.numpy()
+        out, k = [], 0
+        for idx, anns in imgs:
+            sid, iid = self.ts.images[idx]
+            for a in anns:
+                out.append((f"{sid}/{iid}", save_record(a, poses[k], rles[k], rles[n + k], self.use_pnp)))
+                k += 1
+        return out
+
+
+def save_results_dir(cfg, per_object=False):
+    """do_save_results's directory (engine/engine.py:121-131): <OUTPUT_DIR>/inference_<basename(MODEL.WEIGHTS) up to its
+    first ".">/<DATASETS.TEST[0]>; per_object (several per-object checkpoints in one run): inference_per_object."""
+    tests = list(cfg_get(cfg, "DATASETS.TEST", ()) or ())
+    if len(tests) != 1:
+        raise ValueError(f"DATASETS.TEST={tests!r}: the save-results loop writes one dataset's results.pkl; "
+                         "give exactly one DATASETS.TEST entry")
+    model_name = "per_object" if per_object else os.path.basename(str(cfg_get(cfg, "MODEL.WEIGHTS", ""))).split(".")[0]
+    return os.path.join(str(cfg_get(cfg, "OUTPUT_DIR", "output")), f"inference_{model_name}", tests[0])
+
+
+def write_results_pkl(result, output_dir):
+    """mmcv.dump(result, <dir>/results.pkl): pickle protocol 2."""
+    import pickle
+
+    os.makedirs(output_dir, exist_ok=True)
+    path = os.path.join(output_dir, "results.pkl")
+    with open(path, "wb") as f:
+        pickle.dump(result, f, protocol=2)
+    return path
+
+
+@torch.no_grad()
+def gdrn_save_result_of_dataset(cfg, model, datasets_root, output_dir, *, train_obj_ids=None, max_batch=None,
+                                num_workers=8, use_cuda_graph=True, device="cuda", test_set=None, stats=None):
+    """The save-results loop (save_gdrn.sh -> TEST.SAVE_RESULTS_ONLY -> gdrn_save_result_of_dataset,
+    gdrn_evaluator.py:812-1119) on the batching, decode pool, ROI build, CUDA graphs and D2H pipeline of the test loop.
+    -> {"scene_id/im_id": [{obj_id, score, bbox_est, mask, full_mask, R, t}, ...]} in image order, then ROI order (an
+    image without ROIs has no key), also written to <output_dir>/results.pkl.  model must return the geometry maps
+    (built from a config with TEST.SAVE_RESULTS_ONLY=True or TEST.USE_PNP=True)."""
+    if not model.wants_maps:
+        raise ValueError("gdrn_save_result_of_dataset needs the mask maps: build the model from a config with "
+                         "TEST.SAVE_RESULTS_ONLY=True")
+    device = torch.device(device)
+    ts = test_set or TestSet(cfg, datasets_root, train_obj_ids)
+    mask_thr = float(cfg_get(cfg, "MODEL.POSE_NET.GEO_HEAD.MASK_THR_TEST", 0.5))
+    rows = _run_batches(cfg, model, ts, _SaveRecords(cfg, ts, mask_thr, device), False, max_batch, num_workers,
+                        use_cuda_graph, device, stats)
+    result = results_dict(rows)
+    write_results_pkl(result, output_dir)
+    return result
+
+
+def results_dict(rows):
+    """[("scene_id/im_id", record), ...] in image order, then ROI order -> {key: [record, ...]} in the same order."""
+    result = {}
+    for key, rec in rows:
+        result.setdefault(key, []).append(rec)
+    return result
 
 
 # ------------------------------------------------------------------------------------------------ results

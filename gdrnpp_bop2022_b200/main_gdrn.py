@@ -7,6 +7,12 @@
 DATASETS.DET_FILES_TEST that start with ``datasets/`` are resolved against it.  Per-object (class-agnostic) checkpoints:
 ``MODEL.WEIGHTS=<obj_id>=<ckpt> <obj_id>=<ckpt> ...`` runs every object's network in one pass; a single per-object
 checkpoint names its object with ``--obj_ids``.
+
+``--opts TEST.SAVE_RESULTS_ONLY=True`` runs the reference's save_gdrn.sh instead: gdrn_save_result_of_dataset writes
+results.pkl (per ROI the pose and the visible / amodal masks as COCO RLE) to
+``<OUTPUT_DIR>/inference_<model name>/<DATASETS.TEST[0]>`` (or ``--output_dir``), with exactly one DATASETS.TEST
+entry.  Per-object checkpoints given together write one results.pkl under ``inference_per_object/`` (the reference
+runs one process per object).
 """
 import argparse
 import ast
@@ -80,8 +86,21 @@ def main(argv=None):
     if not weights:
         raise SystemExit("MODEL.WEIGHTS is not set (--opts MODEL.WEIGHTS=CKPT)")
     train_obj_ids = [int(x) for x in args.obj_ids.split(",")] if args.obj_ids else (sorted(per_obj) if per_obj else None)
+    save_only = bool(G.cfg_get(cfg, "TEST.SAVE_RESULTS_ONLY", False))
+    if save_only:
+        try:
+            save_dir = G.save_results_dir(cfg, per_object=bool(per_obj))
+        except ValueError as e:
+            raise SystemExit(str(e))
+        save_dir = args.output_dir or save_dir
     ts = G.TestSet(cfg, args.datasets_root, train_obj_ids)
     model = G.build_model(cfg, weights, obj_ids=ts.obj_ids, precision=args.precision, max_batch=args.max_batch)
+    if save_only:
+        G.gdrn_save_result_of_dataset(cfg, model, args.datasets_root, save_dir, train_obj_ids=train_obj_ids,
+                                      max_batch=args.max_batch, test_set=ts)
+        path = os.path.join(save_dir, "results.pkl")
+        print("wrote", path)
+        return {"results": path}
     records = G.gdrn_inference_on_dataset(cfg, model, args.datasets_root, train_obj_ids=train_obj_ids,
                                           max_batch=args.max_batch, test_set=ts)
     out_dir = args.output_dir or os.path.join(str(G.cfg_get(cfg, "OUTPUT_DIR", "output")), "inference",

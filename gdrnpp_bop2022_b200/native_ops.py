@@ -613,3 +613,134 @@ def yolox_letterbox(images, test_size, out=None, workspace=None):
     _lib.check(_lib.lib().yolox_letterbox(_lib.ptr(images), N, H, W, C, th, tw, _lib.ptr(out), _lib.ptr(workspace),
                                           workspace.numel(), _lib.current_stream()), "yolox_letterbox")
     return out
+
+
+# ---------------------------------------------------------------------------------------------------------------
+# Image-space masks and COCO RLE (detectron2 paste_masks_in_image, pycocotools encode; the decode of the reference's
+# mask tools): csrc/mask_rle.cu
+# ---------------------------------------------------------------------------------------------------------------
+def mask_prob_mode(mask_loss_type):
+    """get_out_mask's probability of a MASK_LOSS_TYPE as the kernel's mode: 1 = L1 min-max, 2 = sigmoid."""
+    if mask_loss_type == "L1":
+        return 1
+    if mask_loss_type in ("BCE", "RW_BCE", "dice"):
+        return 2
+    raise NotImplementedError(mask_loss_type)
+
+
+def _check_threshold(threshold):
+    if not float(threshold) > 0:
+        raise ValueError(f"threshold must be > 0, got {threshold} (detectron2 returns uint8 probabilities otherwise)")
+
+
+@_lib.on_device(0)
+def paste_masks_in_image(masks, boxes, image_shape, threshold=0.5):
+    """detectron2's paste_masks_in_image on the GPU for threshold > 0: masks [N,M,M] probabilities (CUDA), boxes [N,4]
+    XYXY (a tensor, or an object with ``.tensor``) -> bool [N,H,W], bit-identical to its grid_sample path."""
+    _check_threshold(threshold)
+    boxes = getattr(boxes, "tensor", boxes)
+    if not masks.is_cuda:
+        raise _lib.GdrnError("paste_masks_in_image needs CUDA tensors (no CPU fallback)")
+    if masks.dim() != 3 or masks.shape[-1] != masks.shape[-2]:
+        raise ValueError(f"masks must be [N,M,M], got {tuple(masks.shape)}")
+    N, H, W = masks.shape[0], int(image_shape[0]), int(image_shape[1])
+    m = masks.detach().to(dtype=torch.float32).contiguous()
+    b = boxes.detach().to(device=masks.device, dtype=torch.float32).contiguous()
+    if tuple(b.shape) != (N, 4):
+        raise ValueError(f"boxes must be [{N},4], got {tuple(b.shape)}")
+    out = torch.empty((N, H, W), dtype=torch.bool, device=masks.device)
+    _lib.check(_lib.lib().gdrn_mask_paste(_lib.ptr(m), N, m.shape[1], m.shape[2], 0, _lib.ptr(b), H, W, float(threshold),
+                                          _lib.ptr(out), _lib.current_stream()), "gdrn_mask_paste")
+    return out
+
+
+class MaskRleBuffers:
+    """Device buffers of gdrn_mask_paste_rle for up to S strings of H x W masks: the boundary workspace, the packed chars
+    (S * gdrn_mask_rle_max_chars(H, W) bytes: the worst case) and the [S,2] (offset, length) table."""
+
+    def __init__(self, device):
+        self.device = torch.device(device)
+        self.ws = self.chars = self.table = None
+
+    def ensure(self, S, H, W):
+        """Grow (never shrink) to S strings at H x W."""
+        L = _lib.lib()
+        ws, nc = L.gdrn_mask_rle_workspace_bytes(S, H, W), S * L.gdrn_mask_rle_max_chars(H, W)
+        if self.ws is None or ws > self.ws.numel():
+            self.ws = torch.empty(ws, dtype=torch.uint8, device=self.device)
+        if self.chars is None or nc > self.chars.numel():
+            self.chars = torch.empty(nc, dtype=torch.uint8, device=self.device)
+        if self.table is None or S > self.table.shape[0]:
+            self.table = torch.empty((S, 2), dtype=torch.int64, device=self.device)
+        return self
+
+
+@_lib.on_device(0)
+def paste_masks_rle_launch(mask, full_mask, roi_center, scale, image_shape, threshold, mask_loss_type, bufs=None):
+    """Enqueue the paste + RLE of n ROIs' raw maps (mask [n,1,h,w], full_mask the same or None) at roi_center [n,2] /
+    scale [n] (the boxes roi_center -/+ scale / 2) on the current stream; no synchronisation.  -> bufs, whose
+    ``table[:S]`` (S = n, or 2n with full_mask: all masks, then all full masks) holds (offset, length) into ``chars``."""
+    _check_threshold(threshold)
+    mode = mask_prob_mode(mask_loss_type)
+    n, H, W = mask.shape[0], int(image_shape[0]), int(image_shape[1])
+    m0 = mask.detach().to(dtype=torch.float32).contiguous()
+    m1 = None if full_mask is None else full_mask.detach().to(dtype=torch.float32).contiguous()
+    c = roi_center.detach().to(device=mask.device, dtype=torch.float32).contiguous()
+    s = scale.detach().to(device=mask.device, dtype=torch.float32).contiguous()
+    if m0.dim() != 4 or m0.shape[1] != 1 or (m1 is not None and m1.shape != m0.shape):
+        raise ValueError(f"maps must be [n,1,h,w], got {tuple(m0.shape)}")
+    if tuple(c.shape) != (n, 2) or tuple(s.reshape(-1).shape) != (n,):
+        raise ValueError("roi_center must be [n,2] and scale [n]")
+    S = n if m1 is None else 2 * n
+    bufs = (bufs or MaskRleBuffers(mask.device)).ensure(S, H, W)
+    _lib.check(_lib.lib().gdrn_mask_paste_rle(_lib.ptr(m0), _lib.ptr(m1), n, m0.shape[2], m0.shape[3], mode, _lib.ptr(c),
+                                              _lib.ptr(s), H, W, float(threshold), _lib.ptr(bufs.ws), bufs.ws.numel(),
+                                              _lib.ptr(bufs.chars), bufs.chars.numel(), _lib.ptr(bufs.table),
+                                              _lib.current_stream()), "gdrn_mask_paste_rle")
+    return bufs
+
+
+def rle_dicts(table, chars, H, W):
+    """Host (offset, length) table [S,2] + the packed chars (bytes-like) -> [{"size": [H, W], "counts": str}]."""
+    b = bytes(chars)
+    return [{"size": [int(H), int(W)], "counts": b[o:o + n].decode("ascii")} for o, n in np.asarray(table).tolist()]
+
+
+def paste_masks_rle(raw_maps, roi_center, scale, image_shape, threshold, mask_loss_type):
+    """The visible or amodal masks of n ROIs as the save-results loop stores them: get_out_mask(raw_maps
+    [n,1,64,64]) pasted into the image at roi_center -/+ scale / 2, thresholded and COCO-RLE encoded (pycocotools
+    encode of the Fortran-ordered uint8 mask) -> [{"size": [H, W], "counts": str}].  Synchronises."""
+    if not raw_maps.is_cuda:
+        raise _lib.GdrnError("paste_masks_rle needs CUDA tensors (no CPU fallback)")
+    bufs = paste_masks_rle_launch(raw_maps, None, roi_center, scale, image_shape, threshold, mask_loss_type)
+    n = raw_maps.shape[0]
+    table = bufs.table[:n].cpu().numpy()
+    total = int(table[-1].sum()) if n else 0
+    return rle_dicts(table, bufs.chars[:total].cpu().numpy().tobytes(), image_shape[0], image_shape[1])
+
+
+def rle_confusion(rles, gt_masks, device="cuda"):
+    """The mask tools' per-pair counts: P compressed RLE dicts decoded at their size against gt_masks [P,H,W] (nonzero =
+    set; numpy or torch) -> [P,4] int64 numpy (TP, FP, FN, TN).  A malformed string raises GdrnError."""
+    gt = torch.as_tensor(gt_masks)
+    if gt.dim() != 3 or gt.shape[0] != len(rles):
+        raise ValueError(f"gt_masks must be [{len(rles)},H,W], got {tuple(gt.shape)}")
+    P, H, W = gt.shape
+    for i, r in enumerate(rles):
+        if [int(v) for v in r["size"]] != [H, W]:
+            raise ValueError(f"rle {i} has size {r['size']}, the GT masks are {H}x{W}")
+    dev = torch.device(device) if not gt.is_cuda else gt.device
+    with torch.cuda.device(dev):
+        enc = [r["counts"].encode("ascii") if isinstance(r["counts"], str) else bytes(r["counts"]) for r in rles]
+        lens = np.array([len(e) for e in enc], np.int64)
+        offs = np.concatenate([[0], np.cumsum(lens)[:-1]]).astype(np.int64) if P else lens
+        blob = b"".join(enc) or b"\0"
+        chars = torch.frombuffer(bytearray(blob), dtype=torch.uint8).to(dev)
+        table = torch.from_numpy(np.stack([offs, lens], 1) if P else np.zeros((0, 2), np.int64)).to(dev)
+        g = (gt != 0).to(dtype=torch.uint8, device=dev).contiguous()
+        status = torch.empty(max(P, 1), dtype=torch.int32, device=dev)
+        counts = torch.zeros((P, 4), dtype=torch.int64, device=dev)
+        _lib.check(_lib.lib().gdrn_rle_confusion(_lib.ptr(chars), chars.numel(), _lib.ptr(table), P, _lib.ptr(g), H, W,
+                                                 _lib.ptr(status), _lib.ptr(counts), _lib.current_stream()),
+                   "gdrn_rle_confusion")
+        return counts.cpu().numpy()

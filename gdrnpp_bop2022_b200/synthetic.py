@@ -280,12 +280,34 @@ def make_yolox_state_dict(forward, depth=0.33, width=0.25, num_classes=8, seed=0
     return {k: (v.float() if v.is_floating_point() else v).cpu() for k, v in sd.items()}
 
 
+def _instance_masks(rng, H, W, x, y, bw, bh):
+    """(full, visible) bool [H,W] masks of one GT instance: an ellipse in its box, minus a random occluder for the
+    visible one.  One in six is empty, one in six is moved to touch the image border, one in six fully occluded."""
+    kind = rng.randint(6)
+    full = np.zeros((H, W), bool)
+    if kind == 0:
+        return full, full.copy()
+    cx, cy = x + bw / 2, y + bh / 2
+    if kind == 1:
+        cx, cy = rng.choice([0.0, W - 1.0]), rng.uniform(0, H)
+    rx, ry = max(bw / 2, 2.0), max(bh / 2, 2.0)
+    yy, xx = np.mgrid[0:H, 0:W]
+    full = ((xx - cx) / rx) ** 2 + ((yy - cy) / ry) ** 2 <= 1
+    if kind == 2:
+        return full, np.zeros_like(full)
+    ox, oy = rng.uniform(cx - rx, cx + rx), rng.uniform(cy - ry, cy + ry)
+    occ = (np.abs(xx - ox) < rx * rng.uniform(0.2, 0.6)) & (np.abs(yy - oy) < ry * rng.uniform(0.2, 0.6))
+    return full, full & ~occ
+
+
 def write_bop_tree(root, dataset="ycbv", num_images=12, num_scenes=2, H=480, W=640, dets_per_image=6, seed=0, gray=False,
-                   obj_ids=None, with_depth=True):
+                   obj_ids=None, with_depth=True, with_masks=False):
     """A small BOP test split under ``root`` (the reference's ``datasets/`` directory): BOP_DATASETS/<dataset>/ with
     test_targets_bop19.json, test/<scene>/{rgb|gray, depth, scene_camera.json, scene_gt.json, scene_gt_info.json},
     models_eval/ (box meshes in mm + models_info.json) and test/test_bboxes/dets.json (detections, XYWH boxes around the
-    ground-truth objects, some partly outside the image).  Colour images are random BGR PNGs (``gray``: 8-bit TIFs in
+    ground-truth objects, some partly outside the image).  ``with_masks``: also mask/ and mask_visib/
+    {im_id:06d}_{k:06d}.png per GT instance (visible within full; some empty, some touching the border), drawn from a
+    random stream of their own so that the rest of the tree stays byte-identical.  Colour images are random BGR PNGs (``gray``: 8-bit TIFs in
     gray/, as ITODD), depth 16-bit PNGs of a tilted plane.  -> path of the detection file relative to ``root``, as "datasets/..."."""
     import json
     import os
@@ -295,6 +317,7 @@ def write_bop_tree(root, dataset="ycbv", num_images=12, num_scenes=2, H=480, W=6
     from .ply import save_ply
 
     rng = np.random.RandomState(seed)
+    mrng = np.random.RandomState(seed + 7919)
     base = os.path.join(root, "BOP_DATASETS", dataset)
     split = os.path.join(base, "test_primesense" if dataset in ("tless", "hb") else "test")
     models = os.path.join(base, "models_eval")
@@ -320,6 +343,9 @@ def write_bop_tree(root, dataset="ycbv", num_images=12, num_scenes=2, H=480, W=6
         sdir = os.path.join(split, "{:06d}".format(scene_id))
         os.makedirs(os.path.join(sdir, color_dir), exist_ok=True)
         os.makedirs(os.path.join(sdir, "depth"), exist_ok=True)
+        if with_masks:
+            os.makedirs(os.path.join(sdir, "mask"), exist_ok=True)
+            os.makedirs(os.path.join(sdir, "mask_visib"), exist_ok=True)
         cams, gts, gt_infos = {}, {}, {}
         for k in range(min(per_scene, num_images - s * per_scene)):
             im_id = 3 * k + 1
@@ -345,6 +371,10 @@ def write_bop_tree(root, dataset="ycbv", num_images=12, num_scenes=2, H=480, W=6
                 gt_infos[str(im_id)].append({"bbox_obj": [int(x), int(y), int(bw), int(bh)],
                                              "bbox_visib": [int(x), int(y), int(bw), int(bh)], "px_count_all": 1000,
                                              "px_count_valid": 1000, "px_count_visib": 900, "visib_fract": 0.9})
+                if with_masks:
+                    full, vis = _instance_masks(mrng, H, W, x, y, bw, bh)
+                    for d, m in (("mask", full), ("mask_visib", vis)):
+                        cv2.imwrite(os.path.join(sdir, d, "{:06d}_{:06d}.png".format(im_id, j)), m.astype(np.uint8) * 255)
                 cur.append({"obj_id": o, "bbox_est": [float(x), float(y), float(bw), float(bh)],
                             "score": float(np.round(rng.uniform(0.05, 1.0), 2)), "time": 0.01})
             dets["{}/{}".format(scene_id, im_id)] = cur

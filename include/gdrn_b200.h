@@ -517,6 +517,30 @@ int coco_eval_accumulate(const double* kept_score, const int* kept_rank, const i
                          const int* max_dets, int M, void* workspace, size_t workspace_bytes, double* precision,
                          double* recall, void* stream);
 
+/* ---------------------------------------------------------------------------------------------
+ * Image-space masks and COCO RLE (csrc/mask_rle.cu): detectron2's GPU paste_masks_in_image + threshold, pycocotools
+ * rleEncode + rleToString, and the decode + confusion counts of the reference's mask tools.  mode picks how a map
+ * becomes probabilities: 0 as given, 1 = L1 ((p - min) / (max - min) per map), 2 = sigmoid.  threshold must be > 0.
+ *
+ * gdrn_mask_paste: masks [n,mh,mw] f32, boxes [n,4] f32 XYXY -> out [n,H,W] u8 (0 / 1).
+ * gdrn_mask_paste_rle: maps0 (and maps1, or null) [n,1,mh,mw] f32, the box of ROI i is roi_center[i] -/+ scale[i] / 2
+ *   (f32).  S = n (2n with maps1) strings, string s = kind * n + roi, packed in string order into chars (at least
+ *   S * gdrn_mask_rle_max_chars(H, W) bytes); table [S,2] i64 = (offset, length).  workspace:
+ *   gdrn_mask_rle_workspace_bytes(S, H, W) bytes.  No synchronisation.
+ * gdrn_rle_confusion: P compressed strings (chars + table [P,2] (offset, length)) decoded at H x W against gt [P,H,W] u8
+ *   (row-major, nonzero = set) -> counts [P,4] i64 = TP, FP, FN, TN; status [P] i32 device scratch.  Synchronises the
+ *   stream; a malformed string (bad char, unterminated group, total != H * W) is an error naming the string.
+ * ------------------------------------------------------------------------------------------- */
+int gdrn_mask_paste(const float* masks, int n, int mh, int mw, int mode, const float* boxes, int H, int W, float threshold,
+                    uint8_t* out, void* stream);
+size_t gdrn_mask_rle_max_chars(int H, int W);
+size_t gdrn_mask_rle_workspace_bytes(int S, int H, int W);
+int gdrn_mask_paste_rle(const float* maps0, const float* maps1, int n, int mh, int mw, int mode, const float* roi_center,
+                        const float* scale, int H, int W, float threshold, void* workspace, size_t workspace_bytes,
+                        char* chars, size_t chars_bytes, long long* table, void* stream);
+int gdrn_rle_confusion(const char* chars, size_t chars_bytes, const long long* table, int P, const uint8_t* gt, int H, int W,
+                       int* status, long long* counts, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
