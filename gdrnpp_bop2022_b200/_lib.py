@@ -132,6 +132,7 @@ _SIGNATURES = {
     "gdrn_mask_paste_rle": (c_int, [c_void_p, c_void_p] + [c_int] * 4 + [c_void_p, c_void_p, c_int, c_int, c_float, c_void_p,
                                                                        c_size_t, c_void_p, c_size_t, c_void_p, c_void_p]),
     "gdrn_rle_confusion": (c_int, [c_void_p, c_size_t, c_void_p, c_int, c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p]),
+    "gdrn_gt_info": (c_int, [c_void_p] * 6 + [c_int] * 3 + [c_float] + [c_void_p] * 5),
 }
 
 EXPORTED_SYMBOLS = tuple(_SIGNATURES.keys())

@@ -12,6 +12,7 @@
 //    partials in chunk order.
 #include <math.h>
 
+#include "bop_visib.cuh"
 #include "common.cuh"
 
 namespace {
@@ -38,21 +39,6 @@ __device__ __forceinline__ unsigned warp_sum_u(unsigned v) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
   return v;
-}
-
-// misc.depth_im_to_dist_im_fast (misc.py:628-647) for one pixel: sqrt((pre_X*d)^2 + (pre_Y*d)^2 + d^2) in f64, summed
-// left to right, with pre_X = (x - cx) / fx and pre_Y = (y - cy) / fy (Precomputer, misc.py:616-623).
-__device__ __forceinline__ double dist_px(double pre_x, double pre_y, float depth) {
-  const double d = (double)depth;
-  const double a = __dmul_rn(pre_x, d), b = __dmul_rn(pre_y, d);
-  return __dsqrt_rn(__dadd_rn(__dadd_rn(__dmul_rn(a, a), __dmul_rn(b, b)), __dmul_rn(d, d)));
-}
-
-// visibility._estimate_visib_mask, bop19 mode (visibility.py:34-36): the difference is taken in f32, as the reference
-// casts both distance images with astype(np.float32) and compares against delta as f32.
-__device__ __forceinline__ bool visib_bop19(double d_model, double d_test, float delta) {
-  const float diff = __fsub_rn(__double2float_rn(d_model), __double2float_rn(d_test));
-  return (diff <= delta || d_test == 0.0) && d_model > 0.0;
 }
 
 // counts[p] = {union, intersection, cost(tau_0), ..., cost(tau_{T-1})}

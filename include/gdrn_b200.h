@@ -541,6 +541,24 @@ int gdrn_mask_paste_rle(const float* maps0, const float* maps1, int n, int mh, i
 int gdrn_rle_confusion(const char* chars, size_t chars_bytes, const long long* table, int P, const uint8_t* gt, int H, int W,
                        int* status, long long* counts, void* stream);
 
+/* ---------------------------------------------------------------------------------------------
+ * Ground-truth annotations of a BOP split (csrc/gt_info.cu): the per-instance math of calc_gt_info.py and
+ * calc_gt_masks.py for n instances of N images of one size H x W.  Results do not depend on the launch shape.
+ *
+ * gdrn_gt_info: depth_large [n,3H,3W] f32 is instance i rendered alone (float z, 0 = background) on the 3x canvas with
+ *   principal point (cx + W, cy + H); depth_img [n,H,W] f32 (or null) the same instance at image size with K.
+ *   depth_test [N,H,W] u16 sensor depth, depth_scale [N] f32, Ks [N,3,3] f64; instance i lies in image inst_img[i]
+ *   (i32).  The test depth is f32(u16) * depth_scale in f32; distances and bop19 visibility (diff in f32 against delta)
+ *   are the ones VSD uses.  counts [n,3] i64 = px_count_all (canvas coverage), px_count_valid, px_count_visib;
+ *   boxes [n,8] i32 = bbox_obj, bbox_visib as (x_min, y_min, x_max - x_min, y_max - y_min), bbox_obj in image
+ *   coordinates (may be negative or extend past the image), both -1 unless px_count_visib > 0.  With depth_img,
+ *   mask / mask_visib [n,H,W] u8 = 0 / 255.  depth_large may be null when depth_img is given (masks only: counts 0,
+ *   boxes -1).  Allocates nothing, does not synchronise.
+ * ------------------------------------------------------------------------------------------- */
+int gdrn_gt_info(const float* depth_large, const float* depth_img, const uint16_t* depth_test, const float* depth_scale,
+                 const double* Ks, const int* inst_img, int n, int H, int W, float delta, long long* counts, int* boxes,
+                 uint8_t* mask, uint8_t* mask_visib, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
