@@ -105,7 +105,7 @@ def main():
         model_dir = gt_info.models_path(tmp, "lmo")
         scenes = gt_info.plan_split(sp)
         ims = scenes[0][1][:a.batch_images]
-        meshes = gt_info.Meshes(gt_info.load_models(model_dir, range(1, 9)), device=dev)
+        meshes = bop_eval.VsdMeshes(gt_info.load_models(model_dir, range(1, 9)), device=dev)
         depth = np.stack([gt_info.read_depth(im["depth"]) for im in ims])
         gts = [(j, g) for j, im in enumerate(ims) for g in im["gts"]]
         args = (meshes, [g["obj_id"] for _, g in gts], np.stack([g["cam_R_m2c"] for _, g in gts]),

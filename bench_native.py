@@ -178,6 +178,7 @@ def bench_flow(dev, T, peaks):
 
 
 def _mesh_and_rois(dev, n=64, subdiv=5):
+    from gdrnpp_bop2022_b200.renderer import Model3D
     from gdrnpp_bop2022_b200.synthetic import make_icosphere_mesh
 
     v, f = make_icosphere_mesh(subdiv, (0.12, 0.09, 0.1))   # subdiv 5: 10242 vertices, 20480 faces
@@ -192,28 +193,28 @@ def _mesh_and_rois(dev, n=64, subdiv=5):
         t = np.array([rs.randn() * 0.02, rs.randn() * 0.02, 0.5 + rs.rand() * 0.3])
         poses.append(np.hstack([R, t[:, None]]))
         Ks.append(np.array([[110.0 + 10 * rs.rand(), 0, 32 + rs.randn()], [0, 112.0, 31 + rs.randn()], [0, 0, 1]]))
-    return (torch.from_numpy(v).to(dev), torch.from_numpy(f).to(dev),
-            torch.from_numpy(np.stack(poses).astype(np.float32)).to(dev), torch.from_numpy(np.stack(Ks).astype(np.float32)).to(dev))
+    return (Model3D(v, f, device=dev), torch.from_numpy(np.stack(poses).astype(np.float32)).to(dev),
+            torch.from_numpy(np.stack(Ks).astype(np.float32)).to(dev))
 
 
 def bench_raster(dev, T, peaks):
     from gdrnpp_bop2022_b200.renderer import depth_refine, render_depth
 
     n, hw = 64, 64
-    V, F, poses, Ks = _mesh_and_rois(dev, n)
-    ms = T.time(lambda: render_depth(V, F, poses, Ks, hw, hw))
-    nv, nf = V.shape[0], F.shape[0]
-    recs = [_rec("rast_render_depth (64 ROI renders of one mesh)", {"rois": n, "V": nv, "F": nf, "H": hw, "W": hw}, ms,
+    model, poses, Ks = _mesh_and_rois(dev, n)
+    ms = T.time(lambda: render_depth(model, poses, Ks, hw, hw))
+    nv, nf = model.vertices.shape[0], model.faces.shape[0]
+    recs = [_rec("rast_render_meshes (64 ROI renders of one mesh)", {"rois": n, "V": nv, "F": nf, "H": hw, "W": hw}, ms,
                  alg_bytes=n * (12 * nv + 12 * nf + 4 * hw * hw), peaks=peaks, renders_per_s=n / (ms * 1e-3),
                  note="mesh is L2-resident after the first ROI; bound by triangle set-up + 64-bit atomicMin, not HBM",
                  reference_note="reference vispy renderer: 7.96 ms per 640x480 render incl. readback "
                                 "(lib/render_vispy/renderer.py:564, hardware not stated); no GL on this box")]
     # fast depth refine, 2 iterations (render + refine step each), configs[2]'s refinement half
-    sensor = render_depth(V, F, poses, Ks, hw, hw) * 1.02
+    sensor = render_depth(model, poses, Ks, hw, hw) * 1.02
     xyz = torch.rand(n, 3, hw, hw, device=dev) - 0.5
     mask = torch.rand(n, 1, hw, hw, device=dev)
     rot, trans = poses[:, :, :3].contiguous(), poses[:, :, 3].contiguous()
-    ms2 = T.time(lambda: depth_refine(V, F, rot, trans, Ks, xyz, mask, sensor, iters=2, thresh=0.8))
+    ms2 = T.time(lambda: depth_refine(model, rot, trans, Ks, xyz, mask, sensor, iters=2, thresh=0.8))
     recs.append(_rec("depth_refine (2 x [render + weighted-median step])", {"rois": n, "F": nf, "iters": 2}, ms2,
                      alg_bytes=2 * n * (12 * nv + 12 * nf + 4 * hw * hw + 28 * hw * hw), peaks=peaks, rois_per_s=n / (ms2 * 1e-3),
                      reference_note="reference: 2 GL draws + 4 glReadPixels per ROI on one CPU thread "
@@ -270,23 +271,23 @@ def bench_config2(dev, T, peaks, precision="bf16x3"):
     model.load_state_dict(make_state_dict())
     model.to(dev)
     b = {k: v.to(dev) for k, v in make_batch(B=B, seed=3).items()}
-    V, F, _, _ = _mesh_and_rois(dev, 1)
+    mesh, _, _ = _mesh_and_rois(dev, 1)
     kw = dict(roi_classes=b["roi_classes"], roi_coord_2d=b["roi_coord_2d"], roi_cams=b["roi_cams"], roi_centers=b["roi_centers"],
               roi_whs=b["roi_whs"], roi_extents=b["roi_extents"], resize_ratios=b["resize_ratios"])
     scale = 64.0 / b["resize_ratios"]
     K_crop = get_K_crop_resize(b["roi_cams"], b["roi_centers"] - scale.view(B, 1) / 2, b["resize_ratios"].view(B, 1))
     out0 = model(b["roi_img"], **kw)
     poses0 = torch.cat([out0["rot"], (out0["trans"] * 1.03)[:, :, None]], dim=2).contiguous()
-    sensor = render_depth(V, F, poses0, K_crop, 64, 64)     # "sensor" = the object a little farther along the ray
+    sensor = render_depth(mesh, poses0, K_crop, 64, 64)     # "sensor" = the object a little farther along the ray
     n_pts = 2048
-    model_pts = V[torch.randperm(V.shape[0], device=dev)[:n_pts]].contiguous()
+    model_pts = mesh.vertices[torch.randperm(mesh.vertices.shape[0], device=dev)[:n_pts]].contiguous()
     d1, d2 = torch.zeros(B, n_pts, device=dev), torch.zeros(B, n_pts, device=dev)
     i1, i2 = torch.zeros(B, n_pts, dtype=torch.int32, device=dev), torch.zeros(B, n_pts, dtype=torch.int32, device=dev)
 
     def step():
         out = model(b["roi_img"], **kw)
         xyz = torch.cat([out["coor_x"], out["coor_y"], out["coor_z"]], dim=1)
-        t2 = depth_refine(V, F, out["rot"], out["trans"], K_crop, xyz, out["mask"], sensor, iters=2, thresh=0.8)
+        t2 = depth_refine(mesh, out["rot"], out["trans"], K_crop, xyz, out["mask"], sensor, iters=2, thresh=0.8)
         # chamfer between the model points under the refined pose and under the initial pose (b=64, n=m=2048)
         pa = (model_pts[None] @ out["rot"].transpose(1, 2) + t2[:, None]).contiguous()
         pb = (model_pts[None] @ out["rot"].transpose(1, 2) + out["trans"][:, None]).contiguous()
@@ -294,7 +295,7 @@ def bench_config2(dev, T, peaks, precision="bf16x3"):
         return t2
 
     ms = T.time(step, iters=8)
-    return [{"op": "configs[2]: forward(+maps) + depth refine x2 + chamfer", "shape": {"B": B, "F": int(F.shape[0]), "chamfer_n": n_pts},
+    return [{"op": "configs[2]: forward(+maps) + depth refine x2 + chamfer", "shape": {"B": B, "F": int(mesh.faces.shape[0]), "chamfer_n": n_pts},
              "precision": precision, "ms": ms, "rois_per_s": B / (ms * 1e-3), "l2": "flushed before every timed step"}]
 
 

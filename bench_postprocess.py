@@ -143,7 +143,7 @@ def main():
     a = ap.parse_args()
     from gdrnpp_bop2022_b200 import _lib
     from gdrnpp_bop2022_b200.pnp_ransac import pnp_net_from_maps, pnp_ransac_from_maps
-    from gdrnpp_bop2022_b200.renderer import render_depth
+    from gdrnpp_bop2022_b200.renderer import Model3D, render_depth
     from gdrnpp_bop2022_b200.synthetic import make_icosphere_mesh
 
     dev = torch.device("cuda:0")
@@ -169,7 +169,7 @@ def main():
         rs = np.random.RandomState(B)
         Kc = np.stack([np.array([[110.0 + 10 * rs.rand(), 0, 32], [0, 112.0, 31], [0, 0, 1]]) for _ in range(B)]).astype(np.float32)
         poses = torch.cat([R, t[:, :, None]], 2).contiguous()
-        ren = render_depth(T(v), T(f), poses, T(Kc), 64, 64)
+        ren = render_depth(Model3D(v, f, device=dev), poses, T(Kc), 64, 64)
         sensor = (ren * 1.02).contiguous()
         xyz = T(np.concatenate([d["cx"][:, None], d["cy"][:, None], d["cz"][:, None]], 1))
         mask = T(d["m"])
@@ -179,9 +179,9 @@ def main():
             tt = t.clone()
 
             def step():
-                _lib.check(_lib.lib().gdrn_depth_refine_step_weighted(_lib.ptr(xyz), _lib.ptr(mask), 1, _lib.ptr(sensor), _lib.ptr(ren),
-                                                                      _lib.ptr(Kd), _lib.ptr(R), int(coor_z), _lib.ptr(tt), B, 64, 0.8,
-                                                                      _lib.current_stream()), "gdrn_depth_refine_step_weighted")
+                _lib.check(_lib.lib().gdrn_depth_refine_step(_lib.ptr(xyz), _lib.ptr(mask), 1, _lib.ptr(sensor), _lib.ptr(ren),
+                                                             _lib.ptr(Kd), _lib.ptr(R), int(coor_z), _lib.ptr(tt), B, 64, 0.8,
+                                                             _lib.current_stream()), "gdrn_depth_refine_step")
             g = cuda_ms(step, a.reps, a.warmup)
             th = d["t"].astype(np.float64).copy()
             h = host_ms(lambda: host_refine_step(xyz_h, mask_h, sen_h, ren_h, Kc.astype(np.float64), d["R"], th, coor_z), a.host_reps)

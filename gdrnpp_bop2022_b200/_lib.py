@@ -69,19 +69,11 @@ _SIGNATURES = {
     "flow_forward_cuda": (c_int, [c_void_p] * 6 + [c_int] * 3 + [c_void_p]),
     "uncertainty_pnp": (None, [c_void_p] * 6 + [c_int]),
     "upnp_batched": (c_int, [c_void_p] * 6 + [c_int, c_int, c_void_p]),
-    "rast_render_depth": (
-        c_int,
-        [c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_int, c_int, c_int, c_float, c_float, c_int]
-        + [c_void_p] * 4,
-    ),
     "rast_scratch_bytes": (c_size_t, [c_int, c_int, c_int]),
-    "gdrn_depth_refine_step": (c_int, [c_void_p] * 6 + [c_int, c_int, c_float, c_void_p]),
-    "gdrn_depth_refine_step_ex": (c_int, [c_void_p, c_void_p, c_int] + [c_void_p] * 4 + [c_int, c_int, c_float, c_void_p]),
-    "gdrn_depth_refine_step_weighted": (c_int, [c_void_p, c_void_p, c_int] + [c_void_p] * 4 + [c_int, c_void_p, c_int, c_int, c_float,
-                                                                                          c_void_p]),
+    "gdrn_depth_refine_step": (c_int, [c_void_p, c_void_p, c_int] + [c_void_p] * 4 + [c_int, c_void_p, c_int, c_int, c_float,
+                                                                                 c_void_p]),
     "rast_upload_mesh": (c_int, [c_void_p, c_int, c_void_p, c_int]),
     "rast_mesh_count": (c_int, []),
-    "rast_free_meshes": (None, []),
     "rast_render_meshes": (c_int, [c_void_p] * 3 + [c_int] * 3 + [c_float, c_float, c_int] + [c_void_p] * 4),
     "gdrn_pnp_ransac_maps": (c_int, [c_void_p] * 9 + [c_int] * 3 + [c_float, c_float, c_uint] + [c_void_p] * 4),
     "gdrn_pnp_ransac_points": (c_int, [c_void_p] * 4 + [c_int] * 3 + [c_float, c_uint] + [c_void_p] * 4),

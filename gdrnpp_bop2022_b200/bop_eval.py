@@ -326,21 +326,14 @@ VSD_ZNEAR, VSD_ZFAR = 0.01, 10000.0
 
 
 class VsdMeshes:
-    """The models_eval meshes of a dataset (mm), uploaded once to the rasteriser's registry.  meshes: {obj_id: (verts
-    [V,3], faces [F,3])} as arrays or tensors."""
+    """The meshes of a dataset (mm), each uploaded once to the rasteriser's registry as a renderer.Model3D; ids maps
+    obj_id to its registry id.  meshes: {obj_id: (verts [V,3], faces [F,3])} as arrays or CPU tensors."""
 
     def __init__(self, meshes, device="cuda"):
-        from . import renderer
+        from .renderer import Model3D
 
         self.device = torch.device(device)
-        self.ids = {}
-        self._keep = []
-        with torch.cuda.device(self.device):
-            for o, (v, f) in meshes.items():
-                vt = torch.as_tensor(np.asarray(v, np.float32)).to(self.device).contiguous()
-                ft = torch.as_tensor(np.asarray(f, np.int32)).to(self.device).contiguous()
-                self._keep.append((vt, ft))
-                self.ids[int(o)] = renderer.upload_mesh(vt, ft)
+        self.ids = {int(o): Model3D(v, f, device=self.device).mesh_id for o, (v, f) in meshes.items()}
 
     def render(self, obj_ids, R, t, K, H, W):
         """Float-z depth [n,H,W] of obj_ids[i] at pose (R[i], t[i]) with intrinsics K[i] (mm)."""

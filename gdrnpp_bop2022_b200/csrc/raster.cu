@@ -21,54 +21,6 @@ __global__ void rast_clear_kernel(unsigned long long* zbuf, long long n) {
     zbuf[i] = 0xFFFFFFFFFFFFFFFFull;
 }
 
-__global__ void __launch_bounds__(256)
-rast_tri_kernel(const float* __restrict__ verts, const int* __restrict__ faces, int V, int F,
-                const float* __restrict__ poses, const float* __restrict__ Ks, int H, int W, float znear, float zfar,
-                unsigned long long* __restrict__ zbuf) {
-  const int r = blockIdx.y;
-  const int f = blockIdx.x * blockDim.x + threadIdx.x;
-  if (f >= F) return;
-  const float* P = poses + r * 12;
-  const float* K = Ks + r * 9;
-  float u[3], v[3], iz[3];
-#pragma unroll
-  for (int k = 0; k < 3; ++k) {
-    const int vi = faces[f * 3 + k];
-    const float x = verts[vi * 3], y = verts[vi * 3 + 1], z = verts[vi * 3 + 2];
-    const float X = P[0] * x + P[1] * y + P[2] * z + P[3];
-    const float Y = P[4] * x + P[5] * y + P[6] * z + P[7];
-    const float Z = P[8] * x + P[9] * y + P[10] * z + P[11];
-    if (Z < znear) return;
-    iz[k] = 1.0f / Z;
-    u[k] = (K[0] * X + K[1] * Y) * iz[k] + K[2];
-    v[k] = (K[4] * Y) * iz[k] + K[5];
-  }
-  const float area = (u[1] - u[0]) * (v[2] - v[0]) - (u[2] - u[0]) * (v[1] - v[0]);
-  if (area == 0.f) return;
-  const float inv_area = 1.0f / area;
-  int c0 = max(0, (int)floorf(fminf(fminf(u[0], u[1]), u[2]) - 0.5f));
-  int c1 = min(W - 1, (int)ceilf(fmaxf(fmaxf(u[0], u[1]), u[2]) - 0.5f));
-  int r0 = max(0, (int)floorf(fminf(fminf(v[0], v[1]), v[2]) - 0.5f));
-  int r1 = min(H - 1, (int)ceilf(fmaxf(fmaxf(v[0], v[1]), v[2]) - 0.5f));
-  unsigned long long* zb = zbuf + (long long)r * H * W;
-  for (int py = r0; py <= r1; ++py) {
-    const float sy = (float)py + 0.5f;
-    for (int px = c0; px <= c1; ++px) {
-      const float sx = (float)px + 0.5f;
-      // barycentrics (signed areas / area)
-      const float w0 = ((u[1] - sx) * (v[2] - sy) - (u[2] - sx) * (v[1] - sy)) * inv_area;
-      const float w1 = ((u[2] - sx) * (v[0] - sy) - (u[0] - sx) * (v[2] - sy)) * inv_area;
-      const float w2 = 1.0f - w0 - w1;
-      if (w0 < 0.f || w1 < 0.f || w2 < 0.f) continue;
-      const float izp = w0 * iz[0] + w1 * iz[1] + w2 * iz[2];
-      const float zp = 1.0f / izp;
-      if (!(zp >= znear) || zp > zfar) continue;
-      const unsigned long long key = ((unsigned long long)__float_as_uint(zp) << 32) | (unsigned)f;
-      atomicMin(zb + (long long)py * W + px, key);
-    }
-  }
-}
-
 // ---- mesh registry: meshes uploaded once (rast_upload_mesh), renders pick one per ROI by id --------------------------
 struct MeshEntry {
   const float* verts;
@@ -307,27 +259,8 @@ depth_refine_kernel(const float* __restrict__ xyz, const float* __restrict__ mas
 
 extern "C" size_t rast_scratch_bytes(int n, int H, int W) { return (size_t)n * H * W * 8; }
 
-extern "C" int rast_render_depth(const float* verts, const int* faces, int V, int F, const float* poses,
-                                 const float* Ks, int n, int H, int W, float znear, float zfar, int quantize_bits,
-                                 float* depth, float* xyz_cam, unsigned long long* zbuf_scratch, void* stream) {
-  GDRN_REQUIRE(verts && faces && poses && Ks && depth && zbuf_scratch, "rast: null argument");
-  GDRN_REQUIRE(V > 0 && F > 0 && n > 0 && H > 0 && W > 0, "rast: empty input");
-  GDRN_REQUIRE(quantize_bits == 0 || quantize_bits == 16 || quantize_bits == 24 || quantize_bits == 32,
-               "rast: quantize_bits must be 0, 16, 24 or 32");
-  GDRN_REQUIRE(znear > 0.f && zfar > znear, "rast: need 0 < znear < zfar");
-  cudaStream_t st = (cudaStream_t)stream;
-  const long long npx = (long long)n * H * W;
-  int blocks = (int)((npx + 255) / 256 > 4096 ? 4096 : (npx + 255) / 256);
-  rast_clear_kernel<<<blocks, 256, 0, st>>>(zbuf_scratch, npx);
-  rast_tri_kernel<<<dim3((F + 255) / 256, n), 256, 0, st>>>(verts, faces, V, F, poses, Ks, H, W, znear, zfar,
-                                                            zbuf_scratch);
-  rast_resolve_kernel<<<blocks, 256, 0, st>>>(zbuf_scratch, Ks, n, H, W, znear, zfar, quantize_bits, depth, xyz_cam);
-  GDRN_CHECK_CUDA(cudaGetLastError());
-  gdrn_count_launch(3);
-  return GDRN_OK;
-}
-
-// ---- mesh registry (process-wide, on the device that is current at the first upload) ------------------------------
+// ---- mesh registry: process-wide and append-only, on the device that is current at the first upload.  An id stays
+// valid for the life of the process; the object that uploaded the mesh holds it (renderer.Model3D.mesh_id). -------
 namespace {
 struct MeshRegistry {
   int device = -1;
@@ -373,12 +306,6 @@ extern "C" int rast_upload_mesh(const float* verts, int V, const int* faces, int
 
 extern "C" int rast_mesh_count(void) { return g_meshes.count; }
 
-extern "C" void rast_free_meshes(void) {
-  for (int i = 0; i < g_meshes.count; ++i) { cudaFree(const_cast<float*>(g_meshes.host[i].verts)); cudaFree(const_cast<int*>(g_meshes.host[i].faces)); }
-  if (g_meshes.dev_table) cudaFree(g_meshes.dev_table);
-  g_meshes = MeshRegistry();
-}
-
 extern "C" int rast_render_meshes(const int* mesh_ids, const float* poses, const float* Ks, int n, int H, int W,
                                   float znear, float zfar, int quantize_bits, float* depth, float* xyz_cam,
                                   unsigned long long* zbuf_scratch, void* stream) {
@@ -400,22 +327,9 @@ extern "C" int rast_render_meshes(const int* mesh_ids, const float* poses, const
   return GDRN_OK;
 }
 
-extern "C" int gdrn_depth_refine_step(const float* xyz, const float* mask, const float* depth_sensor,
-                                      const float* ren_depth, const float* K_crop, float* trans, int n, int hw,
-                                      float thresh, void* stream) {
-  return gdrn_depth_refine_step_ex(xyz, mask, 0, depth_sensor, ren_depth, K_crop, trans, n, hw, thresh, stream);
-}
-
-extern "C" int gdrn_depth_refine_step_ex(const float* xyz, const float* mask, int mask_mode, const float* depth_sensor,
-                                         const float* ren_depth, const float* K_crop, float* trans, int n, int hw,
-                                         float thresh, void* stream) {
-  return gdrn_depth_refine_step_weighted(xyz, mask, mask_mode, depth_sensor, ren_depth, K_crop, nullptr, 0, trans, n, hw,
-                                         thresh, stream);
-}
-
-extern "C" int gdrn_depth_refine_step_weighted(const float* xyz, const float* mask, int mask_mode, const float* depth_sensor,
-                                               const float* ren_depth, const float* K_crop, const float* rot,
-                                               int weight_mode, float* trans, int n, int hw, float thresh, void* stream) {
+extern "C" int gdrn_depth_refine_step(const float* xyz, const float* mask, int mask_mode, const float* depth_sensor,
+                                      const float* ren_depth, const float* K_crop, const float* rot, int weight_mode,
+                                      float* trans, int n, int hw, float thresh, void* stream) {
   GDRN_REQUIRE(xyz && mask && depth_sensor && ren_depth && K_crop && trans, "depth_refine: null argument");
   GDRN_REQUIRE(mask_mode >= 0 && mask_mode <= 2, "depth_refine: mask_mode must be 0 (normalised), 1 (raw L1) or 2 (logits)");
   GDRN_REQUIRE(weight_mode == 0 || weight_mode == 1, "depth_refine: weight_mode must be 0 (||xyz||) or 1 (coor-z)");

@@ -252,9 +252,8 @@ _MESHES = {}
 
 
 def _mesh(models_path, obj_id, device):
-    """One Model3D per (models_eval directory, object, device) for the life of the process: the rasteriser's mesh
-    registry (renderer.upload_mesh) keys meshes by their tensors' addresses, which a freed and re-allocated mesh could
-    reuse for another object."""
+    """One Model3D per (models_eval directory, object, device) for the life of the process, so that a test loop run
+    again in the same process does not read and upload its models again."""
     from .ply import load_ply
     from .renderer import Model3D
 
@@ -338,8 +337,8 @@ def postprocess(cfg, inp, out, meshes=None, mask_thr=0.5):
         crop_xy = inp["roi_center"] - inp["scale"].view(n, 1) / 2
         K_crop = get_K_crop_resize(inp["roi_cam"], crop_xy, (64.0 / inp["scale"]).view(n, 1))
         xyz = torch.cat([out["coor_x"], out["coor_y"], out["coor_z"]], dim=1)
-        trans = depth_refine([m.vertices for m in meshes], [m.faces for m in meshes], rot, trans, K_crop, xyz, out["mask"],
-                             inp["depth_sensor"], iters=cfg_get(cfg, "TEST.DEPTH_REFINE_ITER", 2),
+        trans = depth_refine(meshes, rot, trans, K_crop, xyz, out["mask"], inp["depth_sensor"],
+                             iters=cfg_get(cfg, "TEST.DEPTH_REFINE_ITER", 2),
                              thresh=cfg_get(cfg, "TEST.DEPTH_REFINE_THRESHOLD", 0.8), mesh_ids=inp["roi_cls"],
                              coor_z_refine=bool(cfg_get(cfg, "TEST.USE_COOR_Z_REFINE", False)))
     return rot, trans

@@ -11,7 +11,6 @@ bop19 visibility arithmetic VSD uses.  No CPU fallback: the GPU path needs CUDA 
   python -m gdrnpp_bop2022_b200.gt_info --dataset lmo --dataset_split train --dataset_split_type pbr
 """
 import argparse
-import ctypes
 import json
 import os
 import sys
@@ -88,26 +87,6 @@ def host_annotation(depth_large, depth_img, depth_test, K, delta):
 
 # ---------------------------------------------------------------------------------------------------------------------
 # In-memory API
-class Meshes:
-    """The models of a split (mm) in the rasteriser's registry, keyed by obj_id: the registry bop_eval.VsdMeshes keeps.
-    Each mesh is uploaded from host memory and gets a registry id of its own; renderer.upload_mesh's cache is keyed by
-    device addresses, which a later model can reuse once an earlier one is freed.  meshes: {obj_id: (verts [V,3],
-    faces [F,3])}.  The registry holds at most 1024 meshes per process."""
-
-    def __init__(self, meshes, device="cuda"):
-        self.device = torch.device(device)
-        self.ids = {}
-        with torch.cuda.device(self.device):
-            for o, (v, f) in meshes.items():
-                v = np.ascontiguousarray(v, np.float32).reshape(-1, 3)
-                f = np.ascontiguousarray(f, np.int32).reshape(-1, 3)
-                mid = _lib.lib().rast_upload_mesh(v.ctypes.data_as(ctypes.c_void_p), len(v),
-                                                  f.ctypes.data_as(ctypes.c_void_p), len(f))
-                if mid < 0:
-                    raise GdrnError(f"rast_upload_mesh failed for obj_id {o} (code {mid}): {_lib.last_error()}")
-                self.ids[int(o)] = mid
-
-
 def instance_bytes(H, W, info=True, masks=True):
     """Device bytes one instance takes in a pass: the float-z render and the rasteriser's 64-bit z-buffer for each
     canvas, the masks, and the counters."""
@@ -140,7 +119,7 @@ def _depth_u16(depth, dev):
 
 def annotate_device(meshes, obj_ids, R, t, inst_img, K, depth, depth_scale, delta=15.0, info=True, masks=False,
                     max_bytes=DEFAULT_MAX_BYTES, out=None):
-    """Launch the annotation of n instances; no synchronisation.  meshes: Meshes or bop_eval.VsdMeshes (obj_id -> mesh, mm);
+    """Launch the annotation of n instances; no synchronisation.  meshes: bop_eval.VsdMeshes (obj_id -> mesh, mm);
     obj_ids [n], R [n,3,3], t [n,3] (mm), inst_img [n] (image of each instance); K [N,3,3], depth [N,H,W] u16 (host or
     CUDA), depth_scale [N].  Instances go through the renders in chunks of at most max_bytes (instance_bytes each),
     which changes no output.  out: optional u8 CUDA buffer of at least result_bytes(n, H, W, masks) bytes.
@@ -410,7 +389,7 @@ def _check_scene_size(sizes, scene_id, H, W, path):
 def run_split(sp, model_dir, delta=15.0, what=("info", "masks"), scene_ids=None, max_bytes=DEFAULT_MAX_BYTES,
               batch_images=16, workers=8, device="cuda", log=None, meshes=None):
     """Annotate every GT instance of a split; writes scene_gt_info.json ("info") and mask/, mask_visib/ ("masks") in
-    each scene directory.  meshes: a Meshes of the split's models to reuse (default: loaded from model_dir).
+    each scene directory.  meshes: a bop_eval.VsdMeshes of the split's models to reuse (default: loaded from model_dir).
     -> {"images": int, "instances": int, "seconds": float}."""
     import cv2
 
@@ -477,7 +456,7 @@ def run_split(sp, model_dir, delta=15.0, what=("info", "masks"), scene_ids=None,
             H, W = staged.shape[1:]
             _check_scene_size(sizes, scene_id, H, W, ims[0]["depth"])
             if meshes is None:
-                meshes = Meshes(meshes_host, device=device)
+                meshes = bop_eval.VsdMeshes(meshes_host, device=device)
             dev = meshes.device
             with torch.cuda.device(dev):
                 d_depth = staged.to(dev, non_blocking=True)   # the one H2D copy of the batch

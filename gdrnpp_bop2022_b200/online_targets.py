@@ -9,7 +9,7 @@ fallback.
 import torch
 
 from . import _lib
-from .renderer import render_meshes, upload_mesh
+from .renderer import render_meshes
 
 
 def _f32(t, dev):
@@ -65,12 +65,12 @@ def xyz_to_region_batch(xyz, fps_points, mask=None):
 
 def render_roi_targets(models, roi_cls, ego_rot, trans, roi_zoom_K, roi_extent, roi_fps_points=None, out_res=64, znear=0.1,
                        zfar=100.0):
-    """The rendering block of batch_data (engine_utils.py:131-187) for a whole batch: models = list of Model3D-like objects
-    (``vertices``, ``faces``) indexed by roi_cls.  Returns roi_xyz, roi_mask_obj, roi_region (when fps points are given)
-    and the rendered roi_depth; two launches (rasteriser + target kernel), no host loop over ROIs, no sync."""
+    """The rendering block of batch_data (engine_utils.py:131-187) for a whole batch: models = list of Model3D indexed by
+    roi_cls.  Returns roi_xyz, roi_mask_obj, roi_region (when fps points are given) and the rendered roi_depth; two
+    launches (rasteriser + target kernel), no host loop over ROIs, no sync."""
     dev = ego_rot.device
     with torch.cuda.device(dev):
-        reg = torch.tensor([upload_mesh(m.vertices, m.faces) for m in models], dtype=torch.int32, device=dev)
+        reg = torch.tensor([m.mesh_id for m in models], dtype=torch.int32, device=dev)
         ids = reg[roi_cls.to(device=dev, dtype=torch.long)].contiguous()
         poses = torch.cat([ego_rot.float(), trans.float().reshape(-1, 3, 1)], dim=2).contiguous()
         depth = render_meshes(ids, poses, roi_zoom_K, out_res, out_res, znear, zfar)

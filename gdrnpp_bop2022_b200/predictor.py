@@ -344,8 +344,7 @@ class GdrnPredictor:
             d = d[:, 0]
         if d.shape[-1] == 256:
             d = ((d[:, 1::4, 1::4] + d[:, 1::4, 2::4]) + (d[:, 2::4, 1::4] + d[:, 2::4, 2::4])) * 0.25
-        return depth_refine([m.vertices for m in self.ren_models], [m.faces for m in self.ren_models], out_dict["rot"],
-                            out_dict["trans"], K_crop, xyz, out_dict["mask"], d.contiguous(),
+        return depth_refine(self.ren_models, out_dict["rot"], out_dict["trans"], K_crop, xyz, out_dict["mask"], d.contiguous(),
                             iters=self.cfg.TEST.DEPTH_REFINE_ITER, thresh=self.cfg.TEST.DEPTH_REFINE_THRESHOLD,
                             mesh_ids=inputs["roi_cls"], coor_z_refine=bool(self.cfg.TEST.USE_COOR_Z_REFINE))
 

@@ -19,27 +19,13 @@ def _f32c(t, dev=None):
     return t.detach().to(device=dev or t.device, dtype=torch.float32).contiguous()
 
 
-@_lib.on_device(0)
-def render_depth(verts, faces, poses, Ks, H, W, znear=0.1, zfar=100.0, quantize_bits=0, return_xyz=False):
-    """verts [V,3] f32, faces [F,3] i32, poses [n,3,4], Ks [n,3,3] (CUDA) -> depth [n,H,W] (0 = background)."""
-    if not verts.is_cuda:
-        raise _lib.GdrnError("render_depth needs CUDA tensors (no CPU fallback)")
-    dev = verts.device
-    verts = _f32c(verts)
-    faces = faces.detach().to(device=dev, dtype=torch.int32).contiguous()
+def render_depth(model, poses, Ks, H, W, znear=0.1, zfar=100.0, quantize_bits=0, return_xyz=False):
+    """One Model3D at poses [n,3,4] with Ks [n,3,3] (or one [1,3,3]) -> depth [n,H,W] (0 = background), rendered on the
+    model's device: render_meshes with the model's registry id for every ROI."""
+    dev = model.vertices.device
     poses = _f32c(poses, dev).reshape(-1, 3, 4)
-    Ks = _f32c(Ks, dev).reshape(-1, 3, 3)
-    n = poses.shape[0]
-    if Ks.shape[0] == 1 and n > 1:
-        Ks = Ks.expand(n, 3, 3).contiguous()
-    depth = torch.empty((n, H, W), dtype=torch.float32, device=dev)
-    xyz = torch.empty((n, H, W, 3), dtype=torch.float32, device=dev) if return_xyz else None
-    scratch = torch.empty((n * H * W,), dtype=torch.int64, device=dev)
-    L = _lib.lib()
-    _lib.check(L.rast_render_depth(_lib.ptr(verts), _lib.ptr(faces), verts.shape[0], faces.shape[0], _lib.ptr(poses),
-                                   _lib.ptr(Ks), n, H, W, float(znear), float(zfar), int(quantize_bits), _lib.ptr(depth),
-                                   _lib.ptr(xyz), _lib.ptr(scratch), _lib.current_stream()), "rast_render_depth")
-    return (depth, xyz) if return_xyz else depth
+    ids = torch.full((poses.shape[0],), model.mesh_id, dtype=torch.int32, device=dev)
+    return render_meshes(ids, poses, Ks, H, W, znear, zfar, quantize_bits, return_xyz)
 
 
 def get_out_mask(pred_mask, mask_loss_type="L1"):
@@ -68,24 +54,6 @@ def get_K_crop_resize(K, crop_xy, resize_ratio):
     return new_K
 
 
-_MESH_IDS = {}   # (verts.data_ptr, faces.data_ptr, V, F) -> id in the library's mesh registry (rast_upload_mesh)
-
-
-def upload_mesh(verts, faces):
-    """Register a mesh with the library once (rast_upload_mesh keeps its own device copy) and return its id.  Tensors
-    are identified by (data_ptr, shape): re-uploading the same tensors is free; a Model3D caches its id itself."""
-    key = (verts.data_ptr(), faces.data_ptr(), int(verts.shape[0]), int(faces.shape[0]))
-    mid = _MESH_IDS.get(key)
-    if mid is None:
-        v = _f32c(verts)
-        f = faces.detach().to(dtype=torch.int32).contiguous()
-        mid = _lib.lib().rast_upload_mesh(_lib.ptr(v), int(v.shape[0]), _lib.ptr(f), int(f.shape[0]))
-        if mid < 0:
-            raise _lib.GdrnError(f"rast_upload_mesh failed (code {mid}): {_lib.last_error()}")
-        _MESH_IDS[key] = mid
-    return mid
-
-
 @_lib.on_device(1)
 def render_meshes(mesh_ids, poses, Ks, H, W, znear=0.1, zfar=100.0, quantize_bits=0, return_xyz=False):
     """One render per ROI of the REGISTERED mesh `mesh_ids[i]` (int32 CUDA tensor of registry ids): poses [n,3,4],
@@ -106,14 +74,14 @@ def render_meshes(mesh_ids, poses, Ks, H, W, znear=0.1, zfar=100.0, quantize_bit
     return (depth, xyz) if return_xyz else depth
 
 
-@_lib.on_device(2)
-def depth_refine(verts, faces, rot, trans, K_crop, xyz, mask, depth_sensor, iters=2, thresh=0.8, mesh_ids=None,
+@_lib.on_device(1)
+def depth_refine(models, rot, trans, K_crop, xyz, mask, depth_sensor, iters=2, thresh=0.8, mesh_ids=None,
                  znear=0.1, zfar=100.0, mask_loss_type="L1", coor_z_refine=False):
     """Batched fast depth refine (gdrn_evaluator.py:515-561): `iters` x (render depth at the current pose ->
     weighted-median depth offset along the weighted-centroid ray).  The weights are ||xyz|| * mask, or with
     coor_z_refine (TEST.USE_COOR_Z_REFINE, :528-537) the camera-frame z of the rotated coordinates, (rot @ xyz)_z * mask.
 
-    verts/faces: one mesh (tensors) or lists of meshes with `mesh_ids` [n] selecting per ROI.
+    models: one Model3D, or a sequence of them with `mesh_ids` [n] indexing it per ROI.
     rot [n,3,3], trans [n,3], K_crop [n,3,3], xyz [n,3,h,w] (coor maps), mask [n,1,h,w] RAW visible-mask output
     (get_out_mask -- per-ROI min-max for the L1 head, sigmoid otherwise -- runs inside the refine kernel),
     depth_sensor [n,h,w] metres.  Returns refined trans [n,3].  Per iteration: one render launch over all ROIs (every
@@ -134,32 +102,37 @@ def depth_refine(verts, faces, rot, trans, K_crop, xyz, mask, depth_sensor, iter
         raise NotImplementedError(mask_loss_type)
     sensor = _f32c(depth_sensor).reshape(n, hw, hw)
     L = _lib.lib()
-    meshes = [(verts, faces)] if not isinstance(verts, (list, tuple)) else list(zip(verts, faces))
-    reg = torch.tensor([upload_mesh(v, f) for v, f in meshes], dtype=torch.int32, device=dev)   # list index -> registry id
+    models = [models] if isinstance(models, Model3D) else list(models)
+    reg = torch.tensor([m.mesh_id for m in models], dtype=torch.int32, device=dev)   # sequence index -> registry id
     if mesh_ids is None:
         ids = reg[:1].expand(n).contiguous()
     else:
         ids = reg[torch.as_tensor(mesh_ids).to(device=dev, dtype=torch.long)].contiguous()
+    weight_mode = 1 if coor_z_refine else 0
     for _ in range(iters):
         poses = torch.cat([rot, t[:, :, None]], dim=2).contiguous()
         ren = render_meshes(ids, poses, K_crop, hw, hw, znear, zfar)
-        if coor_z_refine:
-            _lib.check(L.gdrn_depth_refine_step_weighted(_lib.ptr(xyz), _lib.ptr(raw_mask), mask_mode, _lib.ptr(sensor), _lib.ptr(ren),
-                                                         _lib.ptr(K_crop), _lib.ptr(rot), 1, _lib.ptr(t), n, hw, float(thresh),
-                                                         _lib.current_stream()), "gdrn_depth_refine_step_weighted")
-        else:
-            _lib.check(L.gdrn_depth_refine_step_ex(_lib.ptr(xyz), _lib.ptr(raw_mask), mask_mode, _lib.ptr(sensor), _lib.ptr(ren),
-                                                   _lib.ptr(K_crop), _lib.ptr(t), n, hw, float(thresh), _lib.current_stream()),
-                       "gdrn_depth_refine_step_ex")
+        _lib.check(L.gdrn_depth_refine_step(_lib.ptr(xyz), _lib.ptr(raw_mask), mask_mode, _lib.ptr(sensor), _lib.ptr(ren),
+                                            _lib.ptr(K_crop), _lib.ptr(rot), weight_mode, _lib.ptr(t), n, hw, float(thresh),
+                                            _lib.current_stream()), "gdrn_depth_refine_step")
     return t
 
 
 class Model3D:
-    """Minimal stand-in for lib/render_vispy/model3d.py objects: vertices in metres + triangle indices."""
+    """Minimal stand-in for lib/render_vispy/model3d.py objects: vertices [V,3] in metres + triangle indices [F,3] on
+    `device`, and mesh_id, the mesh's id in the library's registry.  The mesh is uploaded once, here; the registry never
+    frees, so the id stays valid for the life of the process and every render of this model goes through it."""
 
     def __init__(self, vertices, faces, device="cuda"):
-        self.vertices = torch.as_tensor(np.asarray(vertices, np.float32)).to(device)
-        self.faces = torch.as_tensor(np.asarray(faces, np.int32)).to(device)
+        v = torch.as_tensor(np.ascontiguousarray(vertices, np.float32))
+        f = torch.as_tensor(np.ascontiguousarray(faces, np.int32))
+        with torch.cuda.device(device):   # the registry lives on the device current at the upload
+            mid = _lib.lib().rast_upload_mesh(_lib.ptr(v), int(v.shape[0]), _lib.ptr(f), int(f.shape[0]))
+        if mid < 0:
+            raise _lib.GdrnError(f"rast_upload_mesh failed (code {mid}): {_lib.last_error()}")
+        self.mesh_id = mid
+        self.vertices = v.to(device)
+        self.faces = f.to(device)
 
 
 def load_models(model_paths, scale_to_meter=1.0, device="cuda", **_):
@@ -210,8 +183,8 @@ class Renderer:
         depth = None
         K = torch.from_numpy(self.cam)[None].to(self.device)
         for model, pose in self._draws:
-            d = render_depth(model.vertices, model.faces, torch.from_numpy(pose)[None].to(self.device), K, self.height,
-                             self.width, self.clip_near, self.clip_far, quantize_bits=self.depth_bits)[0]
+            d = render_depth(model, torch.from_numpy(pose)[None].to(self.device), K, self.height, self.width,
+                             self.clip_near, self.clip_far, quantize_bits=self.depth_bits)[0]
             if depth is None:
                 depth = d
             else:  # nearest surface wins across draws (shared z-buffer in GL)
@@ -226,7 +199,7 @@ class EGLRenderer:
     EGLRenderer(model_paths, K=, width=, height=, vertex_scale=, znear=, zfar=) and
     render(obj_ids, poses, K=, pc_cam_tensor=, seg_tensor=) writing camera-space xyz (float-exact per fragment, like the
     interpolated varying of shader_textureless_texture.vs:36) into the caller's [H,W,4] CUDA tensor.  `model_paths` may
-    also be Model3D-like objects.  Colour / normal / object-space outputs are not rendered."""
+    also be Model3D objects.  Colour / normal / object-space outputs are not rendered."""
 
     def __init__(self, model_paths, K=None, width=640, height=480, vertex_scale=1.0, znear=0.25, zfar=6.0, device="cuda", **_):
         ms = list(model_paths)
@@ -248,7 +221,7 @@ class EGLRenderer:
         for k, (oid, pose) in enumerate(zip(obj_ids, poses)):
             m = self.models[oid]
             p = torch.as_tensor(np.asarray(pose, np.float32)[:3, :4])[None].to(self.device)
-            d, x = render_depth(m.vertices, m.faces, p, Kt, self.height, self.width, self.znear, self.zfar, return_xyz=True)
+            d, x = render_depth(m, p, Kt, self.height, self.width, self.znear, self.zfar, return_xyz=True)
             upd = (d[0] > 0) & ((depth == 0) | (d[0] < depth))
             depth = torch.where(upd, d[0], depth)
             xyz = torch.where(upd[..., None], x[0], xyz)

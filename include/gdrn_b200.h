@@ -243,48 +243,40 @@ int upnp_batched(const double* pts2d, const double* pts3d, const double* wgt2d, 
  * 363-407 (Renderer.set_cam/draw_model/finish -> depth) and lib/egl_renderer/egl_renderer_v3.py:838-1228
  * (EGLRenderer.render(..., pc_cam_tensor=) -> pc_cam[...,2]); C++ side lib/egl_renderer/cpp/
  * egl_renderer.cpp:262-310.
- *   verts [V,3] f32 (model space, metres), faces [F,3] i32; poses [n,3,4] f32 (R|t, OpenCV camera),
- *   Ks [n,3,3] f32 -> depth [n,H,W] f32 (0 = background), optional xyz_cam [n,H,W,3].
+ * Mesh registry (SURVEY.md 8b): rast_upload_mesh copies a mesh (verts [V,3] f32 in model space, metres; faces [F,3]
+ * i32; host or device pointers) to the device once and returns its id (>= 0) or a negative error code.  The registry
+ * is process-wide and append-only (at most 1024 meshes, all on the device current at the first upload): an id stays
+ * valid for the life of the process, and the object that uploaded the mesh holds it.
+ * rast_render_meshes renders n ROIs in one launch, ROI i with mesh mesh_ids[i] (i32, device) -- the multi-object form
+ * of the reference's per-object draw_model loop (engine/gdrn_evaluator.py:520-526) without a host loop or a sync:
+ *   poses [n,3,4] f32 (R|t, OpenCV camera), Ks [n,3,3] f32 -> depth [n,H,W] f32 (0 = background), optional
+ *   xyz_cam [n,H,W,3]; zbuf_scratch of rast_scratch_bytes(n, H, W) bytes.
  *   quantize_bits: 0 = float depth of the interpolated camera-space z (EGL path), 24/16 = emulate the
  *   fixed-point z-buffer decode of the vispy path (renderer.py:176-182) with znear/zfar.
  * ------------------------------------------------------------------------------------------- */
-int rast_render_depth(const float* verts, const int* faces, int V, int F, const float* poses, const float* Ks,
-                      int n, int H, int W, float znear, float zfar, int quantize_bits, float* depth,
-                      float* xyz_cam, unsigned long long* zbuf_scratch, void* stream);
-size_t rast_scratch_bytes(int n, int H, int W);
-/* Mesh registry (SURVEY.md 8b: rast_upload_mesh + rast_render_depth(mesh_ids, ...)): meshes are uploaded once
- * (host or device pointers; the library keeps a device copy) and a batch of ROIs renders one mesh EACH, selected by
- * mesh_ids [n] i32 (device) -- the multi-object form of the reference's per-object draw_model loop
- * (engine/gdrn_evaluator.py:520-526) without a host loop or a sync.  rast_upload_mesh returns the id (>= 0) or a
- * negative error code. */
 int rast_upload_mesh(const float* verts, int V, const int* faces, int F);
 int rast_mesh_count(void);
-void rast_free_meshes(void);
 int rast_render_meshes(const int* mesh_ids, const float* poses, const float* Ks, int n, int H, int W, float znear,
                        float zfar, int quantize_bits, float* depth, float* xyz_cam, unsigned long long* zbuf_scratch,
                        void* stream);
+size_t rast_scratch_bytes(int n, int H, int W);
 
 /* ---------------------------------------------------------------------------------------------
  * Fast depth refinement -- replaces GDRN_Evaluator.process_depth_refine
  * (core/gdrn_modeling/engine/gdrn_evaluator.py:521-561) == GdrnPredictor.process_depth_refine
  * (core/gdrn_modeling/demo/predictor_gdrn.py:239-286), one iteration after a render:
- *   xyz [n,3,64,64], mask [n,64,64], depth_sensor [n,64,64], ren_depth [n,64,64], K_crop [n,3,3],
- *   trans [n,3] in/out; thresh = DEPTH_REFINE_THRESHOLD (0.8).
+ *   xyz [n,3,hw,hw], mask [n,hw,hw], depth_sensor [n,hw,hw], ren_depth [n,hw,hw], K_crop [n,3,3],
+ *   trans [n,3] in/out; thresh = DEPTH_REFINE_THRESHOLD (0.8); 0 < hw <= 128.
+ *   mask_mode: get_out_mask (engine/engine_utils.py:313-333) folded into the kernel: 0 = `mask` is already
+ *   normalised, 1 = raw L1 mask output -> per-ROI min-max normalisation, 2 = raw logits -> sigmoid.
+ *   weight_mode: 0 = ||xyz||, 1 = TEST.USE_COOR_Z_REFINE (gdrn_evaluator.py:528-537): w = (R xyz)_z * mask *
+ *   (ren > 0) * (sensor > 0) with `xyz` the raw [0,1] coordinate maps and rot [n,3,3] the rotation of the pose being
+ *   refined (may be NULL for mode 0).  Signed weights follow the reference's order: divide by the sum, then threshold
+ *   against the max over all pixels; a zero sum leaves t unchanged.
  * ------------------------------------------------------------------------------------------- */
-int gdrn_depth_refine_step(const float* xyz, const float* mask, const float* depth_sensor, const float* ren_depth,
-                           const float* K_crop, float* trans, int n, int hw, float thresh, void* stream);
-/* same with get_out_mask (engine/engine_utils.py:313-333) folded into the kernel: mask_mode 0 = `mask` is already
- * normalised, 1 = raw L1 mask output -> per-ROI min-max normalisation, 2 = raw logits -> sigmoid. */
-int gdrn_depth_refine_step_ex(const float* xyz, const float* mask, int mask_mode, const float* depth_sensor,
-                              const float* ren_depth, const float* K_crop, float* trans, int n, int hw, float thresh,
-                              void* stream);
-/* same with the weighting selectable: weight_mode 0 = ||xyz|| (the two entries above), 1 = TEST.USE_COOR_Z_REFINE
- * (gdrn_evaluator.py:528-537): w = (R xyz)_z * mask * (ren > 0) * (sensor > 0) with `xyz` the raw [0,1] coordinate maps
- * and rot [n,3,3] the rotation of the pose being refined (may be NULL for mode 0).  Signed weights follow the
- * reference's order: divide by the sum, then threshold against the max over all pixels; a zero sum leaves t unchanged. */
-int gdrn_depth_refine_step_weighted(const float* xyz, const float* mask, int mask_mode, const float* depth_sensor,
-                                    const float* ren_depth, const float* K_crop, const float* rot, int weight_mode,
-                                    float* trans, int n, int hw, float thresh, void* stream);
+int gdrn_depth_refine_step(const float* xyz, const float* mask, int mask_mode, const float* depth_sensor,
+                           const float* ren_depth, const float* K_crop, const float* rot, int weight_mode, float* trans,
+                           int n, int hw, float thresh, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
  * ROI crop + resize (SURVEY.md 8f rank 1) -- replaces crop_resize_by_warp_affine = cv2.warpAffine

@@ -873,12 +873,28 @@ def _mesh_and_poses(n, seed):
     return v, f, np.stack(poses).astype(np.float32), np.stack(Ks).astype(np.float32)
 
 
-def test_rasteriser_vs_numpy_oracle(dev):
-    from gdrnpp_bop2022_b200.renderer import render_depth
+def _refine_oracle(v, f, poses, Ks, xyz, mask, sensor):
+    """Two refine iterations with the numpy renderer and the reference's refine arithmetic -> t [n,3] f64."""
+    n = len(poses)
+    mx = mask.view(n, -1).max(1)[0].view(n, 1, 1, 1); mn = mask.view(n, -1).min(1)[0].view(n, 1, 1, 1)
+    mnorm = ((mask - mn) / (mx - mn)).cpu().numpy()
+    out = []
+    for i in range(n):
+        t = poses[i, :, 3].astype(np.float64).copy()
+        for _ in range(2):
+            pose = np.hstack([poses[i, :, :3], t[:, None]]).astype(np.float32)
+            ren = OO.render_depth(v, f, pose, Ks[i], 64, 64)
+            t = OO.depth_refine_step(xyz[i].permute(1, 2, 0).cpu().numpy(), mnorm[i, 0], sensor[i].cpu().numpy(), ren, Ks[i], t)
+        out.append(t)
+    return np.stack(out)
+
+
+def test_model3d_render_vs_numpy_oracle(dev):
+    from gdrnpp_bop2022_b200.renderer import Model3D, render_depth
 
     v, f, poses, Ks = _mesh_and_poses(4, seed=1)
-    d = render_depth(torch.from_numpy(v).to(dev), torch.from_numpy(f).to(dev), torch.from_numpy(poses).to(dev),
-                     torch.from_numpy(Ks).to(dev), 64, 64).cpu().numpy()
+    d = render_depth(Model3D(v, f, device=dev), torch.from_numpy(poses).to(dev), torch.from_numpy(Ks).to(dev), 64,
+                     64).cpu().numpy()
     for i in range(4):
         ref = OO.render_depth(v, f, poses[i], Ks[i], 64, 64)
         both = (d[i] > 0) & (ref > 0)
@@ -889,33 +905,26 @@ def test_rasteriser_vs_numpy_oracle(dev):
         assert np.median(np.abs(d[i][both] - ref[both])) < 2e-6
 
 
-def test_depth_refine_vs_oracle(dev):
-    from gdrnpp_bop2022_b200.renderer import depth_refine, render_depth
+def test_model3d_depth_refine_vs_oracle(dev):
+    from gdrnpp_bop2022_b200.renderer import Model3D, depth_refine, render_depth
 
     n = 5
     v, f, poses, Ks = _mesh_and_poses(n, seed=2)
     rs = np.random.RandomState(9)
-    V, F = torch.from_numpy(v).to(dev), torch.from_numpy(f).to(dev)
+    model = Model3D(v, f, device=dev)
     true_poses = poses.copy()
     true_poses[:, :, 3] *= (1 + rs.uniform(-0.04, 0.04, (n, 1)))   # sensor sees the object a bit nearer / farther
-    sensor = render_depth(V, F, torch.from_numpy(true_poses).to(dev), torch.from_numpy(Ks).to(dev), 64, 64)
+    sensor = render_depth(model, torch.from_numpy(true_poses).to(dev), torch.from_numpy(Ks).to(dev), 64, 64)
     sensor[4] = 0  # one ROI without valid depth -> pose must stay unchanged
     xyz = torch.rand(n, 3, 64, 64, generator=torch.Generator().manual_seed(0)).to(dev) - 0.5
     mask = torch.rand(n, 1, 64, 64, generator=torch.Generator().manual_seed(1)).to(dev)
     rot = torch.from_numpy(poses[:, :, :3]).to(dev).contiguous()
     trans = torch.from_numpy(poses[:, :, 3]).to(dev).contiguous()
-    new_t = depth_refine(V, F, rot, trans, torch.from_numpy(Ks).to(dev), xyz, mask, sensor, iters=2, thresh=0.8)
+    new_t = depth_refine(model, rot, trans, torch.from_numpy(Ks).to(dev), xyz, mask, sensor, iters=2, thresh=0.8)
     torch.cuda.synchronize()
-    # oracle: same loop with the numpy renderer + the reference's refine arithmetic
-    mx = mask.view(n, -1).max(1)[0].view(n, 1, 1, 1); mn = mask.view(n, -1).min(1)[0].view(n, 1, 1, 1)
-    mnorm = ((mask - mn) / (mx - mn)).cpu().numpy()
+    t_ref = _refine_oracle(v, f, poses, Ks, xyz, mask, sensor)   # same loop with the numpy renderer
     for i in range(n):
-        t = poses[i, :, 3].astype(np.float64).copy()
-        for _ in range(2):
-            pose = np.hstack([poses[i, :, :3], t[:, None]]).astype(np.float32)
-            ren = OO.render_depth(v, f, pose, Ks[i], 64, 64)
-            t = OO.depth_refine_step(xyz[i].permute(1, 2, 0).cpu().numpy(), mnorm[i, 0], sensor[i].cpu().numpy(), ren, Ks[i], t)
-        assert np.abs(new_t[i].cpu().numpy() - t).max() < 1e-3, i       # north_star: t within 1e-3
+        assert np.abs(new_t[i].cpu().numpy() - t_ref[i]).max() < 1e-3, i       # north_star: t within 1e-3
     assert torch.equal(new_t[4].cpu(), torch.from_numpy(poses[4, :, 3]))
     # and the refinement actually moves towards the truth
     err0 = np.abs(poses[:4, 2, 3] - true_poses[:4, 2, 3]); err1 = np.abs(new_t[:4, 2].cpu().numpy() - true_poses[:4, 2, 3])
@@ -1182,13 +1191,13 @@ def _plane_quad(K, n_pl, d_pl, half=0.6):
     return np.array(corners, np.float32), np.array([[0, 1, 2], [0, 2, 3]], np.int32)
 
 
-def test_renderer_surfaces_plane_analytic_and_quantised_decode(dev, tmp_path):
+def test_model3d_renderer_surfaces_plane_analytic_and_quantised_decode(dev, tmp_path):
     """lib/render_vispy Renderer (set_cam / draw_model / finish) and lib/egl_renderer EGLRenderer.render(pc_cam_tensor=)
     surfaces on an analytic case: a tilted plane covering the window renders to the ray/plane intersection depth at the
     pixel centres (float path, EGL) and to the 24- / 16-bit fixed-point z-buffer decode of renderer.py:176-182 (vispy);
     model paths are PLY files like the reference; two draws share one z-buffer (nearest wins)."""
     from gdrnpp_bop2022_b200.ply import save_ply
-    from gdrnpp_bop2022_b200.renderer import EGLRenderer, Renderer, render_depth
+    from gdrnpp_bop2022_b200.renderer import EGLRenderer, Model3D, Renderer, render_depth
 
     K = np.array([[110.0, 0, 31.5], [0, 112.0, 30.25], [0, 0, 1]], np.float32)
     n_pl, d_pl = np.array([0.2, -0.1, 1.0]), 0.8
@@ -1197,14 +1206,14 @@ def test_renderer_surfaces_plane_analytic_and_quantised_decode(dev, tmp_path):
     rays = np.stack([(cc - K[0, 2]) / K[0, 0], (rr - K[1, 2]) / K[1, 1], np.ones_like(cc)], -1)
     z_true = d_pl / (rays @ n_pl)
     pose = np.hstack([np.eye(3), np.zeros((3, 1))]).astype(np.float32)
-    V, F = torch.from_numpy(v).to(dev), torch.from_numpy(f).to(dev)
+    plane = Model3D(v, f, device=dev)
     P, Kt = torch.from_numpy(pose)[None].to(dev), torch.from_numpy(K)[None].to(dev)
-    d0 = render_depth(V, F, P, Kt, 64, 64).cpu().numpy()[0]
+    d0 = render_depth(plane, P, Kt, 64, 64).cpu().numpy()[0]
     assert (d0 > 0).all() and np.abs(d0 - z_true).max() < 1e-5
     nc, fc = 0.1, 100.0
     mult, addi = np.float32((nc * fc) / (nc - fc)), np.float32(fc / (nc - fc))
     for bits in (24, 16):
-        dq = render_depth(V, F, P, Kt, 64, 64, nc, fc, quantize_bits=bits).cpu().numpy()[0]
+        dq = render_depth(plane, P, Kt, 64, 64, nc, fc, quantize_bits=bits).cpu().numpy()[0]
         win = (1.0 / d0.astype(np.float64) - 1.0 / nc) / (1.0 / fc - 1.0 / nc)     # window depth of the float z
         q = float((1 << bits) - 1)
         expect = mult / (np.float32(np.floor(win * q + 0.5) / q) + addi)            # fixed point -> GL_FLOAT read-back -> decode
@@ -1236,44 +1245,103 @@ def test_renderer_surfaces_plane_analytic_and_quantised_decode(dev, tmp_path):
     assert np.abs(xyz[..., 0] - rays[..., 0] * z_true).max() < 1e-5 and np.abs(xyz[..., 1] - rays[..., 1] * z_true).max() < 1e-5
 
 
-def test_multi_mesh_refine_matches_per_mesh_path(dev):
+def test_multi_mesh_refine_matches_per_roi_renders(dev):
     """depth_refine with several meshes: every ROI picks its mesh from the library's registry inside ONE render launch
-    (rast_upload_mesh / rast_render_meshes); result == rendering each mesh's ROIs separately; get_out_mask folded into
-    the refine kernel == the torch min-max normalisation + the pre-normalised entry."""
+    (rast_upload_mesh / rast_render_meshes); result == rendering each ROI alone; get_out_mask folded into the refine
+    kernel == the torch min-max normalisation + the pre-normalised mask mode."""
     from gdrnpp_bop2022_b200 import _lib as L
-    from gdrnpp_bop2022_b200.renderer import depth_refine, get_out_mask, render_depth, render_meshes, upload_mesh
+    from gdrnpp_bop2022_b200.renderer import Model3D, depth_refine, get_out_mask, render_depth, render_meshes
     from gdrnpp_bop2022_b200.synthetic import make_icosphere_mesh
 
     n = 6
     _, _, poses, Ks = _mesh_and_poses(n, seed=4)
-    meshes = [make_icosphere_mesh(2, e) for e in ((0.12, 0.08, 0.1), (0.06, 0.1, 0.07), (0.09, 0.09, 0.09))]
-    Vs = [torch.from_numpy(v).to(dev) for v, _ in meshes]
-    Fs = [torch.from_numpy(f).to(dev) for _, f in meshes]
+    exts = ((0.12, 0.08, 0.1), (0.06, 0.1, 0.07), (0.09, 0.09, 0.09))
+    models = [Model3D(*make_icosphere_mesh(2, e), device=dev) for e in exts]
     ids = torch.tensor([0, 2, 1, 1, 0, 2])
     P, Kt = torch.from_numpy(poses).to(dev), torch.from_numpy(Ks).to(dev)
-    reg = torch.tensor([upload_mesh(v, f) for v, f in zip(Vs, Fs)], dtype=torch.int32, device=dev)
+    reg = torch.tensor([m.mesh_id for m in models], dtype=torch.int32, device=dev)
     multi = render_meshes(reg[ids.to(dev)], P, Kt, 64, 64)
     for i in range(n):
-        single = render_depth(Vs[ids[i]], Fs[ids[i]], P[i:i + 1], Kt[i:i + 1], 64, 64)[0]
+        single = render_depth(models[ids[i]], P[i:i + 1], Kt[i:i + 1], 64, 64)[0]
         assert torch.equal(multi[i], single), i
     g = torch.Generator().manual_seed(0)
     xyz = (torch.rand(n, 3, 64, 64, generator=g) - 0.5).to(dev)
     mask = torch.rand(n, 1, 64, 64, generator=g).to(dev)
     sensor = multi * 1.03
     rot, trans = P[:, :, :3].contiguous(), P[:, :, 3].contiguous()
-    t_new = depth_refine(Vs, Fs, rot, trans, Kt, xyz, mask, sensor, iters=2, thresh=0.8, mesh_ids=ids)
-    # reference path: per-mesh renders + torch get_out_mask + the pre-normalised kernel entry
+    t_new = depth_refine(models, rot, trans, Kt, xyz, mask, sensor, iters=2, thresh=0.8, mesh_ids=ids)
+    # reference path: one render per ROI + torch get_out_mask + the kernel's pre-normalised mask mode
     t_ref = trans.clone()
     mnorm = get_out_mask(mask).reshape(n, 64, 64).contiguous()
     lib = L.lib()
     for _ in range(2):
         pp = torch.cat([rot, t_ref[:, :, None]], dim=2).contiguous()
-        ren = torch.stack([render_depth(Vs[ids[i]], Fs[ids[i]], pp[i:i + 1], Kt[i:i + 1], 64, 64)[0] for i in range(n)]).contiguous()
-        L.check(lib.gdrn_depth_refine_step(L.ptr(xyz), L.ptr(mnorm), L.ptr(sensor.contiguous()), L.ptr(ren), L.ptr(Kt), L.ptr(t_ref), n, 64,
-                                           0.8, L.current_stream()), "refine")
+        ren = torch.stack([render_depth(models[ids[i]], pp[i:i + 1], Kt[i:i + 1], 64, 64)[0] for i in range(n)]).contiguous()
+        L.check(lib.gdrn_depth_refine_step(L.ptr(xyz), L.ptr(mnorm), 0, L.ptr(sensor.contiguous()), L.ptr(ren), L.ptr(Kt), None, 0,
+                                           L.ptr(t_ref), n, 64, 0.8, L.current_stream()), "refine")
     torch.cuda.synchronize()
     assert (t_new - t_ref).abs().max().item() < 1e-6
     assert (t_new - trans).abs().max().item() > 1e-3     # it did move
+
+
+def test_registry_id_is_held_by_the_uploading_object(dev):
+    """Two meshes with equal V and F but different geometry, made one after the other with the first dropped in
+    between (so the second's tensors may reuse the first's device memory): each renders its own geometry, through
+    bop_eval.VsdMeshes and through Model3D + depth_refine.  Repeated depth_refine calls upload nothing."""
+    import gc
+
+    from gdrnpp_bop2022_b200 import _lib as L
+    from gdrnpp_bop2022_b200 import bop_eval
+    from gdrnpp_bop2022_b200.renderer import Model3D, depth_refine, render_depth
+    from gdrnpp_bop2022_b200.synthetic import make_icosphere_mesh
+
+    n = 4
+    _, _, poses, Ks = _mesh_and_poses(n, seed=6)
+    (va, fa), (vb, fb) = (make_icosphere_mesh(2, e) for e in ((0.12, 0.08, 0.1), (0.05, 0.11, 0.06)))
+    assert va.shape == vb.shape and np.array_equal(fa, fb)
+    R, t = poses[:, :, :3], poses[:, :, 3]
+    refs = {k: np.stack([OO.render_depth(v, f, poses[i], Ks[i], 64, 64) for i in range(n)])
+            for k, (v, f) in (("a", (va, fa)), ("b", (vb, fb)))}
+    assert all(((refs["a"][i] > 0) != (refs["b"][i] > 0)).sum() > 50 for i in range(n))   # the two render apart
+
+    def assert_renders(d, k):
+        d = d.cpu().numpy()
+        for i in range(n):
+            ref = refs[k][i]
+            both = (d[i] > 0) & (ref > 0)
+            assert ((d[i] > 0) != (ref > 0)).sum() <= 6, (k, i)
+            assert np.abs(d[i][both] - ref[both]).max() < 1e-3, (k, i)
+
+    first = bop_eval.VsdMeshes({1: (va, fa)}, device=dev)
+    assert_renders(first.render([1] * n, R, t, Ks, 64, 64), "a")
+    del first
+    gc.collect()
+    second = bop_eval.VsdMeshes({1: (vb, fb)}, device=dev)
+    assert_renders(second.render([1] * n, R, t, Ks, 64, 64), "b")
+
+    P, Kt = torch.from_numpy(poses).to(dev), torch.from_numpy(Ks).to(dev)
+    first = Model3D(va, fa, device=dev)
+    assert_renders(render_depth(first, P, Kt, 64, 64), "a")
+    del first
+    gc.collect()
+    count = L.lib().rast_mesh_count()
+    second = Model3D(vb, fb, device=dev)
+    assert L.lib().rast_mesh_count() == count + 1
+    assert_renders(render_depth(second, P, Kt, 64, 64), "b")
+    g = torch.Generator().manual_seed(0)
+    xyz = (torch.rand(n, 3, 64, 64, generator=g) - 0.5).to(dev)
+    mask = torch.rand(n, 1, 64, 64, generator=g).to(dev)
+    truth = P.clone()
+    truth[:, :, 3] *= 1.03
+    sensor = render_depth(second, truth, Kt, 64, 64)
+    args = (second, P[:, :, :3].contiguous(), P[:, :, 3].contiguous(), Kt, xyz, mask, sensor)
+    t_new = depth_refine(*args, iters=2, thresh=0.8)
+    assert np.abs(t_new.cpu().numpy() - _refine_oracle(vb, fb, poses, Ks, xyz, mask, sensor)).max() < 1e-3
+    for _ in range(2):
+        assert torch.equal(depth_refine(*args, iters=2, thresh=0.8), t_new)
+        assert torch.equal(depth_refine([second], *args[1:], iters=2, thresh=0.8, mesh_ids=torch.zeros(n, dtype=torch.long)),
+                           t_new)
+    assert L.lib().rast_mesh_count() == count + 1
 
 
 # ------------------------------------------------------------------------------- depthwise 7x7 + LayerNorm kernels

@@ -233,11 +233,11 @@ def _host_renders(meshes, obj_ids, R, t, K, H, W):
 
 
 @pytest.mark.gpu
-def test_in_memory_edge_cases_and_chunking(lib, dev):
+def test_in_memory_edge_cases_and_chunking_on_vsd_meshes(lib, dev):
     from gdrnpp_bop2022_b200 import bop_eval
 
     H, W = 120, 160
-    meshes = gt_info.Meshes(_box_meshes(), device=dev)
+    meshes = bop_eval.VsdMeshes(_box_meshes(), device=dev)
     K = np.array([[[150.0, 0, 80.3], [0, 150.0, 59.6], [0, 0, 1]], [[140.0, 0, 77.0], [0, 145.0, 62.0], [0, 0, 1]],
                   [[150.0, 0, 80.0], [0, 150.0, 60.0], [0, 0, 1]]])
     yy, xx = np.mgrid[0:H, 0:W]
@@ -310,7 +310,7 @@ def _read_outputs(sp):
 
 
 @pytest.mark.gpu
-def test_cli_end_to_end_matches_host_restatement(lib, dev, tmp_path):
+def test_cli_end_to_end_matches_host_restatement_on_vsd_meshes(lib, dev, tmp_path):
     from gdrnpp_bop2022_b200 import bop_eval
 
     root = str(tmp_path / "datasets")
@@ -321,7 +321,7 @@ def test_cli_end_to_end_matches_host_restatement(lib, dev, tmp_path):
                    check=True, cwd=str(tmp_path), env=env)
     got = _read_outputs(sp)
     models = gt_info.load_models(gt_info.models_path(os.path.join(root, "BOP_DATASETS"), "ycbv"), range(1, 7))
-    meshes = gt_info.Meshes(models, device=dev)
+    meshes = bop_eval.VsdMeshes(models, device=dev)
     n_vis = n_occ = 0
     for scene_id, ims in gt_info.plan_split(sp):
         scene_info = {}

@@ -261,10 +261,10 @@ def _coor_z_inputs(seed, n=4, hw=64):
 
 
 @pytest.mark.gpu
-def test_coor_z_depth_refine_step_vs_numpy(dev):
-    """gdrn_depth_refine_step_weighted(weight_mode=1) == the reference's coor-z iteration restated in numpy, with
-    negative weights, a negative sum (the cut then comes from the most negative weight) and an exactly-zero sum (pose
-    unchanged); weight_mode 0 stays torch.equal to gdrn_depth_refine_step_ex."""
+def test_coor_z_single_refine_entry_vs_numpy(dev):
+    """gdrn_depth_refine_step(weight_mode=1) == the reference's coor-z iteration restated in numpy, with negative
+    weights, a negative sum (the cut then comes from the most negative weight) and an exactly-zero sum (pose unchanged);
+    weight_mode 0 ignores the rotations."""
     from gdrnpp_bop2022_b200 import _lib as L
 
     xyz, mask, ren, sensor, K, R, t = _coor_z_inputs(3)
@@ -273,21 +273,15 @@ def test_coor_z_depth_refine_step_vs_numpy(dev):
     xyz_d, mask_d, ren_d, sen_d, K_d, R_d = T(xyz), T(mask), T(ren), T(sensor), T(K), T(R)
     stream = L.current_stream()
 
-    def run(entry, *args):
+    def run(rot, mode):
         out = T(t).clone()
-        if entry == "ex":
-            L.check(L.lib().gdrn_depth_refine_step_ex(L.ptr(xyz_d), L.ptr(mask_d), 1, L.ptr(sen_d), L.ptr(ren_d), L.ptr(K_d), L.ptr(out),
-                                                      n, hw, 0.8, stream), entry)
-        else:
-            rot, mode = args
-            L.check(L.lib().gdrn_depth_refine_step_weighted(L.ptr(xyz_d), L.ptr(mask_d), 1, L.ptr(sen_d), L.ptr(ren_d), L.ptr(K_d),
-                                                            L.ptr(rot), mode, L.ptr(out), n, hw, 0.8, stream), entry)
+        L.check(L.lib().gdrn_depth_refine_step(L.ptr(xyz_d), L.ptr(mask_d), 1, L.ptr(sen_d), L.ptr(ren_d), L.ptr(K_d),
+                                               L.ptr(rot), mode, L.ptr(out), n, hw, 0.8, stream), "gdrn_depth_refine_step")
         torch.cuda.synchronize()
         return out.cpu()
 
-    assert torch.equal(run("weighted", None, 0), run("ex"))
-    assert torch.equal(run("weighted", R_d, 0), run("ex"))
-    got = run("weighted", R_d, 1).numpy()
+    assert torch.equal(run(None, 0), run(R_d, 0))
+    got = run(R_d, 1).numpy()
     mn, mx = mask.reshape(n, -1).min(1)[:, None, None], mask.reshape(n, -1).max(1)[:, None, None]
     mask_n = (mask - mn) / (mx - mn)
     sums = []
@@ -301,16 +295,16 @@ def test_coor_z_depth_refine_step_vs_numpy(dev):
     assert sums[0] > 0 and sums[1] < 0 and sums[3] == 0.0
     assert np.array_equal(got[3], t[3]) and not np.array_equal(got[1], t[1])
     with pytest.raises(L.GdrnError):        # coor-z needs the rotations; unknown weight modes are rejected
-        run("weighted", None, 1)
+        run(None, 1)
     with pytest.raises(L.GdrnError):
-        run("weighted", R_d, 2)
+        run(R_d, 2)
 
 
 @pytest.mark.gpu
-def test_depth_refine_coor_z_vs_oracle(dev):
+def test_model3d_depth_refine_coor_z_vs_oracle(dev):
     """renderer.depth_refine(coor_z_refine=True): render + coor-z refine, 2 iterations, vs the numpy renderer and the
     reference's coor-z arithmetic; the default weighting is unchanged by the new keyword."""
-    from gdrnpp_bop2022_b200.renderer import depth_refine, render_depth
+    from gdrnpp_bop2022_b200.renderer import Model3D, depth_refine, render_depth
     from gdrnpp_bop2022_b200.synthetic import make_icosphere_mesh
 
     n = 4
@@ -324,13 +318,13 @@ def test_depth_refine_coor_z_vs_oracle(dev):
     poses, Ks = np.stack(poses).astype(np.float32), np.stack(Ks).astype(np.float32)
     true_poses = poses.copy()
     true_poses[:, :, 3] *= (1 + rs.uniform(-0.04, 0.04, (n, 1)))
-    V, F = torch.from_numpy(v).to(dev), torch.from_numpy(f).to(dev)
-    sensor = render_depth(V, F, torch.from_numpy(true_poses).to(dev), torch.from_numpy(Ks).to(dev), 64, 64)
+    model = Model3D(v, f, device=dev)
+    sensor = render_depth(model, torch.from_numpy(true_poses).to(dev), torch.from_numpy(Ks).to(dev), 64, 64)
     xyz = torch.rand(n, 3, 64, 64, generator=torch.Generator().manual_seed(0)).to(dev)
     mask = torch.rand(n, 1, 64, 64, generator=torch.Generator().manual_seed(1)).to(dev)
     rot = torch.from_numpy(poses[:, :, :3]).to(dev).contiguous()
     trans = torch.from_numpy(poses[:, :, 3]).to(dev).contiguous()
-    args = (V, F, rot, trans, torch.from_numpy(Ks).to(dev), xyz, mask, sensor)
+    args = (model, rot, trans, torch.from_numpy(Ks).to(dev), xyz, mask, sensor)
     new_t = depth_refine(*args, iters=2, thresh=0.8, coor_z_refine=True).cpu().numpy()
     assert torch.equal(depth_refine(*args, iters=2, thresh=0.8, coor_z_refine=False), depth_refine(*args, iters=2, thresh=0.8))
     mx = mask.view(n, -1).max(1)[0].view(n, 1, 1, 1); mn = mask.view(n, -1).min(1)[0].view(n, 1, 1, 1)

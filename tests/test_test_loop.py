@@ -356,9 +356,9 @@ def _per_image_driver(cfg, model, root, ts, dev):
         K_crop = get_K_crop_resize(cam, f("roi_center") - scale.view(n, 1) / 2, (64.0 / scale).view(n, 1))
         sensor = ((rd[:, 1::4, 1::4] + rd[:, 1::4, 2::4]) + (rd[:, 2::4, 1::4] + rd[:, 2::4, 2::4])) * 0.25
         xyz = torch.cat([out["coor_x"], out["coor_y"], out["coor_z"]], dim=1)
-        t = depth_refine([m.vertices for m in meshes], [m.faces for m in meshes], out["rot"], out["trans"], K_crop, xyz,
-                         out["mask"], sensor.contiguous(), iters=cfg.TEST.DEPTH_REFINE_ITER,
-                         thresh=cfg.TEST.DEPTH_REFINE_THRESHOLD, mesh_ids=cls, coor_z_refine=cfg.TEST.USE_COOR_Z_REFINE)
+        t = depth_refine(meshes, out["rot"], out["trans"], K_crop, xyz, out["mask"], sensor.contiguous(),
+                         iters=cfg.TEST.DEPTH_REFINE_ITER, thresh=cfg.TEST.DEPTH_REFINE_THRESHOLD, mesh_ids=cls,
+                         coor_z_refine=cfg.TEST.USE_COOR_Z_REFINE)
         R = out["rot"].cpu().numpy()
         t = t.cpu().numpy()
         sid, iid = ts.images[idx]
@@ -370,7 +370,7 @@ def _per_image_driver(cfg, model, root, ts, dev):
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("coor_z", [False, True])
-def test_depth_refine_matches_per_image_driver(dev, tmp_path, coor_z):
+def test_depth_refine_matches_per_image_model3d_driver(dev, tmp_path, coor_z):
     root, det = _tree(tmp_path, num_images=6, seed=5)
     cfg = _cfg(det, USE_PNP=False, USE_DEPTH_REFINE=True, USE_COOR_Z_REFINE=coor_z, DEPTH_REFINE_ITER=2,
                DEPTH_REFINE_THRESHOLD=0.8)
