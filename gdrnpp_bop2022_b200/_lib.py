@@ -73,8 +73,10 @@ _SIGNATURES = {
     "gdrn_depth_refine_step": (c_int, [c_void_p, c_void_p, c_int] + [c_void_p] * 4 + [c_int, c_void_p, c_int, c_int, c_float,
                                                                                  c_void_p]),
     "rast_upload_mesh": (c_int, [c_void_p, c_int, c_void_p, c_int]),
+    "rast_upload_mesh_ex": (c_int, [c_void_p, c_int, c_void_p, c_int, c_void_p]),
     "rast_mesh_count": (c_int, []),
     "rast_render_meshes": (c_int, [c_void_p] * 3 + [c_int] * 3 + [c_float, c_float, c_int] + [c_void_p] * 4),
+    "rast_render_meshes_rgb": (c_int, [c_void_p] * 4 + [c_int] * 3 + [c_float, c_float] + [c_void_p] * 5),
     "gdrn_pnp_ransac_maps": (c_int, [c_void_p] * 9 + [c_int] * 3 + [c_float, c_float, c_uint] + [c_void_p] * 4),
     "gdrn_pnp_ransac_points": (c_int, [c_void_p] * 4 + [c_int] * 3 + [c_float, c_uint] + [c_void_p] * 4),
     "gdrn_pnp_net_maps": (c_int, [c_void_p] * 10 + [c_int] * 3 + [c_float, c_float, c_int, c_uint] + [c_void_p] * 3),
@@ -125,6 +127,9 @@ _SIGNATURES = {
                                                                        c_size_t, c_void_p, c_size_t, c_void_p, c_void_p]),
     "gdrn_rle_confusion": (c_int, [c_void_p, c_size_t, c_void_p, c_int, c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p]),
     "gdrn_gt_info": (c_int, [c_void_p] * 6 + [c_int] * 3 + [c_float] + [c_void_p] * 5),
+    "gdrn_vis_poses_workspace_bytes": (c_size_t, [c_int] * 3),
+    "gdrn_vis_poses": (c_int, [c_void_p] * 3 + [c_int] * 3 + [c_void_p] * 2 + [c_int] * 3 + [c_void_p] * 9 + [c_size_t,
+                                                                                                         c_void_p]),
 }
 
 EXPORTED_SYMBOLS = tuple(_SIGNATURES.keys())

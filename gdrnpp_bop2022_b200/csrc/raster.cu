@@ -117,6 +117,80 @@ __global__ void rast_resolve_kernel(const unsigned long long* __restrict__ zbuf,
   }
 }
 
+// Colour resolve: each covered pixel's winning triangle (the low word of the rasteriser's key) is shaded with
+// renderer_py's flat fragment shader (lib/pysixd/renderer_py.py:52-75), light at the eye origin, ambient 0.5:
+//   L = normalize(interp(normalize(-P_k))),  n = face normal turned toward the viewer,
+//   rgb = rint(min(0.5 + max(dot(L, n), 0), 1) * colour * 255).
+// The screen barycentrics are recomputed with the rasteriser's arithmetic and made perspective-correct
+// (b_k = w_k / Z_k / sum(w / Z)), which is how GL interpolates v_L and v_color.  The face normal of a plane through
+// the eye-facing side satisfies dot(n, P) <= 0 for every point P of the triangle, so it is turned once per triangle.
+// Colour: colors [n,3] per render when given, else the mesh's vertex colours, else grey 0.5.  Depth, coverage and
+// tri_ids come straight from the key, so they equal rast_render_meshes' float-z output.
+__global__ void __launch_bounds__(256)
+rast_shade_kernel(const unsigned long long* __restrict__ zbuf, const MeshEntry* __restrict__ table,
+                  const float* const* __restrict__ mesh_colors, const int* __restrict__ mesh_ids,
+                  const float* __restrict__ poses, const float* __restrict__ Ks, const float* __restrict__ colors, int n,
+                  int H, int W, uint8_t* __restrict__ rgb, float* __restrict__ depth, int* __restrict__ tri_ids) {
+  const long long total = (long long)n * H * W;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total;
+       i += (long long)gridDim.x * blockDim.x) {
+    const unsigned long long key = zbuf[i];
+    if (key == 0xFFFFFFFFFFFFFFFFull) {
+      depth[i] = 0.f;
+      rgb[i * 3] = 0; rgb[i * 3 + 1] = 0; rgb[i * 3 + 2] = 0;
+      if (tri_ids) tri_ids[i] = -1;
+      continue;
+    }
+    depth[i] = __uint_as_float((unsigned)(key >> 32));
+    const int f = (int)(unsigned)key;
+    if (tri_ids) tri_ids[i] = f;
+    const int px = (int)(i % W), py = (int)((i / W) % H), r = (int)(i / ((long long)H * W));
+    const MeshEntry me = table[mesh_ids[r]];
+    const float* P = poses + r * 12;
+    const float* K = Ks + r * 9;
+    float X[3], Y[3], Z[3], u[3], v[3], iz[3];
+#pragma unroll
+    for (int k = 0; k < 3; ++k) {
+      const int vi = me.faces[f * 3 + k];
+      const float x = me.verts[vi * 3], y = me.verts[vi * 3 + 1], z = me.verts[vi * 3 + 2];
+      X[k] = P[0] * x + P[1] * y + P[2] * z + P[3];
+      Y[k] = P[4] * x + P[5] * y + P[6] * z + P[7];
+      Z[k] = P[8] * x + P[9] * y + P[10] * z + P[11];
+      iz[k] = 1.0f / Z[k];
+      u[k] = (K[0] * X[k] + K[1] * Y[k]) * iz[k] + K[2];
+      v[k] = (K[4] * Y[k]) * iz[k] + K[5];
+    }
+    const float inv_area = 1.0f / ((u[1] - u[0]) * (v[2] - v[0]) - (u[2] - u[0]) * (v[1] - v[0]));
+    const float sx = (float)px + 0.5f, sy = (float)py + 0.5f;
+    const float w0 = ((u[1] - sx) * (v[2] - sy) - (u[2] - sx) * (v[1] - sy)) * inv_area;
+    const float w1 = ((u[2] - sx) * (v[0] - sy) - (u[0] - sx) * (v[2] - sy)) * inv_area;
+    const float w2 = 1.0f - w0 - w1;
+    const float izp = w0 * iz[0] + w1 * iz[1] + w2 * iz[2];
+    const float b[3] = {w0 * iz[0] / izp, w1 * iz[1] / izp, w2 * iz[2] / izp};
+    float lx = 0.f, ly = 0.f, lz = 0.f;
+#pragma unroll
+    for (int k = 0; k < 3; ++k) {   // v_L = normalize(light - eye_pos) per vertex, light at the eye origin
+      const float il = rsqrtf(X[k] * X[k] + Y[k] * Y[k] + Z[k] * Z[k]);
+      lx -= b[k] * X[k] * il; ly -= b[k] * Y[k] * il; lz -= b[k] * Z[k] * il;
+    }
+    const float ex = X[1] - X[0], ey = Y[1] - Y[0], ez = Z[1] - Z[0];
+    const float gx = X[2] - X[0], gy = Y[2] - Y[0], gz = Z[2] - Z[0];
+    float nx = ey * gz - ez * gy, ny = ez * gx - ex * gz, nz = ex * gy - ey * gx;
+    if (nx * X[0] + ny * Y[0] + nz * Z[0] > 0.f) { nx = -nx; ny = -ny; nz = -nz; }
+    const float dot = (lx * nx + ly * ny + lz * nz) * rsqrtf(lx * lx + ly * ly + lz * lz) * rsqrtf(nx * nx + ny * ny + nz * nz);
+    const float lw = fminf(0.5f + fmaxf(dot, 0.f), 1.f);
+    const float* vc = mesh_colors[mesh_ids[r]];
+#pragma unroll
+    for (int c = 0; c < 3; ++c) {
+      float col = 0.5f;
+      if (colors) col = colors[r * 3 + c];
+      else if (vc) col = b[0] * vc[me.faces[f * 3] * 3 + c] + b[1] * vc[me.faces[f * 3 + 1] * 3 + c] +
+                         b[2] * vc[me.faces[f * 3 + 2] * 3 + c];
+      rgb[i * 3 + c] = (uint8_t)fminf(fmaxf(rintf(lw * col * 255.f), 0.f), 255.f);
+    }
+  }
+}
+
 // ------------------------------------------------------------------------------------------------
 // Fast depth refine, one CTA per ROI (gdrn_evaluator.py:539-561):
 //   w = ||xyz|| * mask * (ren>0) * (sensor>0);  w /= sum(w);  sel = w > thresh*max(w)
@@ -268,12 +342,13 @@ struct MeshRegistry {
   int max_faces = 0;
   MeshEntry host[RAST_MAX_MESHES];
   MeshEntry* dev_table = nullptr;
+  const float** dev_colors = nullptr;   // [RAST_MAX_MESHES] per-vertex RGB [V,3] f32, or null for a mesh without colours
 };
 MeshRegistry g_meshes;
 }  // namespace
 
-extern "C" int rast_upload_mesh(const float* verts, int V, const int* faces, int F) {
-  // verts / faces: host OR device pointers (cudaMemcpyDefault); the library keeps its own device copy.
+extern "C" int rast_upload_mesh_ex(const float* verts, int V, const int* faces, int F, const float* colors) {
+  // verts / faces / colors: host OR device pointers (cudaMemcpyDefault); the library keeps its own device copy.
   // Returns the mesh id (>= 0) or a negative GDRN_ERR_* code.
   if (!(verts && faces && V > 0 && F > 0)) { gdrn_set_last_error(__FILE__, __LINE__, "rast_upload_mesh: empty mesh"); return GDRN_ERR_INVALID; }
   int dev = 0;
@@ -283,15 +358,21 @@ extern "C" int rast_upload_mesh(const float* verts, int V, const int* faces, int
   if (g_meshes.count >= RAST_MAX_MESHES) { gdrn_set_last_error(__FILE__, __LINE__, "rast_upload_mesh: registry full (1024 meshes)"); return GDRN_ERR_STATE; }
   float* dv = nullptr;
   int* df = nullptr;
+  float* dc = nullptr;
   cudaError_t e = cudaMalloc(&dv, (size_t)V * 12);
   if (e == cudaSuccess) e = cudaMalloc(&df, (size_t)F * 12);
   if (e == cudaSuccess) e = cudaMemcpy(dv, verts, (size_t)V * 12, cudaMemcpyDefault);
   if (e == cudaSuccess) e = cudaMemcpy(df, faces, (size_t)F * 12, cudaMemcpyDefault);
+  if (e == cudaSuccess && colors) e = cudaMalloc(&dc, (size_t)V * 12);
+  if (e == cudaSuccess && colors) e = cudaMemcpy(dc, colors, (size_t)V * 12, cudaMemcpyDefault);
   if (e == cudaSuccess && !g_meshes.dev_table) e = cudaMalloc(&g_meshes.dev_table, sizeof(MeshEntry) * RAST_MAX_MESHES);
+  if (e == cudaSuccess && !g_meshes.dev_colors) e = cudaMalloc(&g_meshes.dev_colors, sizeof(float*) * RAST_MAX_MESHES);
   if (e == cudaSuccess) {
     const int id = g_meshes.count;
     g_meshes.host[id] = MeshEntry{dv, df, V, F};
+    const float* dcc = dc;
     e = cudaMemcpy(g_meshes.dev_table + id, &g_meshes.host[id], sizeof(MeshEntry), cudaMemcpyHostToDevice);
+    if (e == cudaSuccess) e = cudaMemcpy(g_meshes.dev_colors + id, &dcc, sizeof(float*), cudaMemcpyHostToDevice);
     if (e == cudaSuccess) {
       g_meshes.count = id + 1;
       if (F > g_meshes.max_faces) g_meshes.max_faces = F;
@@ -299,9 +380,13 @@ extern "C" int rast_upload_mesh(const float* verts, int V, const int* faces, int
     }
   }
   (void)cudaGetLastError();
-  cudaFree(dv); cudaFree(df);
+  cudaFree(dv); cudaFree(df); cudaFree(dc);
   gdrn_set_last_error(__FILE__, __LINE__, cudaGetErrorString(e));
   return GDRN_ERR_CUDA;
+}
+
+extern "C" int rast_upload_mesh(const float* verts, int V, const int* faces, int F) {
+  return rast_upload_mesh_ex(verts, V, faces, F, nullptr);
 }
 
 extern "C" int rast_mesh_count(void) { return g_meshes.count; }
@@ -322,6 +407,26 @@ extern "C" int rast_render_meshes(const int* mesh_ids, const float* poses, const
   rast_tri_multi_kernel<<<dim3((g_meshes.max_faces + 255) / 256, n), 256, 0, st>>>(g_meshes.dev_table, mesh_ids, g_meshes.count, poses, Ks,
                                                                                  H, W, znear, zfar, zbuf_scratch);
   rast_resolve_kernel<<<blocks, 256, 0, st>>>(zbuf_scratch, Ks, n, H, W, znear, zfar, quantize_bits, depth, xyz_cam);
+  GDRN_CHECK_CUDA(cudaGetLastError());
+  gdrn_count_launch(3);
+  return GDRN_OK;
+}
+
+extern "C" int rast_render_meshes_rgb(const int* mesh_ids, const float* poses, const float* Ks, const float* colors, int n,
+                                      int H, int W, float znear, float zfar, uint8_t* rgb, float* depth, int* tri_ids,
+                                      unsigned long long* zbuf_scratch, void* stream) {
+  GDRN_REQUIRE(mesh_ids && poses && Ks && rgb && depth && zbuf_scratch, "rast_render_meshes_rgb: null argument");
+  GDRN_REQUIRE(n > 0 && H > 0 && W > 0, "rast_render_meshes_rgb: empty input");
+  GDRN_REQUIRE(g_meshes.count > 0, "rast_render_meshes_rgb: no mesh uploaded (rast_upload_mesh)");
+  GDRN_REQUIRE(znear > 0.f && zfar > znear, "rast: need 0 < znear < zfar");
+  cudaStream_t st = (cudaStream_t)stream;
+  const long long npx = (long long)n * H * W;
+  int blocks = (int)((npx + 255) / 256 > 4096 ? 4096 : (npx + 255) / 256);
+  rast_clear_kernel<<<blocks, 256, 0, st>>>(zbuf_scratch, npx);
+  rast_tri_multi_kernel<<<dim3((g_meshes.max_faces + 255) / 256, n), 256, 0, st>>>(g_meshes.dev_table, mesh_ids, g_meshes.count, poses, Ks,
+                                                                                 H, W, znear, zfar, zbuf_scratch);
+  rast_shade_kernel<<<blocks, 256, 0, st>>>(zbuf_scratch, g_meshes.dev_table, g_meshes.dev_colors, mesh_ids, poses, Ks, colors,
+                                            n, H, W, rgb, depth, tri_ids);
   GDRN_CHECK_CUDA(cudaGetLastError());
   gdrn_count_launch(3);
   return GDRN_OK;

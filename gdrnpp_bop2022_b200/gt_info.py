@@ -256,16 +256,22 @@ def split_params(datasets_path, dataset, split, split_type=None):
     if split_type is not None and split_type != "bb8":
         split_path += "_" + split_type
     depth_ext = ".tif" if dataset == "itodd" and split_type != "pbr" else ".png"
+    # the colour image: rgb/ (JPEG for pbr), or for ITODD gray/ (.tif); vis_gt_poses.py reads rgb/ for any pbr split
+    im_modality = "gray" if dataset == "itodd" and split_type != "pbr" else "rgb"
+    im_ext = ".jpg" if split_type == "pbr" else (".tif" if im_modality == "gray" else ".png")
     return {"base_path": os.path.join(datasets_path, name), "split_path": split_path, "split_type": split_type,
-            "depth_ext": depth_ext}
+            "depth_ext": depth_ext, "im_modality": im_modality, "im_ext": im_ext}
 
 
-def models_path(datasets_path, dataset, models_dir=None):
-    """The model directory the scripts render: models/ (models_cad/ for T-LESS), or models_dir when given."""
+def models_path(datasets_path, dataset, models_dir=None, model_type=None):
+    """The model directory the scripts render: models/ (models_cad/ for T-LESS), models_{model_type}/ when a model type
+    is given (vis_gt_poses.py: "eval"), or models_dir when given."""
     if models_dir:
         return models_dir
     name = {"hbs": "hb", "ycbvposecnn": "ycbv"}.get(dataset, dataset)
-    return os.path.join(datasets_path, name, "models_cad" if dataset == "tless" else "models")
+    if model_type is None and dataset == "tless":
+        model_type = "cad"
+    return os.path.join(datasets_path, name, "models" + ("_" + model_type if model_type else ""))
 
 
 def depth_path(split_path, scene_id, im_id, depth_ext):
@@ -276,6 +282,15 @@ def depth_path(split_path, scene_id, im_id, depth_ext):
         if not os.path.exists(p2):
             raise GdrnError("missing depth image {}".format(p))
         p = p2
+    return p
+
+
+def image_path(sp, scene_id, im_id):
+    """The colour (or ITODD gray) image of one view, as the split's rgb_tpath / gray_tpath names it.  Raises when it
+    does not exist."""
+    p = os.path.join(sp["split_path"], "{:06d}".format(scene_id), sp["im_modality"], "{:06d}{}".format(im_id, sp["im_ext"]))
+    if not os.path.exists(p):
+        raise GdrnError("missing {} image {}".format(sp["im_modality"], p))
     return p
 
 

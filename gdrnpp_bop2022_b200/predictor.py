@@ -117,6 +117,11 @@ class GdrnPredictor:
             if models is None and len(loaded) == len(self.obj_ids):
                 models = loaded
         self.extents = {k: np.asarray(v, np.float32) for k, v in extents.items()}
+        # model points (metres) that gdrn_visualization projects: the loaded PLYs, else the given meshes' vertices
+        self.model_pts = {i: m["pts"] for i, m in self.obj_models.items()}
+        if models is not None:
+            for i, m in models.items():
+                self.model_pts.setdefault(int(i), np.asarray(m[0], np.float64))
         # ---- model (set_eval_model, predictor_gdrn.py:113-122) ----
         per_object_sd = isinstance(state_dict, Mapping) and bool(state_dict) and all(
             isinstance(v, Mapping) for v in state_dict.values())
@@ -347,6 +352,114 @@ class GdrnPredictor:
         return depth_refine(self.ren_models, out_dict["rot"], out_dict["trans"], K_crop, xyz, out_dict["mask"], d.contiguous(),
                             iters=self.cfg.TEST.DEPTH_REFINE_ITER, thresh=self.cfg.TEST.DEPTH_REFINE_THRESHOLD,
                             mesh_ids=inputs["roi_cls"], coor_z_refine=bool(self.cfg.TEST.USE_COOR_Z_REFINE))
+
+
+    # ---- visualisation (predictor_gdrn.py:583-630) ---------------------------------------------
+    def gdrn_visualization(self, batch, out_dict, image, frame_count=0, *, show=True):
+        """The reference's panels, side by side, returned as one u8 image in the input's channel order:
+          * with "full_mask" in out_dict: every ROI's full mask (get_out_mask with MASK_LOSS_TYPE, pasted into the image
+            at threshold 0.5 on the device by native_ops.paste_masks_in_image) blended in a colour drawn from
+            np.random, with the bbox_est boxes and labels (vis_image_mask_bbox_cv2);
+          * per ROI: the object's model points projected with the ROI's pose (points2d_to_mask) blended in yellow
+            (ROI 0) or blue, with its box and label (vis_image_mask_cv2 + vis_image_bboxes_cv2).
+        The reference flips channels twice before cv2.hstack, which leaves them as they were.  Colours come from
+        np.random exactly as the reference draws them, so a seeded run is reproducible.  Deviation: ROI i's points and
+        label are those of ROI i's object (the reference uses obj_models[i + 1] and cls_names[i]).  cv2.imshow /
+        waitKey(0) only with show.  Needs postprocessing() to have filled batch["cur_res"]."""
+        import cv2
+
+        from .native_ops import paste_masks_in_image
+        from .renderer import get_out_mask
+
+        image = np.ascontiguousarray(image.detach().cpu().numpy() if torch.is_tensor(image) else image, np.uint8)
+        bs = int(batch["roi_cls"].shape[0])
+        im_H, im_W = image.shape[:2]
+        names = [self.objs[self.obj_ids[int(c)]] for c in batch["roi_cls"].tolist()]
+        boxes = [np.asarray(b.detach().cpu().numpy() if torch.is_tensor(b) else b) for b in batch["bbox_est"]]
+        panels = []
+        if "full_mask" in out_dict:
+            masks = np.zeros((0, im_H, im_W), np.uint8)
+            if bs:
+                half = batch["scale"].view(bs, -1) / 2
+                rois = torch.cat([batch["roi_center"] - half, batch["roi_center"] + half], dim=1)
+                probs = get_out_mask(out_dict["full_mask"], str(_cfg_get(self.cfg, "MODEL.POSE_NET.LOSS_CFG.MASK_LOSS_TYPE", "L1")))
+                masks = paste_masks_in_image(probs[:, 0], rois, (im_H, im_W), threshold=0.5).to(torch.uint8).cpu().numpy()
+            panels.append(_vis_image_mask_bbox_cv2(image, masks, boxes, names))
+        K = self.cam.astype(np.float64)
+        for i in range(bs):
+            res = batch["cur_res"][i]
+            oid = self.obj_ids[int(batch["roi_cls"][i])]
+            if oid not in self.model_pts:
+                raise ValueError(f"gdrn_visualization: no model points for obj_id {oid} (path_to_obj_models or models=)")
+            mask = _points2d_to_mask(_project_pts(self.model_pts[oid], K, res["R"], res["t"]), im_H, im_W)
+            im = _vis_image_mask_cv2(image, mask, _YELLOW if i == 0 else _BLUE)
+            panels.append(_vis_image_bboxes_cv2(im, [boxes[i]], [names[i]]))
+        show_ims = np.hstack(panels) if panels else image.copy()
+        if show:
+            cv2.imshow("Main", show_ims)
+            cv2.waitKey(0)
+        return show_ims
+
+
+# lib/vis_utils/image.py drawing helpers (mmcv.color_val colours are BGR tuples)
+_GREEN = (18, 127, 15)
+_TEXT_GREEN, _YELLOW, _BLUE = (0, 255, 0), (0, 255, 255), (255, 0, 0)
+
+
+def _blend(img, mask, color):
+    """img[mask] = img[mask] * 0.5 + color * 0.5 in f64, truncated back to u8 by the assignment."""
+    m = mask.astype(bool)
+    img[m] = img[m] * 0.5 + np.asarray(color, np.uint8).reshape(-1, 3) * 0.5
+
+
+def _vis_image_mask_bbox_cv2(img, masks, bboxes, labels):
+    """vis_image_mask_bbox_cv2 (box_thickness 1, green labels at (x1, max(y1 - 2, 5)), font scale 0.5, thickness 2):
+    one np.random.randint(0, 256, (1, 3), uint8) colour per mask, in mask order."""
+    import cv2
+
+    out = img.copy()
+    for i, mask in enumerate(masks):
+        _blend(out, mask, np.random.randint(0, 256, (1, 3), dtype=np.uint8))
+        x1, y1, x2, y2 = (int(v) for v in bboxes[i].astype(np.int32)[:4])
+        cv2.rectangle(out, (x1, y1), (x2, y2), _GREEN, thickness=1)
+        cv2.putText(out, labels[i], (x1, max(y1 - 2, 5)), cv2.FONT_HERSHEY_SIMPLEX, 0.5, _TEXT_GREEN, 2)
+    return out
+
+
+def _vis_image_mask_cv2(img, mask, color):
+    out = img.copy()
+    _blend(out, mask, color)
+    return out
+
+
+def _vis_image_bboxes_cv2(img, bboxes, labels):
+    """vis_image_bboxes_cv2 (box_thickness 2, green labels at (x1, y1 - 2))."""
+    import cv2
+
+    out = img.copy()
+    for bbox, label in zip(bboxes, labels):
+        x1, y1, x2, y2 = (int(v) for v in np.asarray(bbox).astype(np.int32)[:4])
+        cv2.rectangle(out, (x1, y1), (x2, y2), _GREEN, thickness=2)
+        cv2.putText(out, label, (x1, y1 - 2), cv2.FONT_HERSHEY_SIMPLEX, 0.5, _TEXT_GREEN, 2)
+    return out
+
+
+def _project_pts(pts, K, R, t):
+    """misc.project_pts: K [R | t] applied to [pts, 1], divided by the third row."""
+    P = K.dot(np.hstack((np.asarray(R, np.float64), np.asarray(t, np.float64).reshape(3, 1))))
+    pts_im = P.dot(np.hstack((pts, np.ones((pts.shape[0], 1)))).T)
+    pts_im /= pts_im[2, :]
+    return pts_im[:2, :].T
+
+
+def _points2d_to_mask(points2d, height, width):
+    """misc.points2d_to_mask: mask[int(round(y)), int(round(x))] = 1 inside the image; round half to even, as Python's
+    round of a float."""
+    mask = np.zeros((height, width), dtype=np.uint8)
+    xy = np.rint(points2d)
+    ok = (xy[:, 0] >= 0) & (xy[:, 0] < width) & (xy[:, 1] >= 0) & (xy[:, 1] < height)
+    mask[xy[ok, 1].astype(np.int64), xy[ok, 0].astype(np.int64)] = 1
+    return mask
 
 
 def _arch(cfg):

@@ -75,6 +75,31 @@ def render_meshes(mesh_ids, poses, Ks, H, W, znear=0.1, zfar=100.0, quantize_bit
 
 
 @_lib.on_device(1)
+def render_meshes_rgb(mesh_ids, poses, Ks, H, W, znear=0.1, zfar=100.0, colors=None, return_tri_ids=False):
+    """render_meshes in colour: the registered meshes `mesh_ids` [n] at poses [n,3,4] with Ks [n,3,3], flat-shaded as
+    lib/pysixd/renderer_py.py shades them (light at the eye, ambient 0.5) -> (rgb [n,H,W,3] u8, depth [n,H,W] f32),
+    plus tri_ids [n,H,W] i32 (-1 = background) with return_tri_ids.  colors [n,3] in [0,1]: a uniform colour per
+    render; without it each mesh's vertex colours, or grey 0.5 for a mesh uploaded without them.  Depth and coverage
+    equal render_meshes(quantize_bits=0).  One launch set, no sync."""
+    dev = poses.device
+    poses = _f32c(poses).reshape(-1, 3, 4)
+    n = poses.shape[0]
+    Ks = _f32c(Ks, dev).reshape(-1, 3, 3)
+    if Ks.shape[0] == 1 and n > 1:
+        Ks = Ks.expand(n, 3, 3).contiguous()
+    ids = mesh_ids.detach().to(device=dev, dtype=torch.int32).contiguous()
+    cols = None if colors is None else _f32c(torch.as_tensor(colors), dev).reshape(n, 3)
+    rgb = torch.empty((n, H, W, 3), dtype=torch.uint8, device=dev)
+    depth = torch.empty((n, H, W), dtype=torch.float32, device=dev)
+    tri = torch.empty((n, H, W), dtype=torch.int32, device=dev) if return_tri_ids else None
+    scratch = torch.empty((n * H * W,), dtype=torch.int64, device=dev)
+    _lib.check(_lib.lib().rast_render_meshes_rgb(_lib.ptr(ids), _lib.ptr(poses), _lib.ptr(Ks), _lib.ptr(cols), n, H, W,
+                                                 float(znear), float(zfar), _lib.ptr(rgb), _lib.ptr(depth), _lib.ptr(tri),
+                                                 _lib.ptr(scratch), _lib.current_stream()), "rast_render_meshes_rgb")
+    return (rgb, depth, tri) if return_tri_ids else (rgb, depth)
+
+
+@_lib.on_device(1)
 def depth_refine(models, rot, trans, K_crop, xyz, mask, depth_sensor, iters=2, thresh=0.8, mesh_ids=None,
                  znear=0.1, zfar=100.0, mask_loss_type="L1", coor_z_refine=False):
     """Batched fast depth refine (gdrn_evaluator.py:515-561): `iters` x (render depth at the current pose ->
@@ -121,13 +146,19 @@ def depth_refine(models, rot, trans, K_crop, xyz, mask, depth_sensor, iters=2, t
 class Model3D:
     """Minimal stand-in for lib/render_vispy/model3d.py objects: vertices [V,3] in metres + triangle indices [F,3] on
     `device`, and mesh_id, the mesh's id in the library's registry.  The mesh is uploaded once, here; the registry never
-    frees, so the id stays valid for the life of the process and every render of this model goes through it."""
+    frees, so the id stays valid for the life of the process and every render of this model goes through it.
+    colors: optional per-vertex RGB [V,3] in [0,1], which render_meshes_rgb interpolates."""
 
-    def __init__(self, vertices, faces, device="cuda"):
+    def __init__(self, vertices, faces, device="cuda", colors=None):
         v = torch.as_tensor(np.ascontiguousarray(vertices, np.float32))
         f = torch.as_tensor(np.ascontiguousarray(faces, np.int32))
+        c = None
+        if colors is not None:
+            c = torch.as_tensor(np.ascontiguousarray(colors, np.float32))
+            if tuple(c.shape) != (v.shape[0], 3):
+                raise _lib.GdrnError(f"Model3D: colors must be [V,3] = [{v.shape[0]},3], got {tuple(c.shape)}")
         with torch.cuda.device(device):   # the registry lives on the device current at the upload
-            mid = _lib.lib().rast_upload_mesh(_lib.ptr(v), int(v.shape[0]), _lib.ptr(f), int(f.shape[0]))
+            mid = _lib.lib().rast_upload_mesh_ex(_lib.ptr(v), int(v.shape[0]), _lib.ptr(f), int(f.shape[0]), _lib.ptr(c))
         if mid < 0:
             raise _lib.GdrnError(f"rast_upload_mesh failed (code {mid}): {_lib.last_error()}")
         self.mesh_id = mid

@@ -255,11 +255,22 @@ int upnp_batched(const double* pts2d, const double* pts3d, const double* wgt2d, 
  *   fixed-point z-buffer decode of the vispy path (renderer.py:176-182) with znear/zfar.
  * ------------------------------------------------------------------------------------------- */
 int rast_upload_mesh(const float* verts, int V, const int* faces, int F);
+/* rast_upload_mesh_ex: the same, with optional per-vertex colours [V,3] f32 in [0,1] (null: none), which
+ * rast_render_meshes_rgb interpolates.  rast_upload_mesh(...) is rast_upload_mesh_ex(..., NULL). */
+int rast_upload_mesh_ex(const float* verts, int V, const int* faces, int F, const float* colors);
 int rast_mesh_count(void);
 int rast_render_meshes(const int* mesh_ids, const float* poses, const float* Ks, int n, int H, int W, float znear,
                        float zfar, int quantize_bits, float* depth, float* xyz_cam, unsigned long long* zbuf_scratch,
                        void* stream);
 size_t rast_scratch_bytes(int n, int H, int W);
+/* rast_render_meshes_rgb: the same n renders in colour, with lib/pysixd/renderer_py.py's flat shading (light at the
+ *   eye origin, ambient 0.5, face normal turned toward the viewer): rgb [n,H,W,3] u8 = rint(light_w * colour * 255),
+ *   0 on background, and float-z depth [n,H,W] equal to rast_render_meshes(quantize_bits = 0).  Colour: colors [n,3]
+ *   f32 per render when non-null, else the mesh's vertex colours (interpolated perspective-correctly), else grey 0.5.
+ *   tri_ids [n,H,W] i32 (optional): the triangle seen at each pixel, -1 on background. */
+int rast_render_meshes_rgb(const int* mesh_ids, const float* poses, const float* Ks, const float* colors, int n, int H,
+                           int W, float znear, float zfar, uint8_t* rgb, float* depth, int* tri_ids,
+                           unsigned long long* zbuf_scratch, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
  * Fast depth refinement -- replaces GDRN_Evaluator.process_depth_refine
@@ -550,6 +561,26 @@ int gdrn_rle_confusion(const char* chars, size_t chars_bytes, const long long* t
 int gdrn_gt_info(const float* depth_large, const float* depth_img, const uint16_t* depth_test, const float* depth_scale,
                  const double* Ks, const int* inst_img, int n, int H, int W, float delta, long long* counts, int* boxes,
                  uint8_t* mask, uint8_t* mask_visib, void* stream);
+
+
+/* ---------------------------------------------------------------------------------------------
+ * Pose visualisation composite (csrc/vis_poses.cu): the pixel arithmetic of visualization.vis_object_poses
+ * (lib/pysixd/visualization.py) for N images of one size H x W; image j owns instances [inst_off[j], inst_off[j+1])
+ * of the n instance renders, in drawing order; max_inst >= the largest inst_off[j+1] - inst_off[j] (at most 3000).
+ *   m_rgb [n,H,W,3] u8 and m_depth [n,H,W] f32 (rast_render_meshes_rgb), rgb [N,H,W,3] u8, depth [N,H,W] f32 in mm.
+ *   flags: 1 = rgb visualisation, 2 = resolve visibility, 4 = depth difference.
+ *   -> ren_rgb [N,H,W,3] u8 (resolved, or the saturating sum), ren_depth [N,H,W] f32, blend [N,H,W,3] u8 =
+ *      floor(0.5 * rgb + 0.5 * ren_rgb), boxes [n,4] i32 = x_min, y_min, x_max, y_max of m_rgb > 0 (INT_MAX,
+ *      INT_MAX, INT_MIN, INT_MIN when empty); diff_vis [N,H,W,3] u8 (the depth-difference image without text),
+ *      diff_minmax [N,2] f32, diff_sum [N] f64, diff_count [N] i64 over the valid pixels.  Every output is
+ *      independent of the order in which CTAs run.  workspace of gdrn_vis_poses_workspace_bytes(N, H, W) bytes.
+ * ------------------------------------------------------------------------------------------- */
+size_t gdrn_vis_poses_workspace_bytes(int N, int H, int W);
+int gdrn_vis_poses(const uint8_t* m_rgb, const float* m_depth, const int* inst_off, int max_inst, int N, int n,
+                   const uint8_t* rgb,
+                   const float* depth, int H, int W, int flags, uint8_t* ren_rgb, float* ren_depth, uint8_t* blend,
+                   int* boxes, uint8_t* diff_vis, float* diff_minmax, double* diff_sum, long long* diff_count,
+                   void* workspace, size_t workspace_bytes, void* stream);
 
 #ifdef __cplusplus
 }
