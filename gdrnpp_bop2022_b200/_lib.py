@@ -130,6 +130,11 @@ _SIGNATURES = {
     "gdrn_vis_poses_workspace_bytes": (c_size_t, [c_int] * 3),
     "gdrn_vis_poses": (c_int, [c_void_p] * 3 + [c_int] * 3 + [c_void_p] * 2 + [c_int] * 3 + [c_void_p] * 9 + [c_size_t,
                                                                                                          c_void_p]),
+    "gdrn_train_composite": (c_int, [c_void_p, c_void_p] + [c_int] * 3 + [c_void_p] * 8 + [c_void_p]),
+    "gdrn_train_luma_sum": (c_int, [c_void_p] + [c_int] * 3 + [c_void_p, c_int, c_int, c_void_p, c_void_p]),
+    "gdrn_train_color_step": (c_int, [c_void_p, c_void_p] + [c_int] * 3 + [c_void_p] * 3 + [c_int, c_int, c_void_p, c_int,
+                                                                                        c_int, c_void_p, c_void_p]),
+    "gdrn_train_roi_crop": (c_int, [c_void_p] * 5 + [c_int] * 5 + [c_void_p] * 9),
 }
 
 EXPORTED_SYMBOLS = tuple(_SIGNATURES.keys())

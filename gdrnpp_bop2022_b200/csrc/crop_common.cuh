@@ -77,4 +77,30 @@ __device__ __forceinline__ float f32_blend(const F32Tap& t, float a, float b, fl
   return __fadd_rn(__fadd_rn(__fadd_rn(__fmul_rn(a, t.w[0]), __fmul_rn(b, t.w[1])), __fmul_rn(c, t.w[2])), __fmul_rn(d, t.w[3]));
 }
 
+// get_affine_transform(centre f64, (scale, scale) f64, 0, res) as cv2.getAffineTransform solves it: the three float32
+// point pairs src (X0, Y0), (X0, Y1), (X2, Y1) with X0 = f32(cx), Y0 = f32(cy), Y1 = f32(cy - scale / 2),
+// X2 = f32(X0 - f32(Y0 - Y1)), and dst (r/2, r/2), (r/2, 0), (0, 0); their affine map is diagonal and solved in closed
+// form in float64.
+struct Affine6 { double m[6]; };
+
+__device__ __forceinline__ Affine6 forward_affine(double cx, double cy, double scale, int res) {
+  const float X0 = __double2float_rn(cx), Y0 = __double2float_rn(cy);
+  const float Y1 = __double2float_rn(__dadd_rn(cy, __dmul_rn(scale, -0.5)));
+  const float X2 = __fsub_rn(X0, __fsub_rn(Y0, Y1));
+  const double half = 0.5 * (double)res;
+  Affine6 a;
+  a.m[0] = __ddiv_rn(half, __dsub_rn((double)X0, (double)X2));
+  a.m[1] = 0.0;
+  a.m[2] = __dsub_rn(half, __dmul_rn(a.m[0], (double)X0));
+  a.m[3] = 0.0;
+  a.m[4] = __ddiv_rn(half, __dsub_rn((double)Y0, (double)Y1));
+  a.m[5] = __dsub_rn(half, __dmul_rn(a.m[4], (double)Y0));
+  return a;
+}
+
+// get_2d_coord_np's np.linspace(0, 1, n, endpoint=False, dtype=float32): f32(k * (1.0 / n)) in float64
+__device__ __forceinline__ float grid_value(int k, int n) {
+  return __double2float_rn(__dmul_rn((double)k, __ddiv_rn(1.0, (double)n)));
+}
+
 }  // namespace crop

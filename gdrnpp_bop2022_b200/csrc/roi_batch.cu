@@ -16,23 +16,6 @@
 
 namespace {
 
-struct Affine6 { double m[6]; };
-
-__device__ __forceinline__ Affine6 forward_affine(double cx, double cy, double scale, int res) {
-  const float X0 = __double2float_rn(cx), Y0 = __double2float_rn(cy);
-  const float Y1 = __double2float_rn(__dadd_rn(cy, __dmul_rn(scale, -0.5)));
-  const float X2 = __fsub_rn(X0, __fsub_rn(Y0, Y1));
-  const double half = 0.5 * (double)res;
-  Affine6 a;
-  a.m[0] = __ddiv_rn(half, __dsub_rn((double)X0, (double)X2));
-  a.m[1] = 0.0;
-  a.m[2] = __dsub_rn(half, __dmul_rn(a.m[0], (double)X0));
-  a.m[3] = 0.0;
-  a.m[4] = __ddiv_rn(half, __dsub_rn((double)Y0, (double)Y1));
-  a.m[5] = __dsub_rn(half, __dmul_rn(a.m[4], (double)Y0));
-  return a;
-}
-
 __global__ void __launch_bounds__(128)
 roi_setup_kernel(const int* __restrict__ det_meta, const float* __restrict__ det_xywh, int n, const float* __restrict__ K,
                  const int* __restrict__ im_hw, const float* __restrict__ extents, double dzi_pad_scale, int in_res,
@@ -66,13 +49,8 @@ roi_setup_kernel(const int* __restrict__ det_meta, const float* __restrict__ det
   im_H_out[i] = (float)H;
   im_W_out[i] = (float)W;
   bbox_xyxy[4 * i] = x; bbox_xyxy[4 * i + 1] = y; bbox_xyxy[4 * i + 2] = x2f; bbox_xyxy[4 * i + 3] = y2f;
-  const Affine6 a_in = forward_affine(cx, cy, scale, in_res), a_out = forward_affine(cx, cy, scale, out_res);
+  const crop::Affine6 a_in = crop::forward_affine(cx, cy, scale, in_res), a_out = crop::forward_affine(cx, cy, scale, out_res);
   for (int k = 0; k < 6; ++k) { M_in[6 * i + k] = a_in.m[k]; M_out[6 * i + k] = a_out.m[k]; }
-}
-
-// get_2d_coord_np's np.linspace(0, 1, n, endpoint=False, dtype=float32): f32(k * (1.0 / n)) in float64
-__device__ __forceinline__ float grid_value(int k, int n) {
-  return __double2float_rn(__dmul_rn((double)k, __ddiv_rn(1.0, (double)n)));
 }
 
 // metres as mmcv.imread(depth) / depth_factor, then astype(float32)
@@ -134,8 +112,8 @@ roi_crop_multi_kernel(const uint8_t* __restrict__ images, int H, int W, int C, c
   crop::invert_affine(M_out + 6 * b, iM);
   const crop::F32Tap t = crop::f32_tap(crop::src_coord(iM, x, y, false), H, W);
   // the coordinate grid at the four taps, zero outside the image (the warp's constant border)
-  const float gx0 = grid_value(t.sx, W), gx1 = grid_value(t.sx + 1, W);
-  const float gy0 = grid_value(t.sy, H), gy1 = grid_value(t.sy + 1, H);
+  const float gx0 = crop::grid_value(t.sx, W), gx1 = crop::grid_value(t.sx + 1, W);
+  const float gy0 = crop::grid_value(t.sy, H), gy1 = crop::grid_value(t.sy + 1, H);
   const long long o = (long long)b * 2 * per + (long long)y * out_res + x;
   roi_coord_2d[o] = crop::f32_blend(t, t.in[0] ? gx0 : 0.f, t.in[1] ? gx1 : 0.f, t.in[2] ? gx0 : 0.f, t.in[3] ? gx1 : 0.f);
   roi_coord_2d[o + per] = crop::f32_blend(t, t.in[0] ? gy0 : 0.f, t.in[1] ? gy0 : 0.f, t.in[2] ? gy1 : 0.f, t.in[3] ? gy1 : 0.f);

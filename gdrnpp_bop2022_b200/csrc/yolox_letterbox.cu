@@ -1,43 +1,12 @@
 // The YOLOX test-time letterbox (det/yolox/data/data_augment.py preproc after base_data_from_list.load_resized_img):
 // resize to (int(w * r), int(h * r)) with r = min(th / h, tw / w), place top-left on a 114-filled th x tw canvas, BGR in
-// CHW float32.  The resize is bit-exact to cv2.resize(INTER_LINEAR) on uint8 (OpenCV 4.x resize.cpp), which takes one
-// of three paths:
-//   * identity (dsize == ssize): a copy;
-//   * scale exactly 2 in both axes: INTER_LINEAR silently becomes the INTER_AREA fast path, (a + b + c + d + 2) >> 2;
-//   * otherwise the generic fixed-point bilinear path: per output column fx = f32((dx + 0.5) * scale_x - 0.5) in float64,
-//     sx = floor(fx), fx -= sx; columns left of 0 or at/after the last one are clamped with fx = 0; the weights are
-//     round-half-even(f32(1 - fx) * 2048) and round-half-even(fx * 2048) (11-bit).  Rows use the same formula without
-//     the clamp of fy; the two source rows are clamped to [0, H - 1] instead.  The horizontal pass sums in int, the
-//     vertical one is (((b0 * (h0 >> 4)) >> 16) + ((b1 * (h1 >> 4)) >> 16) + 2) >> 2.
+// CHW float32.  The resize is bit-exact to cv2.resize(INTER_LINEAR) on uint8 (cv_resize.cuh);
 // scale_x = 1 / (dw / W) in float64, as cv::resize derives it from dsize.
 // When the second preproc of ValTransform is not the identity for a size, the host side runs the resize twice through
 // a uint8 intermediate, as the reference does.
-#include "common.cuh"
+#include "cv_resize.cuh"
 
 namespace {
-
-enum ResizeMode { kCopy = 0, kArea2 = 1, kLinear = 2 };
-
-struct Tap {
-  int i0, i1, w0, w1;
-};
-
-// cv::resize's coefficient table entry for output coordinate d (clamp_f: the column rule, else the row rule)
-__device__ __forceinline__ Tap linear_tap(int d, double scale, int n, bool clamp_f) {
-  float f = __double2float_rn(__dsub_rn(__dmul_rn((double)d + 0.5, scale), 0.5));
-  int i = (int)floorf(f);
-  f = __fsub_rn(f, (float)i);
-  if (clamp_f) {
-    if (i < 0) { f = 0.f; i = 0; }
-    if (i >= n - 1) { f = 0.f; i = n - 1; }
-  }
-  Tap t;
-  t.w0 = __float2int_rn(__fmul_rn(__fsub_rn(1.f, f), 2048.f));
-  t.w1 = __float2int_rn(__fmul_rn(f, 2048.f));
-  t.i0 = min(max(i, 0), n - 1);
-  t.i1 = min(max(i + 1, 0), n - 1);
-  return t;
-}
 
 // One thread per (image, output pixel) of the destination: f32 CHW canvas (ch x cw, the resized image top-left, 114
 // elsewhere) when out_f != nullptr, else the u8 HWC resized image (ch = dh, cw = dw).
@@ -52,31 +21,7 @@ letterbox_kernel(const uint8_t* __restrict__ src, int N, int H, int W, int C, in
   int v[3] = {114, 114, 114};
   if (x < dw && y < dh) {
     const uint8_t* img = src + (long long)n * H * W * C;
-    const long long rowC = (long long)W * C;
-    if (mode == kCopy) {
-      const uint8_t* p = img + y * rowC + (long long)x * C;
-#pragma unroll
-      for (int c = 0; c < 3; ++c) v[c] = p[C == 1 ? 0 : c];
-    } else if (mode == kArea2) {
-      const uint8_t* p = img + (2LL * y) * rowC + (2LL * x) * C;
-#pragma unroll
-      for (int c = 0; c < 3; ++c) {
-        const int cs = C == 1 ? 0 : c;
-        v[c] = (p[cs] + p[C + cs] + p[rowC + cs] + p[rowC + C + cs] + 2) >> 2;
-      }
-    } else {
-      const Tap tx = linear_tap(x, scale_x, W, true), ty = linear_tap(y, scale_y, H, false);
-      const uint8_t* r0 = img + ty.i0 * rowC;
-      const uint8_t* r1 = img + ty.i1 * rowC;
-      const long long c0 = (long long)tx.i0 * C, c1 = (long long)tx.i1 * C;
-#pragma unroll
-      for (int c = 0; c < 3; ++c) {
-        const int cs = C == 1 ? 0 : c;
-        const int h0 = r0[c0 + cs] * tx.w0 + r0[c1 + cs] * tx.w1;
-        const int h1 = r1[c0 + cs] * tx.w0 + r1[c1 + cs] * tx.w1;
-        v[c] = (((ty.w0 * (h0 >> 4)) >> 16) + ((ty.w1 * (h1 >> 4)) >> 16) + 2) >> 2;
-      }
-    }
+    cvresize::pixel_u8(img, (long long)W * C, H, W, C, x, y, mode, scale_x, scale_y, v);
   }
   if (out_f != nullptr) {
     float* o = out_f + (long long)n * 3 * plane + (long long)y * cw + x;
@@ -103,9 +48,7 @@ Size2 letterbox_size(int h, int w, int th, int tw) {
 int launch(const uint8_t* src, int N, int H, int W, int C, Size2 d, int ch, int cw, float* out_f, uint8_t* out_u8,
            cudaStream_t stream) {
   const double scale_x = 1.0 / ((double)d.w / W), scale_y = 1.0 / ((double)d.h / H);
-  int mode = kLinear;
-  if (d.h == H && d.w == W) mode = kCopy;
-  else if (scale_x == 2.0 && scale_y == 2.0) mode = kArea2;
+  const int mode = cvresize::resize_mode(H, W, d.h, d.w, scale_x, scale_y);
   const long long total = (long long)N * ch * cw;
   letterbox_kernel<<<(unsigned)((total + 255) / 256), 256, 0, stream>>>(src, N, H, W, C, d.h, d.w, mode, scale_x, scale_y,
                                                                         ch, cw, out_f, out_u8);

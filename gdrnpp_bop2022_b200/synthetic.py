@@ -390,3 +390,134 @@ def write_bop_tree(root, dataset="ycbv", num_images=12, num_scenes=2, H=480, W=6
     with open(os.path.join(split, "test_bboxes", "dets.json"), "w") as f:
         json.dump(dets, f)
     return "datasets/" + os.path.relpath(os.path.join(split, "test_bboxes", "dets.json"), root)
+
+
+def write_bop_train_tree(root, dataset="ycbv", num_images=8, num_scenes=2, H=480, W=640, insts_per_image=4, seed=0,
+                         obj_ids=(1, 2, 3), num_bg=6, jpeg_quality=95):
+    """A small BOP PBR training split and VOC-style backgrounds under ``root`` (the reference's ``datasets/``):
+    BOP_DATASETS/<dataset>/train_pbr/<scene>/{rgb/*.jpg, depth/*.png, mask/, mask_visib/, scene_camera.json,
+    scene_gt.json, scene_gt_info.json}, models/ (box meshes in mm, models_info.json; object 2 with a discrete symmetry)
+    and VOCdevkit/VOC2012/{JPEGImages, ImageSets/Main/diningtable_trainval.txt} with ``num_bg`` backgrounds of
+    assorted sizes and aspect ratios.  Each instance's full mask is an ellipse around its projected centre, its visible
+    mask that ellipse minus an occluder; one instance per image has visib_fract 0.05 (for FILTER_VISIB_THR)."""
+    import json
+    import os
+
+    import cv2
+
+    from .ply import save_ply
+
+    rng = np.random.RandomState(seed)
+    base = os.path.join(root, "BOP_DATASETS", dataset)
+    split = os.path.join(base, "train_pbr")
+    models = os.path.join(base, "models")
+    os.makedirs(models, exist_ok=True)
+    faces = np.array([[0, 1, 3], [0, 3, 2], [4, 6, 7], [4, 7, 5], [0, 4, 5], [0, 5, 1], [2, 3, 7], [2, 7, 6],
+                      [0, 2, 6], [0, 6, 4], [1, 5, 7], [1, 7, 3]], np.int32)
+    info = {}
+    for o in obj_ids:
+        half = rng.uniform(30, 60, 3)
+        pts = np.array([[sx, sy, sz] for sx in (-1, 1) for sy in (-1, 1) for sz in (-1, 1)], np.float32) * half
+        save_ply(os.path.join(models, "obj_{:06d}.ply".format(o)), pts, faces)
+        info[str(o)] = {"diameter": float(2 * np.linalg.norm(half)), "min_x": float(-half[0]), "min_y": float(-half[1]),
+                        "min_z": float(-half[2]), "size_x": float(2 * half[0]), "size_y": float(2 * half[1]),
+                        "size_z": float(2 * half[2])}
+        if o == 2:
+            info[str(o)]["symmetries_discrete"] = [[-1, 0, 0, 0, 0, -1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1]]
+    with open(os.path.join(models, "models_info.json"), "w") as f:
+        json.dump(info, f)
+    per_scene = -(-num_images // num_scenes)
+    yy, xx = np.mgrid[0:H, 0:W]
+    for s in range(num_scenes):
+        sdir = os.path.join(split, "{:06d}".format(s))
+        for d in ("rgb", "depth", "mask", "mask_visib"):
+            os.makedirs(os.path.join(sdir, d), exist_ok=True)
+        cams, gts, gt_infos = {}, {}, {}
+        for im_id in range(min(per_scene, num_images - s * per_scene)):
+            f = W * rng.uniform(0.9, 1.1)
+            K = [f, 0.0, W / 2, 0.0, f, H / 2, 0.0, 0.0, 1.0]
+            cams[str(im_id)] = {"cam_K": K, "depth_scale": 0.1}
+            im = cv2.GaussianBlur(rng.randint(0, 256, (H, W, 3)).astype(np.uint8), (7, 7), 2.0)
+            cv2.imwrite(os.path.join(sdir, "rgb", "{:06d}.jpg".format(im_id)), im, [cv2.IMWRITE_JPEG_QUALITY, jpeg_quality])
+            cv2.imwrite(os.path.join(sdir, "depth", "{:06d}.png".format(im_id)), np.full((H, W), 9000, np.uint16))
+            gts[str(im_id)], gt_infos[str(im_id)] = [], []
+            for k in range(insts_per_image):
+                o = int(obj_ids[rng.randint(len(obj_ids))])
+                R = cv2.Rodrigues(rng.uniform(-1, 1, 3))[0]
+                t = np.array([rng.uniform(-200, 200), rng.uniform(-150, 150), rng.uniform(600, 1000)])
+                if k == 1:   # one instance per image at the border: the AMODAL_CLIP box is clipped
+                    t[0] = rng.choice([-1, 1]) * t[2] * (W / 2) / f
+                gts[str(im_id)].append({"obj_id": o, "cam_R_m2c": R.reshape(-1).tolist(), "cam_t_m2c": t.tolist()})
+                u, v = f * t[0] / t[2] + K[2], f * t[1] / t[2] + K[5]
+                r = f * 0.5 * info[str(o)]["diameter"] / t[2] * 0.6
+                rx, ry = r * rng.uniform(0.7, 1.0), r * rng.uniform(0.7, 1.0)
+                full = ((xx - u) / rx) ** 2 + ((yy - v) / ry) ** 2 <= 1
+                ox, oy = rng.uniform(u - rx, u + rx), rng.uniform(v - ry, v + ry)
+                vis = full & ~((np.abs(xx - ox) < rx * 0.4) & (np.abs(yy - oy) < ry * 0.4))
+                for d, m in (("mask", full), ("mask_visib", vis)):
+                    cv2.imwrite(os.path.join(sdir, d, "{:06d}_{:06d}.png".format(im_id, k)), m.astype(np.uint8) * 255)
+                bo = [int(np.floor(u - rx)), int(np.floor(v - ry)), int(np.ceil(2 * rx)), int(np.ceil(2 * ry))]
+                ys, xs = np.nonzero(vis)
+                bv = [int(xs.min()), int(ys.min()), int(xs.max() - xs.min() + 1), int(ys.max() - ys.min() + 1)] if xs.size \
+                    else [-1, -1, -1, -1]
+                vf = 0.05 if k == 3 else float(vis.sum()) / max(float(full.sum()), 1.0)
+                gt_infos[str(im_id)].append({"bbox_obj": bo, "bbox_visib": bv, "px_count_all": int(full.sum()),
+                                             "px_count_valid": int(full.sum()), "px_count_visib": int(vis.sum()),
+                                             "visib_fract": vf})
+        for name, content in (("scene_camera.json", cams), ("scene_gt.json", gts), ("scene_gt_info.json", gt_infos)):
+            with open(os.path.join(sdir, name), "w") as fh:
+                json.dump(content, fh)
+    voc = os.path.join(root, "VOCdevkit", "VOC2012")
+    os.makedirs(os.path.join(voc, "JPEGImages"), exist_ok=True)
+    os.makedirs(os.path.join(voc, "ImageSets", "Main"), exist_ok=True)
+    sizes = [(375, 500), (500, 375), (480, 640), (333, 500), (500, 500), (240, 320)]
+    lines = []
+    for i in range(num_bg):
+        bh, bw = sizes[i % len(sizes)]
+        bg = cv2.GaussianBlur(rng.randint(0, 256, (bh, bw, 3)).astype(np.uint8), (5, 5), 1.5)
+        name = "2008_{:06d}".format(i)
+        cv2.imwrite(os.path.join(voc, "JPEGImages", name + ".jpg"), bg)
+        lines.append("{} {}".format(name, 1 if i % 5 != 4 else -1))
+    with open(os.path.join(voc, "ImageSets", "Main", "diningtable_trainval.txt"), "w") as fh:
+        fh.write("\n".join(lines) + "\n")
+    return base
+
+
+# the COLOR_AUG_CODE of the shipped GDRN configs (configs/gdrn/*/convnext_AugCosyAAEGray_*)
+SHIPPED_COLOR_AUG_CODE = (
+    "Sequential(["
+    "Sometimes(0.5, CoarseDropout( p=0.2, size_percent=0.05) ),"
+    "Sometimes(0.4, GaussianBlur((0., 3.))),"
+    "Sometimes(0.3, pillike.EnhanceSharpness(factor=(0., 50.))),"
+    "Sometimes(0.3, pillike.EnhanceContrast(factor=(0.2, 50.))),"
+    "Sometimes(0.5, pillike.EnhanceBrightness(factor=(0.1, 6.))),"
+    "Sometimes(0.3, pillike.EnhanceColor(factor=(0., 20.))),"
+    "Sometimes(0.5, Add((-25, 25), per_channel=0.3)),"
+    "Sometimes(0.3, Invert(0.2, per_channel=True)),"
+    "Sometimes(0.5, Multiply((0.6, 1.4), per_channel=0.5)),"
+    "Sometimes(0.5, Multiply((0.6, 1.4))),"
+    "Sometimes(0.1, AdditiveGaussianNoise(scale=10, per_channel=True)),"
+    "Sometimes(0.5, iaa.contrast.LinearContrast((0.5, 2.2), per_channel=0.3)),"
+    "Sometimes(0.5, Grayscale(alpha=(0.0, 1.0))),"
+    "], random_order=True)"
+)
+
+
+def shipped_train_cfg(train=("ycbv_train_pbr",)):
+    """The training settings of the shipped AugCosyAAEGray GDRN configs (configs/gdrn/*/convnext_AugCosyAAEGray_*),
+    as the nested dict the package reads, training on the given DATASETS.TRAIN splits."""
+    return {
+        "INPUT": {"FORMAT": "BGR", "MIN_SIZE_TRAIN": (480,), "MAX_SIZE_TRAIN": 640, "WITH_DEPTH": False,
+                  "DZI_TYPE": "uniform", "DZI_PAD_SCALE": 1.5, "DZI_SCALE_RATIO": 0.25, "DZI_SHIFT_RATIO": 0.25,
+                  "TRUNCATE_FG": True, "CHANGE_BG_PROB": 0.5, "COLOR_AUG_PROB": 0.8, "COLOR_AUG_TYPE": "code",
+                  "COLOR_AUG_CODE": SHIPPED_COLOR_AUG_CODE, "BG_TYPE": "VOC_table", "BG_IMGS_ROOT": "datasets/VOCdevkit/VOC2012/",
+                  "NUM_BG_IMGS": 10000},
+        "DATASETS": {"TRAIN": train},
+        "DATALOADER": {"FILTER_VISIB_THR": 0.3},
+        "SOLVER": {"IMS_PER_BATCH": 48},
+        "TRAIN": {"VIS": False},
+        "MODEL": {"PIXEL_MEAN": [0.0, 0.0, 0.0], "PIXEL_STD": [255.0, 255.0, 255.0], "BBOX_TYPE": "AMODAL_CLIP",
+                  "POSE_NET": {"XYZ_ONLINE": True, "XYZ_BP": True, "INPUT_RES": 256, "OUTPUT_RES": 64,
+                               "GEO_HEAD": {"NUM_REGIONS": 64}, "PNP_NET": {"COORD_2D_TYPE": "abs"},
+                               "LOSS_CFG": {"XYZ_LOSS_TYPE": "L1", "NUM_PM_POINTS": 3000}}},
+    }

@@ -582,6 +582,33 @@ int gdrn_vis_poses(const uint8_t* m_rgb, const float* m_depth, const int* inst_o
                    int* boxes, uint8_t* diff_vis, float* diff_minmax, double* diff_sum, long long* diff_count,
                    void* workspace, size_t workspace_bytes, void* stream);
 
+/* ---------------------------------------------------------------------------------------------
+ * Training batch pipeline (csrc/train_aug.cu): read_data_train's image work for n uint8 BGR images [n,H,W,3] of one size.
+ *   gdrn_train_composite: mask_visib [n,H,W] u8 (0/1); bbox [n,4] i32 the host sets to (H, -1, W, -1) -> the visible
+ *     mask's row / column extent; side [n] (0 top, 1 bottom, 2 left, 3 right, else none) and trunc_u [n] in [0, 1) ->
+ *     keep [n,4] = row0, row1, col0, col1 of the truncated mask; bg_meta [n,7] = do_bg, bg_h, bg_w, crop_h, crop_w,
+ *     resized_h, resized_w; bg_scale [n,2] = 1 / fx, 1 / fy; background j at bg_pool + bg_off[j] (u8 [bg_h,bg_w,3]).
+ *     Pixels outside the kept mask of a do_bg image become the resized background (0 beyond it), in place.
+ *   gdrn_train_luma_sum: sums [n] u64 = sum of PIL's L image of each image whose kind_at[b][step] is EnhanceContrast.
+ *   gdrn_train_color_step: dst = colour op kind_at[b][step] (kinds 0..11, others pass through) of src with params
+ *     fpar [n,S,4] f32, ipar [n,S,12] i32, dropout cells [n,ch,cw] u8, luma_sums from gdrn_train_luma_sum.
+ *   gdrn_train_roi_crop: center_scale [n,3] f64 -> roi_img [n,3,in,in] (normalised), roi_coord_2d [n,2,out,out],
+ *     roi_mask_trunc / visib / full [n,out,out] f32 (nearest), counts [n,2] i32 = trunc and visib pixels of each ROI.
+ * Allocate nothing, do not synchronise.
+ * ------------------------------------------------------------------------------------------- */
+int gdrn_train_composite(uint8_t* images, const uint8_t* mask_visib, int n, int H, int W, const uint8_t* bg_pool,
+                         const long long* bg_off, const int* bg_meta, const double* bg_scale, const int* side,
+                         const double* trunc_u, int* bbox, int* keep, void* stream);
+int gdrn_train_luma_sum(const uint8_t* images, int n, int H, int W, const int* kind_at, int S, int step,
+                        unsigned long long* sums, void* stream);
+int gdrn_train_color_step(const uint8_t* src, uint8_t* dst, int n, int H, int W, const int* kind_at, const float* fpar,
+                          const int* ipar, int S, int step, const uint8_t* cells, int ch, int cw,
+                          const unsigned long long* luma_sums, void* stream);
+int gdrn_train_roi_crop(const uint8_t* images, const uint8_t* mask_visib, const uint8_t* mask_full, const int* keep,
+                        const double* center_scale, int n, int H, int W, int in_res, int out_res, const double* pixel_mean,
+                        const double* pixel_std, float* roi_img, float* roi_coord_2d, float* roi_mask_trunc,
+                        float* roi_mask_visib, float* roi_mask_full, int* counts, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
