@@ -135,6 +135,12 @@ _SIGNATURES = {
     "gdrn_train_color_step": (c_int, [c_void_p, c_void_p] + [c_int] * 3 + [c_void_p] * 3 + [c_int, c_int, c_void_p, c_int,
                                                                                         c_int, c_void_p, c_void_p]),
     "gdrn_train_roi_crop": (c_int, [c_void_p] * 5 + [c_int] * 5 + [c_void_p] * 9),
+    "yolox_train_resize": (c_int, [c_void_p] * 3 + [c_int, c_int64, c_void_p]),
+    "yolox_train_mosaic_affine": (c_int, [c_void_p] * 4 + [c_int] * 3 + [c_void_p, c_void_p]),
+    "yolox_train_mixup": (c_int, [c_void_p] * 4 + [c_int] * 3 + [c_void_p]),
+    "yolox_train_hsv": (c_int, [c_void_p] * 3 + [c_int, c_int64, c_int, c_void_p]),
+    "yolox_train_preproc": (c_int, [c_void_p] * 2 + [c_int] * 3 + [c_void_p, c_void_p]),
+    "yolox_train_pack": (c_int, [c_void_p] * 2 + [c_int] * 3 + [c_void_p, c_void_p]),
 }
 
 EXPORTED_SYMBOLS = tuple(_SIGNATURES.keys())

@@ -1,5 +1,6 @@
 // cv2.resize(INTER_LINEAR) on uint8, bit-exact to OpenCV 4.x resize.cpp, shared by the YOLOX letterbox
-// (yolox_letterbox.cu) and the training background resize (train_aug.cu).  cv::resize takes one of three paths:
+// (yolox_letterbox.cu), the training background resize (train_aug.cu) and the YOLOX training resizes
+// (yolox_train_aug.cu).  cv::resize takes one of three paths:
 //   * identity (dsize == ssize): a copy;
 //   * scale exactly 2 in both axes: INTER_LINEAR silently becomes the INTER_AREA fast path, (a + b + c + d + 2) >> 2;
 //   * otherwise the generic fixed-point bilinear path: per output column fx = f32((dx + 0.5) * scale_x - 0.5) in float64,
@@ -38,15 +39,16 @@ __device__ __forceinline__ Tap linear_tap(int d, double scale, int n, bool clamp
 }
 
 // The three channels of output pixel (x, y) of an H x W source (C = 1 or 3 interleaved channels, rows rowC elements
-// apart; a single-channel source is read as three equal channels) under `mode`.
+// apart; a single-channel source is read as three equal channels) under `mode`.  flip: the source is read mirrored
+// left-right (source column i is img column W - 1 - i), as cv2.resize sees img[:, ::-1].
 __device__ __forceinline__ void pixel_u8(const uint8_t* __restrict__ img, long long rowC, int H, int W, int C, int x, int y,
-                                         int mode, double scale_x, double scale_y, int (&v)[3]) {
+                                         int mode, double scale_x, double scale_y, int (&v)[3], bool flip = false) {
   if (mode == kCopy) {
-    const uint8_t* p = img + y * rowC + (long long)x * C;
+    const uint8_t* p = img + y * rowC + (long long)(flip ? W - 1 - x : x) * C;
 #pragma unroll
     for (int c = 0; c < 3; ++c) v[c] = p[C == 1 ? 0 : c];
-  } else if (mode == kArea2) {
-    const uint8_t* p = img + (2LL * y) * rowC + (2LL * x) * C;
+  } else if (mode == kArea2) {   // the two columns swap under a flip; their sum does not change
+    const uint8_t* p = img + (2LL * y) * rowC + (long long)(flip ? W - 2 - 2 * x : 2 * x) * C;
 #pragma unroll
     for (int c = 0; c < 3; ++c) {
       const int cs = C == 1 ? 0 : c;
@@ -56,7 +58,7 @@ __device__ __forceinline__ void pixel_u8(const uint8_t* __restrict__ img, long l
     const Tap tx = linear_tap(x, scale_x, W, true), ty = linear_tap(y, scale_y, H, false);
     const uint8_t* r0 = img + ty.i0 * rowC;
     const uint8_t* r1 = img + ty.i1 * rowC;
-    const long long c0 = (long long)tx.i0 * C, c1 = (long long)tx.i1 * C;
+    const long long c0 = (long long)(flip ? W - 1 - tx.i0 : tx.i0) * C, c1 = (long long)(flip ? W - 1 - tx.i1 : tx.i1) * C;
 #pragma unroll
     for (int c = 0; c < 3; ++c) {
       const int cs = C == 1 ? 0 : c;

@@ -393,13 +393,15 @@ def write_bop_tree(root, dataset="ycbv", num_images=12, num_scenes=2, H=480, W=6
 
 
 def write_bop_train_tree(root, dataset="ycbv", num_images=8, num_scenes=2, H=480, W=640, insts_per_image=4, seed=0,
-                         obj_ids=(1, 2, 3), num_bg=6, jpeg_quality=95):
+                         obj_ids=(1, 2, 3), num_bg=6, jpeg_quality=95, split="train_pbr"):
     """A small BOP PBR training split and VOC-style backgrounds under ``root`` (the reference's ``datasets/``):
-    BOP_DATASETS/<dataset>/train_pbr/<scene>/{rgb/*.jpg, depth/*.png, mask/, mask_visib/, scene_camera.json,
+    BOP_DATASETS/<dataset>/<split>/<scene>/{rgb/*.jpg, depth/*.png, mask/, mask_visib/, scene_camera.json,
     scene_gt.json, scene_gt_info.json}, models/ (box meshes in mm, models_info.json; object 2 with a discrete symmetry)
     and VOCdevkit/VOC2012/{JPEGImages, ImageSets/Main/diningtable_trainval.txt} with ``num_bg`` backgrounds of
     assorted sizes and aspect ratios.  Each instance's full mask is an ellipse around its projected centre, its visible
-    mask that ellipse minus an occluder; one instance per image has visib_fract 0.05 (for FILTER_VISIB_THR)."""
+    mask that ellipse minus an occluder; one instance per image has visib_fract 0.05 (for FILTER_VISIB_THR).  A split
+    other than train_pbr (train_primesense, train_real) stores its colour images as PNG, so one dataset can hold
+    splits of two image sizes."""
     import json
     import os
 
@@ -409,7 +411,8 @@ def write_bop_train_tree(root, dataset="ycbv", num_images=8, num_scenes=2, H=480
 
     rng = np.random.RandomState(seed)
     base = os.path.join(root, "BOP_DATASETS", dataset)
-    split = os.path.join(base, "train_pbr")
+    im_ext = ".jpg" if split == "train_pbr" else ".png"
+    split = os.path.join(base, split)
     models = os.path.join(base, "models")
     os.makedirs(models, exist_ok=True)
     faces = np.array([[0, 1, 3], [0, 3, 2], [4, 6, 7], [4, 7, 5], [0, 4, 5], [0, 5, 1], [2, 3, 7], [2, 7, 6],
@@ -438,7 +441,7 @@ def write_bop_train_tree(root, dataset="ycbv", num_images=8, num_scenes=2, H=480
             K = [f, 0.0, W / 2, 0.0, f, H / 2, 0.0, 0.0, 1.0]
             cams[str(im_id)] = {"cam_K": K, "depth_scale": 0.1}
             im = cv2.GaussianBlur(rng.randint(0, 256, (H, W, 3)).astype(np.uint8), (7, 7), 2.0)
-            cv2.imwrite(os.path.join(sdir, "rgb", "{:06d}.jpg".format(im_id)), im, [cv2.IMWRITE_JPEG_QUALITY, jpeg_quality])
+            cv2.imwrite(os.path.join(sdir, "rgb", "{:06d}{}".format(im_id, im_ext)), im, [cv2.IMWRITE_JPEG_QUALITY, jpeg_quality])
             cv2.imwrite(os.path.join(sdir, "depth", "{:06d}.png".format(im_id)), np.full((H, W), 9000, np.uint16))
             gts[str(im_id)], gt_infos[str(im_id)] = [], []
             for k in range(insts_per_image):
@@ -521,3 +524,57 @@ def shipped_train_cfg(train=("ycbv_train_pbr",)):
                                "GEO_HEAD": {"NUM_REGIONS": 64}, "PNP_NET": {"COORD_2D_TYPE": "abs"},
                                "LOSS_CFG": {"XYZ_LOSS_TYPE": "L1", "NUM_PM_POINTS": 3000}}},
     }
+
+
+# the training settings of the shipped detector configs (configs/yolox/bop_pbr/yolox_base.py and the
+# yolox_x_640_augCozyAAEhsv_ranger_30_epochs_* configs that import it), as a LazyConfig load_yolox_config reads
+_YOLOX_TRAIN_BASE = '''
+from omegaconf import OmegaConf
+model = L(YOLOX)(backbone=L(YOLOPAFPN)(depth=1.0, width=1.0, in_channels=[256, 512, 1024]),
+                 head=L(YOLOXHead)(num_classes=1, width="${..backbone.width}", in_channels="${..backbone.in_channels}"))
+train = dict(total_epochs=300, no_aug_epochs=2)
+DATASETS = dict(TRAIN=("",), TEST=("",))
+dataloader = OmegaConf.create()
+dataloader.train = L(build_yolox_train_loader)(
+    dataset=L(Base_DatasetFromList)(split="train", lst=L(get_detection_dataset_dicts)(names=DATASETS.TRAIN),
+                                    img_size=(640, 640), preproc=L(TrainTransform)(max_labels=50)),
+    aug_wrapper=L(MosaicDetection)(mosaic=True, img_size="${..dataset.img_size}", preproc=L(TrainTransform)(max_labels=120),
+                                   degrees=10.0, translate=0.1, mosaic_scale=(0.1, 2), mixup_scale=(0.5, 1.5), shear=2.0,
+                                   enable_mixup=True, mosaic_prob=1.0, mixup_prob=1.0),
+    total_batch_size=64, num_workers=4, pin_memory=True)
+test = dict(test_dataset_names=DATASETS.TEST, test_size=(640, 640), conf_thr=0.01, nms_thr=0.65, half_test=True)
+'''
+
+YOLOX_COLOR_AUG_CODE = SHIPPED_COLOR_AUG_CODE.replace("Sometimes(0.5, Grayscale(alpha=(0.0, 1.0))),", "")
+
+
+def write_yolox_train_config(directory, train=("lmo_pbr_train",), test="lmo_bop_test", extra=""):
+    """The shipped detector training settings for the given DATASETS.TRAIN, as <directory>/yolox_base.py and
+    <directory>/yolox_train.py (the derived config, followed by ``extra`` lines) -> the derived config's path."""
+    import os
+
+    os.makedirs(directory, exist_ok=True)
+    with open(os.path.join(directory, "yolox_base.py"), "w") as f:
+        f.write(_YOLOX_TRAIN_BASE)
+    lines = [
+        "from .yolox_base import train, val, test, model, dataloader, DATASETS  # noqa",
+        "model.head.num_classes = 8",
+        f"DATASETS.TRAIN = {list(train)!r}",
+        f"DATASETS.TEST = [{test!r}]",
+        "dataloader.train.total_batch_size = 32",
+        "dataloader.train.aug_wrapper.COLOR_AUG_PROB = 0.8",
+        'dataloader.train.aug_wrapper.COLOR_AUG_TYPE = "code"',
+        f"dataloader.train.aug_wrapper.COLOR_AUG_CODE = {YOLOX_COLOR_AUG_CODE!r}",
+        "dataloader.train.aug_wrapper.AUG_HSV_PROB = 1.0",
+        "dataloader.train.aug_wrapper.HSV_H = 0.015",
+        "dataloader.train.aug_wrapper.HSV_S = 0.7",
+        "dataloader.train.aug_wrapper.HSV_V = 0.4",
+        'dataloader.train.aug_wrapper.FORMAT = "RGB"',
+        "train.total_epochs = 30",
+        "train.no_aug_epochs = 15",
+        "test.test_dataset_names = DATASETS.TEST",
+    ]
+    path = os.path.join(directory, "yolox_train.py")
+    with open(path, "w") as f:
+        f.write("\n".join(lines) + "\n" + extra)
+    return path

@@ -430,7 +430,8 @@ def load_yolox_config(path):
     ``from .yolox_base import ...`` chain.  A model setting the engine cannot honour (depthwise convs, an activation
     other than silu, other strides or channel lists, a head width other than the backbone's) raises ValueError.
     -> SimpleNamespace(depth, width, num_classes, test_size (h, w), conf_thr, nms_thr, augment (default False),
-    scales (a tuple, default None)).  The namespace is also the ``cfg`` of ``YOLOX.forward(augment=True, cfg=cfg)``."""
+    scales (a tuple, default None), the test-loop settings and the training loader's (``_train_loader_settings``)).  The
+    namespace is also the ``cfg`` of ``YOLOX.forward(augment=True, cfg=cfg)``."""
     model, test = _read_config(path, frozenset())
     cfg = dict(_MODEL_DEFAULTS)
     for k, v in model.items():
@@ -469,7 +470,86 @@ def load_yolox_config(path):
                            test_dataset_names=tuple(ex.get("test_dataset_names", ())),
                            half_test=bool(ex.get("half_test", False)), amp_test=bool(ex.get("amp_test", False)),
                            output_dir=output_dir, eval_cached=bool(ex.get("eval_cached", False)),
-                           legacy=bool(ex.get("legacy", False)), filter_scene=bool(ex.get("filter_scene", False)))
+                           legacy=bool(ex.get("legacy", False)), filter_scene=bool(ex.get("filter_scene", False)),
+                           **_train_loader_settings(path))
+
+
+# MosaicDetection's keyword defaults (det/yolox/data/datasets/mosaicdetection.py)
+_AUG_WRAPPER_DEFAULTS = {"mosaic": True, "degrees": 10.0, "translate": 0.1, "mosaic_scale": (0.5, 1.5),
+                         "mixup_scale": (0.5, 1.5), "shear": 2.0, "enable_mixup": True, "mosaic_prob": 1.0,
+                         "mixup_prob": 1.0, "COLOR_AUG_PROB": 0.0, "COLOR_AUG_TYPE": "", "COLOR_AUG_CODE": (),
+                         "AUG_HSV_PROB": 0, "HSV_H": 0, "HSV_S": 0, "HSV_V": 0, "FORMAT": "RGB",
+                         "preproc.max_labels": 50, "preproc.flip_prob": 0.5, "preproc.hsv_prob": 1.0}
+
+
+def _train_loader_settings(path):
+    """The training loader of the config (dataloader.train = L(build_yolox_train_loader)(...) and the
+    dataloader.train.* assignments after it), DATASETS.TRAIN and train.no_aug_epochs -> train_img_size (h, w),
+    train_dataset_names, aug_wrapper (MosaicDetection's keywords with their defaults, preproc.* for its TrainTransform),
+    train_total_batch_size, train_num_workers, no_aug_epochs."""
+    flat = _read_train_settings(path, frozenset())
+    wrap = dict(_AUG_WRAPPER_DEFAULTS)
+    wrap.update({k[len("aug_wrapper."):]: v for k, v in flat.items() if k.startswith("aug_wrapper.")})
+    size = flat.get("dataset.img_size", (416, 416))   # Base_DatasetFromList's default
+    if wrap.get("img_size", "${..dataset.img_size}") != "${..dataset.img_size}":
+        size = wrap["img_size"]
+    wrap.pop("img_size", None)
+    return {"train_img_size": tuple(int(v) for v in size), "train_dataset_names": tuple(flat.get("DATASETS.TRAIN", ())),
+            "aug_wrapper": wrap, "train_total_batch_size": int(flat.get("total_batch_size", 64)),
+            "train_num_workers": int(flat.get("num_workers", 0)), "no_aug_epochs": int(flat.get("train.no_aug_epochs", 0))}
+
+
+def _read_train_settings(path, seen):
+    path = os.path.abspath(path)
+    if path in seen:
+        raise ValueError(f"{path}: import cycle")
+    tree = ast.parse(open(path).read(), path)
+    out = {}
+
+    def lit(node):
+        try:
+            return ast.literal_eval(node)
+        except ValueError:
+            return None
+
+    def call_kwargs(node, prefix):
+        for kw in node.keywords:
+            if isinstance(kw.value, ast.Call) and isinstance(kw.value.func, ast.Call):
+                call_kwargs(kw.value, f"{prefix}{kw.arg}.")
+            else:
+                v = lit(kw.value)
+                if v is not None:
+                    out[prefix + kw.arg] = v
+
+    for node in tree.body:
+        if isinstance(node, ast.ImportFrom) and node.level == 1 and node.module:
+            base = os.path.join(os.path.dirname(path), *node.module.split(".")) + ".py"
+            if os.path.exists(base) and {a.name for a in node.names} & {"dataloader", "train", "DATASETS"}:
+                out.update(_read_train_settings(base, seen | {path}))
+            continue
+        if isinstance(node, ast.Expr) and isinstance(node.value, ast.Call) and _dotted(node.value.func) == "train.update":
+            for kw in node.value.keywords:
+                if kw.arg == "no_aug_epochs" and lit(kw.value) is not None:
+                    out["train.no_aug_epochs"] = lit(kw.value)
+            continue
+        if not (isinstance(node, ast.Assign) and len(node.targets) == 1):
+            continue
+        tgt, val = _dotted(node.targets[0]), node.value
+        if tgt == "dataloader.train" and isinstance(val, ast.Call):
+            out = {k: v for k, v in out.items() if not k.startswith(("dataset.", "aug_wrapper.", "total_batch_size",
+                                                                     "num_workers"))}
+            call_kwargs(val, "")
+        elif tgt and tgt.startswith("dataloader.train."):
+            v = lit(val)
+            if v is not None:
+                out[tgt[len("dataloader.train."):]] = v
+        elif tgt in ("train", "DATASETS") and isinstance(val, ast.Call) and _dotted(val.func) == "dict":
+            for kw in val.keywords:
+                if (tgt, kw.arg) in (("train", "no_aug_epochs"), ("DATASETS", "TRAIN")) and lit(kw.value) is not None:
+                    out[f"{tgt}.{kw.arg}"] = lit(kw.value)
+        elif tgt in ("train.no_aug_epochs", "DATASETS.TRAIN") and lit(val) is not None:
+            out[tgt] = lit(val)
+    return out
 
 
 def _read_test_loop_settings(path, seen):

@@ -609,6 +609,33 @@ int gdrn_train_roi_crop(const uint8_t* images, const uint8_t* mask_visib, const 
                         const double* pixel_std, float* roi_img, float* roi_coord_2d, float* roi_mask_trunc,
                         float* roi_mask_visib, float* roi_mask_full, int* counts, void* stream);
 
+/* ---------------------------------------------------------------------------------------------
+ * YOLOX training batch pipeline (csrc/yolox_train_aug.cu): MosaicDetection + TrainTransform's image work on uint8 BGR
+ * images (HWC, 3 channels), oh x ow the training size.  Offsets are in bytes from the named pool's base.
+ *   yolox_train_resize: jobs [n_jobs,8] i64 = src_off, sh, sw, dst_off, dh, dw, ch, cw: dst (ch x cw) = the source resized
+ *     to dh x dw (cv2.resize INTER_LINEAR) top-left, 114 elsewhere; max_plane >= every ch * cw.
+ *   yolox_train_mosaic_affine: tile_info [n_sel,4,8] i64 = lx1, ly1, lx2, ly2, padw, padh, tile_w, tile_off (tiles pasted
+ *     in order into a 2oh x 2ow mosaic of 114), M [n_sel,6] f64 the forward affine -> out[sel[i]] = cv2.warpAffine of the
+ *     mosaic to (ow, oh), bilinear, border 114.
+ *   yolox_train_mixup: params [n_sel,6] i64 = canvas_off, jit_h, jit_w, flip, x_offset, y_offset; canvas (oh x ow) resized
+ *     to jit_h x jit_w, mirrored when flip, zero-padded and cropped at the offsets, blended 0.5 / 0.5 into images[sel[i]].
+ *   yolox_train_hsv: entries [n,2] i64 = off, npix; luts [n,3,256] u8 (hue, saturation, value); rgb: channel 0 is R.
+ *     In place; max_pix >= every npix.
+ *   yolox_train_preproc: info [n,5] i64 = src_off, sh, sw, flip, transpose -> out [n,oh,ow,3] = the mirrored source
+ *     letterboxed into 114 (TrainTransform's preproc), stored as (ow, oh, 3) when transpose.
+ *   yolox_train_pack: images [n,oh,ow,3] (transposed[b]: stored (ow, oh, 3)) -> out [n,3,oh,ow] f32.
+ * Allocate nothing, do not synchronise.
+ * ------------------------------------------------------------------------------------------- */
+int yolox_train_resize(const uint8_t* src, uint8_t* dst, const long long* jobs, int n_jobs, long long max_plane, void* stream);
+int yolox_train_mosaic_affine(const uint8_t* tiles, const long long* tile_info, const double* M, const int* sel, int n_sel,
+                              int oh, int ow, uint8_t* out, void* stream);
+int yolox_train_mixup(uint8_t* images, const uint8_t* canvases, const long long* params, const int* sel, int n_sel, int oh,
+                      int ow, void* stream);
+int yolox_train_hsv(uint8_t* pool, const long long* entries, const uint8_t* luts, int n, long long max_pix, int rgb,
+                    void* stream);
+int yolox_train_preproc(const uint8_t* pool, const long long* info, int n, int oh, int ow, uint8_t* out, void* stream);
+int yolox_train_pack(const uint8_t* images, const int* transposed, int n, int oh, int ow, float* out, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
