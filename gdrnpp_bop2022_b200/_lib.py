@@ -96,6 +96,10 @@ _SIGNATURES = {
     "yolox_model_num_anchors_tta": (c_int, [c_void_p]),
     "yolox_model_workspace_bytes_tta": (c_size_t, [c_void_p, c_int]),
     "yolox_model_forward_tta": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_size_t, c_void_p]),
+    "yolox_model_plan_info": (c_int, [c_void_p, c_int, POINTER(c_int)]),
+    "yolox_model_step_info": (c_int, [c_void_p, c_int, c_int, POINTER(c_int), c_char_p, c_int]),
+    "yolox_model_buffer_info": (c_int, [c_void_p, c_int, c_int, c_int, POINTER(c_int64)]),
+    "yolox_model_run_step": (c_int, [c_void_p, c_int, c_int, c_void_p, c_int, c_void_p, c_void_p, c_size_t, c_void_p]),
     "yolox_postprocess_single_workspace_bytes": (c_size_t, [c_int] * 3),
     "yolox_postprocess_single": (c_int, [c_void_p] + [c_int] * 3 + [c_float, c_float] + [c_void_p] * 3 + [c_size_t, c_void_p]),
     "gdrn_crop_resize_u8": (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p,

@@ -461,6 +461,7 @@ inline int blocks_for(long long n, int t) { return (int)((n + t - 1) / t); }
 // ---------------------------------------------------------------------------------------------------------------------
 #include <algorithm>
 #include <cmath>
+#include <cstring>
 #include <map>
 #include <string>
 #include <vector>
@@ -766,42 +767,67 @@ bool yx_ready(const YoloxModel* m) {
   return true;
 }
 
+// the buffer pointers of a plan laid out for nb images from the 256-aligned workspace base
+int yx_buffers(YPlan& pl, int nb, uint8_t* base, float** bp) {
+  GDRN_REQUIRE(pl.bufs.size() <= 512, "yolox_model_forward: too many buffers");
+  yx_layout(pl, nb);
+  for (size_t i = 0; i < pl.bufs.size(); ++i) bp[i] = reinterpret_cast<float*>(base + pl.offs[i]);
+  return GDRN_OK;
+}
+
+// one step of a plan over nb images of the original [nb,3,H,W] input x; a head step writes det rows
+// [a_base + s.d_off, a_base + s.d_off + h*w) of [nb, A_row, 5 + nc].  One launch.
+int yx_run_step(YoloxModel* m, const YPlan& pl, const YStep& s, float* const* bp, const float* x, int nb, float* det, int A_row,
+                int a_base, cudaStream_t st) {
+  if (s.kind == YS_CONV) return yx_launch_conv(m, pl, s, m->convs.at(s.w), bp, nb, st);
+  if (s.kind == YS_FOCUS) {
+    const long long n = (long long)nb * (pl.H / 2) * (pl.W / 2);
+    if (pl.resample)
+      GDRN_CHECK_CUDA(gdrn_launch_dep(yolox_focus_resample_kernel, dim3(blocks_for(n, 256)), dim3(256), 0, st, x, nb, m->H, m->W,
+                                      pl.H, pl.W, pl.sh, pl.sw, (float)m->H / (float)pl.sh, (float)m->W / (float)pl.sw, bp[s.dst]));
+    else
+      GDRN_CHECK_CUDA(gdrn_launch_dep(yolox_focus_kernel, dim3(blocks_for(n, 256)), dim3(256), 0, st, x, nb, pl.H, pl.W, bp[s.dst]));
+  } else if (s.kind == YS_SPP) {
+    const long long n = (long long)nb * s.h * s.wd * s.d_c;
+    GDRN_CHECK_CUDA(gdrn_launch_dep(yolox_spp_kernel, dim3(blocks_for(n, 256)), dim3(256), 0, st, bp[s.dst], nb, s.h, s.wd,
+                                    pl.bufs[s.dst].ld, s.d_c));
+  } else if (s.kind == YS_UP) {
+    const long long n = (long long)nb * 4 * s.h * s.wd * s.d_c;
+    GDRN_CHECK_CUDA(gdrn_launch_dep(yolox_upsample2x_kernel, dim3(blocks_for(n, 256)), dim3(256), 0, st,
+                                    (const float*)bp[s.src], pl.bufs[s.src].ld, s.s_off, bp[s.dst], pl.bufs[s.dst].ld, s.d_off,
+                                    nb, s.h, s.wd, s.d_c));
+  } else {
+    const long long n = (long long)nb * s.h * s.wd * (5 + m->nc);
+    GDRN_CHECK_CUDA(gdrn_launch_dep(yolox_head_out_kernel, dim3(blocks_for(n, 256)), dim3(256), 0, st, (const float*)bp[s.src],
+                                    nb, s.h, s.wd, m->nc, s.extra, A_row, a_base + s.d_off, pl.inv_scale, det));
+  }
+  return GDRN_OK;
+}
+
 // one plan over nb images of the original [nb,3,H,W] input x: det rows [a_base, a_base + pl.A) of [nb, A_row, 5 + nc]
 int yx_run_plan(YoloxModel* m, YPlan& pl, const float* x, int nb, float* det, int A_row, int a_base, uint8_t* base, cudaStream_t st,
                 int& launches) {
   float* bp[512];
-  GDRN_REQUIRE(pl.bufs.size() <= 512, "yolox_model_forward: too many buffers");
-  yx_layout(pl, nb);
-  for (size_t i = 0; i < pl.bufs.size(); ++i) bp[i] = reinterpret_cast<float*>(base + pl.offs[i]);
-  const int C = 5 + m->nc;
+  int rc = yx_buffers(pl, nb, base, bp);
+  if (rc != GDRN_OK) return rc;
   for (const YStep& s : pl.steps) {
-    if (s.kind == YS_CONV) {
-      const int rc = yx_launch_conv(m, pl, s, m->convs.at(s.w), bp, nb, st);
-      if (rc != GDRN_OK) return rc;
-    } else if (s.kind == YS_FOCUS) {
-      const long long n = (long long)nb * (pl.H / 2) * (pl.W / 2);
-      if (pl.resample)
-        GDRN_CHECK_CUDA(gdrn_launch_dep(yolox_focus_resample_kernel, dim3(blocks_for(n, 256)), dim3(256), 0, st, x, nb, m->H, m->W,
-                                        pl.H, pl.W, pl.sh, pl.sw, (float)m->H / (float)pl.sh, (float)m->W / (float)pl.sw, bp[s.dst]));
-      else
-        GDRN_CHECK_CUDA(gdrn_launch_dep(yolox_focus_kernel, dim3(blocks_for(n, 256)), dim3(256), 0, st, x, nb, pl.H, pl.W, bp[s.dst]));
-    } else if (s.kind == YS_SPP) {
-      const long long n = (long long)nb * s.h * s.wd * s.d_c;
-      GDRN_CHECK_CUDA(gdrn_launch_dep(yolox_spp_kernel, dim3(blocks_for(n, 256)), dim3(256), 0, st, bp[s.dst], nb, s.h, s.wd,
-                                      pl.bufs[s.dst].ld, s.d_c));
-    } else if (s.kind == YS_UP) {
-      const long long n = (long long)nb * 4 * s.h * s.wd * s.d_c;
-      GDRN_CHECK_CUDA(gdrn_launch_dep(yolox_upsample2x_kernel, dim3(blocks_for(n, 256)), dim3(256), 0, st,
-                                      (const float*)bp[s.src], pl.bufs[s.src].ld, s.s_off, bp[s.dst], pl.bufs[s.dst].ld, s.d_off,
-                                      nb, s.h, s.wd, s.d_c));
-    } else {
-      const long long n = (long long)nb * s.h * s.wd * C;
-      GDRN_CHECK_CUDA(gdrn_launch_dep(yolox_head_out_kernel, dim3(blocks_for(n, 256)), dim3(256), 0, st, (const float*)bp[s.src],
-                                      nb, s.h, s.wd, m->nc, s.extra, A_row, a_base + s.d_off, pl.inv_scale, det));
-    }
+    rc = yx_run_step(m, pl, s, bp, x, nb, det, A_row, a_base, st);
+    if (rc != GDRN_OK) return rc;
     ++launches;
   }
   return GDRN_OK;
+}
+
+// anchor base of a plan in the rows its forward writes: 0 for plan 0 (yolox_model_forward), the anchors of the scales
+// before it for a test-time-augmentation plan (yolox_model_forward_tta); -1 if the plan is not in the scale set
+int yx_anchor_base(const YoloxModel* m, int plan) {
+  if (plan == 0) return 0;
+  int a = 0;
+  for (int k : m->tta_plan) {
+    if (k == plan) return a;
+    a += m->plans[k].A;
+  }
+  return -1;
 }
 
 // the plan of one scale: model_utils.scale_img sizes in double arithmetic from the create-time H x W
@@ -954,6 +980,81 @@ extern "C" int yolox_model_forward_tta(YoloxModel* m, const float* img, int B, f
     }
   }
   gdrn_count_launch(launches);
+  return GDRN_OK;
+}
+
+// ---- test / measurement entries: walk a plan's step table and run one step of it (include/gdrn_b200.h) ----
+extern "C" int yolox_model_plan_info(YoloxModel* m, int plan, int* info) {
+  GDRN_REQUIRE(m && info, "yolox_model_plan_info: bad arguments");
+  GDRN_REQUIRE(plan >= 0 && plan < (int)m->plans.size(), "yolox_model_plan_info: no such plan");
+  const YPlan& pl = m->plans[plan];
+  const int v[9] = {(int)pl.steps.size(), (int)pl.bufs.size(), pl.H, pl.W, pl.sh, pl.sw, pl.A,
+                    plan == 0 ? pl.A : m->A_tta, yx_anchor_base(m, plan)};
+  for (int i = 0; i < 9; ++i) info[i] = v[i];
+  return GDRN_OK;
+}
+
+extern "C" int yolox_model_step_info(YoloxModel* m, int plan, int step, int* info, char* name, int name_len) {
+  GDRN_REQUIRE(m && info && name && name_len > 0, "yolox_model_step_info: bad arguments");
+  GDRN_REQUIRE(plan >= 0 && plan < (int)m->plans.size(), "yolox_model_step_info: no such plan");
+  const YPlan& pl = m->plans[plan];
+  GDRN_REQUIRE(step >= 0 && step < (int)pl.steps.size(), "yolox_model_step_info: no such step");
+  const YStep& s = pl.steps[step];
+  GDRN_REQUIRE((int)s.w.size() < name_len, "yolox_model_step_info: name buffer too small");
+  const int C = 5 + m->nc;
+  // kind, src, s_off, s_c, dst, d_off, d_c, res, r_off, in h, in w, out h, out w, ks, stride, act, level stride, anchor offset
+  int v[18] = {s.kind, s.src, s.s_off, s.s_c, s.dst, s.d_off, s.d_c, s.res, s.r_off, s.h, s.wd, s.h, s.wd, 0, 0, 0, 0, 0};
+  if (s.kind == YS_CONV) {
+    const int k = m->convs.at(s.w).k, pad = (k - 1) / 2;
+    v[11] = (s.h + 2 * pad - k) / s.stride + 1;
+    v[12] = (s.wd + 2 * pad - k) / s.stride + 1;
+    v[13] = k; v[14] = s.stride; v[15] = s.act;
+  } else if (s.kind == YS_FOCUS) {   // reads the [B,3,H,W] input (the create-time size: a scaled plan resamples it)
+    v[1] = -1; v[2] = 0; v[3] = 3; v[6] = 16; v[9] = m->H; v[10] = m->W; v[11] = pl.H / 2; v[12] = pl.W / 2;
+  } else if (s.kind == YS_SPP) {     // pools slice [0, C) of its buffer into slices C, 2C, 3C
+    v[1] = s.dst; v[2] = 0; v[3] = s.d_c; v[5] = s.d_c; v[6] = 3 * s.d_c; v[13] = 13; v[14] = 1;
+  } else if (s.kind == YS_UP) {
+    v[3] = s.d_c; v[11] = 2 * s.h; v[12] = 2 * s.wd;
+  } else {                           // reads the level's raw buffer, writes det rows
+    v[2] = 0; v[3] = C; v[4] = -1; v[5] = 0; v[6] = C; v[16] = s.extra; v[17] = s.d_off;
+  }
+  for (int i = 0; i < 18; ++i) info[i] = v[i];
+  std::memcpy(name, s.w.c_str(), s.w.size() + 1);
+  return GDRN_OK;
+}
+
+extern "C" int yolox_model_buffer_info(YoloxModel* m, int plan, int buf, int batch, int64_t* info) {
+  GDRN_REQUIRE(m && info, "yolox_model_buffer_info: bad arguments");
+  GDRN_REQUIRE(plan >= 0 && plan < (int)m->plans.size(), "yolox_model_buffer_info: no such plan");
+  YPlan& pl = m->plans[plan];
+  GDRN_REQUIRE(buf >= 0 && buf < (int)pl.bufs.size(), "yolox_model_buffer_info: no such buffer");
+  GDRN_REQUIRE(batch > 0 && batch <= m->max_batch, "yolox_model_buffer_info: batch must be 1..max_batch");
+  const size_t need = yx_layout(pl, batch) + 256;
+  info[0] = (int64_t)pl.offs[buf];
+  info[1] = pl.bufs[buf].pix;
+  info[2] = pl.bufs[buf].ld;
+  info[3] = (int64_t)need;
+  return GDRN_OK;
+}
+
+extern "C" int yolox_model_run_step(YoloxModel* m, int plan, int step, const float* img, int batch, float* det_preds, void* workspace,
+                                    size_t workspace_bytes, void* stream) {
+  GDRN_REQUIRE(m && img && det_preds && workspace, "yolox_model_run_step: bad arguments");
+  GDRN_REQUIRE(plan >= 0 && plan < (int)m->plans.size(), "yolox_model_run_step: no such plan");
+  YPlan& pl = m->plans[plan];
+  GDRN_REQUIRE(step >= 0 && step < (int)pl.steps.size(), "yolox_model_run_step: no such step");
+  GDRN_REQUIRE(batch > 0 && batch <= m->max_batch, "yolox_model_run_step: batch must be 1..max_batch");
+  GDRN_REQUIRE(yx_ready(m), "yolox_model_run_step: weights missing (load every tensor, then yolox_model_missing)");
+  const int a_base = yx_anchor_base(m, plan);
+  GDRN_REQUIRE(a_base >= 0, "yolox_model_run_step: the plan is not in the scale set");
+  GDRN_REQUIRE(workspace_bytes >= yx_layout(pl, batch) + 256, "yolox_model_run_step: workspace too small");
+  uint8_t* base = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(workspace) + 255) & ~(uintptr_t)255);
+  float* bp[512];
+  int rc = yx_buffers(pl, batch, base, bp);
+  if (rc != GDRN_OK) return rc;
+  rc = yx_run_step(m, pl, pl.steps[step], bp, img, batch, det_preds, plan == 0 ? pl.A : m->A_tta, a_base, (cudaStream_t)stream);
+  if (rc != GDRN_OK) return rc;
+  gdrn_count_launch(1);
   return GDRN_OK;
 }
 

@@ -154,7 +154,9 @@ def _base_convs(module):
 # engine: the C ABI model of csrc/yolox_net.cu for one (device, max_batch, H, W, precision)
 # ---------------------------------------------------------------------------------------------------------------------
 class _Engine:
-    def __init__(self, model, device, H, W):
+    def __init__(self, model, device, H, W, load=True):
+        """``load=False`` leaves the weights out: such an engine only lays plans out (host only, no device call), for
+        the step-table entries below."""
         L = _lib.lib()
         self.device = device
         h = ctypes.c_void_p()
@@ -164,6 +166,8 @@ class _Engine:
         self.A = L.yolox_model_num_anchors(h)
         self.scales, self.A_tta = None, 0   # the test-time-augmentation scale set (yolox_model_set_scales)
         self.workspace = None
+        if not load:
+            return
         st = _lib.current_stream()
         for k, v in model.state_dict().items():
             if k.endswith("num_batches_tracked"):
@@ -193,6 +197,52 @@ class _Engine:
         fn, name = (_lib.lib().yolox_model_forward_tta, "yolox_model_forward_tta") if tta else (_lib.lib().yolox_model_forward,
                                                                                               "yolox_model_forward")
         _lib.check(fn(self.handle, _lib.ptr(x), x.shape[0], _lib.ptr(det), _lib.ptr(ws), ws.numel(), _lib.current_stream()), name)
+
+    # -- test / measurement entries (yolox_model_plan_info / step_info / buffer_info / run_step in include/gdrn_b200.h) --
+    STEP_KINDS = ("conv", "focus", "spp", "upsample", "head")
+    STEP_SLOTS = ("kind", "src", "s_off", "s_c", "dst", "d_off", "d_c", "res", "r_off", "in_h", "in_w", "out_h", "out_w", "ks",
+                  "stride", "act", "level_stride", "anchor_off")
+
+    def plan_info(self, plan=0):
+        """-> dict(n_steps, n_bufs, H, W, sh, sw, A, A_row, a_base) of plan ``plan`` (0: the create-time size; 1..: the
+        non-unit scales of the current scale set)."""
+        info = (ctypes.c_int * 9)()
+        _lib.check(_lib.lib().yolox_model_plan_info(self.handle, plan, info), "yolox_model_plan_info")
+        return dict(zip(("n_steps", "n_bufs", "H", "W", "sh", "sw", "A", "A_row", "a_base"), info))
+
+    def steps(self, plan=0):
+        """The step table of a plan: one dict per step with the slots of yolox_model_step_info, ``kind`` as a name and
+        ``name`` the packed conv name ("" for other kinds)."""
+        out = []
+        info, name = (ctypes.c_int * len(self.STEP_SLOTS))(), ctypes.create_string_buffer(256)
+        for i in range(self.plan_info(plan)["n_steps"]):
+            _lib.check(_lib.lib().yolox_model_step_info(self.handle, plan, i, info, name, 256), "yolox_model_step_info")
+            d = dict(zip(self.STEP_SLOTS, info))
+            d["kind"], d["name"] = self.STEP_KINDS[d["kind"]], name.value.decode()
+            out.append(d)
+        return out
+
+    def buffer_info(self, plan, buf, batch):
+        """-> (byte offset from the 256-aligned workspace base, pixels per image, ld, workspace bytes the plan needs) of
+        buffer ``buf`` of a plan laid out for ``batch`` images."""
+        info = (ctypes.c_int64 * 4)()
+        _lib.check(_lib.lib().yolox_model_buffer_info(self.handle, plan, buf, batch, info), "yolox_model_buffer_info")
+        return tuple(info)
+
+    def buffer(self, ws, plan, buf, batch):
+        """The fp32 view [batch, pixels, ld] of buffer ``buf`` of a plan laid out for ``batch`` images inside the uint8
+        workspace tensor ``ws``."""
+        off, pix, ld, need = self.buffer_info(plan, buf, batch)
+        if ws.numel() < need:
+            raise _lib.GdrnError(f"workspace of {ws.numel()} bytes, plan {plan} needs {need} at batch {batch}")
+        start = (-ws.data_ptr()) % 256 + off
+        return ws[start:start + batch * pix * ld * 4].view(torch.float32).view(batch, pix, ld)
+
+    def run_step(self, x, det, ws, plan, step):
+        """Run step ``step`` of ``plan`` for the x.shape[0] <= max_batch images of x, writing det's rows as the forward
+        (plan 0) or the TTA forward (plan >= 1) does."""
+        _lib.check(_lib.lib().yolox_model_run_step(self.handle, plan, step, _lib.ptr(x), x.shape[0], _lib.ptr(det), _lib.ptr(ws),
+                                                   ws.numel(), _lib.current_stream()), "yolox_model_run_step")
 
     def __del__(self):
         try:

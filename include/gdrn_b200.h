@@ -128,6 +128,36 @@ int gdrn_model_run_stage(GdrnModel* m, const char* stage, int batch, const float
                          const float* roi_coord_2d, const GdrnMaps* maps, void* workspace, size_t workspace_bytes,
                          void* stream);
 
+/* Test / measurement entries of the YOLOX engine (yolox_model_*, below): walk the layer plan of a forward and run ONE of
+ * its steps -- the same host function and kernel the forward launches for it -- on a caller's workspace.  plan indexes the
+ * engine's plans: 0 is the create-time size (yolox_model_forward), 1.. the non-unit scales of the current
+ * yolox_model_set_scales set in the order they were added (yolox_model_forward_tta).  Buffers are fp32 NHWC
+ * [batch, pix, ld] at an offset from the workspace pointer rounded up to 256 bytes.
+ *   yolox_model_plan_info: info[9] = {n_steps, n_buffers, H, W, content h, content w (= H, W for plan 0), A (the plan's
+ *     anchors), A_row (det_preds row count the forward writes: A for plan 0, A_tta otherwise), anchor base of the plan}.
+ *   yolox_model_step_info: info[18] =
+ *      0 kind (0 conv, 1 Focus, 2 SPP, 3 nearest x2 upsample, 4 head output)
+ *      1 src buffer (-1: the [B,3,H,W] input), 2 src channel offset, 3 src channel count,
+ *      4 dst buffer (-1: det_preds), 5 dst channel offset, 6 dst channel count,
+ *      7 residual buffer (-1: none; conv only, added after the activation), 8 residual channel offset,
+ *      9 / 10 input map h / w, 11 / 12 output map h / w, 13 kernel size (conv; 13 for SPP), 14 stride (conv, SPP),
+ *     15 SiLU flag (conv), 16 level stride (head), 17 anchor offset of the level within the plan (head).
+ *     SPP reads slice [0, C) of its buffer and writes slices C, 2C, 3C (dst offset C, count 3C).  The head step reads
+ *     the level's raw [pix, 5 + nc] buffer and writes det rows anchor base + anchor offset + [0, h*w).  name (name_len
+ *     bytes) receives the packed conv name ("backbone.backbone.dark2.0", "head.conv0.1" = [cls_convs.1.0 | reg_convs.1.0]
+ *     along N, "head.regobj.2" = [reg_preds.2 | obj_preds.2], "head.cls.0" = cls_preds.0), "" for other kinds.
+ *   yolox_model_buffer_info: info[4] = {byte offset from the aligned base, pixels per image, ld (channels), workspace bytes
+ *     the plan needs} for a chunk of batch <= max_batch images, laid out as the forward lays it out.
+ *   yolox_model_run_step: step of plan for batch <= max_batch images of img [batch,3,H,W]; a head step writes det_preds
+ *     rows of stride A_row at the plan's anchor base.  Rejects a bad plan / step index, a batch above max_batch, a
+ *     workspace smaller than the plan needs and missing weights.  No allocation, no synchronisation. */
+typedef struct YoloxModel YoloxModel;
+int yolox_model_plan_info(YoloxModel* m, int plan, int* info);
+int yolox_model_step_info(YoloxModel* m, int plan, int step, int* info, char* name, int name_len);
+int yolox_model_buffer_info(YoloxModel* m, int plan, int buf, int batch, int64_t* info);
+int yolox_model_run_step(YoloxModel* m, int plan, int step, const float* img, int batch, float* det_preds, void* workspace,
+                         size_t workspace_bytes, void* stream);
+
 /* Plain GEMM through the same wgmma kernel, exported for tests and roofline measurement:
  * out[M,N] = epi(A[M,K] @ W[N,K]^T + bias); A, W bf16 row-major (K contiguous, lda/ldw = K).
  * epi: 0 = store (out bf16 or fp32 by out_f32), 1 = GELU -> bf16, 2 = resid + gamma*(.) -> fp32. */

@@ -134,3 +134,118 @@ def keep_single_instance(det, num_classes, conf_thre, nms_thre, ious=None):
             kept.append(i)
     out = r[sorted(kept, key=lambda i: r[i, 6])]
     return out
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# the engine's layer plan, one step at a time (yolox_model_step_info / yolox_model_run_step): the folded and merged
+# weights of every packed conv, restated from the reference's modules, and one torch op per step kind
+# ---------------------------------------------------------------------------------------------------------------------
+def fold(sd, prefix):
+    """(w [Cout, Cin, k, k], b [Cout]) float64 of one BaseConv with its BatchNorm folded in (fuse_conv_and_bn,
+    det/yolox/utils/model_utils.py:33-58, eps 1e-3), from an unfused (conv + bn) or a fused (conv bias) state dict."""
+    w = sd[prefix + ".conv.weight"].double()
+    cb = sd.get(prefix + ".conv.bias")
+    cb = torch.zeros(w.shape[0], dtype=torch.float64, device=w.device) if cb is None else cb.double()
+    if prefix + ".bn.weight" not in sd:
+        return w, cb
+    g, beta = sd[prefix + ".bn.weight"].double(), sd[prefix + ".bn.bias"].double()
+    mean, var = sd[prefix + ".bn.running_mean"].double(), sd[prefix + ".bn.running_var"].double()
+    s = g / torch.sqrt(var + BN_EPS)
+    return w * s[:, None, None, None], s * cb + (beta - g * mean / torch.sqrt(var + BN_EPS))
+
+
+def packed_conv(sd, name):
+    """(w, b) float64 of one conv of the engine's step table by its packed name: a BaseConv prefix folded; the merged head
+    convs head.conv0.k = [cls_convs.k.0 | reg_convs.k.0] and head.regobj.k = [reg_preds.k | obj_preds.k] along N;
+    head.cls.k = cls_preds.k; the stem's 12 Focus input channels padded to 16 with zero weights."""
+    level = name.rsplit(".", 1)[-1]
+    pred = lambda p: (sd[p + ".weight"].double(), sd[p + ".bias"].double())  # noqa: E731
+    if name.startswith("head.conv0."):
+        parts = [fold(sd, f"head.cls_convs.{level}.0"), fold(sd, f"head.reg_convs.{level}.0")]
+    elif name.startswith("head.regobj."):
+        parts = [pred(f"head.reg_preds.{level}"), pred(f"head.obj_preds.{level}")]
+    elif name.startswith("head.cls."):
+        parts = [pred(f"head.cls_preds.{level}")]
+    else:
+        parts = [fold(sd, name)]
+    w, b = torch.cat([p[0] for p in parts]), torch.cat([p[1] for p in parts])
+    if name.endswith("stem.conv"):
+        w = F.pad(w, (0, 0, 0, 0, 0, 16 - w.shape[1]))
+    return w, b
+
+
+def conv_op(x, w, b, stride, act, resid=None):
+    """x [B, Cin, h, w] -> act(conv(x) + b) (+ resid): the engine's conv epilogue adds the shortcut after SiLU."""
+    y = F.conv2d(x, w, b, stride=stride, padding=(w.shape[-1] - 1) // 2)
+    if act:
+        y = y * torch.sigmoid(y)
+    return y if resid is None else y + resid
+
+
+def focus_op(x):
+    """[B, 3, H, W] -> [B, 16, H/2, W/2]: Focus's space-to-depth (TL, BL, TR, BR) x 3, then 4 zero channels."""
+    y = torch.cat((x[..., ::2, ::2], x[..., 1::2, ::2], x[..., ::2, 1::2], x[..., 1::2, 1::2]), 1)
+    return F.pad(y, (0, 0, 0, 0, 0, 4))
+
+
+def spp_op(x):
+    """[B, C, h, w] -> [B, 3C, h, w]: the 5 / 9 / 13 max-pools of SPPBottleneck (stride 1, -inf padding)."""
+    return torch.cat([F.max_pool2d(x, k, 1, k // 2) for k in (5, 9, 13)], 1)
+
+
+def upsample_op(x):
+    return F.interpolate(x, scale_factor=2, mode="nearest")
+
+
+def head_op(raw, stride, inv_scale=1.0):
+    """raw [B, 5 + nc, h, w] (reg 4 | obj | cls) -> [B, h*w, 5 + nc] decoded as YOLOXHead.decode_outputs:
+    (xy + grid) * stride, exp(wh) * stride, sigmoid(obj), sigmoid(cls); then the box columns times inv_scale (the
+    test-time-augmentation de-scale, 1 for the plain forward).  In the dtype of raw: float32 restates the kernel's
+    round-to-nearest ops one for one."""
+    B, C, h, w = raw.shape
+    o = raw.flatten(2).permute(0, 2, 1)
+    yv, xv = torch.meshgrid(torch.arange(h, device=raw.device), torch.arange(w, device=raw.device), indexing="ij")
+    grid = torch.stack((xv, yv), 2).view(1, -1, 2).to(o)
+    box = torch.cat([(o[..., :2] + grid) * stride, torch.exp(o[..., 2:4]) * stride], -1)
+    if inv_scale != 1.0:
+        box = box * inv_scale
+    return torch.cat([box, torch.sigmoid(o[..., 4:])], -1)
+
+
+def nchw(buf, off, c, h, w):
+    """Channel slice [off, off + c) of an engine buffer [B, h*w, ld] as [B, c, h, w]."""
+    return buf[:, :, off:off + c].reshape(buf.shape[0], h, w, c).permute(0, 3, 1, 2)
+
+
+def store(buf, off, y):
+    """Write y [B, c, h, w] into channel slice [off, off + c) of an engine buffer [B, h*w, ld]."""
+    buf[:, :, off:off + y.shape[1]] = y.permute(0, 2, 3, 1).reshape(buf.shape[0], -1, y.shape[1])
+
+
+def replay_step(step, bufs, x, det, weights, scale=1.0, a_base=0):
+    """Run one step of the engine's step table (a dict with the slots of yolox_model_step_info) on torch buffers
+    ``bufs`` ([B, pix, ld] each, any dtype), the input x [B, 3, H, W] and det [B, A_row, 5 + nc]: one torch op per step
+    kind.  ``weights``: packed name -> (w, b); ``scale``: the plan's test-time-augmentation scale (1 for plan 0);
+    ``a_base``: the plan's anchor base."""
+    k = step["kind"]
+    if k == "conv":
+        w, b = weights[step["name"]]
+        inp = nchw(bufs[step["src"]], step["s_off"], step["s_c"], step["in_h"], step["in_w"])
+        res = None
+        if step["res"] >= 0:
+            res = nchw(bufs[step["res"]], step["r_off"], step["d_c"], step["out_h"], step["out_w"])
+        y = conv_op(inp, w.to(inp), b.to(inp), step["stride"], step["act"], res)
+        store(bufs[step["dst"]], step["d_off"], y)
+    elif k == "focus":
+        from .yolox_tta_oracle import tta_scale_input
+
+        store(bufs[step["dst"]], 0, focus_op(tta_scale_input(x, scale).to(bufs[step["dst"]])))
+    elif k == "spp":
+        store(bufs[step["dst"]], step["d_off"], spp_op(nchw(bufs[step["src"]], 0, step["s_c"], step["in_h"], step["in_w"])))
+    elif k == "upsample":
+        store(bufs[step["dst"]], step["d_off"],
+              upsample_op(nchw(bufs[step["src"]], step["s_off"], step["s_c"], step["in_h"], step["in_w"])))
+    else:
+        raw = nchw(bufs[step["src"]], 0, step["s_c"], step["in_h"], step["in_w"])
+        a0 = a_base + step["anchor_off"]
+        det[:, a0:a0 + step["in_h"] * step["in_w"]] = head_op(raw, step["level_stride"], 1.0 / scale).to(det)

@@ -187,7 +187,10 @@ def _fp32_errs(sd, x, depth, nc, ref):
     return _errs(r32, ref)
 
 
-BARS = {"bf16x3": (0.05, 1e-4), "bf16": (2.0, 2e-2)}   # max box-coordinate error (px), max score error
+# max box-coordinate error (px), max score error; also the bars of test_yolox_tta.  Largest errors measured over the
+# cases of both files (H100 80GB HBM3, 700 W power limit): bf16x3 0.00145 px (YOLOX-X 640x640 TTA B=2) / 4.38e-5 (YOLOX-X
+# TTA), bf16 0.371 px (width 0.25 480x640 B=5 TTA) / 0.0112 (YOLOX-X 640x640 TTA B=2).
+BARS = {"bf16x3": (0.005, 1e-4), "bf16": (1.4, 2e-2)}
 
 
 _SD = {}
