@@ -79,6 +79,7 @@ _SIGNATURES = {
     "rast_render_meshes_rgb": (c_int, [c_void_p] * 4 + [c_int] * 3 + [c_float, c_float] + [c_void_p] * 5),
     "gdrn_pnp_ransac_maps": (c_int, [c_void_p] * 9 + [c_int] * 3 + [c_float, c_float, c_uint] + [c_void_p] * 4),
     "gdrn_pnp_ransac_points": (c_int, [c_void_p] * 4 + [c_int] * 3 + [c_float, c_uint] + [c_void_p] * 4),
+    "gdrn_pnp_ransac_trace": (c_int, [c_void_p] * 11 + [c_int] * 3 + [c_float, c_float, c_uint] + [c_void_p] * 15),
     "gdrn_pnp_net_maps": (c_int, [c_void_p] * 10 + [c_int] * 3 + [c_float, c_float, c_int, c_uint] + [c_void_p] * 3),
     "gdrn_pnp_iterative_points": (c_int, [c_void_p] * 5 + [c_int, c_int, c_void_p, c_void_p]),
     "gdrn_xyz_region_targets": (c_int, [c_void_p] * 6 + [c_int] * 4 + [c_void_p] * 5),

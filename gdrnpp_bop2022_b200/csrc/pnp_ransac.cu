@@ -11,8 +11,8 @@
 //      roi_coord_2d * (im_W, im_H); selection mask > thr & |xyz_k| > 1e-4 * extent_k, compacted in row-major order
 //      (the order numpy boolean indexing gives the reference).
 //   2. `iters` hypotheses: 4 sampled correspondences each (counter-based hash RNG of (seed, roi, hypothesis), or caller
-//      supplied indices), Grunert P3P on the first three (quartic by Ferrari + Newton polish), the fourth picks among
-//      the <= 4 solutions; one thread per hypothesis.
+//      supplied indices; four distinct ids, a repeated caller id gives no model), Grunert P3P on the first three (quartic
+//      by Ferrari + Newton polish, then Newton on the depths), the fourth picks among the <= 4 solutions; a thread each.
 //   3. inlier count of every hypothesis over all correspondences (reprojection error < thr px; a warp per hypothesis,
 //      lanes over points), best = max count (lowest index on ties).
 //   4. refit on the inliers of the best hypothesis: Levenberg-Marquardt on the reprojection error (6x6 normal equations
@@ -34,6 +34,22 @@ constexpr int PR_MAX_HYP = 256;
 constexpr int PNP_ITERATIVE_MAX_ITERS = 20;   // OpenCV's SOLVEPNP_ITERATIVE cap (cvFindExtrinsicCameraParams2 max_iter)
 enum { PNP_NET_ITER = 0, PNP_NET_RANSAC = 1, PNP_NET_RANSAC_ROT = 2 };   // gdrn_pnp_net_maps pnp_type
 
+// Per-stage record of pnp_ransac_kernel (gdrn_pnp_ransac_trace), all device pointers; every member null in production
+// calls.  Entries a ROI does not reach (after an early sentinel return) are left as the caller initialised them.
+struct PnpTrace {
+  int* count;               // [n] selected correspondences N
+  int* src;                 // [n, PR_MAX_PTS] source pixel / point of compacted entry i (-1 from N on)
+  int* samples;             // [n, iters, 4] ids each hypothesis used (after % N and de-duplication)
+  int* nsol;                // [n, iters] P3P solutions
+  double* hyp;              // [n, iters, 12] the solution the fourth point chose
+  int* cnt;                 // [n, iters] inlier count (-1: no model)
+  int* best;                // [n]
+  unsigned char* inl;       // [n, 2, PR_MAX_PTS] inlier flags at the start of each refit round, compacted order
+  double* round_pose;       // [n, 2, 2, 12] start / end pose of each refit round
+  double* round_cost;       // [n, 2, 3] cost at the start, the lowest cost LM evaluated, the cost at the returned pose
+  double* pose;             // [n, 12] final pose (-100 for the sentinel)
+};
+
 struct PnpParams {
   const float* coor_x; const float* coor_y; const float* coor_z;   // [n, hw*hw] network outputs in [0,1]
   const float* mask;        // [n, hw*hw] raw visible-mask output, or null (then `sel` picks)
@@ -51,6 +67,7 @@ struct PnpParams {
   float* poses;             // [n, 12]
   int* n_inliers;           // [n] (or null)
   unsigned char* inlier_mask;   // [n, npts] over the INPUT pixels/points (or null)
+  PnpTrace tr;
 };
 
 __device__ __forceinline__ unsigned hash32(unsigned x) {
@@ -100,8 +117,10 @@ __device__ int solve_quartic(double a4, double a3, double a2, double a1, double 
     for (int sg = 1; sg >= -1; sg -= 2) {
       const double cc = p / 2.0 + m - sg * q / (2.0 * s);
       const double disc = s * s - 4.0 * cc;
-      if (disc >= 0.0) {
-        const double sd = sqrt(disc);
+      // a double root rounded into a complex pair is still a root: keep it within a relative 1e-9 (p3p_grunert's
+      // depth refinement then settles it or drops it)
+      if (disc >= -1e-9 * (s * s + fabs(4.0 * cc))) {
+        const double sd = sqrt(fmax(disc, 0.0));
         y[n++] = (-sg * s + sd) / 2.0;
         y[n++] = (-sg * s - sd) / 2.0;
       }
@@ -175,7 +194,29 @@ __device__ int p3p_grunert(const double (*P)[3], const double (*f)[3], double (*
     if (!(u > 0.0)) continue;
     const double s1sq = c2 / (1.0 + u * u - 2.0 * u * cg);
     if (!(s1sq > 0.0)) continue;
-    const double s1 = sqrt(s1sq), s2 = u * s1, s3 = v * s1;
+    double s1 = sqrt(s1sq), s2 = u * s1, s3 = v * s1;
+    // Grunert's quartic loses precision when the bearings are close (samples a few pixels apart): Newton on the three
+    // depths with the law-of-cosines system s_i^2 + s_j^2 - 2 cos_ij s_i s_j = d_ij^2 restores it.
+    for (int it = 0; it < 3; ++it) {
+      const double F0 = s1 * s1 + s2 * s2 - 2.0 * cg * s1 * s2 - c2;   // pair (0, 1)
+      const double F1 = s1 * s1 + s3 * s3 - 2.0 * cb * s1 * s3 - b2;   // pair (0, 2)
+      const double F2 = s2 * s2 + s3 * s3 - 2.0 * ca * s2 * s3 - a2;   // pair (1, 2)
+      const double j00 = 2.0 * (s1 - cg * s2), j01 = 2.0 * (s2 - cg * s1);
+      const double j10 = 2.0 * (s1 - cb * s3), j12 = 2.0 * (s3 - cb * s1);
+      const double j21 = 2.0 * (s2 - ca * s3), j22 = 2.0 * (s3 - ca * s2);
+      // J = [[j00, j01, 0], [j10, 0, j12], [0, j21, j22]]: Cramer's rule
+      const double det = j00 * (-j12 * j21) - j01 * (j10 * j22);
+      if (!(fabs(det) > 1e-300)) break;
+      const double d1 = (F0 * (-j12 * j21) - j01 * (F1 * j22 - j12 * F2)) / det;
+      const double d2 = (j00 * (F1 * j22 - j12 * F2) - F0 * (j10 * j22)) / det;
+      const double d3 = (F0 * (j10 * j21) - j00 * (j21 * F1) - j01 * (j10 * F2)) / det;
+      s1 -= d1; s2 -= d2; s3 -= d3;
+    }
+    {   // a candidate the refinement did not bring onto the system is not a pose
+      const double r0 = s1 * s1 + s2 * s2 - 2.0 * cg * s1 * s2 - c2, r1 = s1 * s1 + s3 * s3 - 2.0 * cb * s1 * s3 - b2;
+      const double r2 = s2 * s2 + s3 * s3 - 2.0 * ca * s2 * s3 - a2;
+      if (!(s1 > 0.0 && s2 > 0.0 && s3 > 0.0 && fabs(r0) <= 1e-6 * c2 && fabs(r1) <= 1e-6 * b2 && fabs(r2) <= 1e-6 * a2)) continue;
+    }
     double Q0[3] = {s1 * f[0][0], s1 * f[0][1], s1 * f[0][2]};
     double Q1[3] = {s2 * f[1][0], s2 * f[1][1], s2 * f[1][2]};
     double Q2[3] = {s3 * f[2][0], s3 * f[2][1], s3 * f[2][2]};
@@ -347,16 +388,48 @@ __device__ __forceinline__ int gather_correspondences(const PnpParams& p, int ro
 //   kFromGuess = true (network-initialised PnP): like OpenCV's iterative solver, every point with z != 0 counts (from a
 //     poor start some may lie behind the camera; dropping them would reward steps that push points there), and only
 //     accepted steps count towards `max_iters` (at most 4 * max_iters solves in all).
+// The cost lm_refine minimises (sum of squared reprojection errors over the same points) at s_pose, summed in the order
+// lm_refine sums it; returned in every thread.  Every thread must call it.
+template <bool kFromGuess>
+__device__ double pose_cost(const double* s_pose, const unsigned char* inl, int N, const PnpShared& sh) {
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const float* s3 = sh.s3;
+  const float* s2 = sh.s2;
+  const double* s_K = sh.s_K;
+  double acc = 0.0;
+  for (int i = tid; i < N; i += PR_THREADS) {
+    if (inl && !inl[i]) continue;
+    const double X = s3[i * 3], Y = s3[i * 3 + 1], Z = s3[i * 3 + 2];
+    const double xc = s_pose[0] * X + s_pose[1] * Y + s_pose[2] * Z + s_pose[3];
+    const double yc = s_pose[4] * X + s_pose[5] * Y + s_pose[6] * Z + s_pose[7];
+    const double zc = s_pose[8] * X + s_pose[9] * Y + s_pose[10] * Z + s_pose[11];
+    if (kFromGuess ? zc == 0.0 : !(zc > 1e-9)) continue;
+    const double iz = 1.0 / zc;
+    const double eu = s_K[0] * xc * iz + s_K[1] * yc * iz + s_K[2] - s2[i * 2], ev = s_K[4] * yc * iz + s_K[5] - s2[i * 2 + 1];
+    acc += eu * eu + ev * ev;
+  }
+  for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
+  __syncthreads();   // s_red may still be read by the caller's last reduction
+  if (lane == 0) sh.s_red[warp][0] = acc;
+  __syncthreads();
+  double tot = 0.0;
+  for (int w = 0; w < PR_THREADS / 32; ++w) tot += sh.s_red[w][0];
+  __syncthreads();
+  return tot;
+}
+
+// trace_cost (global [3], or null): cost at the start, the lowest cost evaluated, the cost at the returned pose.
 template <bool kFromGuess>
 __device__ __forceinline__ void lm_refine(double* s_pose, double* s_save, const unsigned char* inl, int N, int max_iters,
-                                          const PnpShared& sh) {
+                                          const PnpShared& sh, double* trace_cost = nullptr) {
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const float* s3 = sh.s3;
   const float* s2 = sh.s2;
   const double* s_K = sh.s_K;
   double (*s_red)[28] = sh.s_red;
   double* s_step = sh.s_step;
-  double lambda = 1e-4, prev_cost = -1.0;
+  double lambda = 1e-4, prev_cost = -1.0, lowest = INFINITY;   // lowest: thread 0's least cost evaluated
+  bool pending = false;   // the pose holds a step whose cost has not been evaluated
   for (int it = 0, solves = 0; it < max_iters && solves < 4 * max_iters; ++it, ++solves) {
     // normal equations: 21 (upper JtJ) + 6 (Jt r) + 1 (cost) sums
     double acc[28];
@@ -404,6 +477,8 @@ __device__ __forceinline__ void lm_refine(double* s_pose, double* s_save, const 
         for (int b = a; b < 6; ++b) { A[a * 6 + b] = tot[k]; A[b * 6 + a] = tot[k]; ++k; }
       for (int a = 0; a < 6; ++a) g[a] = -tot[21 + a];
       const double cost = tot[27];
+      if (trace_cost && prev_cost < 0.0) trace_cost[0] = cost;
+      lowest = fmin(lowest, cost);
       int stop = 0;
       if (prev_cost >= 0.0 && cost > prev_cost) {
         // the previous step made it worse: undo it and raise the damping
@@ -432,10 +507,23 @@ __device__ __forceinline__ void lm_refine(double* s_pose, double* s_save, const 
     __syncthreads();
     const bool accepted = s_step[6] != 0.0;
     if (accepted) prev_cost = s_step[5];
+    pending = accepted;
     const bool stop = s_step[7] == 1.0;
     __syncthreads();
     if (stop) break;
     if (kFromGuess && !accepted) --it;   // a rejected step does not count
+  }
+  if (pending) {   // the loop ended on a step it never evaluated: keep it only if it did not raise the cost
+    const double c = pose_cost<kFromGuess>(s_pose, inl, N, sh);
+    if (tid == 0) {
+      lowest = fmin(lowest, c);
+      if (c > prev_cost) for (int a = 0; a < 12; ++a) s_pose[a] = s_save[a];
+    }
+    __syncthreads();
+  }
+  if (trace_cost) {
+    const double c = pose_cost<kFromGuess>(s_pose, inl, N, sh);
+    if (tid == 0) { trace_cost[1] = lowest; trace_cost[2] = c; }
   }
 }
 
@@ -462,9 +550,16 @@ pnp_ransac_kernel(const PnpParams p) {
   // ---------------- 1. correspondences ----------------
   const int N = gather_correspondences(p, roi, sh);
   float* out = p.poses + (long long)roi * 12;
+  const PnpTrace& tr = p.tr;
+  const bool trace = tr.count != nullptr;
+  if (trace) {
+    if (tid == 0) tr.count[roi] = N;
+    for (int i = tid; i < PR_MAX_PTS; i += PR_THREADS) tr.src[(long long)roi * PR_MAX_PTS + i] = i < N ? (int)s_src[i] : -1;
+  }
   if (p.inlier_mask) for (int i = tid; i < npts; i += PR_THREADS) p.inlier_mask[(long long)roi * npts + i] = 0;
   if (N < 4) {   // gdrn_evaluator.py:1178-1179
     if (tid < 12) out[tid] = -100.f;
+    if (trace && tid < 12) tr.pose[roi * 12 + tid] = -100.0;
     if (tid == 0 && p.n_inliers) p.n_inliers[roi] = 0;
     return;
   }
@@ -474,8 +569,11 @@ pnp_ransac_kernel(const PnpParams p) {
   const double ifx = 1.0 / s_K[0], ify = 1.0 / s_K[4];
   for (int h = tid; h < H; h += PR_THREADS) {
     int id[4];
+    bool distinct = true;
     if (p.idxs) {
       for (int k = 0; k < 4; ++k) id[k] = (int)((unsigned)p.idxs[((long long)roi * H + h) * 4 + k] % (unsigned)N);
+      for (int k = 1; k < 4; ++k)
+        for (int j = 0; j < k; ++j) distinct = distinct && id[j] != id[k];
     } else {
       unsigned st = hash32(p.seed ^ hash32((unsigned)roi * 0x9E3779B9u + (unsigned)h));
       for (int k = 0; k < 4; ++k) {
@@ -483,6 +581,11 @@ pnp_ransac_kernel(const PnpParams p) {
         for (int tries = 0; tries < 8 && dup; ++tries) {
           st = hash32(st + 0x6D2B79F5u);
           id[k] = (int)(st % (unsigned)N);
+          dup = false;
+          for (int j = 0; j < k; ++j) dup = dup || (id[j] == id[k]);
+        }
+        while (dup) {   // eight draws collided: the next free id (N >= 4, so one exists) keeps the four distinct
+          id[k] = id[k] + 1 == N ? 0 : id[k] + 1;
           dup = false;
           for (int j = 0; j < k; ++j) dup = dup || (id[j] == id[k]);
         }
@@ -497,7 +600,7 @@ pnp_ransac_kernel(const PnpParams p) {
       f[k][0] = xn / nn; f[k][1] = yn / nn; f[k][2] = 1.0 / nn;
     }
     double sols[4][12];
-    const int ns = p3p_grunert(P, f, sols);
+    const int ns = distinct ? p3p_grunert(P, f, sols) : 0;   // a repeated correspondence gives no model
     double best = 1e300;
     int bi = -1;
     for (int s = 0; s < ns; ++s) {
@@ -512,6 +615,12 @@ pnp_ransac_kernel(const PnpParams p) {
       s_cnt[h] = 0;
     } else {
       s_cnt[h] = -1;   // no valid model from this sample
+    }
+    if (trace) {
+      const long long rh = (long long)roi * H + h;
+      for (int k = 0; k < 4; ++k) tr.samples[rh * 4 + k] = id[k];
+      tr.nsol[rh] = ns;
+      if (bi >= 0) for (int k = 0; k < 12; ++k) tr.hyp[rh * 12 + k] = sols[bi][k];
     }
   }
   __syncthreads();
@@ -538,10 +647,13 @@ pnp_ransac_kernel(const PnpParams p) {
       if (s_cnt[h] > bc) { bc = s_cnt[h]; bh = h; }
     s_flag = bh;
     if (bh >= 0) for (int k = 0; k < 12; ++k) s_pose[k] = s_hyp[bh][k];
+    if (trace) tr.best[roi] = bh;
   }
   __syncthreads();
+  if (trace) for (int h = tid; h < H; h += PR_THREADS) tr.cnt[(long long)roi * H + h] = s_cnt[h];
   if (s_flag < 0 || s_cnt[s_flag] < 4) {   // RANSAC found no model: the reference's solvePnPRansac returns garbage/false here
     if (tid < 12) out[tid] = -100.f;
+    if (trace && tid < 12) tr.pose[roi * 12 + tid] = -100.0;
     if (tid == 0 && p.n_inliers) p.n_inliers[roi] = 0;
     return;
   }
@@ -556,10 +668,15 @@ pnp_ransac_kernel(const PnpParams p) {
         in = du * du + dv * dv < thr2;
       }
       s_inl[i] = in ? 1 : 0;
+      if (trace) tr.inl[((long long)roi * 2 + round) * PR_MAX_PTS + i] = in ? 1 : 0;
     }
     __syncthreads();
-    lm_refine<false>(s_pose, s_hyp[0], s_inl, N, 12, sh);   // s_hyp[0] doubles as the saved pose
+    double* rp = trace ? tr.round_pose + ((long long)roi * 2 + round) * 24 : nullptr;
+    if (trace && tid < 12) rp[tid] = s_pose[tid];
+    // s_hyp[0] doubles as the saved pose
+    lm_refine<false>(s_pose, s_hyp[0], s_inl, N, 12, sh, trace ? tr.round_cost + ((long long)roi * 2 + round) * 3 : nullptr);
     __syncthreads();
+    if (trace && tid < 12) rp[12 + tid] = s_pose[tid];
   }
   // final inlier set of the refined pose
   int cnt = 0;
@@ -582,6 +699,7 @@ pnp_ransac_kernel(const PnpParams p) {
     if (p.n_inliers) p.n_inliers[roi] = c;
   }
   if (tid < 12) out[tid] = (float)s_pose[tid];
+  if (trace && tid < 12) tr.pose[roi * 12 + tid] = s_pose[tid];
 }
 
 // Network-initialised iterative PnP (TEST.PNP_TYPE = "net_iter_pnp", gdrn_evaluator.py:241-371): the reference calls
@@ -685,6 +803,34 @@ extern "C" int gdrn_pnp_ransac_points(const float* pts3d, const float* pts2d, co
   PnpParams p = {};
   p.pts3d = pts3d; p.pts2d = pts2d; p.Ks = Ks; p.idxs = idxs; p.npts = npts; p.iters = iters; p.reproj_thr = reproj_thr;
   p.seed = seed; p.poses = poses; p.n_inliers = n_inliers; p.inlier_mask = inlier_mask;
+  return launch_pnp(p, n, (cudaStream_t)stream);
+}
+
+extern "C" int gdrn_pnp_ransac_trace(const float* coor_x, const float* coor_y, const float* coor_z, const float* mask,
+                                     const float* roi_coord_2d, const float* im_hw, const float* extents,
+                                     const float* pts3d, const float* pts2d, const float* Ks, const int* idxs, int n,
+                                     int npts, int iters, float mask_thr, float reproj_thr, unsigned seed, float* poses,
+                                     int* n_inliers, unsigned char* inlier_mask, int* tr_count, int* tr_src,
+                                     int* tr_samples, int* tr_nsol, double* tr_hyp, int* tr_cnt, int* tr_best,
+                                     unsigned char* tr_inl, double* tr_round_pose, double* tr_round_cost,
+                                     double* tr_pose, void* stream) {
+  const bool maps = pts3d == nullptr;
+  GDRN_REQUIRE(Ks && poses && (maps ? (coor_x && coor_y && coor_z && mask && roi_coord_2d && im_hw && extents) : pts2d != nullptr),
+               "pnp_ransac_trace: null argument");
+  GDRN_REQUIRE(tr_count && tr_src && tr_samples && tr_nsol && tr_hyp && tr_cnt && tr_best && tr_inl && tr_round_pose &&
+               tr_round_cost && tr_pose, "pnp_ransac_trace: null trace buffer");
+  GDRN_REQUIRE(n > 0 && npts >= 1 && npts <= PR_MAX_PTS, "pnp_ransac_trace: need n > 0 and 1 <= npts <= 4096");
+  GDRN_REQUIRE(iters >= 1 && iters <= PR_MAX_HYP, "pnp_ransac_trace: iters must be in [1, 256]");
+  PnpParams p = {};
+  if (maps) {
+    p.coor_x = coor_x; p.coor_y = coor_y; p.coor_z = coor_z; p.mask = mask; p.coord2d = roi_coord_2d; p.im_hw = im_hw;
+    p.extents = extents; p.mask_thr = mask_thr;
+  } else {
+    p.pts3d = pts3d; p.pts2d = pts2d;
+  }
+  p.Ks = Ks; p.idxs = idxs; p.npts = npts; p.iters = iters; p.reproj_thr = reproj_thr; p.seed = seed; p.poses = poses;
+  p.n_inliers = n_inliers; p.inlier_mask = inlier_mask;
+  p.tr = {tr_count, tr_src, tr_samples, tr_nsol, tr_hyp, tr_cnt, tr_best, tr_inl, tr_round_pose, tr_round_cost, tr_pose};
   return launch_pnp(p, n, (cudaStream_t)stream);
 }
 

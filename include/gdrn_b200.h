@@ -388,6 +388,23 @@ int gdrn_pnp_ransac_maps(const float* coor_x, const float* coor_y, const float* 
 int gdrn_pnp_ransac_points(const float* pts3d, const float* pts2d, const float* Ks, const int* idxs, int n, int npts,
                            int iters, float reproj_thr, unsigned seed, float* poses, int* n_inliers,
                            unsigned char* inlier_mask, void* stream);
+/* gdrn_pnp_ransac_trace: the same kernel and outputs (bit-identical to the two entries above), plus a record of every
+ * stage.  Maps form when pts3d is null (npts = hw*hw), points form otherwise (the map arguments are then ignored).
+ * Trace buffers (device, all required; the caller initialises them, entries a ROI does not reach keep that value):
+ *   tr_count [n] i32 selected correspondences N; tr_src [n,4096] i32 source pixel / point of compacted entry i (-1 from N);
+ *   tr_samples [n,iters,4] i32 the ids each hypothesis used (after % N and de-duplication); tr_nsol [n,iters] i32 P3P
+ *   solutions; tr_hyp [n,iters,12] f64 the solution chosen by the fourth point; tr_cnt [n,iters] i32 inlier count
+ *   (-1 no model); tr_best [n] i32; tr_inl [n,2,4096] u8 inlier flags at the start of each refit round (compacted
+ *   order); tr_round_pose [n,2,2,12] f64 start / end pose of each round; tr_round_cost [n,2,3] f64 cost at the start,
+ *   the lowest cost the LM evaluated and the cost at the returned pose; tr_pose [n,12] f64 final pose (-100 for the
+ *   sentinel). */
+int gdrn_pnp_ransac_trace(const float* coor_x, const float* coor_y, const float* coor_z, const float* mask,
+                          const float* roi_coord_2d, const float* im_hw, const float* extents, const float* pts3d,
+                          const float* pts2d, const float* Ks, const int* idxs, int n, int npts, int iters,
+                          float mask_thr, float reproj_thr, unsigned seed, float* poses, int* n_inliers,
+                          unsigned char* inlier_mask, int* tr_count, int* tr_src, int* tr_samples, int* tr_nsol,
+                          double* tr_hyp, int* tr_cnt, int* tr_best, unsigned char* tr_inl, double* tr_round_pose,
+                          double* tr_round_cost, double* tr_pose, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
  * Network-initialised PnP (TEST.PNP_TYPE = net_*) -- replaces the per-ROI host loop process_net_and_pnp

@@ -13,6 +13,7 @@ import torch
 from conftest import ROOT
 from oracle import gdrn_model_oracle as O
 from oracle import ops_oracle as OO
+from oracle import pnp_oracle as PNO
 
 pytestmark = pytest.mark.gpu
 
@@ -1120,18 +1121,14 @@ def test_pnp_ransac_from_maps_vs_reference_recipe(dev):
     poses = poses.cpu().numpy().astype(np.float64)
     for i in range(n):
         # host restatement of the reference recipe on the same float32 maps
-        m32 = np.stack(mk).astype(np.float32)[i]
-        mn = (m32 - m32.min()) / (m32.max() - m32.min())
-        e32 = ext[i].astype(np.float32)
-        xyz = np.stack([(np.float32(cx_[i]) - np.float32(0.5)) * e32[0], (np.float32(cy_[i]) - np.float32(0.5)) * e32[1],
-                        (np.float32(cz_[i]) - np.float32(0.5)) * e32[2]], -1).astype(np.float32)
-        sel = (mn > 0.5) & (np.abs(xyz[..., 0]) > 1e-4 * e32[0]) & (np.abs(xyz[..., 1]) > 1e-4 * e32[1]) & (np.abs(xyz[..., 2]) > 1e-4 * e32[2])
-        img = np.stack([np.float32(c2d[i][0]) * imW, np.float32(c2d[i][1]) * imH], -1)
+        xyz, img, src = PNO.correspondences(cx_[i], cy_[i], cz_[i], mk[i], c2d[i], ext[i], imH, imW)
+        sel = np.zeros(hw * hw, bool)
+        sel[src] = True
         if sel.sum() < 4:
             assert (poses[i] == -100).all() and int(ninl[i]) == 0
             continue
-        assert int(imask[i].sum()) <= int(sel.sum()) and not bool((imask[i].cpu().numpy().astype(bool) & ~sel).any())
-        ok, rvec, tvec, _ = cv2.solvePnPRansac(xyz[sel][None].astype(np.float64), img[sel][None].astype(np.float64), K, np.zeros((8, 1)),
+        assert int(imask[i].sum()) <= int(sel.sum()) and not bool((imask[i].cpu().numpy().astype(bool).reshape(-1) & ~sel).any())
+        ok, rvec, tvec, _ = cv2.solvePnPRansac(xyz[None].astype(np.float64), img[None].astype(np.float64), K, np.zeros((8, 1)),
                                                flags=cv2.SOLVEPNP_EPNP, reprojectionError=3.0, iterationsCount=100)
         Rc = cv2.Rodrigues(rvec)[0]
         R, t = GT[i]

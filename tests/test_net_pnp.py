@@ -7,6 +7,7 @@ import torch
 
 from oracle import gdrn_model_oracle as O
 from oracle import ops_oracle as OO
+from oracle import pnp_oracle as PO
 
 K_CAM = np.array([[1066.778, 0, 312.9869], [0, 1067.487, 241.3109], [0, 0, 1]])
 NET_TYPES = ("net_iter_pnp", "net_ransac_pnp", "net_ransac_pnp_rot")
@@ -56,14 +57,7 @@ def ref_net_pnp(points_3d, points_2d, K, rot_est_net, out_transes, i, pnp_type):
 
 def ref_correspondences(cx, cy, cz, m, c2d, ext, imH, imW, mask_thr=0.5):
     """get_out_mask (L1) + get_img_model_points_with_coords2d (gdrn_evaluator.py:1183-1221) on float32 maps."""
-    m32 = m.astype(np.float32)
-    mn = (m32 - m32.min()) / (m32.max() - m32.min())
-    e32 = ext.astype(np.float32)
-    xyz = np.stack([(cx.astype(np.float32) - np.float32(0.5)) * e32[0], (cy.astype(np.float32) - np.float32(0.5)) * e32[1],
-                    (cz.astype(np.float32) - np.float32(0.5)) * e32[2]], -1).astype(np.float32)
-    sel = (mn > mask_thr) & (np.abs(xyz[..., 0]) > 1e-4 * e32[0]) & (np.abs(xyz[..., 1]) > 1e-4 * e32[1]) & (np.abs(xyz[..., 2]) > 1e-4 * e32[2])
-    img = np.stack([np.float32(c2d[0]) * np.float32(imW), np.float32(c2d[1]) * np.float32(imH)], -1)
-    return xyz[sel], img[sel]
+    return PO.correspondences(cx, cy, cz, m, c2d, ext, imH, imW, mask_thr)[:2]
 
 
 def ref_coor_z_step(xyz01, mask_n, sensor, ren, K_crop, rot_est, trans, thresh=0.8):
