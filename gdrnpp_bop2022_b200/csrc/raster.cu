@@ -7,14 +7,27 @@
 // coverage = sample inside the projected triangle (either winding, no culling: renderer.py:102);
 // the z-buffer value is affine in window space, i.e. 1/Z is interpolated with screen-space
 // barycentrics (== the perspective-correct interpolation of camera-space Z in the EGL shader);
-// nearest fragment wins; background = 0.  Triangles with a vertex closer than znear are dropped
-// (GL would clip them; objects in front of the camera never hit this).
+// nearest fragment wins, and on equal depth the lower triangle index; background = 0.  Triangles with a vertex closer
+// than znear are dropped whole (GL would clip them; objects in front of the camera never hit this); a fragment with
+// z < znear or z > zfar is dropped at its pixel.  Coverage is watertight: the triangles sharing an edge evaluate its
+// edge function bit for bit alike up to sign (edge_fn), so a sample on the shared side of one is covered by the other.
 //
 // Algorithmic HBM traffic per render: 12*V + 12*F bytes of mesh + 8*H*W z-buffer scratch + 4*H*W out.
 // One thread per (render, triangle); 64-bit atomicMin on (z_bits << 32 | triangle) resolves visibility.
 #include "common.cuh"
 
 namespace {
+
+// Edge function of the edge a -> b at the sample (sx, sy), (ua - sx)(vb - sy) - (ub - sx)(va - sy).  The endpoints are
+// taken in a canonical order (by screen position) and the products are not contracted into an fma, so the two
+// triangles sharing an edge get the same magnitude with opposite signs whatever their vertex order: a sample is covered
+// by at least one of them, and by both only when it lies exactly on the edge.
+__device__ __forceinline__ float edge_fn(float ua, float va, float ub, float vb, float sx, float sy) {
+  const bool swap = ub < ua || (ub == ua && vb < va);
+  const float x0 = swap ? ub : ua, y0 = swap ? vb : va, x1 = swap ? ua : ub, y1 = swap ? va : vb;
+  const float e = __fsub_rn(__fmul_rn(__fsub_rn(x0, sx), __fsub_rn(y1, sy)), __fmul_rn(__fsub_rn(x1, sx), __fsub_rn(y0, sy)));
+  return swap ? -e : e;
+}
 
 __global__ void rast_clear_kernel(unsigned long long* zbuf, long long n) {
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x)
@@ -29,19 +42,14 @@ struct MeshEntry {
 };
 constexpr int RAST_MAX_MESHES = 1024;
 
-// one thread per (ROI, triangle of that ROI's mesh); grid.x covers the largest registered mesh
-__global__ void __launch_bounds__(256)
-rast_tri_multi_kernel(const MeshEntry* __restrict__ table, const int* __restrict__ mesh_ids, int n_meshes,
-                      const float* __restrict__ poses, const float* __restrict__ Ks, int H, int W, float znear, float zfar,
-                      unsigned long long* __restrict__ zbuf) {
-  const int r = blockIdx.y;
-  int mid = mesh_ids[r];
-  if (mid < 0 || mid >= n_meshes) return;   // unknown id: the ROI renders as background
+// the triangles of one ROI: mesh `mid` (an unknown id renders as background) at pose P [3,4] with intrinsics K, into zb
+__device__ __forceinline__ void rast_tri_one(const MeshEntry* __restrict__ table, int mid, int n_meshes,
+                                             const float* __restrict__ P, const float* __restrict__ K, int H, int W,
+                                             float znear, float zfar, unsigned long long* __restrict__ zb) {
+  if (mid < 0 || mid >= n_meshes) return;
   const MeshEntry me = table[mid];
   const int f = blockIdx.x * blockDim.x + threadIdx.x;
   if (f >= me.F) return;
-  const float* P = poses + r * 12;
-  const float* K = Ks + r * 9;
   float u[3], v[3], iz[3];
 #pragma unroll
   for (int k = 0; k < 3; ++k) {
@@ -62,15 +70,15 @@ rast_tri_multi_kernel(const MeshEntry* __restrict__ table, const int* __restrict
   int c1 = min(W - 1, (int)ceilf(fmaxf(fmaxf(u[0], u[1]), u[2]) - 0.5f));
   int r0 = max(0, (int)floorf(fminf(fminf(v[0], v[1]), v[2]) - 0.5f));
   int r1 = min(H - 1, (int)ceilf(fmaxf(fmaxf(v[0], v[1]), v[2]) - 0.5f));
-  unsigned long long* zb = zbuf + (long long)r * H * W;
   for (int py = r0; py <= r1; ++py) {
     const float sy = (float)py + 0.5f;
     for (int px = c0; px <= c1; ++px) {
       const float sx = (float)px + 0.5f;
-      const float w0 = ((u[1] - sx) * (v[2] - sy) - (u[2] - sx) * (v[1] - sy)) * inv_area;
-      const float w1 = ((u[2] - sx) * (v[0] - sy) - (u[0] - sx) * (v[2] - sy)) * inv_area;
-      const float w2 = 1.0f - w0 - w1;
-      if (w0 < 0.f || w1 < 0.f || w2 < 0.f) continue;
+      const float w0 = edge_fn(u[1], v[1], u[2], v[2], sx, sy) * inv_area;
+      const float w1 = edge_fn(u[2], v[2], u[0], v[0], sx, sy) * inv_area;
+      const float e2 = edge_fn(u[0], v[0], u[1], v[1], sx, sy) * inv_area;
+      if (w0 < 0.f || w1 < 0.f || e2 < 0.f) continue;
+      const float w2 = 1.0f - w0 - w1;   // interpolation weights that sum to 1: a plane of constant Z keeps its depth
       const float izp = w0 * iz[0] + w1 * iz[1] + w2 * iz[2];
       const float zp = 1.0f / izp;
       if (!(zp >= znear) || zp > zfar) continue;
@@ -78,6 +86,16 @@ rast_tri_multi_kernel(const MeshEntry* __restrict__ table, const int* __restrict
       atomicMin(zb + (long long)py * W + px, key);
     }
   }
+}
+
+// one thread per (ROI, triangle of that ROI's mesh); grid.x covers the largest registered mesh, grid.y strides over
+// the ROIs (gridDim.y is capped at 65535, so each block row may take several ROIs)
+__global__ void __launch_bounds__(256)
+rast_tri_multi_kernel(const MeshEntry* __restrict__ table, const int* __restrict__ mesh_ids, int n_meshes, int n,
+                      const float* __restrict__ poses, const float* __restrict__ Ks, int H, int W, float znear, float zfar,
+                      unsigned long long* __restrict__ zbuf) {
+  for (int r = blockIdx.y; r < n; r += gridDim.y) rast_tri_one(table, mesh_ids[r], n_meshes, poses + r * 12, Ks + r * 9,
+                                                               H, W, znear, zfar, zbuf + (long long)r * H * W);
 }
 
 __global__ void rast_resolve_kernel(const unsigned long long* __restrict__ zbuf, const float* __restrict__ Ks, int n,
@@ -404,8 +422,8 @@ extern "C" int rast_render_meshes(const int* mesh_ids, const float* poses, const
   const long long npx = (long long)n * H * W;
   int blocks = (int)((npx + 255) / 256 > 4096 ? 4096 : (npx + 255) / 256);
   rast_clear_kernel<<<blocks, 256, 0, st>>>(zbuf_scratch, npx);
-  rast_tri_multi_kernel<<<dim3((g_meshes.max_faces + 255) / 256, n), 256, 0, st>>>(g_meshes.dev_table, mesh_ids, g_meshes.count, poses, Ks,
-                                                                                 H, W, znear, zfar, zbuf_scratch);
+  rast_tri_multi_kernel<<<dim3((g_meshes.max_faces + 255) / 256, n < 65535 ? n : 65535), 256, 0, st>>>(
+      g_meshes.dev_table, mesh_ids, g_meshes.count, n, poses, Ks, H, W, znear, zfar, zbuf_scratch);
   rast_resolve_kernel<<<blocks, 256, 0, st>>>(zbuf_scratch, Ks, n, H, W, znear, zfar, quantize_bits, depth, xyz_cam);
   GDRN_CHECK_CUDA(cudaGetLastError());
   gdrn_count_launch(3);
@@ -423,8 +441,8 @@ extern "C" int rast_render_meshes_rgb(const int* mesh_ids, const float* poses, c
   const long long npx = (long long)n * H * W;
   int blocks = (int)((npx + 255) / 256 > 4096 ? 4096 : (npx + 255) / 256);
   rast_clear_kernel<<<blocks, 256, 0, st>>>(zbuf_scratch, npx);
-  rast_tri_multi_kernel<<<dim3((g_meshes.max_faces + 255) / 256, n), 256, 0, st>>>(g_meshes.dev_table, mesh_ids, g_meshes.count, poses, Ks,
-                                                                                 H, W, znear, zfar, zbuf_scratch);
+  rast_tri_multi_kernel<<<dim3((g_meshes.max_faces + 255) / 256, n < 65535 ? n : 65535), 256, 0, st>>>(
+      g_meshes.dev_table, mesh_ids, g_meshes.count, n, poses, Ks, H, W, znear, zfar, zbuf_scratch);
   rast_shade_kernel<<<blocks, 256, 0, st>>>(zbuf_scratch, g_meshes.dev_table, g_meshes.dev_colors, mesh_ids, poses, Ks, colors,
                                             n, H, W, rgb, depth, tri_ids);
   GDRN_CHECK_CUDA(cudaGetLastError());
