@@ -72,6 +72,8 @@ _SIGNATURES = {
     "rast_scratch_bytes": (c_size_t, [c_int, c_int, c_int]),
     "gdrn_depth_refine_step": (c_int, [c_void_p, c_void_p, c_int] + [c_void_p] * 4 + [c_int, c_void_p, c_int, c_int, c_float,
                                                                                  c_void_p]),
+    "gdrn_depth_refine_trace": (c_int, [c_void_p, c_void_p, c_int] + [c_void_p] * 4 + [c_int, c_void_p, c_int, c_int, c_float]
+                                + [c_void_p] * 14),
     "rast_upload_mesh": (c_int, [c_void_p, c_int, c_void_p, c_int]),
     "rast_upload_mesh_ex": (c_int, [c_void_p, c_int, c_void_p, c_int, c_void_p]),
     "rast_mesh_count": (c_int, []),

@@ -219,10 +219,26 @@ rast_shade_kernel(const unsigned long long* __restrict__ zbuf, const MeshEntry* 
 // raw weight.
 constexpr int DR_THREADS = 1024;
 
+// Per-stage record of depth_refine_kernel (gdrn_depth_refine_trace), device pointers, used only by the TRACE = true
+// instantiation.  Entries a ROI does not reach (zero sum, empty selection) keep what the caller initialised them to.
+struct DrTrace {
+  float* m_lo; float* m_scale;      // [n] mask normalisation (0 and 1 unless mask_mode 1)
+  float* w;                         // [n, hw*hw] raw weights before the division by the sum
+  double* sum;                      // [n]
+  float* max; float* min; float* cut;   // [n] reduced max / min (zero included) and the selection cut
+  unsigned char* sel;               // [n, hw*hw] selected pixels
+  int* count;                       // [n]
+  float* median;                    // [n]
+  double* centroid;                 // [n, 2] (y, x)
+  double* ray;                      // [n, 3] K^-1 (x, y, 1) / z
+  float* t;                         // [n, 3] the output translation
+};
+
+template <bool TRACE>
 __global__ void __launch_bounds__(DR_THREADS)
 depth_refine_kernel(const float* __restrict__ xyz, const float* __restrict__ mask, const float* __restrict__ sensor,
                     const float* __restrict__ ren, const float* __restrict__ Kc, float* __restrict__ trans, int hw,
-                    float thresh, int mask_mode, const float* __restrict__ rot, int weight_mode) {
+                    float thresh, int mask_mode, const float* __restrict__ rot, int weight_mode, DrTrace tr) {
   extern __shared__ float sm[];  // [npix] weights, then [npow2] diffs for the sort
   const int roi = blockIdx.x;
   const int npix = hw * hw;
@@ -252,6 +268,7 @@ depth_refine_kernel(const float* __restrict__ xyz, const float* __restrict__ mas
     for (int k = 0; k < DR_THREADS / 32; ++k) { mn = fminf(mn, red_mm[0][k]); mx = fmaxf(mx, red_mm[1][k]); }
     m_lo = mn; m_scale = mx - mn;    // applied as a DIVISION below, like torch's (mask - min) / (max - min)
   }
+  if constexpr (TRACE) { if (tid == 0) { tr.m_lo[roi] = m_lo; tr.m_scale[roi] = m_scale; } }
   // pass 1: weights, sum (double), max (and min for the signed coor-z weights)
   const float Rz0 = weight_mode == 1 ? rot[roi * 9 + 6] : 0.f, Rz1 = weight_mode == 1 ? rot[roi * 9 + 7] : 0.f,
               Rz2 = weight_mode == 1 ? rot[roi * 9 + 8] : 0.f;
@@ -266,6 +283,7 @@ depth_refine_kernel(const float* __restrict__ xyz, const float* __restrict__ mas
     const float rd = ren[(long long)roi * npix + i], sd = sensor[(long long)roi * npix + i];
     if (!(rd > 0.f) || !(sd > 0.f)) wv = 0.f;
     sw[i] = wv;
+    if constexpr (TRACE) tr.w[(long long)roi * npix + i] = wv;
     lsum += (double)wv;
     lmax = fmaxf(lmax, wv);
     lmin = fminf(lmin, wv);
@@ -281,11 +299,17 @@ depth_refine_kernel(const float* __restrict__ xyz, const float* __restrict__ mas
   double tsum = 0.0;
   float tmax = 0.f, tmin = 0.f;
   for (int k = 0; k < DR_THREADS / 32; ++k) { tsum += red_d[k]; tmax = fmaxf(tmax, red_f[k]); tmin = fminf(tmin, red_n[k]); }
+  if constexpr (TRACE) { if (tid == 0) { tr.sum[roi] = tsum; tr.max[roi] = tmax; tr.min[roi] = tmin; } }
   if (tsum == 0.0) return;  // reference: `continue` (pose unchanged)
-  const float inv = (float)(1.0 / tsum);
+  // w / sum is formed as (w * pre) * inv.  Below |sum| = 2^-128 the float reciprocal would overflow to inf and select
+  // nothing; there the weights are scaled by pre = 2^64 and the reciprocal by 2^-64, which rounds every w / sum as the
+  // unscaled product would round it if float had the exponent range.  Elsewhere pre = 1 and nothing changes.
+  float inv = (float)(1.0 / tsum), pre = 1.f;
+  if (isinf(inv)) { pre = 0x1p64f; inv = (float)(1.0 / (tsum * 0x1p64)); }
   // max over all pixels of w / sum: from the largest raw weight when the sum is positive, from the most negative one
   // (zeros included in both) when it is negative
-  const float cut = ((weight_mode == 1 && inv < 0.f ? tmin : tmax) * inv) * thresh;
+  const float cut = (((weight_mode == 1 && inv < 0.f ? tmin : tmax) * pre) * inv) * thresh;
+  if constexpr (TRACE) { if (tid == 0) tr.cut[roi] = cut; }
   // pass 2: weighted centroid (double) and selection of depth differences
   int npow2 = 1;
   while (npow2 < npix) npow2 <<= 1;
@@ -294,9 +318,10 @@ depth_refine_kernel(const float* __restrict__ xyz, const float* __restrict__ mas
   __syncthreads();
   double ly = 0.0, lx = 0.0;
   for (int i = tid; i < npix; i += DR_THREADS) {
-    const float wn = sw[i] * inv;
+    const float wn = (sw[i] * pre) * inv;
     ly += (double)wn * (double)(i / hw);
     lx += (double)wn * (double)(i % hw);
+    if constexpr (TRACE) tr.sel[(long long)roi * npix + i] = wn > cut;
     if (wn > cut) {
       const int slot = atomicAdd(&s_count, 1);
       sdiff[slot] = sensor[(long long)roi * npix + i] - ren[(long long)roi * npix + i];
@@ -326,6 +351,7 @@ depth_refine_kernel(const float* __restrict__ xyz, const float* __restrict__ mas
   }
   if (tid == 0) {
     const int cnt = s_count;
+    if constexpr (TRACE) tr.count[roi] = cnt;
     if (cnt > 0) {
       // np.median: mean of the two middle elements for an even count
       const float med = (cnt & 1) ? sdiff[cnt >> 1] : 0.5f * (sdiff[(cnt >> 1) - 1] + sdiff[cnt >> 1]);
@@ -343,8 +369,29 @@ depth_refine_kernel(const float* __restrict__ xyz, const float* __restrict__ mas
       t[0] = (float)((double)t[0] + rx / rz * (double)med);
       t[1] = (float)((double)t[1] + ry / rz * (double)med);
       t[2] = (float)((double)t[2] + 1.0 * (double)med);
+      if constexpr (TRACE) {
+        tr.median[roi] = med;
+        tr.centroid[roi * 2] = cy; tr.centroid[roi * 2 + 1] = cx;
+        tr.ray[roi * 3] = rx / rz; tr.ray[roi * 3 + 1] = ry / rz; tr.ray[roi * 3 + 2] = 1.0;
+      }
     }
+    if constexpr (TRACE) { for (int k = 0; k < 3; ++k) tr.t[roi * 3 + k] = trans[roi * 3 + k]; }
   }
+}
+
+template <bool TRACE>
+int launch_depth_refine(const float* xyz, const float* mask, int mask_mode, const float* depth_sensor,
+                        const float* ren_depth, const float* K_crop, const float* rot, int weight_mode, float* trans,
+                        int n, int hw, float thresh, const DrTrace& tr, cudaStream_t stream) {
+  int npix = hw * hw, npow2 = 1;
+  while (npow2 < npix) npow2 <<= 1;
+  size_t smem = (size_t)(npix + npow2) * 4;
+  GDRN_OPT_IN_SMEM(depth_refine_kernel<TRACE>, 160 * 1024);
+  depth_refine_kernel<TRACE><<<n, DR_THREADS, smem, stream>>>(xyz, mask, depth_sensor, ren_depth, K_crop, trans, hw,
+                                                               thresh, mask_mode, rot, weight_mode, tr);
+  GDRN_CHECK_CUDA(cudaGetLastError());
+  gdrn_count_launch(1);
+  return GDRN_OK;
 }
 
 }  // namespace
@@ -458,13 +505,25 @@ extern "C" int gdrn_depth_refine_step(const float* xyz, const float* mask, int m
   GDRN_REQUIRE(weight_mode == 0 || weight_mode == 1, "depth_refine: weight_mode must be 0 (||xyz||) or 1 (coor-z)");
   GDRN_REQUIRE(weight_mode == 0 || rot, "depth_refine: the coor-z weighting needs the rotations");
   GDRN_REQUIRE(n > 0 && hw > 0 && hw <= 128, "depth_refine: need 0 < hw <= 128");
-  int npix = hw * hw, npow2 = 1;
-  while (npow2 < npix) npow2 <<= 1;
-  size_t smem = (size_t)(npix + npow2) * 4;
-  GDRN_OPT_IN_SMEM(depth_refine_kernel, 160 * 1024);
-  depth_refine_kernel<<<n, DR_THREADS, smem, (cudaStream_t)stream>>>(xyz, mask, depth_sensor, ren_depth, K_crop, trans,
-                                                                    hw, thresh, mask_mode, rot, weight_mode);
-  GDRN_CHECK_CUDA(cudaGetLastError());
-  gdrn_count_launch(1);
-  return GDRN_OK;
+  return launch_depth_refine<false>(xyz, mask, mask_mode, depth_sensor, ren_depth, K_crop, rot, weight_mode, trans, n,
+                                    hw, thresh, DrTrace{}, (cudaStream_t)stream);
+}
+
+extern "C" int gdrn_depth_refine_trace(const float* xyz, const float* mask, int mask_mode, const float* depth_sensor,
+                                       const float* ren_depth, const float* K_crop, const float* rot, int weight_mode,
+                                       float* trans, int n, int hw, float thresh, float* tr_m_lo, float* tr_m_scale,
+                                       float* tr_w, double* tr_sum, float* tr_max, float* tr_min, float* tr_cut,
+                                       unsigned char* tr_sel, int* tr_count, float* tr_median, double* tr_centroid,
+                                       double* tr_ray, float* tr_t, void* stream) {
+  GDRN_REQUIRE(xyz && mask && depth_sensor && ren_depth && K_crop && trans, "depth_refine_trace: null argument");
+  GDRN_REQUIRE(tr_m_lo && tr_m_scale && tr_w && tr_sum && tr_max && tr_min && tr_cut && tr_sel && tr_count && tr_median &&
+               tr_centroid && tr_ray && tr_t, "depth_refine_trace: null trace buffer");
+  GDRN_REQUIRE(mask_mode >= 0 && mask_mode <= 2, "depth_refine: mask_mode must be 0 (normalised), 1 (raw L1) or 2 (logits)");
+  GDRN_REQUIRE(weight_mode == 0 || weight_mode == 1, "depth_refine: weight_mode must be 0 (||xyz||) or 1 (coor-z)");
+  GDRN_REQUIRE(weight_mode == 0 || rot, "depth_refine: the coor-z weighting needs the rotations");
+  GDRN_REQUIRE(n > 0 && hw > 0 && hw <= 128, "depth_refine: need 0 < hw <= 128");
+  const DrTrace tr = {tr_m_lo, tr_m_scale, tr_w, tr_sum, tr_max, tr_min, tr_cut, tr_sel, tr_count, tr_median,
+                      tr_centroid, tr_ray, tr_t};
+  return launch_depth_refine<true>(xyz, mask, mask_mode, depth_sensor, ren_depth, K_crop, rot, weight_mode, trans, n,
+                                   hw, thresh, tr, (cudaStream_t)stream);
 }

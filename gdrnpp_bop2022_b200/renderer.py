@@ -143,6 +143,37 @@ def depth_refine(models, rot, trans, K_crop, xyz, mask, depth_sensor, iters=2, t
     return t
 
 
+@_lib.on_device(0)
+def depth_refine_trace(xyz, mask, depth_sensor, ren, K_crop, trans, rot=None, mask_mode=1, weight_mode=0, thresh=0.8):
+    """One refine step of depth_refine on a given render, with a record of every stage (gdrn_depth_refine_trace), for
+    tests.  xyz [n,3,hw,hw], mask [n,hw,hw] (mask_mode 0 normalised, 1 raw L1, 2 logits), depth_sensor and ren
+    [n,hw,hw], K_crop [n,3,3], trans [n,3], rot [n,3,3] (weight_mode 1 only).  Returns a dict of tensors on the device:
+    t [n,3] (the refined translation, as gdrn_depth_refine_step returns it) and the trace m_lo, m_scale [n], w [n,hw,hw],
+    sum [n] f64, max, min, cut [n], sel [n,hw,hw] bool, count [n], median [n], centroid [n,2] f64 (y, x), ray [n,3] f64
+    and t_trace [n,3].  Entries a ROI does not reach hold NaN (count -1)."""
+    if not xyz.is_cuda:
+        raise _lib.GdrnError("depth_refine_trace needs CUDA tensors (no CPU fallback)")
+    dev = xyz.device
+    n, hw = xyz.shape[0], xyz.shape[-1]
+    xyz, K_crop = _f32c(xyz), _f32c(K_crop)
+    mask, sensor, ren = (_f32c(a).reshape(n, hw, hw) for a in (mask, depth_sensor, ren))
+    rot = None if rot is None else _f32c(rot)
+    f32 = lambda *s: torch.full(s, float("nan"), dtype=torch.float32, device=dev)
+    f64 = lambda *s: torch.full(s, float("nan"), dtype=torch.float64, device=dev)
+    out = dict(t=_f32c(trans).clone(), m_lo=f32(n), m_scale=f32(n), w=f32(n, hw, hw), sum=f64(n), max=f32(n), min=f32(n),
+               cut=f32(n), sel=torch.zeros((n, hw, hw), dtype=torch.uint8, device=dev),
+               count=torch.full((n,), -1, dtype=torch.int32, device=dev), median=f32(n), centroid=f64(n, 2), ray=f64(n, 3),
+               t_trace=f32(n, 3))
+    P = lambda k: _lib.ptr(out[k])
+    _lib.check(_lib.lib().gdrn_depth_refine_trace(_lib.ptr(xyz), _lib.ptr(mask), int(mask_mode), _lib.ptr(sensor), _lib.ptr(ren),
+                                                  _lib.ptr(K_crop), _lib.ptr(rot), int(weight_mode), P("t"), n, hw, float(thresh),
+                                                  P("m_lo"), P("m_scale"), P("w"), P("sum"), P("max"), P("min"), P("cut"),
+                                                  P("sel"), P("count"), P("median"), P("centroid"), P("ray"), P("t_trace"),
+                                                  _lib.current_stream()), "gdrn_depth_refine_trace")
+    out["sel"] = out["sel"].bool()
+    return out
+
+
 class Model3D:
     """Minimal stand-in for lib/render_vispy/model3d.py objects: vertices [V,3] in metres + triangle indices [F,3] on
     `device`, and mesh_id, the mesh's id in the library's registry.  The mesh is uploaded once, here; the registry never

@@ -313,11 +313,25 @@ int rast_render_meshes_rgb(const int* mesh_ids, const float* poses, const float*
  *   weight_mode: 0 = ||xyz||, 1 = TEST.USE_COOR_Z_REFINE (gdrn_evaluator.py:528-537): w = (R xyz)_z * mask *
  *   (ren > 0) * (sensor > 0) with `xyz` the raw [0,1] coordinate maps and rot [n,3,3] the rotation of the pose being
  *   refined (may be NULL for mode 0).  Signed weights follow the reference's order: divide by the sum, then threshold
- *   against the max over all pixels; a zero sum leaves t unchanged.
+ *   against the max over all pixels; a zero sum leaves t unchanged.  So does an empty selection (a constant L1
+ *   mask, thresh >= 1), where the reference's median of nothing is NaN.  Sums below 2^-128 in magnitude are
+ *   normalised without overflowing the f32 reciprocal (INTEGRATION.md section 7).
  * ------------------------------------------------------------------------------------------- */
 int gdrn_depth_refine_step(const float* xyz, const float* mask, int mask_mode, const float* depth_sensor,
                            const float* ren_depth, const float* K_crop, const float* rot, int weight_mode, float* trans,
                            int n, int hw, float thresh, void* stream);
+/* gdrn_depth_refine_trace: the same kernel and output (trans bit-identical to gdrn_depth_refine_step), plus a record
+ * of every stage.  Trace buffers (device, all required; the caller initialises them, entries a ROI does not reach --
+ * after a zero sum, or with nothing selected -- keep that value):
+ *   tr_m_lo, tr_m_scale [n] f32 the mask normalisation (m - m_lo) / m_scale (0 and 1 unless mask_mode 1);
+ *   tr_w [n,hw*hw] f32 raw weights; tr_sum [n] f64; tr_max, tr_min [n] f32 (zero included); tr_cut [n] f32;
+ *   tr_sel [n,hw*hw] u8 selected pixels; tr_count [n] i32; tr_median [n] f32; tr_centroid [n,2] f64 (y, x);
+ *   tr_ray [n,3] f64 K^-1 (x, y, 1) / z; tr_t [n,3] f32 the output translation. */
+int gdrn_depth_refine_trace(const float* xyz, const float* mask, int mask_mode, const float* depth_sensor,
+                            const float* ren_depth, const float* K_crop, const float* rot, int weight_mode, float* trans,
+                            int n, int hw, float thresh, float* tr_m_lo, float* tr_m_scale, float* tr_w, double* tr_sum,
+                            float* tr_max, float* tr_min, float* tr_cut, unsigned char* tr_sel, int* tr_count,
+                            float* tr_median, double* tr_centroid, double* tr_ray, float* tr_t, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
  * ROI crop + resize (SURVEY.md 8f rank 1) -- replaces crop_resize_by_warp_affine = cv2.warpAffine
