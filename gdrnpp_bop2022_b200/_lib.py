@@ -86,6 +86,7 @@ _SIGNATURES = {
     "gdrn_pnp_iterative_points": (c_int, [c_void_p] * 5 + [c_int, c_int, c_void_p, c_void_p]),
     "gdrn_xyz_region_targets": (c_int, [c_void_p] * 6 + [c_int] * 4 + [c_void_p] * 5),
     "yolox_postprocess_workspace_bytes": (c_size_t, [c_int, c_int]),
+    "yolox_postprocess_layout": (c_int, [c_int, c_int, POINTER(c_size_t)]),
     "yolox_postprocess": (c_int, [c_void_p] + [c_int] * 3 + [c_void_p, c_void_p, c_int, c_float, c_float, c_int, c_int, c_void_p, c_void_p,
                                   c_void_p, c_size_t, c_void_p]),
     "yolox_model_create": (c_int, [POINTER(c_void_p), c_double, c_double] + [c_int] * 5),
@@ -104,7 +105,8 @@ _SIGNATURES = {
     "yolox_model_buffer_info": (c_int, [c_void_p, c_int, c_int, c_int, POINTER(c_int64)]),
     "yolox_model_run_step": (c_int, [c_void_p, c_int, c_int, c_void_p, c_int, c_void_p, c_void_p, c_size_t, c_void_p]),
     "yolox_postprocess_single_workspace_bytes": (c_size_t, [c_int] * 3),
-    "yolox_postprocess_single": (c_int, [c_void_p] + [c_int] * 3 + [c_float, c_float] + [c_void_p] * 3 + [c_size_t, c_void_p]),
+    "yolox_postprocess_single_layout": (c_int, [c_int] * 3 + [POINTER(c_size_t)]),
+    "yolox_postprocess_single": (c_int, [c_void_p] + [c_int] * 3 + [c_float, c_double] + [c_void_p] * 3 + [c_size_t, c_void_p]),
     "gdrn_crop_resize_u8": (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p,
                                     c_void_p]),
     "gdrn_crop_resize_f32": (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p]),

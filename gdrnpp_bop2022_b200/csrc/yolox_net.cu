@@ -348,6 +348,9 @@ __global__ void yolox_head_out_kernel(const float* __restrict__ raw, int B, int 
 }
 
 // ---- keep-single-instance post-process (predictor_yolo.py:84-140 with keep_single_instance=True, class_agnostic=True) ----
+// The reference scores and filters on the device (torch compares the CUDA tensor with conf_thre rounded to fp32), copies
+// the selected rows into a host tensor (instance_detections = torch.rand(num_classes, 7)) and so runs torchvision's CPU
+// nms: every product rounded on its own and the fp32 IoU compared with the threshold as a double.
 // per anchor: class_conf / class_pred = first max over the class scores, score = obj * class_conf
 __global__ void yolox_ksi_score_kernel(const float* __restrict__ preds, int B, int A, int nc, float* __restrict__ score,
                                        int* __restrict__ cls) {
@@ -392,7 +395,7 @@ __global__ void __launch_bounds__(256) yolox_ksi_select_kernel(const float* __re
 
 constexpr int KSI_MAX_CLASSES = 1024;
 
-__device__ __forceinline__ float ksi_iou(const float* a, const float* b) {   // torchvision devIoU (as yolox_post.cu)
+__device__ __forceinline__ float ksi_iou(const float* a, const float* b) {   // torchvision's CPU nms: (Sa + Sb) - inter
   const float left = fmaxf(a[0], b[0]), right = fminf(a[2], b[2]);
   const float top = fmaxf(a[1], b[1]), bottom = fminf(a[3], b[3]);
   const float width = fmaxf(__fsub_rn(right, left), 0.f), height = fmaxf(__fsub_rn(bottom, top), 0.f);
@@ -405,7 +408,7 @@ __device__ __forceinline__ float ksi_iou(const float* a, const float* b) {   // 
 // one thread per image: the (at most nc) selected rows, class-agnostic greedy NMS in descending score order, kept rows
 // written in ascending class order
 __global__ void yolox_ksi_nms_kernel(const float* __restrict__ preds, const int* __restrict__ sel, const float* __restrict__ score,
-                                     int A, int nc, float nms_thre, float* __restrict__ dets, int* __restrict__ n_det) {
+                                     int A, int nc, double nms_thre, float* __restrict__ dets, int* __restrict__ n_det) {
   const int b = blockIdx.x;
   int n_in = 0;
   // sorted insertion by (score desc, class asc) into the output area itself: rows are 7 floats, class kept in row[6]
@@ -426,11 +429,11 @@ __global__ void yolox_ksi_nms_kernel(const float* __restrict__ preds, const int*
     for (int k = 0; k < 7; ++k) out[pos * 7 + k] = row[k];
     ++n_in;
   }
-  // greedy suppression: a kept row removes every later row with IoU > nms_thre; removed rows get class -1
+  // greedy suppression: a kept row removes every later row with (double)IoU > nms_thre; removed rows get class -1
   for (int i = 0; i < n_in; ++i) {
     if (out[i * 7 + 6] < 0.f) continue;
     for (int j = i + 1; j < n_in; ++j)
-      if (out[j * 7 + 6] >= 0.f && ksi_iou(out + i * 7, out + j * 7) > nms_thre) out[j * 7 + 6] = -1.f;
+      if (out[j * 7 + 6] >= 0.f && (double)ksi_iou(out + i * 7, out + j * 7) > nms_thre) out[j * 7 + 6] = -1.f;
   }
   // compact in ascending class order (selection sort over the survivors: at most nc rows)
   int kept = 0;
@@ -1058,23 +1061,37 @@ extern "C" int yolox_model_run_step(YoloxModel* m, int plan, int step, const flo
   return GDRN_OK;
 }
 
+// workspace layout, byte offsets from the 256-byte-aligned base: score [B,A] f32, cls [B,A] i32, sel [B,nc] i32
+static void ksi_layout(int B, int A, size_t off[3]) {
+  off[0] = 0;
+  off[1] = ((size_t)B * A * 4 + 255) & ~(size_t)255;
+  off[2] = off[1] + (((size_t)B * A * 4 + 255) & ~(size_t)255);
+}
+
 extern "C" size_t yolox_postprocess_single_workspace_bytes(int B, int A, int num_classes) {
   if (B <= 0 || A <= 0 || num_classes <= 0) return 0;
   return (size_t)B * A * 8 + (size_t)B * num_classes * 4 + 4 * 256;
 }
 
-extern "C" int yolox_postprocess_single(const float* preds, int B, int A, int num_classes, float conf_thre, float nms_thre, float* dets,
-                                        int* n_det, void* workspace, size_t workspace_bytes, void* stream) {
+extern "C" int yolox_postprocess_single_layout(int B, int A, int num_classes, size_t* offsets) {
+  GDRN_REQUIRE(offsets && B > 0 && A > 0 && num_classes > 0, "yolox_postprocess_single_layout: bad arguments");
+  ksi_layout(B, A, offsets);
+  return GDRN_OK;
+}
+
+extern "C" int yolox_postprocess_single(const float* preds, int B, int A, int num_classes, float conf_thre, double nms_thre,
+                                        float* dets, int* n_det, void* workspace, size_t workspace_bytes, void* stream) {
   GDRN_REQUIRE(preds && dets && n_det && workspace, "yolox_postprocess_single: null argument");
   GDRN_REQUIRE(B > 0 && A > 0 && num_classes > 0 && num_classes <= KSI_MAX_CLASSES, "yolox_postprocess_single: bad problem size");
   GDRN_REQUIRE(workspace_bytes >= yolox_postprocess_single_workspace_bytes(B, A, num_classes),
                "yolox_postprocess_single: workspace too small");
   cudaStream_t st = (cudaStream_t)stream;
-  uint8_t* p = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(workspace) + 255) & ~(uintptr_t)255);
-  auto take = [&](size_t bytes) { uint8_t* r = p; p += (bytes + 255) & ~(size_t)255; return r; };
-  float* score = reinterpret_cast<float*>(take((size_t)B * A * 4));
-  int* cls = reinterpret_cast<int*>(take((size_t)B * A * 4));
-  int* sel = reinterpret_cast<int*>(take((size_t)B * num_classes * 4));
+  uint8_t* base = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(workspace) + 255) & ~(uintptr_t)255);
+  size_t off[3];
+  ksi_layout(B, A, off);
+  float* score = reinterpret_cast<float*>(base + off[0]);
+  int* cls = reinterpret_cast<int*>(base + off[1]);
+  int* sel = reinterpret_cast<int*>(base + off[2]);
   yolox_ksi_score_kernel<<<blocks_for((long long)B * A, 256), 256, 0, st>>>(preds, B, A, num_classes, score, cls);
   yolox_ksi_select_kernel<<<dim3(num_classes, B), 256, 0, st>>>(score, cls, A, num_classes, conf_thre, sel);
   yolox_ksi_nms_kernel<<<B, 1, 0, st>>>(preds, sel, score, A, num_classes, nms_thre, dets, n_det);

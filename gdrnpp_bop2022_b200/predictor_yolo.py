@@ -35,10 +35,12 @@ def preproc(img, input_size):
 
 
 @_lib.on_device(0)
-def postprocess_single_instance(det_preds, num_classes, conf_thre, nms_thre):
+def postprocess_single_instance(det_preds, num_classes, conf_thre, nms_thre, workspace=None):
     """YoloPredictor.postprocess(class_agnostic=True, keep_single_instance=True) (predictor_yolo.py:84-140) on the
     device: per class the highest-scoring anchor with obj * class_conf >= conf_thre (the first one on ties), then
-    class-agnostic NMS, rows sorted by class.  -> (dets [B, nc, 7], n_det [B] int32), no synchronisation."""
+    class-agnostic NMS as torchvision's CPU nms decides it (IoU compared with nms_thre as a double), rows sorted by
+    class.  -> (dets [B, nc, 7], n_det [B] int32), no synchronisation.  ``workspace``: a one-element list that holds
+    the workspace across calls (grown when a call needs more)."""
     if not det_preds.is_cuda:
         raise _lib.GdrnError("keep-single-instance post-process needs CUDA tensors (no CPU fallback)")
     B, A, C = det_preds.shape
@@ -48,7 +50,13 @@ def postprocess_single_instance(det_preds, num_classes, conf_thre, nms_thre):
     dets = torch.zeros((B, num_classes, 7), dtype=torch.float32, device=p.device)
     n_det = torch.zeros((B,), dtype=torch.int32, device=p.device)
     L = _lib.lib()
-    ws = torch.empty(L.yolox_postprocess_single_workspace_bytes(B, A, num_classes), dtype=torch.uint8, device=p.device)
+    nb = L.yolox_postprocess_single_workspace_bytes(B, A, num_classes)
+    if workspace is None:
+        ws = torch.empty(nb, dtype=torch.uint8, device=p.device)
+    else:
+        if workspace[0] is None or workspace[0].numel() < nb or workspace[0].device != p.device:
+            workspace[0] = torch.empty(nb, dtype=torch.uint8, device=p.device)
+        ws = workspace[0]
     _lib.check(L.yolox_postprocess_single(_lib.ptr(p), B, A, int(num_classes), float(conf_thre), float(nms_thre),
                                           _lib.ptr(dets), _lib.ptr(n_det), _lib.ptr(ws), ws.numel(), _lib.current_stream()),
                "yolox_postprocess_single")

@@ -460,8 +460,16 @@ int gdrn_xyz_region_targets(const float* depth, const float* R, const float* T, 
  *   n_levels > 0: raw head outputs, decoded here with hw [n_levels,2] i32 (rows, cols per level) and strides [n_levels]
  *   i32 (both device arrays); n_levels = 0: preds are already decoded (cx, cy, w, h).
  *   dets [B, max_out, 7] = (x1, y1, x2, y2, obj_conf, class_conf, class) in descending score order, n_det [B] i32.
+ *   The NMS decides as torchvision on CUDA does (sm_90 build): class-aware with n <= 25 000 candidates in an image
+ *   (boxes.numel() <= 100 000) is _batched_nms_coordinate_trick -- boxes shifted by cls * (max coordinate + 1) in fp32,
+ *   every pair compared; above that _batched_nms_vanilla -- per class, unshifted; class-agnostic is nms.  IoU as
+ *   nms_kernel_impl<float>: fma(bw, bh, Sa) - inter in the denominator (b the later-ranked box), IoU > nms_thre.
+ *   yolox_postprocess_layout: offsets[6] = byte offsets, from the workspace rounded up to 256 bytes, of the stage
+ *   results a call leaves there: cand [B,A,7] f32 (the compacted decoded rows), score [B,A] f32, order [B,A] i32
+ *   (candidate index by rank), n_cand [B] i32, max_coord [B] f32, mask [B,A,(A+63)/64] u64 (words jb >= ib written).
  * ------------------------------------------------------------------------------------------- */
 size_t yolox_postprocess_workspace_bytes(int B, int A);
+int yolox_postprocess_layout(int B, int A, size_t* offsets);
 int yolox_postprocess(const float* preds, int B, int A, int num_classes, const int* hw, const int* strides, int n_levels,
                       float conf_thre, float nms_thre, int class_agnostic, int max_out, float* dets, int* n_det,
                       void* workspace, size_t workspace_bytes, void* stream);
@@ -490,7 +498,11 @@ int yolox_postprocess(const float* preds, int B, int A, int num_classes, const i
  *     run one after the other per max_batch chunk in one workspace.  No allocation, no synchronisation.
  *   yolox_postprocess_single: keep-single-instance post-process of the reference predictor (predictor_yolo.py:84-140):
  *     per class the highest-scoring anchor with obj * cls_conf >= conf_thre, class-agnostic NMS, rows in ascending
- *     class order; dets [B, num_classes, 7], n_det [B] i32.  Classes without such an anchor are left out.
+ *     class order; dets [B, num_classes, 7], n_det [B] i32.  Classes without such an anchor are left out.  The
+ *     reference runs this NMS with torchvision's CPU nms: products rounded one by one, and the fp32 IoU compared with
+ *     nms_thre as a double (so a threshold that rounds up in fp32, such as 0.3, is honoured); num_classes <= 1024.
+ *   yolox_postprocess_single_layout: offsets[3] = byte offsets, from the workspace rounded up to 256 bytes, of score
+ *     [B,A] f32, cls [B,A] i32 and sel [B,num_classes] i32 (selected anchor per class, -1 = none) a call leaves there.
  * ------------------------------------------------------------------------------------------- */
 typedef struct YoloxModel YoloxModel;
 int yolox_model_create(YoloxModel** out, double depth, double width, int num_classes, int max_batch, int H, int W, int precision);
@@ -507,7 +519,8 @@ size_t yolox_model_workspace_bytes_tta(YoloxModel* m, int B);
 int yolox_model_forward_tta(YoloxModel* m, const float* img, int B, float* det_preds, void* workspace, size_t workspace_bytes,
                             void* stream);
 size_t yolox_postprocess_single_workspace_bytes(int B, int A, int num_classes);
-int yolox_postprocess_single(const float* preds, int B, int A, int num_classes, float conf_thre, float nms_thre, float* dets,
+int yolox_postprocess_single_layout(int B, int A, int num_classes, size_t* offsets);
+int yolox_postprocess_single(const float* preds, int B, int A, int num_classes, float conf_thre, double nms_thre, float* dets,
                              int* n_det, void* workspace, size_t workspace_bytes, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
