@@ -135,6 +135,6 @@ extern "C" int gdrn_dwconv_ln(const float* x, const float* w49c, const float* bi
                               void* out, int B, int H, int W, int C, float eps, int split, int variant, void* stream) {
   GDRN_REQUIRE(x && w49c && bias && ln_w && ln_b && out, "dwconv_ln: null argument");
   GDRN_REQUIRE(variant >= -1 && variant <= 1, "dwconv_ln: variant must be -1 (default), 0 (per-tile cluster kernel) or 1 (ping-pong)");
-  return launch_dwconv_ln_variant(x, w49c, bias, ln_w, ln_b, reinterpret_cast<__nv_bfloat16*>(out), B, H, W, C, eps, split, variant,
-                                  (cudaStream_t)stream);
+  return launch_dwconv_ln(x, w49c, bias, ln_w, ln_b, reinterpret_cast<__nv_bfloat16*>(out), B, H, W, C, eps, split, variant,
+                          (cudaStream_t)stream);
 }

@@ -4,8 +4,6 @@
 // heads/conv_pnp_net.py, core/utils/rot_reps.py:34-55, models/pose_from_pred_centroid_z.py:56-154,
 // core/utils/utils.py:31-88.
 #include <cooperative_groups.h>
-#include <stdio.h>
-#include <stdlib.h>
 
 #include "common.cuh"
 #include "dense_ops.h"
@@ -89,133 +87,8 @@ __global__ void stem_patchify_kernel(const float* __restrict__ img, __nv_bfloat1
 }
 
 // ------------------------------------------------------------------------------------------------
-// depthwise 7x7 + bias + LayerNorm(C).  Block = 256 threads = S strips x (C/4) channel-quads; a strip is TW
-// consecutive output pixels of one image row; a thread owns 4 channels of its strip's TW pixels.
-template <int TW>
-__global__ void __launch_bounds__(256)
-dwconv_ln_kernel(const float* __restrict__ x, const float* __restrict__ w49c, const float* __restrict__ bias,
-                 const float* __restrict__ ln_w, const float* __restrict__ ln_b, __nv_bfloat16* __restrict__ out,
-                 int B, int H, int W, int C, float eps) {
-  ptx::griddep_launch();
-  ptx::griddep_wait();
-  __shared__ float red[8][TW];  // [warp][pixel]
-  const int cq = C >> 2;                 // threads per strip
-  const int S = 256 / cq;                // strips per block
-  const int strip = threadIdx.x / cq;
-  const int c4 = (threadIdx.x % cq) * 4;
-  const int strips_per_row = W / TW;
-  const long long strip_id = (long long)blockIdx.x * S + strip;  // over B*H*strips_per_row
-  const long long n_strips = (long long)B * H * strips_per_row;
-  const bool live = strip_id < n_strips;
-  const int sx = live ? (int)(strip_id % strips_per_row) : 0;
-  const int y = live ? (int)((strip_id / strips_per_row) % H) : 0;
-  const int b = live ? (int)(strip_id / ((long long)strips_per_row * H)) : 0;
-  const int x0 = sx * TW;
-
-  float4 acc[TW];
-  {
-    const float4 bv = *reinterpret_cast<const float4*>(bias + c4);
-#pragma unroll
-    for (int i = 0; i < TW; ++i) acc[i] = bv;
-  }
-  if (live) {
-    for (int ky = 0; ky < 7; ++ky) {
-      const int iy = y + ky - 3;
-      if (iy < 0 || iy >= H) continue;
-      float4 wr[7];
-#pragma unroll
-      for (int kx = 0; kx < 7; ++kx) wr[kx] = __ldg(reinterpret_cast<const float4*>(w49c + (ky * 7 + kx) * C + c4));
-      const float* rowp = x + (((long long)b * H + iy) * W) * C + c4;
-#pragma unroll
-      for (int j = 0; j < TW + 6; ++j) {
-        const int ix = x0 + j - 3;
-        if (ix < 0 || ix >= W) continue;
-        const float4 v = *reinterpret_cast<const float4*>(rowp + (long long)ix * C);
-#pragma unroll
-        for (int kx = 0; kx < 7; ++kx) {
-          const int o = j - kx;  // output pixel index in the strip: ix = x0 + o + kx - 3
-          if (o >= 0 && o < TW) {
-            acc[o].x = fmaf(v.x, wr[kx].x, acc[o].x);
-            acc[o].y = fmaf(v.y, wr[kx].y, acc[o].y);
-            acc[o].z = fmaf(v.z, wr[kx].z, acc[o].z);
-            acc[o].w = fmaf(v.w, wr[kx].w, acc[o].w);
-          }
-        }
-      }
-    }
-  }
-  // LayerNorm over C: two-pass (mean, then centred variance), reductions over the strip's cq threads.
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int wps = cq >> 5;               // warps per strip (1, 2, 4, 8)
-  const int w0 = strip * wps;            // first warp of this strip
-  float mean[TW];
-#pragma unroll
-  for (int i = 0; i < TW; ++i) {
-    float s = (acc[i].x + acc[i].y) + (acc[i].z + acc[i].w);
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
-    mean[i] = s;
-  }
-  if (wps > 1) {
-    if (lane == 0) {
-#pragma unroll
-      for (int i = 0; i < TW; ++i) red[warp][i] = mean[i];
-    }
-    __syncthreads();
-#pragma unroll
-    for (int i = 0; i < TW; ++i) {
-      float s = 0.f;
-      for (int k = 0; k < wps; ++k) s += red[w0 + k][i];
-      mean[i] = s;
-    }
-    __syncthreads();
-  }
-  const float invC = 1.0f / (float)C;
-  float rstd[TW];
-#pragma unroll
-  for (int i = 0; i < TW; ++i) {
-    mean[i] *= invC;
-    float dx = acc[i].x - mean[i], dy = acc[i].y - mean[i], dz = acc[i].z - mean[i], dw = acc[i].w - mean[i];
-    float s = (dx * dx + dy * dy) + (dz * dz + dw * dw);
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
-    rstd[i] = s;
-  }
-  if (wps > 1) {
-    if (lane == 0) {
-#pragma unroll
-      for (int i = 0; i < TW; ++i) red[warp][i] = rstd[i];
-    }
-    __syncthreads();
-#pragma unroll
-    for (int i = 0; i < TW; ++i) {
-      float s = 0.f;
-      for (int k = 0; k < wps; ++k) s += red[w0 + k][i];
-      rstd[i] = s;
-    }
-  }
-  if (!live) return;
-  const float4 gw = *reinterpret_cast<const float4*>(ln_w + c4);
-  const float4 gb = *reinterpret_cast<const float4*>(ln_b + c4);
-  __nv_bfloat16* orow = out + ((((long long)b * H + y) * W) + x0) * C + c4;
-#pragma unroll
-  for (int i = 0; i < TW; ++i) {
-    const float r = rsqrtf(rstd[i] * invC + eps);
-    float o0 = fmaf((acc[i].x - mean[i]) * r, gw.x, gb.x);
-    float o1 = fmaf((acc[i].y - mean[i]) * r, gw.y, gb.y);
-    float o2 = fmaf((acc[i].z - mean[i]) * r, gw.z, gb.z);
-    float o3 = fmaf((acc[i].w - mean[i]) * r, gw.w, gb.w);
-    __nv_bfloat162 p0 = __floats2bfloat162_rn(o0, o1), p1 = __floats2bfloat162_rn(o2, o3);
-    uint2 u;
-    u.x = *reinterpret_cast<uint32_t*>(&p0);
-    u.y = *reinterpret_cast<uint32_t*>(&p1);
-    *reinterpret_cast<uint2*>(orow + (long long)i * C) = u;
-  }
-}
-
-
-// ------------------------------------------------------------------------------------------------
-// depthwise 7x7 + bias + LayerNorm(C), thread-block-cluster + packed-FP32 version (the one the forward uses).
+// depthwise 7x7 + bias + LayerNorm(C), thread-block-cluster + packed-FP32 version: one tile per CTA, for the shapes the
+// persistent ping-pong kernel (dwconv_pp.cu) does not take or is not chosen for.
 //   CTA  = one TW x TH output tile of one image x CPC channels (16x8 x 64 ch, two CTAs per SM so that one CTA's tile
 //          load overlaps the other's arithmetic; 8x8 x 128 ch for 8x8 images).  The zero-padded (TW+6)x(TH+6) x CPC
 //          fp32 input tile is fetched by ONE TMA box load (halo = out-of-bounds zero fill).
@@ -225,33 +98,22 @@ dwconv_ln_kernel(const float* __restrict__ x, const float* __restrict__ w49c, co
 //   cluster = the C/CPC CTAs (2/4/8) that together hold all channels of the tile: the LayerNorm statistics are
 //          combined across them through distributed shared memory with ONE cluster barrier (see below).
 // In-warp per-pixel channel sums use a transposing shuffle reduction.
-// Depthwise 7x7 + bias + LayerNorm(C) -> bf16 GEMM operand.  One CTA = (TW x TH pixel tile) x CPC channels of one
-// image; the CTAs of a cluster hold the C / CPC channel slices of the same tile.  A thread owns one channel PAIR
-// (packed fma.rn.f32x2) and R consecutive output rows x TW pixels.  It walks the R + 6 input rows once: each row is
-// loaded from shared memory a single time (TW + 6 LDS.64) and applied to every output row it contributes to, and
-// the filter row fetched for output row r is kept in registers for output row r + 1 of the next step, so that one
-// step costs TW + 6 + 7 shared-memory loads for R * 7 * TW packed FMAs (R = 2: 0.13 loads per FMA instead of 0.26;
-// the R = 1 form was co-limited by shared-memory bandwidth, see profiles/).
-template <int TW, int TH, int CPC, int R, int MINB>
-__global__ void __launch_bounds__((CPC / 2) * TH / R, MINB)
+template <int TW, int TH, int CPC, int MINB>
+__global__ void __launch_bounds__((CPC / 2) * TH, MINB)
 dwconv_ln_cluster_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_constant__ CUtensorMap tmap_w,
                          const float* __restrict__ bias, const float* __restrict__ ln_w,
                          const float* __restrict__ ln_b, __nv_bfloat16* __restrict__ out, int B, int H, int W, int C,
-                         int c_real, float eps, int split, long long* trace) {
+                         int c_real, float eps, int split) {
   ptx::griddep_launch();
   ptx::griddep_wait();
-  static_assert(R == 1 || R == 2, "rows per thread");
-  const bool trc = trace != nullptr && blockIdx.x == 0 && blockIdx.y == 0 && blockIdx.z == B / 2 && threadIdx.x == 0;
-  long long tt[6];
-  if (trc) tt[0] = clock64();
   constexpr int PAIRS = CPC / 2;              // channel pairs = threads per thread-row (CPC = channels per CTA)
   constexpr int IW = TW + 6;
   constexpr int IH = TH + 6;
   constexpr int NPIX = TW * TH;
   constexpr int WPR = PAIRS / 32;             // warps per thread-row
-  constexpr int NV = R * TW;                  // pixels per thread
-  constexpr int LPP = 32 / NV;                // lanes per pixel after the transposing reduction (1, 2 or 4)
-  static_assert(NV == 8 || NV == 16 || NV == 32, "pixels per thread");
+  constexpr int NV = TW;                      // pixels per thread
+  constexpr int LPP = 32 / NV;                // lanes per pixel after the transposing reduction (2 or 4)
+  static_assert(NV == 8 || NV == 16, "pixels per thread");
   extern __shared__ __align__(1024) float smem_dw[];   // TMA destination first: 128-byte aligned
   float* tile = smem_dw;                      // [IH][IW][CPC]
   float* wsm = tile + IH * IW * CPC;          // [49][CPC]
@@ -267,7 +129,7 @@ dwconv_ln_cluster_kernel(const __grid_constant__ CUtensorMap tmap_x, const __gri
   const int b = blockIdx.z;
   const int tid = threadIdx.x, lane = tid & 31;
   const int pair = tid % PAIRS;
-  const int row0 = (tid / PAIRS) * R;         // first output row of this thread
+  const int row0 = tid / PAIRS;               // output row of this thread
   const int wc = (tid >> 5) % WPR;            // which 64-channel group of the CTA this warp holds
   const int cl = 2 * pair;                    // first channel of the pair (CTA-local)
 
@@ -289,52 +151,31 @@ dwconv_ln_cluster_kernel(const __grid_constant__ CUtensorMap tmap_x, const __gri
   // split-phase cluster barrier: "my barriers exist" is announced here and only waited for right before the push
   // (a conv later), so the start-up skew between the CTAs of a cluster is off the critical path
   asm volatile("barrier.cluster.arrive.release;" ::: "memory");
-  f32x2_t acc[R][TW];
+  f32x2_t acc[TW];
   {
     const f32x2_t bv = f2_pack(__ldg(bias + c0 + cl), __ldg(bias + c0 + cl + 1));
 #pragma unroll
-    for (int r = 0; r < R; ++r)
-#pragma unroll
-      for (int i = 0; i < TW; ++i) acc[r][i] = bv;
+    for (int i = 0; i < TW; ++i) acc[i] = bv;
   }
   ptx::mbar_wait(bar, 0);    // filter taps + input tile landed
-  if (trc) tt[1] = clock64();
 
-  // ---- convolution: input row i feeds output row r with filter row ky = i - r ----
-  {
-    f32x2_t wprev[7];
+  // ---- convolution, per output ky = 0..6, kx = 0..6 (the ping-pong kernel's order) ----
 #pragma unroll
-    for (int i = 0; i < R + 6; ++i) {
-      f32x2_t v[IW], wk[7];
-      const float* rowp = tile + ((row0 + i) * IW) * CPC + cl;
+  for (int ky = 0; ky < 7; ++ky) {
+    f32x2_t v[IW], wk[7];
+    const float* rowp = tile + ((row0 + ky) * IW) * CPC + cl;
 #pragma unroll
-      for (int j = 0; j < IW; ++j) v[j] = *reinterpret_cast<const f32x2_t*>(rowp + j * CPC);
-      if (i < 7) {
+    for (int j = 0; j < IW; ++j) v[j] = *reinterpret_cast<const f32x2_t*>(rowp + j * CPC);
 #pragma unroll
-        for (int kx = 0; kx < 7; ++kx) wk[kx] = *reinterpret_cast<const f32x2_t*>(wsm + (i * 7 + kx) * CPC + cl);
+    for (int kx = 0; kx < 7; ++kx) wk[kx] = *reinterpret_cast<const f32x2_t*>(wsm + (ky * 7 + kx) * CPC + cl);
 #pragma unroll
-        for (int kx = 0; kx < 7; ++kx)
+    for (int kx = 0; kx < 7; ++kx)
 #pragma unroll
-          for (int ox = 0; ox < TW; ++ox) acc[0][ox] = f2_fma(v[ox + kx], wk[kx], acc[0][ox]);
-      }
-      if (R == 2 && i >= 1) {
-#pragma unroll
-        for (int kx = 0; kx < 7; ++kx)
-#pragma unroll
-          for (int ox = 0; ox < TW; ++ox) acc[R - 1][ox] = f2_fma(v[ox + kx], wprev[kx], acc[R - 1][ox]);
-      }
-      if (R == 2 && i < 7) {
-#pragma unroll
-        for (int kx = 0; kx < 7; ++kx) wprev[kx] = wk[kx];
-      }
-    }
+      for (int ox = 0; ox < TW; ++ox) acc[ox] = f2_fma(v[ox + kx], wk[kx], acc[ox]);
   }
-  if (trc) tt[2] = clock64();
   float ax[NV], ay[NV];
 #pragma unroll
-  for (int r = 0; r < R; ++r)
-#pragma unroll
-    for (int i = 0; i < TW; ++i) { const float2 t = f2_unpack(acc[r][i]); ax[r * TW + i] = t.x; ay[r * TW + i] = t.y; }
+  for (int i = 0; i < TW; ++i) { const float2 t = f2_unpack(acc[i]); ax[i] = t.x; ay[i] = t.y; }
 
   // ---- LayerNorm over all C channels of each pixel ----
   // A warp holds 64 channels of its NV pixels: it computes (sum, M2 about its own mean) per pixel with
@@ -342,7 +183,7 @@ dwconv_ln_cluster_kernel(const __grid_constant__ CUtensorMap tmap_x, const __gri
   // ONE cluster barrier each warp combines the C/64 partials with Chan's parallel-variance formula.  No block-level
   // barrier, no remote loads, and nothing remote is touched after the barrier (so no exit barrier is needed).
   // Zero pad channels (c >= c_real, all in the last 64-channel group) are left out of the group's mean and M2.
-  const int pix = row0 * TW + lane / LPP;   // the thread's R rows are contiguous in the row-major tile
+  const int pix = row0 * TW + lane / LPP;
   float s_loc, m2_loc;
   {
     const int cw = c0 + wc * 64;             // first channel of this warp's group
@@ -372,9 +213,7 @@ dwconv_ln_cluster_kernel(const __grid_constant__ CUtensorMap tmap_x, const __gri
         ptx::st_async_f32x2(ptx::mapa_shared(la, rk), s_loc, m2_loc, ptx::mapa_shared(parts_bar, rk));
     }
   }
-  if (trc) tt[3] = clock64();
   ptx::mbar_wait_cluster(parts_bar, 0);
-  if (trc) tt[4] = clock64();
   float mean_p, rstd_p;
   {
     float tot = 0.f;
@@ -394,26 +233,18 @@ dwconv_ln_cluster_kernel(const __grid_constant__ CUtensorMap tmap_x, const __gri
   const float gw0 = __ldg(ln_w + c0 + cl), gw1 = __ldg(ln_w + c0 + cl + 1);
   const float gb0 = __ldg(ln_b + c0 + cl), gb1 = __ldg(ln_b + c0 + cl + 1);
   const int ldc = split ? 2 * C : C;  // split mode: rows are [hi C | lo C]
+  __nv_bfloat16* orow = out + (((long long)b * H + (y0 + row0)) * W + x0) * ldc + c0 + cl;
 #pragma unroll
-  for (int r = 0; r < R; ++r) {
-    __nv_bfloat16* orow = out + (((long long)b * H + (y0 + row0 + r)) * W + x0) * ldc + c0 + cl;
-#pragma unroll
-    for (int ox = 0; ox < TW; ++ox) {
-      const int i = r * TW + ox;
-      const float m = __shfl_sync(0xffffffffu, mean_p, i * LPP);
-      const float rs = __shfl_sync(0xffffffffu, rstd_p, i * LPP);
-      const float o0 = fmaf((ax[i] - m) * rs, gw0, gb0), o1 = fmaf((ay[i] - m) * rs, gw1, gb1);
-      const __nv_bfloat162 o = __floats2bfloat162_rn(o0, o1);
-      *reinterpret_cast<__nv_bfloat162*>(orow + (long long)ox * ldc) = o;
-      if (split) {
-        const float2 of = __bfloat1622float2(o);
-        *reinterpret_cast<__nv_bfloat162*>(orow + (long long)ox * ldc + C) = __floats2bfloat162_rn(o0 - of.x, o1 - of.y);
-      }
+  for (int ox = 0; ox < TW; ++ox) {
+    const float m = __shfl_sync(0xffffffffu, mean_p, ox * LPP);
+    const float rs = __shfl_sync(0xffffffffu, rstd_p, ox * LPP);
+    const float o0 = fmaf((ax[ox] - m) * rs, gw0, gb0), o1 = fmaf((ay[ox] - m) * rs, gw1, gb1);
+    const __nv_bfloat162 o = __floats2bfloat162_rn(o0, o1);
+    *reinterpret_cast<__nv_bfloat162*>(orow + (long long)ox * ldc) = o;
+    if (split) {
+      const float2 of = __bfloat1622float2(o);
+      *reinterpret_cast<__nv_bfloat162*>(orow + (long long)ox * ldc + C) = __floats2bfloat162_rn(o0 - of.x, o1 - of.y);
     }
-  }
-  if (trc) {
-    tt[5] = clock64();
-    for (int i = 0; i < 5; ++i) trace[i] = tt[i + 1] - tt[i];
   }
 }
 
@@ -992,32 +823,34 @@ int launch_stem_patchify(const float* img, __nv_bfloat16* out, int B, int H, int
   return GDRN_OK;
 }
 
-template <int TW, int TH, int CPC, int R, int MINB>
+int make_dwconv_tmaps(CUtensorMap* tmap_x, CUtensorMap* tmap_w, const float* x, const float* w49c, int B, int H, int W,
+                      int C, int cpc, int box_w, int box_h) {
+  {
+    const uint64_t dims[4] = {(uint64_t)C, (uint64_t)W, (uint64_t)H, (uint64_t)B};
+    const uint64_t str[3] = {(uint64_t)C * 4, (uint64_t)W * C * 4, (uint64_t)H * W * C * 4};
+    const uint32_t box[4] = {(uint32_t)cpc, (uint32_t)box_w, (uint32_t)box_h, 1};
+    const int rc = make_tmap_f32_plain(tmap_x, x, 4, dims, str, box);
+    if (rc != GDRN_OK) return rc;
+  }
+  const uint64_t dims[2] = {(uint64_t)C, 49};
+  const uint64_t str[1] = {(uint64_t)C * 4};
+  const uint32_t box[2] = {(uint32_t)cpc, 49};
+  return make_tmap_f32_plain(tmap_w, w49c, 2, dims, str, box);
+}
+
+template <int TW, int TH, int CPC, int MINB>
 static int launch_dwconv_cluster(const float* x, const float* w49c, const float* bias, const float* ln_w,
                                  const float* ln_b, __nv_bfloat16* out, int B, int H, int W, int C, float eps,
                                  int split, cudaStream_t st, int c_real) {
   constexpr int IW = TW + 6, IH = TH + 6;
   constexpr int NPIX = TW * TH;
-  constexpr int NTHREADS = (CPC / 2) * TH / R;
+  constexpr int NTHREADS = (CPC / 2) * TH;
   const size_t smem = (size_t)(IH * IW * CPC + 49 * CPC + 2 * 8 * (CPC / 64) * NPIX) * sizeof(float) + 32;
-  auto kfn = dwconv_ln_cluster_kernel<TW, TH, CPC, R, MINB>;
+  auto kfn = dwconv_ln_cluster_kernel<TW, TH, CPC, MINB>;
   GDRN_OPT_IN_SMEM(kfn, smem);
-  CUtensorMap tmap;
-  {
-    const uint64_t dims[4] = {(uint64_t)C, (uint64_t)W, (uint64_t)H, (uint64_t)B};
-    const uint64_t str[3] = {(uint64_t)C * 4, (uint64_t)W * C * 4, (uint64_t)H * W * C * 4};
-    const uint32_t box[4] = {(uint32_t)CPC, (uint32_t)IW, (uint32_t)IH, 1};
-    int rc = make_tmap_f32_plain(&tmap, x, 4, dims, str, box);
-    if (rc != GDRN_OK) return rc;
-  }
-  CUtensorMap tmap_w;
-  {
-    const uint64_t dims[2] = {(uint64_t)C, 49};
-    const uint64_t str[1] = {(uint64_t)C * 4};
-    const uint32_t box[2] = {(uint32_t)CPC, 49};
-    int rc = make_tmap_f32_plain(&tmap_w, w49c, 2, dims, str, box);
-    if (rc != GDRN_OK) return rc;
-  }
+  CUtensorMap tmap, tmap_w;
+  const int rc = make_dwconv_tmaps(&tmap, &tmap_w, x, w49c, B, H, W, C, CPC, IW, IH);
+  if (rc != GDRN_OK) return rc;
   cudaLaunchConfig_t cfg = {};
   cfg.gridDim = dim3(C / CPC, (H / TH) * (W / TW), B);
   cfg.blockDim = dim3(NTHREADS);
@@ -1032,72 +865,29 @@ static int launch_dwconv_cluster(const float* x, const float* w49c, const float*
   attr[1].val.programmaticStreamSerializationAllowed = 1;
   cfg.attrs = attr;
   cfg.numAttrs = gdrn_pdl_enabled() ? 2 : 1;
-  static int trace_on = -1;  // GDRN_DW_TRACE=1: phase cycle counts of one mid-grid CTA on stderr (synchronises)
-  if (trace_on < 0) trace_on = getenv("GDRN_DW_TRACE") ? 1 : 0;
-  static long long* d_trace = nullptr;
-  if (trace_on && !d_trace) GDRN_CHECK_CUDA(cudaMalloc(&d_trace, 8 * sizeof(long long)));
-  long long* trp = trace_on ? d_trace : nullptr;
-  GDRN_CHECK_CUDA(cudaLaunchKernelEx(&cfg, kfn, tmap, tmap_w, bias, ln_w, ln_b, out, B, H, W, C, c_real, eps, split, trp));
+  GDRN_CHECK_CUDA(cudaLaunchKernelEx(&cfg, kfn, tmap, tmap_w, bias, ln_w, ln_b, out, B, H, W, C, c_real, eps, split));
   gdrn_count_launch(1);
-  if (trace_on) {
-    long long h[5];
-    GDRN_CHECK_CUDA(cudaMemcpyAsync(h, d_trace, sizeof(h), cudaMemcpyDeviceToHost, st));
-    GDRN_CHECK_CUDA(cudaStreamSynchronize(st));
-    fprintf(stderr, "[dwconv trace] %dx%d C=%d tile %dx%d R=%d: load-wait=%lld conv=%lld ln-local=%lld cluster-sync=%lld finish=%lld\n",
-            H, W, C, TW, TH, R, h[0], h[1], h[2], h[3], h[4]);
-  }
   return GDRN_OK;
 }
 
 int launch_dwconv_ln(const float* x, const float* w49c, const float* bias, const float* ln_w, const float* ln_b,
-                     __nv_bfloat16* out, int B, int H, int W, int C, float eps, int split, cudaStream_t st, int c_real) {
-  return launch_dwconv_ln_variant(x, w49c, bias, ln_w, ln_b, out, B, H, W, C, eps, split, -1, st, c_real);
-}
-
-// variant: -1 = default choice (env GDRN_DW_PP), 0 = one-tile-per-CTA cluster kernel, 1 = persistent ping-pong kernel
-int launch_dwconv_ln_variant(const float* x, const float* w49c, const float* bias, const float* ln_w, const float* ln_b,
-                             __nv_bfloat16* out, int B, int H, int W, int C, float eps, int split, int variant,
-                             cudaStream_t st, int c_real) {
+                     __nv_bfloat16* out, int B, int H, int W, int C, float eps, int split, int variant, cudaStream_t st,
+                     int c_real) {
   GDRN_REQUIRE(C % 64 == 0 && C <= 1024, "dwconv: C must be a multiple of 64 and <= 1024");
   if (c_real <= 0) c_real = C;
   GDRN_REQUIRE(c_real <= C && C - c_real < 64, "dwconv: c_real must be within the last 64-channel slice of C");
-  // cluster kernel: 16x8 tiles x 64 channels (cluster C/64 <= 8) or 8x8 tiles x 128 channels (cluster C/128 <= 8)
-  static int rows = -1;  // GDRN_DW_ROWS=2: two output rows per thread (half the LDS traffic, half the warps: measured 4 % slower)
-  if (rows < 0) { const char* e = getenv("GDRN_DW_ROWS"); rows = (e && atoi(e) == 2) ? 2 : 1; }
-  static int var = -1;   // GDRN_DW_VARIANT: tile-shape experiments
-  if (var < 0) { const char* e = getenv("GDRN_DW_VARIANT"); var = e ? atoi(e) : 0; }
 #define DW_ARGS x, w49c, bias, ln_w, ln_b, out, B, H, W, C, eps, split, st, c_real
-  static int pp = -1;    // GDRN_DW_PP=0: one-tile-per-CTA kernel instead of the persistent ping-pong kernel (A/B experiments)
-  if (pp < 0) { const char* e = getenv("GDRN_DW_PP"); pp = e ? atoi(e) : 1; }
-  const bool want_pp = variant == 1 || (variant < 0 && pp && var == 0 && rows == 1 && (long long)B * (H / 8) * (W / 16) >= 32);
-  if (want_pp) {
+  if (variant == 1 || (variant < 0 && (long long)B * (H / 8) * (W / 16) >= 32)) {
     const int rc = launch_dwconv_ln_pp(DW_ARGS);
     if (rc != 1) return rc;
     GDRN_REQUIRE(variant != 1, "dwconv: shape not handled by the ping-pong kernel");
   }
-  if (H % 8 == 0 && W % 16 == 0 && C / 64 <= 8) {
-    if (var == 1) return launch_dwconv_cluster<16, 4, 64, 1, 3>(DW_ARGS);   // 73 KB: 3 CTAs / SM, 128 threads
-    if (var == 2) return launch_dwconv_cluster<8, 8, 64, 1, 3>(DW_ARGS);    // 67 KB: 3 CTAs / SM, 256 threads
-    if (var == 3) return launch_dwconv_cluster<8, 4, 64, 1, 4>(DW_ARGS);    // 50 KB: 4 CTAs / SM, 128 threads
-    return rows == 2 ? launch_dwconv_cluster<16, 8, 64, 2, 2>(DW_ARGS) : launch_dwconv_cluster<16, 8, 64, 1, 2>(DW_ARGS);
-  }
-  if (H % 8 == 0 && W % 8 == 0 && C % 128 == 0 && C / 128 <= 8)
-    return rows == 2 ? launch_dwconv_cluster<8, 8, 128, 2, 1>(DW_ARGS) : launch_dwconv_cluster<8, 8, 128, 1, 1>(DW_ARGS);
+  if (H % 8 == 0 && W % 16 == 0 && C / 64 <= 8) return launch_dwconv_cluster<16, 8, 64, 2>(DW_ARGS);
+  if (H % 8 == 0 && W % 8 == 0 && C % 128 == 0 && C / 128 <= 8) return launch_dwconv_cluster<8, 8, 128, 1>(DW_ARGS);
 #undef DW_ARGS
-  GDRN_REQUIRE(!split, "dwconv: the non-cluster fallback kernel has no split-bf16 output");
-  GDRN_REQUIRE(c_real == C && C % 128 == 0, "dwconv: the non-cluster fallback kernel needs C % 128 == 0 and no pad channels");
-  const int S = 256 / (C / 4);
-  if (W % 16 == 0) {
-    long long strips = (long long)B * H * (W / 16);
-    GDRN_CHECK_CUDA(gdrn_launch_dep(dwconv_ln_kernel<16>, dim3((int)((strips + S - 1) / S)), dim3(256), 0, st, x, w49c, bias, ln_w, ln_b, out, B, H, W, C, eps));
-  } else {
-    GDRN_REQUIRE(W % 8 == 0, "dwconv: W must be a multiple of 8");
-    long long strips = (long long)B * H * (W / 8);
-    GDRN_CHECK_CUDA(gdrn_launch_dep(dwconv_ln_kernel<8>, dim3((int)((strips + S - 1) / S)), dim3(256), 0, st, x, w49c, bias, ln_w, ln_b, out, B, H, W, C, eps));
-  }
-  GDRN_CHECK_CUDA(cudaGetLastError());
-  gdrn_count_launch(1);
-  return GDRN_OK;
+  GDRN_REQUIRE(false, "dwconv: unsupported shape: needs H % 8 == 0 and either W % 16 == 0 with C <= 512, or W % 8 == 0 "
+                      "with C a multiple of 128");
+  return GDRN_ERR_INVALID;
 }
 
 int launch_ln_patchify2(const float* x, const float* ln_w, const float* ln_b, __nv_bfloat16* out, int B, int H, int W,

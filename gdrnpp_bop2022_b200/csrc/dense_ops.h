@@ -1,5 +1,6 @@
 // Internal launchers of the CUDA-core kernels around the wgmma GEMMs (dense_ops.cu).
 #pragma once
+#include <cuda.h>
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -21,14 +22,19 @@ int launch_stem_patchify(const float* img, __nv_bfloat16* out, int B, int H, int
 // x: fp32 NHWC; w: [49][C] (tap-major, repacked); all fp32.
 // c_real (0 = C): the tensor carries C - c_real trailing zero PAD channels (zero filter taps / bias / LN affine), e.g. the
 // 96-channel stage of convnext_tiny/small stored 128 wide; LayerNorm statistics are taken over the c_real channels.
+// variant -1 picks the kernel from the shape: the persistent ping-pong kernel when B * (H/8) * (W/16) >= 32 and it takes
+// the shape, else the 16x8-pixel x 64-channel cluster kernel (H % 8 == 0, W % 16 == 0, C <= 512), else the 8x8 x 128 one
+// (H % 8 == 0, W % 8 == 0, C % 128 == 0).  0 = cluster kernel, 1 = ping-pong kernel.  Other shapes: GDRN_ERR_INVALID.
 int launch_dwconv_ln(const float* x, const float* w49c, const float* bias, const float* ln_w, const float* ln_b,
-                     __nv_bfloat16* out, int B, int H, int W, int C, float eps, int split, cudaStream_t st, int c_real = 0);
-int launch_dwconv_ln_variant(const float* x, const float* w49c, const float* bias, const float* ln_w, const float* ln_b,
-                             __nv_bfloat16* out, int B, int H, int W, int C, float eps, int split, int variant,
-                             cudaStream_t st, int c_real = 0);
+                     __nv_bfloat16* out, int B, int H, int W, int C, float eps, int split, int variant, cudaStream_t st,
+                     int c_real = 0);
 // persistent two-warpgroup ping-pong version (dwconv_pp.cu) for 16x8x64 tiles; returns 1 if the shape is not handled
 int launch_dwconv_ln_pp(const float* x, const float* w49c, const float* bias, const float* ln_w, const float* ln_b,
                         __nv_bfloat16* out, int B, int H, int W, int C, float eps, int split, cudaStream_t st, int c_real = 0);
+// the tensor maps both depthwise kernels load through: x [B,H,W,C] in (cpc x box_w x box_h) halo boxes (out-of-bounds
+// zero fill) and w49c [49][C] in (cpc x 49) boxes
+int make_dwconv_tmaps(CUtensorMap* tmap_x, CUtensorMap* tmap_w, const float* x, const float* w49c, int B, int H, int W,
+                      int C, int cpc, int box_w, int box_h);
 
 // downsample front half: per-pixel LayerNorm over C then 2x2/s2 patchify -> bf16 [B*(H/2)*(W/2), 4*C]
 // (k = (ky*2+kx)*C + c)

@@ -529,7 +529,7 @@ int stage_block(GdrnModel* m, const Workspace& w, int B, int s, int i, cudaStrea
   const int H4 = 4 * Cr;      // hidden width of the MLP
   const long long M = (long long)B * res * res;
   const BlockW& bw = m->blocks[s][i];
-  RCP(1, launch_dwconv_ln(w.X, bw.dw_w, bw.dw_b, bw.ln_w, bw.ln_b, w.A, B, res, res, C, 1e-6f, PR, st, Cr));
+  RCP(1, launch_dwconv_ln(w.X, bw.dw_w, bw.dw_b, bw.ln_w, bw.ln_b, w.A, B, res, res, C, 1e-6f, PR, -1, st, Cr));
   if (!PR && m->fuse_mlp && m->gelu_mode == 1 && Cr == C && mlp_fused_supported(C, M)) {
     // stage 0: fc1 -> GELU -> fc2 -> residual in one kernel (no 4C-wide Hb round trip through HBM)
     RCP(0, mlp_fused_launch(w.A, bw.fc1_w, bw.fc1_b, bw.fc2_w, bw.fc2_b, bw.gamma, w.X, M, C, st));

@@ -186,7 +186,11 @@ int gdrn_mlp_fused_x3(const void* A, const void* W1, const float* b1, const void
 
 /* ConvNeXt block front half exported for tests and roofline measurement: depthwise 7x7 (pad 3) + bias + LayerNorm(C)
  * on an NHWC fp32 tensor x [B,H,W,C] with tap-major weights w49c [49][C] -> bf16 [B*H*W, C] (split = 1: [hi C | lo C]).
- * variant: -1 default, 0 = one-tile-per-CTA cluster kernel, 1 = persistent two-warpgroup ping-pong kernel. */
+ * variant: -1 default, 0 = one-tile-per-CTA cluster kernel, 1 = persistent two-warpgroup ping-pong kernel.
+ * Supported shapes: C a multiple of 64 up to 1024, H % 8 == 0, and either W % 16 == 0 with C <= 512 or W % 8 == 0 with
+ * C % 128 == 0; variant 1 also needs W % 16 == 0 and C / 64 in {2, 3, 4, 6, 8}.  The default takes the ping-pong kernel
+ * when B * (H/8) * (W/16) >= 32 and the shape allows it.  Any other shape or variant returns GDRN_ERR_INVALID before
+ * anything is launched. */
 int gdrn_dwconv_ln(const float* x, const float* w49c, const float* bias, const float* ln_w, const float* ln_b, void* out,
                    int B, int H, int W, int C, float eps, int split, int variant, void* stream);
 

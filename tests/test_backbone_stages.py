@@ -14,7 +14,7 @@ LayerNorm kernels write (ln_patchify2 for down<s>, the depthwise conv + LayerNor
 largest error measured on an H100 (80GB HBM3, 400 W power limit) over all cases of the quantity; BARS lists that maximum
 and where it occurred.
 
-Depthwise kernel per (stage, B) (launch_dwconv_ln_variant; _dw_kernel below restates the rule and
+Depthwise kernel per (stage, B) (launch_dwconv_ln; _dw_kernel below restates the rule and
 test_dwconv_kernel_coverage checks that every kernel is reached):
   * ping-pong kernel when B * (H/8) * (W/16) >= 32: stage 0 at every B, stage 1 at B = 5, 64, stage 2 at B = 64;
   * 16x8x64 cluster kernel: stage 1 at B = 1, 3, stage 2 at B = 1, 3, 5;
@@ -85,7 +85,7 @@ CASES = [(a, st) for a in ARCHS for st in _stages(a)]
 
 
 def _dw_kernel(s, B):
-    """The depthwise kernel launch_dwconv_ln_variant picks for stage s at batch B (default settings)."""
+    """The depthwise kernel launch_dwconv_ln picks for stage s at batch B (variant -1, as the forward calls it)."""
     r = 64 >> s
     if B * (r // 8) * (r // 16) >= 32:
         return "ping-pong"

@@ -1367,6 +1367,25 @@ def test_dwconv_ln_pingpong_vs_cluster_kernel_and_torch(dev, lib, B, H, C, split
     assert (got - ref).abs().max().item() < (2e-4 if split else 0.03)
 
 
+def test_dwconv_ln_rejects_shape_without_kernel(dev, lib):
+    """H = 12 fits neither the 8-row tiles of the ping-pong kernel nor those of the two cluster kernels: every variant
+    returns GDRN_ERR_INVALID, names the supported shapes, and leaves the output buffer untouched (nothing launched)."""
+    L = _lib()
+    B, H, W, C = 2, 12, 16, 128
+    g = torch.Generator().manual_seed(12)
+    x = torch.randn(B, H, W, C, generator=g).to(dev)
+    w49c = (torch.randn(49, C, generator=g) / 7).to(dev)
+    bias, lw, lb = torch.zeros(C, device=dev), torch.ones(C, device=dev), torch.zeros(C, device=dev)
+    o = torch.full((B * H * W, C), float("nan"), dtype=torch.bfloat16, device=dev)
+    for variant in (-1, 0, 1):
+        rc = lib.gdrn_dwconv_ln(L.ptr(x), L.ptr(w49c), L.ptr(bias), L.ptr(lw), L.ptr(lb), L.ptr(o), B, H, W, C, 1e-6, 0, variant,
+                                L.current_stream())
+        assert rc == -1, (variant, rc)   # GDRN_ERR_INVALID
+        assert "dwconv" in L.last_error(), (variant, L.last_error())
+    torch.cuda.synchronize()
+    assert torch.isnan(o.float()).all()
+
+
 def test_upnp_vs_vendored_ceres_and_epnp_wrapper(dev):
     """csrc/upnp.cu (batched device LM) and the reference-signature host entry against the REFERENCE's vendored Ceres 2.0
     (ceres::Jet autodiff + ceres::TinySolver on the residual of uncertainty_pnp.cpp:16-34, minimisers stored in
