@@ -79,6 +79,9 @@ _SIGNATURES = {
     "rast_mesh_count": (c_int, []),
     "rast_render_meshes": (c_int, [c_void_p] * 3 + [c_int] * 3 + [c_float, c_float, c_int] + [c_void_p] * 4),
     "rast_render_meshes_rgb": (c_int, [c_void_p] * 4 + [c_int] * 3 + [c_float, c_float] + [c_void_p] * 5),
+    "rast_upload_mesh_tex": (c_int, [c_void_p, c_int, c_void_p, c_int] + [c_void_p] * 4 + [c_int, c_int]),
+    "rast_render_scene": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_int, c_int, c_float, c_float] + [c_void_p] * 9),
+    "rast_scene_scratch_bytes": (c_size_t, [c_int, c_int, c_int]),
     "gdrn_pnp_ransac_maps": (c_int, [c_void_p] * 9 + [c_int] * 3 + [c_float, c_float, c_uint] + [c_void_p] * 4),
     "gdrn_pnp_ransac_points": (c_int, [c_void_p] * 4 + [c_int] * 3 + [c_float, c_uint] + [c_void_p] * 4),
     "gdrn_pnp_ransac_trace": (c_int, [c_void_p] * 11 + [c_int] * 3 + [c_float, c_float, c_uint] + [c_void_p] * 15),

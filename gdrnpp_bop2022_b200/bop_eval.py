@@ -328,13 +328,15 @@ VSD_ZNEAR, VSD_ZFAR = 0.01, 10000.0
 class VsdMeshes:
     """The meshes of a dataset (mm), each uploaded once to the rasteriser's registry as a renderer.Model3D; ids maps
     obj_id to its registry id.  meshes: {obj_id: (verts [V,3], faces [F,3])} or {obj_id: (verts, faces, colors [V,3]
-    in [0,1] or None)} as arrays or CPU tensors."""
+    in [0,1] or None)}, optionally followed by uvs [V,2] and texture [h,w,3] u8 (row 0 at t = 0), as arrays or CPU
+    tensors."""
 
     def __init__(self, meshes, device="cuda"):
         from .renderer import Model3D
 
         self.device = torch.device(device)
-        self.ids = {int(o): Model3D(m[0], m[1], device=self.device, colors=m[2] if len(m) > 2 else None).mesh_id
+        self.ids = {int(o): Model3D(m[0], m[1], device=self.device, colors=m[2] if len(m) > 2 else None,
+                                    uvs=m[3] if len(m) > 3 else None, texture=m[4] if len(m) > 4 else None).mesh_id
                     for o, m in meshes.items()}
 
     def render(self, obj_ids, R, t, K, H, W):

@@ -42,10 +42,23 @@ struct MeshEntry {
 };
 constexpr int RAST_MAX_MESHES = 1024;
 
-// the triangles of one ROI: mesh `mid` (an unknown id renders as background) at pose P [3,4] with intrinsics K, into zb
+// Per-mesh shading attributes of rast_upload_mesh_tex; null / 0 for what a mesh was uploaded without.
+constexpr int RAST_MAX_MIPS = 16;
+struct MeshTex {
+  const float* normals;                    // [V,3] model-space vertex normals
+  const float* uvs;                        // [V,2] per-vertex texture coordinates
+  const uint8_t* tex;                      // mip chain: level l is [h[l], w[l], 3] u8 at tex + off[l], row 0 at t = 0
+  int levels;                              // 0 = no texture
+  int w[RAST_MAX_MIPS], h[RAST_MAX_MIPS];
+  long long off[RAST_MAX_MIPS];
+};
+
+// the triangles of one ROI: mesh `mid` (an unknown id renders as background) at pose P [3,4] with intrinsics K, into zb.
+// The key's low word is tri_base + the triangle's index in the mesh.
 __device__ __forceinline__ void rast_tri_one(const MeshEntry* __restrict__ table, int mid, int n_meshes,
                                              const float* __restrict__ P, const float* __restrict__ K, int H, int W,
-                                             float znear, float zfar, unsigned long long* __restrict__ zb) {
+                                             float znear, float zfar, unsigned long long* __restrict__ zb,
+                                             unsigned tri_base = 0u) {
   if (mid < 0 || mid >= n_meshes) return;
   const MeshEntry me = table[mid];
   const int f = blockIdx.x * blockDim.x + threadIdx.x;
@@ -82,7 +95,7 @@ __device__ __forceinline__ void rast_tri_one(const MeshEntry* __restrict__ table
       const float izp = w0 * iz[0] + w1 * iz[1] + w2 * iz[2];
       const float zp = 1.0f / izp;
       if (!(zp >= znear) || zp > zfar) continue;
-      const unsigned long long key = ((unsigned long long)__float_as_uint(zp) << 32) | (unsigned)f;
+      const unsigned long long key = ((unsigned long long)__float_as_uint(zp) << 32) | (tri_base + (unsigned)f);
       atomicMin(zb + (long long)py * W + px, key);
     }
   }
@@ -142,11 +155,13 @@ __global__ void rast_resolve_kernel(const unsigned long long* __restrict__ zbuf,
 // The screen barycentrics are recomputed with the rasteriser's arithmetic and made perspective-correct
 // (b_k = w_k / Z_k / sum(w / Z)), which is how GL interpolates v_L and v_color.  The face normal of a plane through
 // the eye-facing side satisfies dot(n, P) <= 0 for every point P of the triangle, so it is turned once per triangle.
-// Colour: colors [n,3] per render when given, else the mesh's vertex colours, else grey 0.5.  Depth, coverage and
+// Colour: colors [n,3] per render when given, else the mesh's texture (renderer_py's texture2D, here the nearest texel of
+// level 0 with clamp to edge at the interpolated UV), else its vertex colours, else grey 0.5.  Depth, coverage and
 // tri_ids come straight from the key, so they equal rast_render_meshes' float-z output.
 __global__ void __launch_bounds__(256)
 rast_shade_kernel(const unsigned long long* __restrict__ zbuf, const MeshEntry* __restrict__ table,
-                  const float* const* __restrict__ mesh_colors, const int* __restrict__ mesh_ids,
+                  const float* const* __restrict__ mesh_colors, const MeshTex* __restrict__ mesh_tex,
+                  const int* __restrict__ mesh_ids,
                   const float* __restrict__ poses, const float* __restrict__ Ks, const float* __restrict__ colors, int n,
                   int H, int W, uint8_t* __restrict__ rgb, float* __restrict__ depth, int* __restrict__ tri_ids) {
   const long long total = (long long)n * H * W;
@@ -198,13 +213,255 @@ rast_shade_kernel(const unsigned long long* __restrict__ zbuf, const MeshEntry* 
     const float dot = (lx * nx + ly * ny + lz * nz) * rsqrtf(lx * lx + ly * ly + lz * lz) * rsqrtf(nx * nx + ny * ny + nz * nz);
     const float lw = fminf(0.5f + fmaxf(dot, 0.f), 1.f);
     const float* vc = mesh_colors[mesh_ids[r]];
+    const MeshTex& mt = mesh_tex[mesh_ids[r]];
+    float tx[3] = {0.f, 0.f, 0.f};
+    const bool textured = !colors && mt.levels > 0 && mt.uvs;
+    if (textured) {   // renderer_py's texture2D(u_texture, v_texcoord): nearest texel of level 0, clamp to edge
+      const float* t0 = mt.uvs + me.faces[f * 3] * 2;
+      const float* t1 = mt.uvs + me.faces[f * 3 + 1] * 2;
+      const float* t2 = mt.uvs + me.faces[f * 3 + 2] * 2;
+      const float s = b[0] * t0[0] + b[1] * t1[0] + b[2] * t2[0];
+      const float t = b[0] * t0[1] + b[1] * t1[1] + b[2] * t2[1];
+      const int w = mt.w[0], h = mt.h[0];
+      const float xs = isfinite(s) ? fminf(fmaxf(floorf(s * (float)w), 0.f), (float)(w - 1)) : 0.f;
+      const float ys = isfinite(t) ? fminf(fmaxf(floorf(t * (float)h), 0.f), (float)(h - 1)) : 0.f;
+      const uint8_t* T = mt.tex + ((long long)ys * w + (long long)xs) * 3;
+      tx[0] = T[0] * (1.f / 255.f); tx[1] = T[1] * (1.f / 255.f); tx[2] = T[2] * (1.f / 255.f);
+    }
 #pragma unroll
     for (int c = 0; c < 3; ++c) {
       float col = 0.5f;
       if (colors) col = colors[r * 3 + c];
+      else if (textured) col = tx[c];
       else if (vc) col = b[0] * vc[me.faces[f * 3] * 3 + c] + b[1] * vc[me.faces[f * 3 + 1] * 3 + c] +
                          b[2] * vc[me.faces[f * 3 + 2] * 3 + c];
       rgb[i * 3 + c] = (uint8_t)fminf(fmaxf(rintf(lw * col * 255.f), 0.f), 255.f);
+    }
+  }
+}
+
+// ---- scene render: the n instances of one call in one image, one z-buffer (EGLRenderer.render) ---------------------
+// The key's low word is the triangle's index in the concatenation of the instances' triangles in call order, so a depth
+// tie between instances goes to the earlier one.  tri_off [n+1] holds each instance's first index (an unknown mesh id
+// contributes no triangles); block 0 of the clear kernel fills it, before the rasteriser reads it in stream order.
+__global__ void rast_scene_clear_kernel(unsigned long long* zbuf, long long npx, const MeshEntry* __restrict__ table,
+                                        int n_meshes, const int* __restrict__ mesh_ids, int n, unsigned* __restrict__ tri_off) {
+  if (blockIdx.x == 0 && threadIdx.x == 0) {
+    unsigned acc = 0;
+    for (int r = 0; r < n; ++r) {
+      tri_off[r] = acc;
+      const int mid = mesh_ids[r];
+      if (mid >= 0 && mid < n_meshes) acc += (unsigned)table[mid].F;
+    }
+    tri_off[n] = acc;
+  }
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < npx; i += (long long)gridDim.x * blockDim.x)
+    zbuf[i] = 0xFFFFFFFFFFFFFFFFull;
+}
+
+__global__ void __launch_bounds__(256)
+rast_scene_tri_kernel(const MeshEntry* __restrict__ table, const int* __restrict__ mesh_ids, int n_meshes, int n,
+                      const float* __restrict__ poses, const float* __restrict__ K, int H, int W, float znear, float zfar,
+                      const unsigned* __restrict__ tri_off, unsigned long long* __restrict__ zbuf) {
+  for (int r = blockIdx.y; r < n; r += gridDim.y)
+    rast_tri_one(table, mesh_ids[r], n_meshes, poses + r * 12, K, H, W, znear, zfar, zbuf, tri_off[r]);
+}
+
+// Bilinear sample of one mip level with clamp-to-edge (GL_LINEAR): texel centres at (i + 0.5) / w, row 0 at t = 0.
+__device__ __forceinline__ void tex_bilinear(const MeshTex& mt, int l, float s, float t, float out[3]) {
+  const int w = mt.w[l], h = mt.h[l];
+  const uint8_t* T = mt.tex + mt.off[l];
+  const float x = s * (float)w - 0.5f, y = t * (float)h - 0.5f;
+  const float fx = floorf(x), fy = floorf(y);
+  const float a = x - fx, b = y - fy;
+  const int i0 = min(max((int)fx, 0), w - 1), i1 = min(max((int)fx + 1, 0), w - 1);
+  const int j0 = min(max((int)fy, 0), h - 1), j1 = min(max((int)fy + 1, 0), h - 1);
+#pragma unroll
+  for (int c = 0; c < 3; ++c) {
+    const float t00 = T[((long long)j0 * w + i0) * 3 + c], t10 = T[((long long)j0 * w + i1) * 3 + c];
+    const float t01 = T[((long long)j1 * w + i0) * 3 + c], t11 = T[((long long)j1 * w + i1) * 3 + c];
+    out[c] = ((1.f - a) * (1.f - b) * t00 + a * (1.f - b) * t10 + (1.f - a) * b * t01 + a * b * t11) * (1.f / 255.f);
+  }
+}
+
+// GL_LINEAR_MIPMAP_LINEAR with GL_LINEAR magnification: lambda = log2(rho), rho the larger screen-space derivative
+// length of (s w0, t h0) in level-0 texels.  lambda <= 0: level 0; lambda >= q (the last level): level q; otherwise the
+// levels floor(lambda) and floor(lambda) + 1 blended by frac(lambda).
+__device__ __forceinline__ void tex_sample(const MeshTex& mt, float s, float t, float dsdx, float dtdx, float dsdy,
+                                           float dtdy, float out[3]) {
+  if (!isfinite(s) || !isfinite(t)) { s = 0.f; t = 0.f; }
+  const float W0 = (float)mt.w[0], H0 = (float)mt.h[0];
+  const float rx = sqrtf((dsdx * W0) * (dsdx * W0) + (dtdx * H0) * (dtdx * H0));
+  const float ry = sqrtf((dsdy * W0) * (dsdy * W0) + (dtdy * H0) * (dtdy * H0));
+  const float lambda = log2f(fmaxf(rx, ry));
+  const int q = mt.levels - 1;
+  if (!(lambda > 0.f)) { tex_bilinear(mt, 0, s, t, out); return; }
+  if (lambda >= (float)q) { tex_bilinear(mt, q, s, t, out); return; }
+  const float d1 = floorf(lambda), fr = lambda - d1;
+  float a[3], b[3];
+  tex_bilinear(mt, (int)d1, s, t, a);
+  tex_bilinear(mt, (int)d1 + 1, s, t, b);
+#pragma unroll
+  for (int c = 0; c < 3; ++c) out[c] = (1.f - fr) * a[c] + fr * b[c];
+}
+
+struct SceneLight {
+  float pos[3], col[3];       // light position (camera frame) and colour
+  float mat_diffuse[3], mat_ambient[3];
+};
+
+// Resolve: depth and pc_cam from the key with rast_resolve_kernel's arithmetic; the other outputs from the winner's
+// perspective-correct barycentrics (rast_shade_kernel's arithmetic), shaded as shader_textureless_texture.{vs,frag}
+// with the view matrix at identity (camera frame = world frame):
+//   pc_obj = interp(x), normal = 0.5 interp(normalize(R n)) + 0.5, diff = max(dot(interp(normalize(R n)),
+//   normalize(light - interp(P))), 0);  textureless: colour (diff + 0.2) light;  textured: texture (diff light
+//   mat_diffuse + mat_ambient light) (the specular term is 0: with the identity view its view direction is
+//   normalize(0)); every channel clamped at 1.  seg = instance index + 1.  Background: every output 0.
+__global__ void __launch_bounds__(256)
+rast_scene_resolve_kernel(const unsigned long long* __restrict__ zbuf, const MeshEntry* __restrict__ table,
+                          const float* const* __restrict__ mesh_colors, const MeshTex* __restrict__ mesh_tex,
+                          const int* __restrict__ mesh_ids, const unsigned* __restrict__ tri_off, int n,
+                          const float* __restrict__ poses, const float* __restrict__ K, int H, int W, SceneLight lt,
+                          float* __restrict__ depth, float* __restrict__ pc_cam, float* __restrict__ pc_obj,
+                          float* __restrict__ normal, float* __restrict__ image, float* __restrict__ seg) {
+  const long long total = (long long)H * W;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total;
+       i += (long long)gridDim.x * blockDim.x) {
+    const unsigned long long key = zbuf[i];
+    const int px = (int)(i % W), py = (int)(i / W);
+    if (key == 0xFFFFFFFFFFFFFFFFull) {
+      depth[i] = 0.f;
+#pragma unroll
+      for (int c = 0; c < 3; ++c) {
+        if (pc_cam) pc_cam[i * 3 + c] = 0.f;
+        if (pc_obj) pc_obj[i * 3 + c] = 0.f;
+        if (normal) normal[i * 3 + c] = 0.f;
+        if (image) image[i * 3 + c] = 0.f;
+      }
+      if (seg) seg[i] = 0.f;
+      continue;
+    }
+    const float z = __uint_as_float((unsigned)(key >> 32));
+    depth[i] = z;
+    if (pc_cam) {
+      float X = 0.f, Y = 0.f;
+      if (z > 0.f) {
+        Y = ((float)py + 0.5f - K[5]) / K[4] * z;
+        X = ((float)px + 0.5f - K[2] - K[1] * Y / z) / K[0] * z;
+      }
+      pc_cam[i * 3] = X; pc_cam[i * 3 + 1] = Y; pc_cam[i * 3 + 2] = z;
+    }
+    const unsigned g = (unsigned)key;
+    int lo = 0, hi = n - 1;              // the last instance whose first triangle index is <= g
+    while (lo < hi) {
+      const int mid = (lo + hi + 1) >> 1;
+      if (tri_off[mid] <= g) lo = mid; else hi = mid - 1;
+    }
+    const int r = lo;
+    if (seg) seg[i] = (float)(r + 1);
+    if (!pc_obj && !normal && !image) continue;
+    const int f = (int)(g - tri_off[r]);
+    const int mid = mesh_ids[r];
+    const MeshEntry me = table[mid];
+    const float* P = poses + r * 12;
+    int vi[3];
+    float X[3], Y[3], Z[3], u[3], v[3], iz[3];
+#pragma unroll
+    for (int k = 0; k < 3; ++k) {
+      vi[k] = me.faces[f * 3 + k];
+      const float x = me.verts[vi[k] * 3], y = me.verts[vi[k] * 3 + 1], zz = me.verts[vi[k] * 3 + 2];
+      X[k] = P[0] * x + P[1] * y + P[2] * zz + P[3];
+      Y[k] = P[4] * x + P[5] * y + P[6] * zz + P[7];
+      Z[k] = P[8] * x + P[9] * y + P[10] * zz + P[11];
+      iz[k] = 1.0f / Z[k];
+      u[k] = (K[0] * X[k] + K[1] * Y[k]) * iz[k] + K[2];
+      v[k] = (K[4] * Y[k]) * iz[k] + K[5];
+    }
+    const float inv_area = 1.0f / ((u[1] - u[0]) * (v[2] - v[0]) - (u[2] - u[0]) * (v[1] - v[0]));
+    const float sx = (float)px + 0.5f, sy = (float)py + 0.5f;
+    const float w0 = ((u[1] - sx) * (v[2] - sy) - (u[2] - sx) * (v[1] - sy)) * inv_area;
+    const float w1 = ((u[2] - sx) * (v[0] - sy) - (u[0] - sx) * (v[2] - sy)) * inv_area;
+    const float w2 = 1.0f - w0 - w1;
+    const float izp = w0 * iz[0] + w1 * iz[1] + w2 * iz[2];
+    const float b[3] = {w0 * iz[0] / izp, w1 * iz[1] / izp, w2 * iz[2] / izp};
+    if (pc_obj) {
+#pragma unroll
+      for (int c = 0; c < 3; ++c)
+        pc_obj[i * 3 + c] = b[0] * me.verts[vi[0] * 3 + c] + b[1] * me.verts[vi[1] * 3 + c] + b[2] * me.verts[vi[2] * 3 + c];
+    }
+    if (!normal && !image) continue;
+    const MeshTex& mt = mesh_tex[mid];
+    float N[3] = {0.f, 0.f, 0.f};
+    if (mt.normals) {
+#pragma unroll
+      for (int k = 0; k < 3; ++k) {   // vNormalCam = normalize(R n) per vertex, interpolated, not renormalised
+        const float* nk = mt.normals + vi[k] * 3;
+        const float a = P[0] * nk[0] + P[1] * nk[1] + P[2] * nk[2];
+        const float bb = P[4] * nk[0] + P[5] * nk[1] + P[6] * nk[2];
+        const float c = P[8] * nk[0] + P[9] * nk[1] + P[10] * nk[2];
+        const float d2 = a * a + bb * bb + c * c;
+        const float s = d2 > 0.f ? rsqrtf(d2) : 0.f;
+        N[0] += b[k] * (a * s); N[1] += b[k] * (bb * s); N[2] += b[k] * (c * s);
+      }
+    }
+    if (normal) {
+#pragma unroll
+      for (int c = 0; c < 3; ++c) normal[i * 3 + c] = 0.5f * N[c] + 0.5f;
+    }
+    if (!image) continue;
+    const float Fx = b[0] * X[0] + b[1] * X[1] + b[2] * X[2];
+    const float Fy = b[0] * Y[0] + b[1] * Y[1] + b[2] * Y[2];
+    const float Fz = b[0] * Z[0] + b[1] * Z[1] + b[2] * Z[2];
+    float lx = lt.pos[0] - Fx, ly = lt.pos[1] - Fy, lz = lt.pos[2] - Fz;
+    const float l2 = lx * lx + ly * ly + lz * lz;
+    const float ls = l2 > 0.f ? rsqrtf(l2) : 0.f;
+    const float diff = fmaxf(N[0] * (lx * ls) + N[1] * (ly * ls) + N[2] * (lz * ls), 0.f);
+    float rgb[3];
+    if (mt.levels > 0 && mt.uvs) {
+      const float* t0 = mt.uvs + vi[0] * 2;
+      const float* t1 = mt.uvs + vi[1] * 2;
+      const float* t2 = mt.uvs + vi[2] * 2;
+      const float s = b[0] * t0[0] + b[1] * t1[0] + b[2] * t2[0];
+      const float t = b[0] * t0[1] + b[1] * t1[1] + b[2] * t2[1];
+      // screen derivatives of the perspective-correct attribute a = sum(w_k iz_k a_k) / sum(w_k iz_k):
+      // da/dx = sum(dw_k/dx iz_k (a_k - a)) / izp, with the edge-function gradients of the screen barycentrics
+      const float gx[3] = {(v[1] - v[2]) * inv_area, (v[2] - v[0]) * inv_area, 0.f};
+      const float gy[3] = {(u[2] - u[1]) * inv_area, (u[0] - u[2]) * inv_area, 0.f};
+      const float gx2 = -(gx[0] + gx[1]), gy2 = -(gy[0] + gy[1]);
+      const float dsdx = (gx[0] * iz[0] * (t0[0] - s) + gx[1] * iz[1] * (t1[0] - s) + gx2 * iz[2] * (t2[0] - s)) / izp;
+      const float dtdx = (gx[0] * iz[0] * (t0[1] - t) + gx[1] * iz[1] * (t1[1] - t) + gx2 * iz[2] * (t2[1] - t)) / izp;
+      const float dsdy = (gy[0] * iz[0] * (t0[0] - s) + gy[1] * iz[1] * (t1[0] - s) + gy2 * iz[2] * (t2[0] - s)) / izp;
+      const float dtdy = (gy[0] * iz[0] * (t0[1] - t) + gy[1] * iz[1] * (t1[1] - t) + gy2 * iz[2] * (t2[1] - t)) / izp;
+      float tx[3];
+      tex_sample(mt, s, t, dsdx, dtdx, dsdy, dtdy, tx);
+#pragma unroll
+      for (int c = 0; c < 3; ++c) rgb[c] = tx[c] * (diff * lt.col[c] * lt.mat_diffuse[c] + lt.mat_ambient[c] * lt.col[c]);
+    } else {
+      const float* vc = mesh_colors[mid];
+      const float cad[3] = {223.f / 255.f, 214.f / 255.f, 205.f / 255.f};   // meshutil.py:484-486, a mesh without colours
+#pragma unroll
+      for (int c = 0; c < 3; ++c) {
+        const float col = vc ? b[0] * vc[vi[0] * 3 + c] + b[1] * vc[vi[1] * 3 + c] + b[2] * vc[vi[2] * 3 + c] : cad[c];
+        rgb[c] = col * (diff * lt.col[c] + 0.2f * lt.col[c]);
+      }
+    }
+#pragma unroll
+    for (int c = 0; c < 3; ++c) image[i * 3 + c] = fminf(rgb[c], 1.f);
+  }
+}
+
+// One level of the mip chain: 2x2 box filter of the level above, rounded to nearest, (a + b + c + d + 2) >> 2 per
+// channel; a source index past the last row / column is clamped to it (a dimension of 1 halves to 1).
+__global__ void rast_mip_kernel(const uint8_t* __restrict__ src, int sw, int sh, uint8_t* __restrict__ dst, int dw, int dh) {
+  const long long total = (long long)dw * dh;
+  for (long long k = (long long)blockIdx.x * blockDim.x + threadIdx.x; k < total; k += (long long)gridDim.x * blockDim.x) {
+    const int i = (int)(k % dw), j = (int)(k / dw);
+    const int x0 = min(2 * i, sw - 1), x1 = min(2 * i + 1, sw - 1), y0 = min(2 * j, sh - 1), y1 = min(2 * j + 1, sh - 1);
+#pragma unroll
+    for (int c = 0; c < 3; ++c) {
+      const unsigned s = src[((long long)y0 * sw + x0) * 3 + c] + src[((long long)y0 * sw + x1) * 3 + c] +
+                         src[((long long)y1 * sw + x0) * 3 + c] + src[((long long)y1 * sw + x1) * 3 + c];
+      dst[k * 3 + c] = (uint8_t)((s + 2u) >> 2);
     }
   }
 }
@@ -408,36 +665,72 @@ struct MeshRegistry {
   MeshEntry host[RAST_MAX_MESHES];
   MeshEntry* dev_table = nullptr;
   const float** dev_colors = nullptr;   // [RAST_MAX_MESHES] per-vertex RGB [V,3] f32, or null for a mesh without colours
+  MeshTex* dev_tex = nullptr;           // [RAST_MAX_MESHES] normals, UVs and texture mip chain (rast_upload_mesh_tex)
 };
 MeshRegistry g_meshes;
 }  // namespace
 
-extern "C" int rast_upload_mesh_ex(const float* verts, int V, const int* faces, int F, const float* colors) {
-  // verts / faces / colors: host OR device pointers (cudaMemcpyDefault); the library keeps its own device copy.
-  // Returns the mesh id (>= 0) or a negative GDRN_ERR_* code.
+extern "C" int rast_upload_mesh_tex(const float* verts, int V, const int* faces, int F, const float* colors,
+                                    const float* normals, const float* uvs, const uint8_t* texture, int tex_h, int tex_w) {
+  // verts / faces / colors / normals / uvs / texture: host OR device pointers (cudaMemcpyDefault); the library keeps
+  // its own device copy.  Returns the mesh id (>= 0) or a negative GDRN_ERR_* code.
   if (!(verts && faces && V > 0 && F > 0)) { gdrn_set_last_error(__FILE__, __LINE__, "rast_upload_mesh: empty mesh"); return GDRN_ERR_INVALID; }
+  if (texture && !(uvs && tex_h > 0 && tex_w > 0)) { gdrn_set_last_error(__FILE__, __LINE__, "rast_upload_mesh_tex: a texture needs uvs and tex_h, tex_w > 0"); return GDRN_ERR_INVALID; }
   int dev = 0;
   cudaGetDevice(&dev);
   if (g_meshes.device < 0) g_meshes.device = dev;
   if (g_meshes.device != dev) { gdrn_set_last_error(__FILE__, __LINE__, "rast_upload_mesh: the mesh registry lives on another device"); return GDRN_ERR_STATE; }
   if (g_meshes.count >= RAST_MAX_MESHES) { gdrn_set_last_error(__FILE__, __LINE__, "rast_upload_mesh: registry full (1024 meshes)"); return GDRN_ERR_STATE; }
+  MeshTex mt = {};
+  long long tex_bytes = 0;
+  if (texture) {    // level sizes: halve each dimension (floor, at least 1) until both are 1
+    int w = tex_w, h = tex_h;
+    for (;;) {
+      mt.w[mt.levels] = w; mt.h[mt.levels] = h; mt.off[mt.levels] = tex_bytes;
+      tex_bytes += (long long)w * h * 3;
+      ++mt.levels;
+      if (w == 1 && h == 1) break;
+      if (mt.levels == RAST_MAX_MIPS) { gdrn_set_last_error(__FILE__, __LINE__, "rast_upload_mesh_tex: texture larger than 32768 texels"); return GDRN_ERR_INVALID; }
+      w = w > 1 ? w / 2 : 1; h = h > 1 ? h / 2 : 1;
+    }
+  }
   float* dv = nullptr;
   int* df = nullptr;
   float* dc = nullptr;
+  float* dn = nullptr;
+  float* du = nullptr;
+  uint8_t* dt = nullptr;
   cudaError_t e = cudaMalloc(&dv, (size_t)V * 12);
   if (e == cudaSuccess) e = cudaMalloc(&df, (size_t)F * 12);
   if (e == cudaSuccess) e = cudaMemcpy(dv, verts, (size_t)V * 12, cudaMemcpyDefault);
   if (e == cudaSuccess) e = cudaMemcpy(df, faces, (size_t)F * 12, cudaMemcpyDefault);
   if (e == cudaSuccess && colors) e = cudaMalloc(&dc, (size_t)V * 12);
   if (e == cudaSuccess && colors) e = cudaMemcpy(dc, colors, (size_t)V * 12, cudaMemcpyDefault);
+  if (e == cudaSuccess && normals) e = cudaMalloc(&dn, (size_t)V * 12);
+  if (e == cudaSuccess && normals) e = cudaMemcpy(dn, normals, (size_t)V * 12, cudaMemcpyDefault);
+  if (e == cudaSuccess && uvs) e = cudaMalloc(&du, (size_t)V * 8);
+  if (e == cudaSuccess && uvs) e = cudaMemcpy(du, uvs, (size_t)V * 8, cudaMemcpyDefault);
+  if (e == cudaSuccess && texture) e = cudaMalloc(&dt, (size_t)tex_bytes);
+  if (e == cudaSuccess && texture) e = cudaMemcpy(dt, texture, (size_t)tex_w * tex_h * 3, cudaMemcpyDefault);
+  for (int l = 1; e == cudaSuccess && l < mt.levels; ++l) {
+    const long long npx = (long long)mt.w[l] * mt.h[l];
+    rast_mip_kernel<<<(int)((npx + 255) / 256 > 4096 ? 4096 : (npx + 255) / 256), 256>>>(
+        dt + mt.off[l - 1], mt.w[l - 1], mt.h[l - 1], dt + mt.off[l], mt.w[l], mt.h[l]);
+    e = cudaGetLastError();
+    gdrn_count_launch(1);
+  }
+  if (e == cudaSuccess && mt.levels > 1) e = cudaStreamSynchronize(0);
   if (e == cudaSuccess && !g_meshes.dev_table) e = cudaMalloc(&g_meshes.dev_table, sizeof(MeshEntry) * RAST_MAX_MESHES);
   if (e == cudaSuccess && !g_meshes.dev_colors) e = cudaMalloc(&g_meshes.dev_colors, sizeof(float*) * RAST_MAX_MESHES);
+  if (e == cudaSuccess && !g_meshes.dev_tex) e = cudaMalloc(&g_meshes.dev_tex, sizeof(MeshTex) * RAST_MAX_MESHES);
   if (e == cudaSuccess) {
     const int id = g_meshes.count;
     g_meshes.host[id] = MeshEntry{dv, df, V, F};
     const float* dcc = dc;
+    mt.normals = dn; mt.uvs = du; mt.tex = dt;
     e = cudaMemcpy(g_meshes.dev_table + id, &g_meshes.host[id], sizeof(MeshEntry), cudaMemcpyHostToDevice);
     if (e == cudaSuccess) e = cudaMemcpy(g_meshes.dev_colors + id, &dcc, sizeof(float*), cudaMemcpyHostToDevice);
+    if (e == cudaSuccess) e = cudaMemcpy(g_meshes.dev_tex + id, &mt, sizeof(MeshTex), cudaMemcpyHostToDevice);
     if (e == cudaSuccess) {
       g_meshes.count = id + 1;
       if (F > g_meshes.max_faces) g_meshes.max_faces = F;
@@ -445,9 +738,13 @@ extern "C" int rast_upload_mesh_ex(const float* verts, int V, const int* faces, 
     }
   }
   (void)cudaGetLastError();
-  cudaFree(dv); cudaFree(df); cudaFree(dc);
+  cudaFree(dv); cudaFree(df); cudaFree(dc); cudaFree(dn); cudaFree(du); cudaFree(dt);
   gdrn_set_last_error(__FILE__, __LINE__, cudaGetErrorString(e));
   return GDRN_ERR_CUDA;
+}
+
+extern "C" int rast_upload_mesh_ex(const float* verts, int V, const int* faces, int F, const float* colors) {
+  return rast_upload_mesh_tex(verts, V, faces, F, colors, nullptr, nullptr, nullptr, 0, 0);
 }
 
 extern "C" int rast_upload_mesh(const float* verts, int V, const int* faces, int F) {
@@ -490,8 +787,40 @@ extern "C" int rast_render_meshes_rgb(const int* mesh_ids, const float* poses, c
   rast_clear_kernel<<<blocks, 256, 0, st>>>(zbuf_scratch, npx);
   rast_tri_multi_kernel<<<dim3((g_meshes.max_faces + 255) / 256, n < 65535 ? n : 65535), 256, 0, st>>>(
       g_meshes.dev_table, mesh_ids, g_meshes.count, n, poses, Ks, H, W, znear, zfar, zbuf_scratch);
-  rast_shade_kernel<<<blocks, 256, 0, st>>>(zbuf_scratch, g_meshes.dev_table, g_meshes.dev_colors, mesh_ids, poses, Ks, colors,
+  rast_shade_kernel<<<blocks, 256, 0, st>>>(zbuf_scratch, g_meshes.dev_table, g_meshes.dev_colors, g_meshes.dev_tex, mesh_ids, poses, Ks, colors,
                                             n, H, W, rgb, depth, tri_ids);
+  GDRN_CHECK_CUDA(cudaGetLastError());
+  gdrn_count_launch(3);
+  return GDRN_OK;
+}
+
+// zbuf [H*W] u64, then the per-instance first-triangle table [n_inst + 1] u32
+extern "C" size_t rast_scene_scratch_bytes(int n_inst, int H, int W) {
+  return (size_t)H * W * 8 + (((size_t)n_inst + 1) * 4 + 7) / 8 * 8;
+}
+
+extern "C" int rast_render_scene(const int* mesh_ids, const float* poses, int n_inst, const float* K, int H, int W,
+                                 float znear, float zfar, const float* light, float* depth, float* pc_cam, float* pc_obj,
+                                 float* normal, float* image, float* seg, void* scratch, void* stream) {
+  GDRN_REQUIRE(mesh_ids && poses && K && light && depth && scratch, "rast_render_scene: null argument");
+  GDRN_REQUIRE(n_inst > 0 && H > 0 && W > 0, "rast_render_scene: empty input");
+  GDRN_REQUIRE(g_meshes.count > 0, "rast_render_scene: no mesh uploaded (rast_upload_mesh)");
+  GDRN_REQUIRE(znear > 0.f && zfar > znear, "rast: need 0 < znear < zfar");
+  SceneLight lt;
+  for (int c = 0; c < 3; ++c) {
+    lt.pos[c] = light[c]; lt.col[c] = light[3 + c]; lt.mat_diffuse[c] = light[6 + c]; lt.mat_ambient[c] = light[9 + c];
+  }
+  cudaStream_t st = (cudaStream_t)stream;
+  const long long npx = (long long)H * W;
+  unsigned long long* zbuf = (unsigned long long*)scratch;
+  unsigned* tri_off = (unsigned*)(zbuf + npx);
+  int blocks = (int)((npx + 255) / 256 > 4096 ? 4096 : (npx + 255) / 256);
+  rast_scene_clear_kernel<<<blocks, 256, 0, st>>>(zbuf, npx, g_meshes.dev_table, g_meshes.count, mesh_ids, n_inst, tri_off);
+  rast_scene_tri_kernel<<<dim3((g_meshes.max_faces + 255) / 256, n_inst < 65535 ? n_inst : 65535), 256, 0, st>>>(
+      g_meshes.dev_table, mesh_ids, g_meshes.count, n_inst, poses, K, H, W, znear, zfar, tri_off, zbuf);
+  rast_scene_resolve_kernel<<<blocks, 256, 0, st>>>(zbuf, g_meshes.dev_table, g_meshes.dev_colors, g_meshes.dev_tex,
+                                                    mesh_ids, tri_off, n_inst, poses, K, H, W, lt, depth, pc_cam, pc_obj,
+                                                    normal, image, seg);
   GDRN_CHECK_CUDA(cudaGetLastError());
   gdrn_count_launch(3);
   return GDRN_OK;

@@ -1,7 +1,9 @@
 """PLY mesh I/O for the object models the predictor / renderers take as paths.
 
 Mirrors ``lib/pysixd/inout.py:489-720`` (``load_ply(path, vertex_scale)`` -> dict with 'pts' [n,3], optional 'normals',
-'colors', 'faces' [m,3]) for the two encodings BOP models ship in (ascii and binary_little_endian, triangular faces).
+'colors', 'texture_uv' [n,2], 'texture_file', 'faces' [m,3]) for the two encodings BOP models ship in (ascii and
+binary_little_endian, triangular faces).  Per-face texture coordinates ('texcoord', the reference's 'texture_uv_face')
+are rejected: the BOP models carry per-vertex UVs, and the renderers read only those.
 Parsing is vectorised (one structured ``np.frombuffer`` per element) instead of the reference's per-vertex
 ``struct.unpack`` loop; a 100 k-vertex model loads in milliseconds.
 """
@@ -13,7 +15,9 @@ _PLY_DTYPES = {"char": "i1", "int8": "i1", "uchar": "u1", "uint8": "u1", "short"
 
 
 def load_ply(path, vertex_scale=1.0):
-    """-> {'pts': [n,3] float64 (scaled by vertex_scale), 'faces': [m,3] int64 (if present), 'normals', 'colors'}."""
+    """-> {'pts': [n,3] float64 (scaled by vertex_scale), 'faces': [m,3] int64 (if present), 'normals', 'colors',
+    'texture_uv' [n,2] float64 (vertex properties texture_u / texture_v, or s / t), 'texture_file' (the last word of a
+    `comment TextureFile` line)}."""
     with open(path, "rb") as f:
         raw = f.read()
     end = raw.find(b"end_header")
@@ -23,11 +27,14 @@ def load_ply(path, vertex_scale=1.0):
     header = raw[:end].decode("ascii", "replace").splitlines()
     fmt = "ascii"
     elements = []   # [name, count, [(prop_name, type) | (prop_name, count_type, item_type)]]
+    texture_file = None
     for line in header:
         tok = line.split()
         if not tok:
             continue
-        if tok[0] == "format":
+        if line.startswith("comment TextureFile"):
+            texture_file = tok[-1]
+        elif tok[0] == "format":
             fmt = tok[1]
         elif tok[0] == "element":
             elements.append([tok[1], int(tok[2]), []])
@@ -35,11 +42,18 @@ def load_ply(path, vertex_scale=1.0):
             if tok[1] == "list":
                 elements[-1][2].append((tok[4], tok[2], tok[3]))
             else:
-                elements[-1][2].append((tok[2], tok[1]))
+                name = {"s": "texture_u", "t": "texture_v"}.get(tok[2], tok[2]) if elements[-1][0] == "vertex" else tok[2]
+                elements[-1][2].append((name, tok[1]))
     if fmt not in ("ascii", "binary_little_endian", "binary_big_endian"):
         raise ValueError(f"{path}: unsupported PLY format {fmt}")
+    for name, _, props in elements:
+        if name == "face" and any(p[0] == "texcoord" for p in props):
+            raise ValueError(f"{path}: per-face texture coordinates (texcoord) are not supported; "
+                             "the models need per-vertex texture_u / texture_v")
     end_c = ">" if fmt == "binary_big_endian" else "<"
     model = {}
+    if texture_file is not None:
+        model["texture_file"] = texture_file
     if fmt == "ascii":
         lines = raw[body_off:].decode("ascii", "replace").split("\n")
         pos = 0
@@ -93,6 +107,8 @@ def load_ply(path, vertex_scale=1.0):
                 model["normals"] = np.stack([cols["nx"], cols["ny"], cols["nz"]], axis=1)
             if {"red", "green", "blue"} <= set(cols):
                 model["colors"] = np.stack([cols["red"], cols["green"], cols["blue"]], axis=1)
+            if {"texture_u", "texture_v"} <= set(cols):
+                model["texture_uv"] = np.stack([cols["texture_u"], cols["texture_v"]], axis=1)
     if "pts" not in model:
         raise ValueError(f"{path}: no vertex element")
     return model

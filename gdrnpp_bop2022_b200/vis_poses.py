@@ -416,6 +416,7 @@ def run_split(sp, model_dir, vis_path, dataset, split, scene_ids=None, im_ids=No
     """Visualise every selected image of a split; writes {vis_path}/{dataset}/{split}/{scene:06d}/{im:06d}.jpg and
     {im:06d}_depth_diff.jpg.  -> {"images", "instances", "seconds"}."""
     from .ply import load_ply
+    from .renderer import load_texture
 
     flags = _flags(resolve_visib, rgb_vis, depth_diff)
     need_depth = bool(depth_diff or (rgb_vis and resolve_visib))
@@ -434,15 +435,21 @@ def run_split(sp, model_dir, vis_path, dataset, split, scene_ids=None, im_ids=No
             m = load_ply(p)
             if "faces" not in m:
                 raise GdrnError("obj_id {}: {} has no faces".format(o, p))
-            col = None
+            col = uvs = tex = None
             if vis_orig_color:
-                with open(p, "rb") as f:
-                    if b"TextureFile" in f.read(4096).split(b"end_header")[0]:
-                        raise GdrnError("obj_id {}: {} is textured; --vis_orig_color renders vertex colours only "
-                                        "(texture sampling is not supported)".format(o, p))
-                if "colors" in m:
+                # renderer_py.py:340-365: the PLY's texture (comment TextureFile, beside the model) with its per-vertex
+                # UVs, else its vertex colours
+                if "texture_file" in m:
+                    tp = os.path.join(os.path.dirname(p), m["texture_file"])
+                    if "texture_uv" not in m:
+                        raise GdrnError("obj_id {}: {} is textured; --vis_orig_color needs per-vertex texture_u / "
+                                        "texture_v".format(o, p))
+                    if not os.path.exists(tp):
+                        raise GdrnError("obj_id {}: {} is textured; --vis_orig_color needs its texture {}".format(o, p, tp))
+                    uvs, tex = m["texture_uv"], load_texture(tp)
+                elif "colors" in m:
                     col = m["colors"] / 255.0 if m["colors"].max() > 1.0 else m["colors"]
-            models[o] = (m["pts"], m["faces"], col)
+            models[o] = (m["pts"], m["faces"], col, uvs, tex)
         meshes = bop_eval.VsdMeshes(models, device=device) if models else None
     batches = _batches(images, max_bytes, need_depth)
     decode_pool, write_pool = ThreadPoolExecutor(max(1, workers)), ThreadPoolExecutor(max(1, workers))
@@ -506,7 +513,7 @@ def parse_args(argv=None):
     ap.add_argument("--no_vis_rgb", action="store_true")
     ap.add_argument("--no_resolve_visib", action="store_true")
     ap.add_argument("--no_depth_diff", action="store_true")
-    ap.add_argument("--vis_orig_color", action="store_true", help="render the models' vertex colours (grey without)")
+    ap.add_argument("--vis_orig_color", action="store_true", help="render the models' textures or vertex colours (grey without)")
     ap.add_argument("--shading", default="flat", help="flat (the only shading vis_gt_poses.py uses)")
     ap.add_argument("--colors_json", default=None, help="colour list, e.g. the BOP toolkit's colors.json")
     ap.add_argument("--result_filename", default=None, help="BOP results CSV: draw its estimates instead of GT")

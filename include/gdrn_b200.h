@@ -300,11 +300,31 @@ size_t rast_scratch_bytes(int n, int H, int W);
 /* rast_render_meshes_rgb: the same n renders in colour, with lib/pysixd/renderer_py.py's flat shading (light at the
  *   eye origin, ambient 0.5, face normal turned toward the viewer): rgb [n,H,W,3] u8 = rint(light_w * colour * 255),
  *   0 on background, and float-z depth [n,H,W] equal to rast_render_meshes(quantize_bits = 0).  Colour: colors [n,3]
- *   f32 per render when non-null, else the mesh's vertex colours (interpolated perspective-correctly), else grey 0.5.
+ *   f32 per render when non-null, else the mesh's texture (rast_upload_mesh_tex: the nearest level-0 texel at the
+ *   interpolated UV, clamp to edge -- renderer_py's texture2D), else its vertex colours (interpolated
+ *   perspective-correctly), else grey 0.5.
  *   tri_ids [n,H,W] i32 (optional): the triangle seen at each pixel, -1 on background. */
 int rast_render_meshes_rgb(const int* mesh_ids, const float* poses, const float* Ks, const float* colors, int n, int H,
                            int W, float znear, float zfar, uint8_t* rgb, float* depth, int* tri_ids,
                            unsigned long long* zbuf_scratch, void* stream);
+/* rast_upload_mesh_tex: rast_upload_mesh_ex with optional shading attributes (null: none): normals [V,3] f32 (model
+ *   space), uvs [V,2] f32 and texture [tex_h, tex_w, 3] u8 (row 0 at t = 0, i.e. the image already flipped as GL
+ *   takes it; needs uvs).  The texture's mip chain (2x2 box filter, rounded) is built on the device here, once.
+ *   rast_upload_mesh_ex(...) is rast_upload_mesh_tex(..., NULL, NULL, NULL, 0, 0). */
+int rast_upload_mesh_tex(const float* verts, int V, const int* faces, int F, const float* colors, const float* normals,
+                         const float* uvs, const uint8_t* texture, int tex_h, int tex_w);
+/* rast_render_scene: the n_inst instances mesh_ids[i] (i32, device) at poses [n_inst,3,4] f32 rendered into ONE image
+ *   with one z-buffer and one K [3,3] f32 -- the draw loop of lib/egl_renderer/egl_renderer_v3.py:998-1177 in one
+ *   launch set.  A depth tie between instances goes to the earlier one.  light: HOST [12] f32 = light position (camera
+ *   frame), light colour, material diffuse, material ambient.  depth [H,W] is required; every other output is written
+ *   only when non-null: pc_cam [H,W,3] (== rast_render_meshes' xyz_cam), pc_obj [H,W,3] (model-space point), normal
+ *   [H,W,3] (0.5 n + 0.5 of the interpolated camera-frame normal), image [H,W,3] (shader_textureless_texture.frag
+ *   colour in [0,1], RGB), seg [H,W] (instance index + 1); all 0 on background.  scratch: rast_scene_scratch_bytes
+ *   (n_inst, H, W) bytes, 8-aligned. */
+int rast_render_scene(const int* mesh_ids, const float* poses, int n_inst, const float* K, int H, int W, float znear,
+                      float zfar, const float* light, float* depth, float* pc_cam, float* pc_obj, float* normal,
+                      float* image, float* seg, void* scratch, void* stream);
+size_t rast_scene_scratch_bytes(int n_inst, int H, int W);
 
 /* ---------------------------------------------------------------------------------------------
  * Fast depth refinement -- replaces GDRN_Evaluator.process_depth_refine
