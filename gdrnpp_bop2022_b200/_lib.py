@@ -139,6 +139,8 @@ _SIGNATURES = {
                                                                        c_size_t, c_void_p, c_size_t, c_void_p, c_void_p]),
     "gdrn_rle_confusion": (c_int, [c_void_p, c_size_t, c_void_p, c_int, c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p]),
     "gdrn_gt_info": (c_int, [c_void_p] * 6 + [c_int] * 3 + [c_float] + [c_void_p] * 5),
+    "gdrn_xyz_crop_boxes": (c_int, [c_void_p] + [c_int] * 3 + [c_void_p, c_void_p]),
+    "gdrn_xyz_crop_pack": (c_int, [c_void_p] * 6 + [c_int] * 3 + [c_void_p, c_void_p]),
     "gdrn_vis_poses_workspace_bytes": (c_size_t, [c_int] * 3),
     "gdrn_vis_poses": (c_int, [c_void_p] * 3 + [c_int] * 3 + [c_void_p] * 2 + [c_int] * 3 + [c_void_p] * 9 + [c_size_t,
                                                                                                          c_void_p]),

@@ -301,9 +301,10 @@ def present_scene_ids(split_path):
     return sorted(int(d) for d in os.listdir(split_path) if d.isdigit() and os.path.isdir(os.path.join(split_path, d)))
 
 
-def plan_split(sp, scene_ids=None):
+def plan_split(sp, scene_ids=None, need_depth=True):
     """Every image of the selected scenes in order: [(scene_id, [image records])], image record = {im_id, depth path,
-    K [3,3], depth_scale, gts}.  Rejects a missing depth image or depth_scale before any work."""
+    K [3,3], depth_scale, gts}.  Rejects a missing depth image or depth_scale before any work.  need_depth=False (for
+    tools that only render, such as gen_xyz) leaves depth and depth_scale out of the records and checks neither."""
     scenes = []
     for scene_id in (present_scene_ids(sp["split_path"]) if scene_ids is None else scene_ids):
         sdir = os.path.join(sp["split_path"], "{:06d}".format(scene_id))
@@ -314,10 +315,13 @@ def plan_split(sp, scene_ids=None):
             cam = scene_cam.get(im_id)
             if cam is None:
                 raise GdrnError("scene {} image {}: no entry in scene_camera.json".format(scene_id, im_id))
-            if "depth_scale" not in cam:
-                raise GdrnError("scene {} image {}: scene_camera.json has no depth_scale".format(scene_id, im_id))
-            ims.append({"im_id": im_id, "depth": depth_path(sp["split_path"], scene_id, im_id, sp["depth_ext"]),
-                        "K": cam["cam_K"], "depth_scale": float(cam["depth_scale"]), "gts": scene_gt[im_id]})
+            rec = {"im_id": im_id, "K": cam["cam_K"], "gts": scene_gt[im_id]}
+            if need_depth:
+                if "depth_scale" not in cam:
+                    raise GdrnError("scene {} image {}: scene_camera.json has no depth_scale".format(scene_id, im_id))
+                rec["depth"] = depth_path(sp["split_path"], scene_id, im_id, sp["depth_ext"])
+                rec["depth_scale"] = float(cam["depth_scale"])
+            ims.append(rec)
         scenes.append((scene_id, ims))
     return scenes
 

@@ -660,6 +660,21 @@ int gdrn_gt_info(const float* depth_large, const float* depth_img, const uint16_
                  const double* Ks, const int* inst_img, int n, int H, int W, float delta, long long* counts, int* boxes,
                  uint8_t* mask, uint8_t* mask_visib, void* stream);
 
+/* ---------------------------------------------------------------------------------------------
+ * xyz_crop training targets of a BOP split (csrc/xyz_crop.cu): the per-instance math of the *_1_gen_xyz.py scripts for
+ * n instances rendered alone at one size H x W (depth [n,H,W] f32, float z, 0 = background).
+ *   gdrn_xyz_crop_boxes: boxes [n,4] i32 = x1, y1, x2, y2, the inclusive pixel box of depth != 0; an empty render gives
+ *     (INT_MAX, INT_MAX, INT_MIN, INT_MIN).  Integer min / max only: independent of the launch shape.
+ *   gdrn_xyz_crop_pack: R [n,9] (row-major cam_R_m2c), t [n,3] (metres), K [n,9], all f32; boxes from
+ *     gdrn_xyz_crop_boxes; offsets [n] i64 in fp16 elements.  Writes instance i's crop at out + offsets[i] as
+ *     [y2-y1+1, x2-x1+1, 3] fp16 (round to nearest even) of R^T (((u - cx) z / fx, (v - cy) z / fy, z) - t), computed
+ *     in f32 with the product rounded before the division, and 0 where z == 0; an empty instance gets [H, W, 3] zeros.
+ * Allocate nothing, do not synchronise.
+ * ------------------------------------------------------------------------------------------- */
+int gdrn_xyz_crop_boxes(const float* depth, int n, int H, int W, int* boxes, void* stream);
+int gdrn_xyz_crop_pack(const float* depth, const float* R, const float* t, const float* K, const int* boxes,
+                       const long long* offsets, int n, int H, int W, uint16_t* out, void* stream);
+
 
 /* ---------------------------------------------------------------------------------------------
  * Pose visualisation composite (csrc/vis_poses.cu): the pixel arithmetic of visualization.vis_object_poses
