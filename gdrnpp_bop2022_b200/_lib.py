@@ -92,6 +92,12 @@ _SIGNATURES = {
     "yolox_postprocess_layout": (c_int, [c_int, c_int, POINTER(c_size_t)]),
     "yolox_postprocess": (c_int, [c_void_p] + [c_int] * 3 + [c_void_p, c_void_p, c_int, c_float, c_float, c_int, c_int, c_void_p, c_void_p,
                                   c_void_p, c_size_t, c_void_p]),
+    "yolox_loss_workspace_bytes": (c_size_t, [c_int] * 3),
+    "yolox_loss_layout": (c_int, [c_int] * 3 + [POINTER(c_size_t)]),
+    "yolox_loss_forward": (c_int, [c_void_p, c_void_p, c_int] + [c_void_p] * 2 + [c_int] * 5 + [c_void_p] * 2
+                           + [c_size_t, c_void_p]),
+    "yolox_loss_backward": (c_int, [c_void_p, c_void_p, c_int] + [c_void_p] * 2 + [c_int] * 5 + [c_void_p] * 2
+                            + [c_size_t] + [c_void_p] * 3),
     "yolox_model_create": (c_int, [POINTER(c_void_p), c_double, c_double] + [c_int] * 5),
     "yolox_model_destroy": (None, [c_void_p]),
     "yolox_model_load_tensor": (c_int, [c_void_p, c_char_p, c_void_p, c_int64, c_void_p]),

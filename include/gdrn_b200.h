@@ -499,6 +499,32 @@ int yolox_postprocess(const float* preds, int B, int A, int num_classes, const i
                       void* workspace, size_t workspace_bytes, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
+ * YOLOX training loss (csrc/yolox_loss.cu) -- replaces YOLOXHead.get_losses (det/yolox/models/yolo_head.py:256-426):
+ * SimOTA assignment and the IoU, objectness, class and L1 terms for a batch, no host synchronisation (DESIGN.md §7q).
+ *   outputs [B, A, 5 + num_classes] (decoded cx, cy, w, h; objectness and class logits) and origin_preds [B, A, 4] (raw
+ *   regression; may be NULL when use_l1 = 0), both of dtype 0 = f32, 1 = f16, 2 = bf16; labels [B, M, 5] f32 (class,
+ *   cx, cy, w, h; the GTs of an image are its first n rows, n = rows with a positive sum; M <= 1024); shifts [3, A] f32 =
+ *   x shift, y shift, stride per anchor.  Everything is computed in f32.
+ *   yolox_loss_forward: trace (NULL or [B, M, A, 3] f32) receives (IoU, unpenalised cost, cost) of every candidate pair.
+ *   yolox_loss_backward: grad_losses [4] f32 (device) = upstream gradients of loss_iou (already x5), loss_conf,
+ *   loss_cls, loss_l1; reads the assignment the forward left in the same workspace; grad_outputs like outputs,
+ *   grad_origin like origin_preds (written when use_l1).
+ *   yolox_loss_layout: offsets[16] = byte offsets, from the workspace rounded up to 256 bytes, of nlabel [B] i32,
+ *   cand [B,A] u8, cls_sum [B,A] f32, count [B,A] i32, chooser [B,A] i32, n_cand [B] i32, k [B,M] i32, iou_sum [B,M]
+ *   f32, chosen [B,M,10] i32 (-1 padded), fg [B,A] u8, matched [B,A] i32, iou_t [B,A] f32, partial [P,4] f32,
+ *   partial_fg [P] i32, err [B] i32 and result [8] f32 = loss_iou * 5, loss_conf, loss_cls, loss_l1, max(num_fg, 1),
+ *   num_fg / max(num_gt, 1), class-id error flag, num_fg.
+ * ------------------------------------------------------------------------------------------- */
+size_t yolox_loss_workspace_bytes(int B, int A, int M);
+int yolox_loss_layout(int B, int A, int M, size_t* offsets);
+int yolox_loss_forward(const void* outputs, const void* origin_preds, int dtype, const float* labels, const float* shifts,
+                       int B, int A, int num_classes, int M, int use_l1, float* trace, void* workspace,
+                       size_t workspace_bytes, void* stream);
+int yolox_loss_backward(const void* outputs, const void* origin_preds, int dtype, const float* labels, const float* shifts,
+                        int B, int A, int num_classes, int M, int use_l1, const float* grad_losses, void* workspace,
+                        size_t workspace_bytes, void* grad_outputs, void* grad_origin, void* stream);
+
+/* ---------------------------------------------------------------------------------------------
  * YOLOX detector network (det/yolox/models: CSPDarknet + YOLOPAFPN + YOLOXHead, inference), csrc/yolox_net.cu.
  *   yolox_model_create: one engine per (depth, width, num_classes, max_batch, H, W, precision); H, W multiples of 32;
  *     precision 1 = bf16x3 (split-bf16 operands), 0 = bf16.  Channel counts must be multiples of 8.
