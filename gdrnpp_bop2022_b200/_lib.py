@@ -98,6 +98,10 @@ _SIGNATURES = {
                            + [c_size_t, c_void_p]),
     "yolox_loss_backward": (c_int, [c_void_p, c_void_p, c_int] + [c_void_p] * 2 + [c_int] * 5 + [c_void_p] * 2
                             + [c_size_t] + [c_void_p] * 3),
+    "gdrn_loss_workspace_bytes": (c_size_t, [c_int, c_int]),
+    "gdrn_loss_layout": (c_int, [c_int, c_int, POINTER(c_size_t)]),
+    "gdrn_loss_forward": (c_int, [c_void_p] * 3 + [c_int] * 5 + [c_void_p, c_size_t, c_void_p]),
+    "gdrn_loss_backward": (c_int, [c_void_p] * 3 + [c_int] * 5 + [c_void_p] * 3 + [c_size_t, c_void_p]),
     "yolox_model_create": (c_int, [POINTER(c_void_p), c_double, c_double] + [c_int] * 5),
     "yolox_model_destroy": (None, [c_void_p]),
     "yolox_model_load_tensor": (c_int, [c_void_p, c_char_p, c_void_p, c_int64, c_void_p]),

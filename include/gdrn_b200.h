@@ -525,6 +525,38 @@ int yolox_loss_backward(const void* outputs, const void* origin_preds, int dtype
                         size_t workspace_bytes, void* grad_outputs, void* grad_origin, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
+ * GDRN training loss (csrc/gdrn_loss.cu) -- replaces GDRN_DoubleMask.gdrn_loss
+ * (core/gdrn_modeling/models/GDRN_double_mask.py:287-536) with PyPMLoss and get_closest_rot_batch: the coordinate,
+ * mask, full-mask and region terms, symmetry-aware point matching (PM_R_ONLY) and the centroid / z terms, all f32, no
+ * host synchronisation (DESIGN.md §7r).
+ *   inputs[22] (device pointers, NULL where a term is off): out_x, out_y, out_z, out_mask_vis, out_mask_full [B,1,H,W]
+ *   (plane contiguous, batch strides in batch_strides[5], in elements); the GT masks the config selects for xyz, mask,
+ *   full mask and region [B,H,W]; gt_xyz [B,3,H,W]; out_region [B,R1,H,W]; gt_region [B,H,W] i64; out_rot, gt_rot
+ *   [B,3,3]; points [B,N,3]; extents [B,3]; symmetry table [T,3,3] and per-ROI (first row, count) [B,2] i32 (both NULL:
+ *   no symmetry); out_centroid [B,2]; out_trans_z [B]; gt_trans_ratio [B,3]; gt_trans [B,3].  HW = H * W.
+ *   weights[7] = XYZ_LW, MASK_LW, FULL_MASK_LW, REGION_LW, PM_LW, CENTROID_LW, Z_LW.  flags: 1 geometry terms (xyz,
+ *   mask, region), 2 full mask, 4 mask BCE (else L1), 8 full mask BCE, 16 point matching, 32 PM_NORM_BY_EXTENT,
+ *   64 centroid, 128 z, 256 Z_TYPE ABS (else REL).
+ *   gdrn_loss_backward: grad_losses [9] f32 (device) = upstream gradients of the result's losses; grads[9] = device
+ *   outputs for out_x, out_y, out_z, out_mask_vis, out_mask_full [B,HW], out_region [B,R1,HW], out_rot [B,9],
+ *   out_centroid [B,2], out_trans_z [B] (NULL where a term is off); reads what the forward left in the workspace.
+ *   gdrn_loss_layout: offsets[10] = byte offsets, from the workspace rounded up to 256 bytes, of partial [P,8] f64
+ *   (per CTA: |dx|, |dy|, |dz|, mask, full mask and region CE sums, xyz and region mask counts; P = B * ceil(HW / 512)),
+ *   partial_err [P] i32, lse [B,HW] f32, sym_idx [B] i32 (-1 = R_gt, k = R_gt S_k), rot_sel [B,3,3] f32 (R_gt'),
+ *   pm_abs [B] f64, pm_sign [B,3,3] f64 (sum of sign(w (R_est - R_gt') p)_i w p_j), sym_err [B] f32 (degrees),
+ *   norm [4] f32 (xyz count, region count, each at least 1; B * HW; B * N * 3) and result [10] f32 = loss_coor_x / y /
+ *   z, loss_mask, loss_mask_full, loss_region, loss_PM_R, loss_centroid, loss_z (each times its weight), region-label
+ *   error flag.
+ * ------------------------------------------------------------------------------------------- */
+size_t gdrn_loss_workspace_bytes(int B, int HW);
+int gdrn_loss_layout(int B, int HW, size_t* offsets);
+int gdrn_loss_forward(const void* const* inputs, const long long* batch_strides, const float* weights, int B, int HW,
+                      int R1, int N, int flags, void* workspace, size_t workspace_bytes, void* stream);
+int gdrn_loss_backward(const void* const* inputs, const long long* batch_strides, const float* weights, int B, int HW,
+                       int R1, int N, int flags, const float* grad_losses, void* const* grads, void* workspace,
+                       size_t workspace_bytes, void* stream);
+
+/* ---------------------------------------------------------------------------------------------
  * YOLOX detector network (det/yolox/models: CSPDarknet + YOLOPAFPN + YOLOXHead, inference), csrc/yolox_net.cu.
  *   yolox_model_create: one engine per (depth, width, num_classes, max_batch, H, W, precision); H, W multiples of 32;
  *     precision 1 = bf16x3 (split-bf16 operands), 0 = bf16.  Channel counts must be multiples of 8.
