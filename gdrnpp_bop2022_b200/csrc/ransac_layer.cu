@@ -27,7 +27,9 @@ __device__ __forceinline__ unsigned rl_hash(unsigned x) {
 }
 
 // one CTA per image: count the foreground, optionally subsample it to ~max_num (ransac_voting_gpu.py:34-38), and compact
-// coords (x, y) / direct in row-major order -- the order torch.nonzero / masked_select produce
+// coords (x, y) / direct in row-major order -- the order torch.nonzero / masked_select produce.  The mask holds integer
+// weights (int)m: a pixel of non-zero weight is foreground, and foreground_num -- which decides min_num, max_num and
+// the keep probability -- is the sum of the weights, as torch.sum of the reference's byte mask is
 __global__ void __launch_bounds__(RL_THREADS)
 rv_compact_kernel(const float* __restrict__ mask, const float* __restrict__ vertex, int h, int w, int vn, int min_num,
                   int max_num, unsigned seed, float* __restrict__ coords, float* __restrict__ direct, int* __restrict__ tn_out) {
@@ -38,21 +40,23 @@ rv_compact_kernel(const float* __restrict__ mask, const float* __restrict__ vert
   float* co = coords + (size_t)bi * npix * 2;
   float* di = direct + (size_t)bi * npix * vn * 2;
   __shared__ int s_scan[RL_THREADS / 32 + 1];
-  __shared__ int s_total, s_base;
-  // pass 1: foreground count
-  int c = 0;
-  for (int i = tid; i < npix; i += RL_THREADS) c += m[i] != 0.f ? 1 : 0;
+  __shared__ long long s_wsum[RL_THREADS / 32];
+  __shared__ long long s_total;
+  __shared__ int s_base;
+  // pass 1: foreground weight
+  long long c = 0;
+  for (int i = tid; i < npix; i += RL_THREADS) c += (int)m[i];
   for (int o = 16; o > 0; o >>= 1) c += __shfl_xor_sync(0xffffffffu, c, o);
-  if (lane == 0) s_scan[warp] = c;
+  if (lane == 0) s_wsum[warp] = c;
   __syncthreads();
   if (tid == 0) {
-    int t = 0;
-    for (int k = 0; k < RL_THREADS / 32; ++k) t += s_scan[k];
+    long long t = 0;
+    for (int k = 0; k < RL_THREADS / 32; ++k) t += s_wsum[k];
     s_total = t;
     s_base = 0;
   }
   __syncthreads();
-  const int fg = s_total;
+  const long long fg = s_total;
   if (fg < min_num) {   // "if too few points, just skip it": zeros come out of the refit kernel
     if (tid == 0) tn_out[bi] = 0;
     return;
@@ -62,7 +66,7 @@ rv_compact_kernel(const float* __restrict__ mask, const float* __restrict__ vert
   // pass 2: ordered compaction, chunks of RL_THREADS pixels
   for (int base = 0; base < npix; base += RL_THREADS) {
     const int i = base + tid;
-    bool sel = i < npix && m[i] != 0.f;
+    bool sel = i < npix && (int)m[i] != 0;
     if (sel && subsample) {
       const float u = (float)(rl_hash(seed ^ rl_hash((unsigned)bi * 0x9E3779B9u + (unsigned)i)) >> 8) * (1.0f / 16777216.0f);
       sel = u < keep_p;
@@ -121,6 +125,8 @@ __global__ void rv_gen_batched_kernel(const float* __restrict__ direct, const fl
 
 // fused vote + count, batched: grid (pixel tiles of the LARGEST possible image, hypothesis chunks, images); tn per image
 constexpr int RL_TILE_T = 256, RL_H_CHUNK = 32;
+// largest dynamic shared memory of a launch (vn <= 84); the kernel opts in to all of it once, whatever vn comes first
+constexpr size_t RL_SMEM_MAX = 200 * 1024;
 __global__ void __launch_bounds__(RL_TILE_T)
 rv_count_batched_kernel(const float* __restrict__ direct, const float* __restrict__ coords, const int* __restrict__ tn_p,
                         const float* __restrict__ hypo, int npix, int vn, int hn, float thresh, int* __restrict__ counts) {
@@ -253,7 +259,7 @@ extern "C" int rv_ransac_voting_layer(const float* mask, const float* vertex, in
   GDRN_REQUIRE(b > 0 && h > 0 && w > 0 && vn > 0 && hn > 0, "ransac_voting_layer: empty problem");
   GDRN_REQUIRE(workspace_bytes >= rv_layer_workspace_bytes(b, h, w, vn, hn), "ransac_voting_layer: workspace too small");
   const size_t smem = (size_t)RL_TILE_T * vn * 8 + (size_t)RL_H_CHUNK * vn * 8 + (size_t)RL_H_CHUNK * vn * 4;
-  GDRN_REQUIRE(smem <= 200 * 1024, "ransac_voting_layer: vn too large for the shared-memory tile");
+  GDRN_REQUIRE(smem <= RL_SMEM_MAX, "ransac_voting_layer: vn too large for the shared-memory tile");
   cudaStream_t st = (cudaStream_t)stream;
   const int npix = h * w;
   uint8_t* p = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(workspace) + 255) & ~(uintptr_t)255);
@@ -265,7 +271,7 @@ extern "C" int rv_ransac_voting_layer(const float* mask, const float* vertex, in
   rv_compact_kernel<<<b, RL_THREADS, 0, st>>>(mask, vertex, h, w, vn, min_num, max_num, seed, coords, direct, tn);
   rv_gen_batched_kernel<<<dim3((hn * vn + 255) / 256, b), 256, 0, st>>>(direct, coords, tn, idxs, seed, npix, vn, hn, hypo);
   GDRN_CHECK_CUDA(cudaMemsetAsync(counts, 0, (size_t)b * hn * vn * 4, st));
-  if (smem > 48 * 1024) GDRN_OPT_IN_SMEM(rv_count_batched_kernel, smem);
+  if (smem > 48 * 1024) GDRN_OPT_IN_SMEM(rv_count_batched_kernel, RL_SMEM_MAX);
   rv_count_batched_kernel<<<dim3((npix + RL_TILE_T - 1) / RL_TILE_T, (hn + RL_H_CHUNK - 1) / RL_H_CHUNK, b), RL_TILE_T, smem, st>>>(
       direct, coords, tn, hypo, npix, vn, hn, inlier_thresh, counts);
   rv_refit_kernel<<<dim3(vn, b), 256, 0, st>>>(direct, coords, tn, hypo, counts, npix, vn, hn, inlier_thresh, win_pts, inliers);

@@ -128,15 +128,16 @@ class _RansacVotingModule:
 ransac_voting = _RansacVotingModule()
 
 
-def _ransac_layer_call(mask, vertex, hn, inlier_thresh, min_num, max_num, idxs, seed, want_hyp=False, want_inliers=False):
+def _ransac_layer_call(weights, vertex, hn, inlier_thresh, min_num, max_num, idxs, seed, want_hyp=False, want_inliers=False):
     """One call of rv_ransac_voting_layer for the whole batch: compaction of the foreground, hypotheses, fused
-    vote + count, per-keypoint winner, inlier set of the winner and its least-squares refit -- all on the device."""
+    vote + count, per-keypoint winner, inlier set of the winner and its least-squares refit -- all on the device.
+    ``weights`` [b,h,w] holds non-negative integers: a non-zero pixel is foreground, and the foreground count that
+    min_num / max_num and the subsampling probability see is the sum of the weights."""
     if not vertex.is_cuda:
         raise RuntimeError("ransac_voting_layer: CUDA tensors required (no CPU fallback)")
     dev = vertex.device
     b, h, w, vn, _ = vertex.shape
-    m = mask.detach().to(device=dev).reshape(b, h, w)
-    m = (m != 0).to(torch.float32).contiguous()
+    m = weights.detach().to(device=dev).reshape(b, h, w).to(torch.float32).contiguous()
     vtx = vertex.detach().to(dtype=torch.float32).contiguous()
     L = _lib.lib()
     ws = torch.empty(L.rv_layer_workspace_bytes(b, h, w, vn, hn), dtype=torch.uint8, device=dev)
@@ -162,6 +163,12 @@ def ransac_voting_layer(mask, vertex, round_hyp_num, inlier_thresh=0.999, confid
                         max_num=30000, idxs=None, seed=None, return_inliers=False):
     """ransac_voting_gpu.py:7-104 on the device: mask [b,h,w], vertex [b,h,w,vn,2] -> keypoints [b,vn,2].
 
+    The mask is read as the reference reads it, as a byte mask (`mask[bi].byte()`, :28): values are truncated to
+    uint8, so a value in (0, 1) is background, and a pixel of value k >= 1 is one foreground pixel that counts k times
+    in `foreground_num` (:29), the count min_num, max_num and the subsampling probability see.  Masks of 0 / 1 give the
+    same result as ransac_voting_layer_v3.  A singular 2x2 refit takes b_inv's identity fallback for that keypoint, as
+    v3 does (the reference's v1 returns zeros for the whole image when torch.inverse fails).
+
     The reference draws its hypothesis pixel pairs ONCE per image, outside its `while` loop (:48), so every round
     regenerates the same hypotheses and counts and its strict `<` update never fires after round 1: `confidence` and
     `max_iter` only decide when that loop stops, not what it returns.  One device-side round is therefore the same
@@ -169,16 +176,20 @@ def ransac_voting_layer(mask, vertex, round_hyp_num, inlier_thresh=0.999, confid
     ``idxs`` [b,hn,vn,2] int32 (optional, taken modulo the foreground count) replaces the on-device RNG (tests);
     ``return_inliers`` also returns (inlier mask [b,vn,h*w] u8 in compacted-pixel order, tn [b])."""
     del confidence, max_iter   # see the docstring: they do not influence the reference's result
-    win, _, _, tn, inl = _ransac_layer_call(mask, vertex, int(round_hyp_num), inlier_thresh, min_num, max_num, idxs, seed,
-                                            want_inliers=return_inliers)
+    win, _, _, tn, inl = _ransac_layer_call(mask.to(torch.uint8), vertex, int(round_hyp_num), inlier_thresh, min_num, max_num,
+                                            idxs, seed, want_inliers=return_inliers)
     return (win, inl, tn) if return_inliers else win
 
 
+@_lib.on_device(1)
 def ransac_voting_layer_v3(mask, vertex, round_hyp_num, inlier_thresh=0.999, confidence=0.99, max_iter=20, min_num=5,
-                           max_num=30000, **kw):
-    """ransac_voting_gpu.py:123-218: the v3 variant differs from ransac_voting_layer only in using bool masks and a
-    batched inverse for the final 2x2 solves -- numerically the same function; same device-side implementation."""
-    return ransac_voting_layer(mask, vertex, round_hyp_num, inlier_thresh, confidence, max_iter, min_num, max_num, **kw)
+                           max_num=30000, idxs=None, seed=None, return_inliers=False):
+    """ransac_voting_gpu.py:123-218: ransac_voting_layer with the reference's bool mask (`.to(torch.bool)`, :144):
+    every non-zero value is one foreground pixel and counts once.  Arguments and outputs as ransac_voting_layer."""
+    del confidence, max_iter
+    win, _, _, tn, inl = _ransac_layer_call(mask.to(torch.bool), vertex, int(round_hyp_num), inlier_thresh, min_num, max_num,
+                                            idxs, seed, want_inliers=return_inliers)
+    return (win, inl, tn) if return_inliers else win
 
 
 @_lib.on_device(1)
@@ -203,10 +214,19 @@ def estimate_voting_distribution_with_mean(mask, vertex, mean, round_hyp_num=256
     hn = int(np.ceil(min_hyp_num / round_hyp_num)) * int(round_hyp_num)
     fg = (mask.reshape(b, h, w) == 1)
     _, hyp, cnt, tn, _ = _ransac_layer_call(fg, vertex, hn, inlier_thresh, min_num, max_num, None, seed, want_hyp=True)
+    return mean, _voting_distribution(hyp, cnt, tn, mean)
+
+
+def _voting_distribution(hyp, cnt, tn, mean):
+    """The covariance of estimate_voting_distribution_with_mean (ransac_voting_gpu.py:290-304) from the layer's
+    hypotheses hyp [b,hn,vn,2], counts cnt [b,hn,vn] and foreground counts tn [b]: ratio = cnt / tn in fp32, an image
+    without foreground (tn = 0) weighs its hn zero hypotheses by 1 (:241-249 emits min_hyp_num of them; hn is that
+    rounded up to whole rounds), ratios below max - 0.1 are dropped -> [b,vn,2,2]."""
+    b = hyp.shape[0]
     tnf = tn.to(torch.float32).clamp_min(1.0).view(b, 1, 1)
     ratio = cnt.to(torch.float32) / tnf                                       # [b,hn,vn]
     empty = (tn <= 0).view(b, 1, 1)
-    ratio = torch.where(empty, torch.ones_like(ratio), ratio)                 # too few pixels: zeros / ones like the reference (:237-247)
+    ratio = torch.where(empty, torch.ones_like(ratio), ratio)                 # too few pixels: zeros / ones like the reference (:241-249)
     all_hyp = hyp.permute(0, 2, 1, 3)                                         # b,vn,hn,2
     all_ratio = ratio.permute(0, 2, 1).clone()                                # b,vn,hn
     thresh = torch.max(all_ratio, 2)[0] - 0.1
@@ -214,7 +234,7 @@ def estimate_voting_distribution_with_mean(mask, vertex, mean, round_hyp_num=256
     diff = all_hyp - mean.unsqueeze(2)
     cov = torch.matmul(diff.transpose(2, 3), diff * all_ratio.unsqueeze(3))
     cov = cov / (torch.sum(all_ratio, 2).unsqueeze(2).unsqueeze(3) + 1e-3)
-    return mean, cov
+    return cov
 
 
 # ------------------------------------------------------------------------------------------------ nnd

@@ -230,11 +230,12 @@ int rv_vote_count(const float* direct, const float* coords, const float* hypo, i
 
 /* The whole RANSAC voting layer for a batch of images on the device (SURVEY.md 8b "rv_ransac_round"): replaces the
  * Python driver ransac_voting_layer / ransac_voting_layer_v3 (core/csrc/ransac_voting/ransac_voting_gpu.py:7-104,
- * 123-218).  mask [b,h,w] f32 (non-zero = foreground), vertex [b,h,w,vn,2] f32 -> win_pts [b,vn,2]: ordered
- * compaction of the foreground (tn stays on the device; images with fewer than min_num pixels give zeros, more than
- * max_num are randomly subsampled), hn hypotheses per keypoint from pixel pairs idxs [b,hn,vn,2] i32 (optional;
- * taken modulo tn; NULL = counter-based RNG(seed)), fused vote + count, per-keypoint winner, inlier set of the winner
- * and least-squares refit of its lines.  No host synchronisation.  Optional outputs: hypo [b,hn,vn,2], counts
+ * 123-218).  mask [b,h,w] f32 of non-negative integer weights (0 = background; a pixel of non-zero (int)weight is
+ * one foreground pixel and adds its weight to the foreground count), vertex [b,h,w,vn,2] f32 -> win_pts [b,vn,2]:
+ * ordered compaction of the foreground (tn stays on the device; images whose foreground count is below min_num give
+ * zeros, above max_num keep each pixel with probability max_num / count), hn hypotheses per keypoint from pixel
+ * pairs idxs [b,hn,vn,2] i32 (optional; taken modulo tn; NULL = counter-based RNG(seed)), fused vote + count,
+ * per-keypoint winner, inlier set of the winner and least-squares refit of its lines.  No host synchronisation.  Optional outputs: hypo [b,hn,vn,2], counts
  * [b,hn,vn] i32, tn [b] i32, inliers [b,vn,h*w] u8 (compacted pixel order, first tn[b] entries valid). */
 size_t rv_layer_workspace_bytes(int b, int h, int w, int vn, int hn);
 int rv_ransac_voting_layer(const float* mask, const float* vertex, int b, int h, int w, int vn, int hn,
