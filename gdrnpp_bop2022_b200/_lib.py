@@ -165,6 +165,11 @@ _SIGNATURES = {
     "yolox_train_hsv": (c_int, [c_void_p] * 3 + [c_int, c_int64, c_int, c_void_p]),
     "yolox_train_preproc": (c_int, [c_void_p] * 2 + [c_int] * 3 + [c_void_p, c_void_p]),
     "yolox_train_pack": (c_int, [c_void_p] * 2 + [c_int] * 3 + [c_void_p, c_void_p]),
+    "gdrn_ranger_plan": (c_int, [c_void_p, c_int, POINTER(ctypes.c_longlong), POINTER(ctypes.c_longlong)]),
+    "gdrn_ranger_workspace_bytes": (c_size_t, [ctypes.c_longlong]),
+    "gdrn_ranger_step": (c_int, [c_void_p, c_int, ctypes.c_longlong, ctypes.c_longlong, c_void_p, c_size_t, c_void_p]),
+    "gdrn_ema_plan": (c_int, [c_void_p, c_int, POINTER(ctypes.c_longlong)]),
+    "gdrn_ema_update": (c_int, [c_void_p, c_int, ctypes.c_longlong, c_float, c_float, c_void_p]),
 }
 
 EXPORTED_SYMBOLS = tuple(_SIGNATURES.keys())

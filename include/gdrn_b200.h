@@ -808,6 +808,60 @@ int yolox_train_hsv(uint8_t* pool, const long long* entries, const uint8_t* luts
 int yolox_train_preproc(const uint8_t* pool, const long long* info, int n, int oh, int ow, uint8_t* out, void* stream);
 int yolox_train_pack(const uint8_t* images, const int* transposed, int n, int oh, int ow, float* out, void* stream);
 
+/* ---------------------------------------------------------------------------------------------
+ * Parameter update of both trainers (csrc/train_step.cu): one step of Ranger (lib/torch_utils/solver/ranger.py: GC,
+ * RAdam, lookahead) over every parameter of a model in one launch, and the model EMA (det/yolox/utils/ema.py,
+ * lib/torch_utils/torch_utils.py ModelEMA) in one launch.  DESIGN.md §7s pins every rule.
+ *
+ * GdrnRangerParam: one fp32 parameter with a gradient, dense with dim 0 outermost; grad, exp_avg, exp_avg_sq and
+ *   slow_buffer have the parameter's strides.  The caller fills param .. row_len, flags and the scalars;
+ *   gdrn_ranger_plan fills unit_begin, mean_begin, units, rows_per_unit and path on the host.
+ *   row_len = numel / size(0) (the GC mean length).  flags: 1 gradient centralisation (grad is replaced in place by
+ *   grad - mean over each dim-0 slice), 2 state created this step (moments read as 0, slow_buffer = the parameter
+ *   before the update), 4 weight decay (p += neg_wd_lr * p first), 8 adaptive branch (p += neg_step_lr * exp_avg /
+ *   (sqrt(exp_avg_sq) + eps); else p += neg_step_lr * exp_avg), 16 lookahead (slow += alpha (p - slow); p = slow).
+ * gdrn_ranger_plan: host only.  n_units = the update grid; n_long_rows = the dim-0 slices longer than the on-chip bound
+ *   (their means come from a separate fixed-order pass into the workspace).
+ * gdrn_ranger_workspace_bytes(n_long_rows): workspace of gdrn_ranger_step.
+ * gdrn_ranger_step: params = the planned table in DEVICE memory.  One launch, two with long rows.  Results do not
+ *   depend on the launch order of CTAs.
+ * GdrnEmaEntry / gdrn_ema_plan / gdrn_ema_update: ema = fl(fl(ema * decay) + fl(one_minus_decay * model)) per element,
+ *   no FMA, over every entry of the DEVICE table (ema and model of equal numel and strides, dense); one launch.
+ * ------------------------------------------------------------------------------------------- */
+typedef struct GdrnRangerParam {
+  float* param;
+  float* grad;
+  float* exp_avg;
+  float* exp_avg_sq;
+  float* slow_buffer;
+  long long numel;
+  long long row_len;
+  long long unit_begin;
+  long long mean_begin;
+  int units;
+  int flags;
+  float beta1, one_minus_beta1, beta2, one_minus_beta2;
+  float neg_step_lr, neg_wd_lr, eps, alpha;
+  int rows_per_unit;
+  int path;
+  long long reserved;
+} GdrnRangerParam; /* 128 bytes */
+
+typedef struct GdrnEmaEntry {
+  float* ema;
+  const float* model;
+  long long numel;
+  long long unit_begin;
+} GdrnEmaEntry; /* 32 bytes */
+
+int gdrn_ranger_plan(GdrnRangerParam* params, int n, long long* n_units, long long* n_long_rows);
+size_t gdrn_ranger_workspace_bytes(long long n_long_rows);
+int gdrn_ranger_step(const GdrnRangerParam* params, int n, long long n_units, long long n_long_rows, void* workspace,
+                     size_t workspace_bytes, void* stream);
+int gdrn_ema_plan(GdrnEmaEntry* entries, int n, long long* n_units);
+int gdrn_ema_update(const GdrnEmaEntry* entries, int n, long long n_units, float decay, float one_minus_decay,
+                    void* stream);
+
 #ifdef __cplusplus
 }
 #endif
