@@ -5,9 +5,6 @@ of bench.py's B = 64 forward, with the tile widths the forward picks for them.
   python bench_gemm_x3.py [--reps R]    CUDA-event time per call (L2 flushed before each call: the forward reads A from
                                         HBM), algorithmic (2MNK) and executed (3 products) TFLOP/s, card name, power limit
                                         and the SM clock sampled while each shape runs
-  python bench_gemm_x3.py --trace       the kernel's cycle accounting of CTA 0 per shape (GDRN_GEMM_TRACE): producer
-                                        empty-wait, consumer full-wait, accumulator hand-over.  Run it on its own: the
-                                        traced calls synchronise and time nothing.
 
 The conv GEMMs (head 3x3, deconv, Patch-PnP) have no stand-alone entry; bench.py's roofline.gemm_ms_per_step covers them.
 Prints one JSON line at the end.
@@ -65,10 +62,7 @@ def make_operands(M, N, K, epi, dev):
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--reps", type=int, default=30, help="timed calls per shape (median reported)")
-    ap.add_argument("--trace", action="store_true", help="print the kernel's cycle accounting instead of timing")
     args = ap.parse_args()
-    if args.trace:
-        os.environ["GDRN_GEMM_TRACE"] = "1"   # read once, at the first gdrn_gemm_x3 call
     import torch
 
     from bench import ClockSampler
@@ -90,12 +84,6 @@ def main():
             L.check(lib.gdrn_gemm_x3(L.ptr(A), L.ptr(W), L.ptr(bias), L.ptr(gamma), L.ptr(out), L.ptr(out), M, N, K, epi, bn,
                                      L.current_stream()), "gemm_x3")
 
-        if args.trace:
-            for _ in range(3):   # the first call loads the module; the last two show the steady state
-                sys.stderr.write("%s: " % name)
-                sys.stderr.flush()
-                call()
-            continue
         # warm up for half a second: it settles the clock and lets nvidia-smi deliver its first samples
         sampler = ClockSampler(0)
         sampler.start()
@@ -124,9 +112,8 @@ def main():
         records.append(rec)
         print(json.dumps(rec), flush=True)
         del A, W, bias, gamma, out
-    if not args.trace:
-        total_us = sum(r["us_median"] for r in records)
-        print(json.dumps({"bench": "gemm_x3", **info, "total_us": round(total_us, 1), "shapes": records}))
+    total_us = sum(r["us_median"] for r in records)
+    print(json.dumps({"bench": "gemm_x3", **info, "total_us": round(total_us, 1), "shapes": records}))
 
 
 if __name__ == "__main__":

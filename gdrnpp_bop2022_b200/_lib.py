@@ -51,7 +51,6 @@ _SIGNATURES = {
     "gdrn_mlp_fused_x3": (c_int, [c_void_p] * 7 + [ctypes.c_longlong, c_int, c_void_p]),
     "gdrn_dwconv_ln": (c_int, [c_void_p] * 6 + [c_int] * 4 + [c_float, c_int, c_int, c_void_p]),
     "gdrn_gemm_x3": (c_int, [c_void_p] * 6 + [c_int] * 5 + [c_void_p]),
-    "gdrn_gemm_x3_ksplit": (c_int, [c_void_p] * 5 + [c_int] * 4 + [c_void_p, c_int, c_void_p]),
     "farthest_point_sampling": (None, [c_void_p, c_void_p, c_int, c_int]),
     "farthest_point_sampling_init_center": (None, [c_void_p, c_void_p, c_int, c_int]),
     "gdrn_fps_set_seed": (None, [c_uint]),

@@ -1,10 +1,9 @@
 // Error channel, version, and the exported plain-GEMM entry (tests + roofline measurement).
+#include <stdio.h>
 #include <stdlib.h>
 #include <string.h>
 #include <atomic>
 
-#include <stdio.h>
-#include <stdlib.h>
 #include "common.cuh"
 #include "dense_ops.h"
 #include "gemm_tc.h"
@@ -49,23 +48,7 @@ extern "C" int gdrn_gemm_bf16(const void* A, const void* W, const float* bias, c
   p.bias = bias;
   p.gamma = gamma;
   p.resid = resid;
-  static int trace_on = -1;
-  if (trace_on < 0) trace_on = getenv("GDRN_GEMM_TRACE") ? 1 : 0;
-  if (!trace_on) return gemm_tc_launch(p, block_n, (cudaStream_t)stream);
-  // debug: cycle accounting of CTA 0, printed to stderr (synchronises the stream)
-  static long long* d_trace = nullptr;
-  if (!d_trace) GDRN_CHECK_CUDA(cudaMalloc(&d_trace, 16 * sizeof(long long)));
-  GDRN_CHECK_CUDA(cudaMemsetAsync(d_trace, 0, 16 * sizeof(long long), (cudaStream_t)stream));
-  p.trace = d_trace;
-  int rc = gemm_tc_launch(p, block_n, (cudaStream_t)stream);
-  if (rc != GDRN_OK) return rc;
-  long long h[16];
-  GDRN_CHECK_CUDA(cudaMemcpyAsync(h, d_trace, sizeof(h), cudaMemcpyDeviceToHost, (cudaStream_t)stream));
-  GDRN_CHECK_CUDA(cudaStreamSynchronize((cudaStream_t)stream));
-  fprintf(stderr, "[gemm trace] M=%lld N=%d K=%d epi=%d bn=%d: cta0 cycles=%lld tiles=%lld | producer empty-wait=%lld | "
-                  "consumer full-wait=%lld acc hand-over=%lld | epi0 acc-ld=%lld compute=%lld flush=%lld\n",
-          (long long)M, N, K, epi, block_n, h[6], h[7], h[0], h[1], h[3], h[8], h[9], h[10]);
-  return GDRN_OK;
+  return gemm_tc_launch(p, block_n, (cudaStream_t)stream);
 }
 
 extern "C" int gdrn_mlp_fused_x3(const void* A, const void* W1, const float* b1, const void* W2, const float* b2,
@@ -75,21 +58,14 @@ extern "C" int gdrn_mlp_fused_x3(const void* A, const void* W1, const float* b1,
 }
 
 extern "C" int gdrn_gemm_x3(const void* A, const void* W, const float* bias, const float* gamma, const float* resid,
-                            void* out, int M, int N, int K, int epi, int block_n, void* stream);
-
-extern "C" int gdrn_gemm_x3_ksplit(const void* A, const void* W, const float* bias, const float* gamma, float* x, int M, int N,
-                                   int K, int block_n, unsigned* flags, int flag_words, void* stream) {
-  GDRN_REQUIRE(flags != nullptr && flag_words > 0, "gemm_x3_ksplit: flags must be a zeroed device buffer");
-  return gdrn_gemm_x3(A, W, bias, gamma, x, x, M, N, K, EPI_RESID, block_n, stream);
-}
-
-extern "C" int gdrn_gemm_x3(const void* A, const void* W, const float* bias, const float* gamma, const float* resid,
                             void* out, int M, int N, int K, int epi, int block_n, void* stream) {
   GDRN_REQUIRE(M > 0 && N > 0 && K > 0, "gemm_x3: empty problem");
   GDRN_REQUIRE(K % 64 == 0, "gemm_x3: K must be a multiple of 64 (the lo half starts at a k-chunk boundary)");
   GDRN_REQUIRE(epi >= 0 && epi <= 2, "gemm_x3: epi must be 0 (store fp32), 1 (gelu -> split bf16) or 2 (resid)");
   GDRN_REQUIRE(block_n == 64 || block_n == 128 || block_n == 256, "gemm_x3: block_n must be 64, 128 or 256");
   GDRN_REQUIRE(N % 64 == 0, "gemm_x3: N must be a multiple of 64");
+  GDRN_REQUIRE(epi != 1 || (uintptr_t)out % 16 == 0,
+               "gemm_x3: epi 1 needs a 16-byte aligned out (the split hi / lo rows leave through TMA stores)");
   GemmPlan p;
   memset(&p, 0, sizeof(p));
   p.a_ptr = A; p.a_dims[0] = 2ULL * K; p.a_dims[1] = M; p.a_str[0] = 4ULL * K; p.a_box[1] = 128; p.a_k = K;
@@ -104,30 +80,12 @@ extern "C" int gdrn_gemm_x3(const void* A, const void* W, const float* bias, con
   p.epi = epi;
   p.out_f32 = epi == 1 ? 0 : 1;
   p.gelu_mode = 3;
-  if (const char* e = getenv("GDRN_X3_GELU_MODE")) p.gelu_mode = atoi(e);   // 4 = libm erff (A/B experiments)
   p.split = 1; p.x3_a_lo = K; p.x3_b_lo = K;
   p.out = out;
   p.ldo = epi == 1 ? 2LL * N : N;
   p.bias = bias;
   p.gamma = gamma;
   p.resid = resid;
-  static int trace_on = -1;
-  if (trace_on < 0) trace_on = getenv("GDRN_GEMM_TRACE") ? 1 : 0;
-  if (trace_on) {
-    static long long* d_trace = nullptr;
-    if (!d_trace) GDRN_CHECK_CUDA(cudaMalloc(&d_trace, 16 * sizeof(long long)));
-    GDRN_CHECK_CUDA(cudaMemsetAsync(d_trace, 0, 16 * sizeof(long long), (cudaStream_t)stream));
-    p.trace = d_trace;
-    int rc = gemm_tc_launch(p, block_n, (cudaStream_t)stream);
-    if (rc != GDRN_OK) return rc;
-    long long h[16];
-    GDRN_CHECK_CUDA(cudaMemcpyAsync(h, d_trace, sizeof(h), cudaMemcpyDeviceToHost, (cudaStream_t)stream));
-    GDRN_CHECK_CUDA(cudaStreamSynchronize((cudaStream_t)stream));
-    fprintf(stderr, "[gemm x3 trace] M=%d N=%d K=%d epi=%d bn=%d: cta0 cycles=%lld tiles=%lld | producer empty-wait=%lld | "
-                    "consumer full-wait=%lld acc hand-over=%lld | epi0 acc-ld=%lld compute=%lld flush=%lld\n",
-            M, N, K, epi, block_n, h[6], h[7], h[0], h[1], h[3], h[8], h[9], h[10]);
-    return GDRN_OK;
-  }
   return gemm_tc_launch(p, block_n, (cudaStream_t)stream);
 }
 

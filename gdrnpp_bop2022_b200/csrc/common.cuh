@@ -311,7 +311,8 @@ __device__ __forceinline__ uint64_t make_sw64_kmajor_desc(uint32_t smem_addr) {
 //   12 FMA-pipe instructions.  Max abs error of the GELU against the fp64 erf form over [-12, 12]: 4.2e-7
 //   (tools/check_erf.py; torch's own fp32 GELU: 1.2e-6), and no cancellation for x < 0 (h is used directly).
 // CUDA's erff() costs ~25 FMA-pipe instructions and takes a data-dependent branch; the fc1 epilogue of the split-bf16
-// mode is FMA-pipe / issue bound (GDRN_GEMM_TRACE: ~30 instructions per element), so the instruction count is what matters.
+// mode is FMA-pipe / issue bound (~30 instructions per element, from cycle counts of its warps), so the instruction count
+// is what matters.
 __device__ __forceinline__ float gelu_erf(float x) {
   const float z = fabsf(x) * 0.70710678118654752440f;
   float t;

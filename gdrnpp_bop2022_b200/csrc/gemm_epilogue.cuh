@@ -108,7 +108,7 @@ __device__ __forceinline__ void load_vec(const float* __restrict__ src, int col,
 
 // The accumulator tile lives in shared memory, [BLOCK_M][acc_pitch] fp32 at the 1024-aligned start of the GEMM kernel's
 // dynamic shared memory (gemm_tc.cu writes it from the wgmma register fragments).  Epilogues address it as
-// (row << 16) | column (the tmem_* names below); lane l of a warp reads row `row + l`, CH consecutive columns.
+// (row << 16) | column (the acc_* arguments below); lane l of a warp reads row `row + l`, CH consecutive columns.
 // Widths that are multiples of 32 keep dense rows and XOR-swizzle the 16-byte column groups by (row & 7), the others
 // pad each row by 16 bytes: either way the 16-byte row reads of 8 consecutive lanes hit distinct banks.
 template <int BLOCK_N>
@@ -138,7 +138,7 @@ __device__ __forceinline__ void acc_load_chunk(uint32_t aaddr, float (&v)[CH]) {
 // Epilogues.  Each of the 128 epilogue threads owns one accumulator row.
 // ------------------------------------------------------------------------------------------------
 template <int BLOCK_N, int EPI>
-__device__ __forceinline__ void epilogue_tile(const GemmPlan& p, int m_tile, int n_tile, uint32_t tmem_row, int lane,
+__device__ __forceinline__ void epilogue_tile(const GemmPlan& p, int m_tile, int n_tile, uint32_t acc_row, int lane,
                                               uint8_t* stg) {
   constexpr int CH = BLOCK_N >= 32 ? 32 : 16;
   const int r = ((threadIdx.x >> 5) & 3) * 32 + lane;
@@ -149,7 +149,7 @@ __device__ __forceinline__ void epilogue_tile(const GemmPlan& p, int m_tile, int
 #pragma unroll 1
     for (int c = 0; c < BLOCK_N; c += CH) {
       float v[CH];
-      acc_load_chunk<BLOCK_N, CH>(tmem_row + c, v);
+      acc_load_chunk<BLOCK_N, CH>(acc_row + c, v);
       const int col = n0 + c;
       if (!ri.valid || col >= p.N) continue;
       float bias[CH];
@@ -181,7 +181,7 @@ __device__ __forceinline__ void epilogue_tile(const GemmPlan& p, int m_tile, int
 #pragma unroll 1
     for (int c = 0; c < BLOCK_N; c += CH) {
       float v[CH];
-      acc_load_chunk<BLOCK_N, CH>(tmem_row + c, v);
+      acc_load_chunk<BLOCK_N, CH>(acc_row + c, v);
       const int col = n0 + c;
       if (col >= p.N) continue;
       if (ri.valid) store_row_chunk<CH>(p, ri, col, v, p.out_f32 != 0);
@@ -228,7 +228,7 @@ __device__ __forceinline__ void epilogue_tile(const GemmPlan& p, int m_tile, int
 #pragma unroll 1
     for (int c = 0; c < p.N; c += CH) {
       float v[CH], bias[CH];
-      acc_load_chunk<BLOCK_N, CH>(tmem_row + c, v);
+      acc_load_chunk<BLOCK_N, CH>(acc_row + c, v);
       load_vec<CH>(p.bias, c, p.N, bias);
 #pragma unroll
       for (int j = 0; j < CH; ++j) sum += v[j] + bias[j];
@@ -241,7 +241,7 @@ __device__ __forceinline__ void epilogue_tile(const GemmPlan& p, int m_tile, int
 #pragma unroll 1
     for (int c = 0; c < p.N; c += CH) {
       float v[CH], bias[CH];
-      acc_load_chunk<BLOCK_N, CH>(tmem_row + c, v);
+      acc_load_chunk<BLOCK_N, CH>(acc_row + c, v);
       load_vec<CH>(p.bias, c, p.N, bias);
 #pragma unroll
       for (int j = 0; j < CH; ++j) { const float d = c + j < ln_n ? v[j] + bias[j] - mean : 0.f; sq = fmaf(d, d, sq); }
@@ -250,7 +250,7 @@ __device__ __forceinline__ void epilogue_tile(const GemmPlan& p, int m_tile, int
 #pragma unroll 1
     for (int c = 0; c < p.N; c += CH) {
       float v[CH], bias[CH], w[CH], bb[CH];
-      acc_load_chunk<BLOCK_N, CH>(tmem_row + c, v);
+      acc_load_chunk<BLOCK_N, CH>(acc_row + c, v);
       load_vec<CH>(p.bias, c, p.N, bias);
       load_vec<CH>(p.ln_w, c, p.N, w);
       load_vec<CH>(p.ln_b, c, p.N, bb);
@@ -283,14 +283,14 @@ __device__ __forceinline__ void epilogue_tile(const GemmPlan& p, int m_tile, int
     float v[80];
     {
       float t[32];
-      acc_load_chunk<BLOCK_N, 32>(tmem_row, t);
+      acc_load_chunk<BLOCK_N, 32>(acc_row, t);
 #pragma unroll
       for (int j = 0; j < 32; ++j) v[j] = t[j];
-      acc_load_chunk<BLOCK_N, 32>(tmem_row + 32, t);
+      acc_load_chunk<BLOCK_N, 32>(acc_row + 32, t);
 #pragma unroll
       for (int j = 0; j < 32; ++j) v[32 + j] = t[j];
       float t16[16];
-      acc_load_chunk<BLOCK_N, 16>(tmem_row + 64, t16);
+      acc_load_chunk<BLOCK_N, 16>(acc_row + 64, t16);
 #pragma unroll
       for (int j = 0; j < 16; ++j) v[64 + j] = t16[j];
     }
@@ -393,7 +393,7 @@ __device__ __forceinline__ float gelu_tanh_f32(float x) {
 // first read) with 16-byte accesses in which 4 lanes cover one row segment: every warp-wide access touches
 // eight full 64-byte runs (16 whole sectors) instead of 32 scattered 16-byte pieces.
 template <int BLOCK_N, int EPI, bool F32>
-__device__ __forceinline__ void epilogue_tile_staged_t(const GemmPlan& p, int m_tile, int n_tile, uint32_t tmem_acc,
+__device__ __forceinline__ void epilogue_tile_staged_t(const GemmPlan& p, int m_tile, int n_tile, uint32_t acc_base,
                                                        int ew, int lane, uint8_t* stg) {
   static_assert(BLOCK_N >= 64, "staged epilogue needs BLOCK_N >= 64");
   constexpr int CPW = BLOCK_N / 2;      // columns per warp
@@ -407,12 +407,10 @@ __device__ __forceinline__ void epilogue_tile_staged_t(const GemmPlan& p, int m_
   s_orow[lane] = ri.valid ? ri.orow : -1;
   __syncwarp();
   const int n0 = n_tile * BLOCK_N + half * CPW;
-  const uint32_t tmem_row = tmem_acc + ((uint32_t)(q * 32) << 16) + half * CPW;
+  const uint32_t acc_row = acc_base + ((uint32_t)(q * 32) << 16) + half * CPW;
   uint8_t* my_row = stg + lane * EPI_STAGE_PITCH;
   const int cpg = p.gn_cpg;
   const int fl_row = lane >> 2, fl_piece = lane & 3;  // flush / prefetch mapping: 8 rows x 4 pieces per pass
-  const bool trc = (p.trace != nullptr) && blockIdx.x == 0 && ew == 0;
-  long long tq_tmem = 0, tq_comp = 0, tq_flush = 0;
   uint4 rres[4];
   if constexpr (EPI == EPI_RESID) {
     if (n0 < p.N) {
@@ -445,9 +443,7 @@ __device__ __forceinline__ void epilogue_tile_staged_t(const GemmPlan& p, int m_
       __syncwarp();
     }
     float v[CH];
-    long long tq0 = trc ? clock64() : 0;
-    acc_load_chunk<BLOCK_N, CH>(tmem_row + c, v);
-    if (trc) { const long long t = clock64(); tq_tmem += t - tq0; tq0 = t; }
+    acc_load_chunk<BLOCK_N, CH>(acc_row + c, v);
     if constexpr (EPI == EPI_STORE || EPI == EPI_GELU) {
       const float4* sb = reinterpret_cast<const float4*>(s_bias + c);  // warp-wide broadcast reads
 #pragma unroll
@@ -478,7 +474,6 @@ __device__ __forceinline__ void epilogue_tile_staged_t(const GemmPlan& p, int m_
       }
     }
     // ---- registers -> staging row ----
-    float lo[F32 ? 1 : CH];  // split mode: residual of the bf16 rounding, written in a second round
     if constexpr (F32) {
       float4* dst = reinterpret_cast<float4*>(my_row);
 #pragma unroll
@@ -506,26 +501,12 @@ __device__ __forceinline__ void epilogue_tile_staged_t(const GemmPlan& p, int m_
             for (int j = 0; j < CH; ++j) v[j] = gelu_fast(v[j]);
           }
         }
-        if (p.split) {  // hi must be exactly the cvt.rn value the lo halves are computed against
 #pragma unroll
-          for (int j = 0; j < CH; j += 8) {
-            uint4 w;
-            w.x = pack_bf16(v[j], v[j + 1]); w.y = pack_bf16(v[j + 2], v[j + 3]);
-            w.z = pack_bf16(v[j + 4], v[j + 5]); w.w = pack_bf16(v[j + 6], v[j + 7]);
-            dst[j >> 3] = w;
-          }
-        } else {
-#pragma unroll
-          for (int j = 0; j < CH; j += 8) {
-            uint4 w;
-            w.x = pack_bf16(v[j], v[j + 1]); w.y = pack_bf16(v[j + 2], v[j + 3]);
-            w.z = pack_bf16(v[j + 4], v[j + 5]); w.w = pack_bf16(v[j + 6], v[j + 7]);
-            dst[j >> 3] = w;
-          }
-        }
-        if (p.split) {
-#pragma unroll
-          for (int j = 0; j < CH; ++j) lo[j] = v[j] - __bfloat162float(__float2bfloat16(v[j]));
+        for (int j = 0; j < CH; j += 8) {
+          uint4 w;
+          w.x = pack_bf16(v[j], v[j + 1]); w.y = pack_bf16(v[j + 2], v[j + 3]);
+          w.z = pack_bf16(v[j + 4], v[j + 5]); w.w = pack_bf16(v[j + 6], v[j + 7]);
+          dst[j >> 3] = w;
         }
       }
     }
@@ -569,7 +550,6 @@ __device__ __forceinline__ void epilogue_tile_staged_t(const GemmPlan& p, int m_
       }
     }
     __syncwarp();
-    if (trc) { const long long t = clock64(); tq_comp += t - tq0; tq0 = t; }
     // ---- coalesced flush of the 32 row segments ----
 #pragma unroll
     for (int pass = 0; pass < 32; pass += 8) {
@@ -580,31 +560,7 @@ __device__ __forceinline__ void epilogue_tile_staged_t(const GemmPlan& p, int m_
             *reinterpret_cast<const uint4*>(stg + rr * EPI_STAGE_PITCH + fl_piece * 16);
     }
     __syncwarp();
-    if (trc) { const long long t = clock64(); tq_flush += t - tq0; tq0 = t; }
-    if constexpr (!F32) {
-      if (p.split) {  // second round: the lo halves go to columns [N + col, ...)
-        uint4* dst = reinterpret_cast<uint4*>(my_row);
-#pragma unroll
-        for (int j = 0; j < CH; j += 8) {
-          uint4 w;
-          w.x = pack_bf16(lo[j], lo[j + 1]); w.y = pack_bf16(lo[j + 2], lo[j + 3]);
-          w.z = pack_bf16(lo[j + 4], lo[j + 5]); w.w = pack_bf16(lo[j + 6], lo[j + 7]);
-          dst[j >> 3] = w;
-        }
-        __syncwarp();
-#pragma unroll
-        for (int pass = 0; pass < 32; pass += 8) {
-          const int rr = pass + fl_row;
-          const long long orow = s_orow[rr];
-          if (orow >= 0)
-            *reinterpret_cast<uint4*>(reinterpret_cast<uint8_t*>(p.out) + (orow * p.ldo + p.N + col) * ESZ + fl_piece * 16) =
-                *reinterpret_cast<const uint4*>(stg + rr * EPI_STAGE_PITCH + fl_piece * 16);
-        }
-        __syncwarp();
-      }
-    }
   }
-  if (trc && lane == 0) { p.trace[8] += tq_tmem; p.trace[9] += tq_comp; p.trace[10] += tq_flush; }
 }
 
 
@@ -615,37 +571,30 @@ __device__ __forceinline__ void epilogue_tile_staged_t(const GemmPlan& p, int m_
 // issues a single cp.async.bulk.tensor store per tile.  No address arithmetic, LDS or STG in the flush; rows beyond
 // M are clipped by the tensor map.  The residual of EPI_RESID is read by its owner thread (64 contiguous bytes per
 // half, register-prefetched one half ahead).
-template <int BLOCK_N, int EPI, bool F32, int NEW = NUM_EPI_WARPS>
-__device__ __forceinline__ void epilogue_tile_tma(const GemmPlan& p, int m_tile, int n_tile, uint32_t tmem_acc, int ew,
-                                                  int lane, uint8_t* stg, int g_begin = 0, int g_end = 1 << 30,
-                                                  bool use_bias = true) {
-  // use_bias = false: a k-split PART of a tile that does not contain k = 0 (the bias travels with the k = 0 part)
-  // [g_begin, g_end): sub-range of this warp's columns (multiples of GW) -- lets a caller interleave the 128-byte groups
-  // of a tile with other work so that the wait for the previous TMA store never blocks (fused MLP kernel)
+template <int BLOCK_N, int EPI, bool F32>
+__device__ __forceinline__ void epilogue_tile_tma(const GemmPlan& p, int m_tile, int n_tile, uint32_t acc_base, int ew,
+                                                  int lane, uint8_t* stg) {
   static_assert(BLOCK_N >= 128, "TMA-store epilogue needs BLOCK_N >= 128");
-  constexpr int CPW = BLOCK_N / (NEW / 4);  // columns per warp (NEW / 4 warps share one quarter of the rows)
-  static_assert(CPW * (F32 ? 4 : 2) >= 128, "a warp must own at least one 128-byte row segment");
+  constexpr int CPW = BLOCK_N / 2;      // columns per warp
   constexpr int CH = F32 ? 16 : 32;     // columns per 64-byte half row
   constexpr int GW = 2 * CH;            // columns per staged 128-byte row (one TMA store)
   const int q = ew & 3, half = ew >> 2;
   const long long grow = (long long)m_tile * BLOCK_M + q * 32 + lane;
   const bool rvalid = grow < p.M;
   const int n0 = n_tile * BLOCK_N + half * CPW;
-  const uint32_t tmem_row = tmem_acc + ((uint32_t)(q * 32) << 16) + half * CPW;
+  const uint32_t acc_row = acc_base + ((uint32_t)(q * 32) << 16) + half * CPW;
   const uint32_t stg_u32 = ptx::smem_u32(stg);
   uint8_t* my_row = stg + lane * 128;
   const int sw = lane & 7;
-  const bool trc = (p.trace != nullptr) && blockIdx.x == 0 && ew == 0;
-  long long tq_tmem = 0, tq_comp = 0, tq_flush = 0;
 
   uint4 rres[4];
   const float* rrow = nullptr;
   const bool red = (EPI == EPI_RESID) && p.resid_reduce;  // launch-uniform: out += gamma*(acc+bias) by TMA reduce-add
   if constexpr (EPI == EPI_RESID) {
     rrow = p.resid + grow * p.ldo + n0;
-    if (rvalid && n0 + g_begin < p.N && !red) {
+    if (rvalid && n0 < p.N && !red) {
 #pragma unroll
-      for (int k = 0; k < 4; ++k) rres[k] = *reinterpret_cast<const uint4*>(rrow + g_begin + 4 * k);
+      for (int k = 0; k < 4; ++k) rres[k] = *reinterpret_cast<const uint4*>(rrow + 4 * k);
     } else {
 #pragma unroll
       for (int k = 0; k < 4; ++k) rres[k] = make_uint4(0, 0, 0, 0);
@@ -653,22 +602,20 @@ __device__ __forceinline__ void epilogue_tile_tma(const GemmPlan& p, int m_tile,
   }
 
 #pragma unroll 1
-  for (int g = g_begin; g < CPW && g < g_end; g += GW) {
+  for (int g = 0; g < CPW; g += GW) {
     const int gcol = n0 + g;
     if (gcol >= p.N) break;  // warp-uniform
-    long long tq0 = trc ? clock64() : 0;
     // the previous store of this warp must have finished reading the staging tile
     if (lane == 0) ptx::bulk_wait_read0();
     __syncwarp();
-    if (trc) { const long long t = clock64(); tq_flush += t - tq0; tq0 = t; }
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
       const int c = g + h * CH;
       const int col = n0 + c;
-      // bias is read four columns at a time right where it is consumed (keeps the live register set small
-      // enough for the 16-warp epilogue variant); the loads are warp-uniform L1 hits
+      // bias is read four columns at a time right where it is consumed (keeps the live register set small); the loads
+      // are warp-uniform L1 hits
       auto bias4 = [&](int j) {
-        return (p.bias && use_bias) ? __ldg(reinterpret_cast<const float4*>(p.bias + col + j)) : make_float4(0.f, 0.f, 0.f, 0.f);
+        return p.bias ? __ldg(reinterpret_cast<const float4*>(p.bias + col + j)) : make_float4(0.f, 0.f, 0.f, 0.f);
       };
       float x[EPI == EPI_RESID ? CH : 1], gm[EPI == EPI_RESID ? CH : 1];
       if constexpr (EPI == EPI_RESID) {
@@ -686,9 +633,7 @@ __device__ __forceinline__ void epilogue_tile_tma(const GemmPlan& p, int m_tile,
         }
       }
       float v[CH];
-      long long tq1 = trc ? clock64() : 0;
-      acc_load_chunk<BLOCK_N, CH>(tmem_row + c, v);
-      if (trc) { const long long t = clock64(); tq_tmem += t - tq1; }
+      acc_load_chunk<BLOCK_N, CH>(acc_row + c, v);
       uint4* dst = reinterpret_cast<uint4*>(my_row);
       if constexpr (F32) {
         if constexpr (EPI == EPI_RESID) {
@@ -749,7 +694,6 @@ __device__ __forceinline__ void epilogue_tile_tma(const GemmPlan& p, int m_tile,
         }
       }
     }
-    if (trc) { const long long t = clock64(); tq_comp += t - tq0; tq0 = t; }
     ptx::fence_proxy_async();  // generic-proxy smem writes -> visible to the TMA (async proxy)
     __syncwarp();
     if (lane == 0) {
@@ -757,9 +701,7 @@ __device__ __forceinline__ void epilogue_tile_tma(const GemmPlan& p, int m_tile,
       else ptx::tma_store_2d(&p.tmap_out, stg_u32, gcol, m_tile * BLOCK_M + q * 32);
       ptx::bulk_commit();
     }
-    if (trc) { const long long t = clock64(); tq_flush += t - tq0; }
   }
-  if (trc && lane == 0) { p.trace[8] += tq_tmem; p.trace[9] += tq_comp; p.trace[10] += tq_flush; }
 }
 
 // Epilogues straight from the wgmma accumulator fragments: split-bf16 rank-2 GEMMs with EPI_STORE (fp32 out), EPI_GELU
@@ -817,21 +759,8 @@ __device__ __forceinline__ void epilogue_regs(const GemmPlan& p, int m_tile, int
           v2[2 * jj + 1] = f2_add(v2[2 * jj + 1], f2_pack(b.x, b.y));
         }
       }
-      if (p.gelu_mode == 3) {
 #pragma unroll
-        for (int j = 0; j < 8; ++j) v2[j] = gelu_erf2(v2[j]);
-      } else {                         // A/B knobs: 5 = scalar A&S form, 4 = libm erff, else the bf16-mode fit
-#pragma unroll
-        for (int j = 0; j < 8; ++j) {
-          float2 f = f2_unpack(v2[j]);
-          if (p.gelu_mode == 5) { f.x = gelu_erf(f.x); f.y = gelu_erf(f.y); }
-          else if (p.gelu_mode == 4) {
-            f.x = 0.5f * f.x * (1.0f + erff(f.x * 0.70710678118654752440f));
-            f.y = 0.5f * f.y * (1.0f + erff(f.y * 0.70710678118654752440f));
-          } else { f.x = gelu_fast(f.x); f.y = gelu_fast(f.y); }
-          v2[j] = f2_pack(f.x, f.y);
-        }
-      }
+      for (int j = 0; j < 8; ++j) v2[j] = gelu_erf2(v2[j]);
       uint32_t hi[8], lo[8];
 #pragma unroll
       for (int j = 0; j < 8; ++j) {
@@ -886,28 +815,28 @@ __device__ __forceinline__ void epilogue_regs(const GemmPlan& p, int m_tile, int
 }
 
 template <int BLOCK_N, int EPI>
-__device__ __forceinline__ void epilogue_tile_staged(const GemmPlan& p, int m_tile, int n_tile, uint32_t tmem_acc,
+__device__ __forceinline__ void epilogue_tile_staged(const GemmPlan& p, int m_tile, int n_tile, uint32_t acc_base,
                                                      int ew, int lane, uint8_t* stg) {
   if constexpr (BLOCK_N >= 128 && (EPI == EPI_STORE || EPI == EPI_GELU || EPI == EPI_RESID)) {
     if (p.use_tma_store) {  // launch-uniform
       if constexpr (EPI == EPI_RESID) {
-        epilogue_tile_tma<BLOCK_N, EPI, true>(p, m_tile, n_tile, tmem_acc, ew, lane, stg);
+        epilogue_tile_tma<BLOCK_N, EPI, true>(p, m_tile, n_tile, acc_base, ew, lane, stg);
       } else if constexpr (EPI == EPI_GELU) {
-        epilogue_tile_tma<BLOCK_N, EPI, false>(p, m_tile, n_tile, tmem_acc, ew, lane, stg);
+        epilogue_tile_tma<BLOCK_N, EPI, false>(p, m_tile, n_tile, acc_base, ew, lane, stg);
       } else {
-        if (p.out_f32) epilogue_tile_tma<BLOCK_N, EPI, true>(p, m_tile, n_tile, tmem_acc, ew, lane, stg);
-        else epilogue_tile_tma<BLOCK_N, EPI, false>(p, m_tile, n_tile, tmem_acc, ew, lane, stg);
+        if (p.out_f32) epilogue_tile_tma<BLOCK_N, EPI, true>(p, m_tile, n_tile, acc_base, ew, lane, stg);
+        else epilogue_tile_tma<BLOCK_N, EPI, false>(p, m_tile, n_tile, acc_base, ew, lane, stg);
       }
       return;
     }
   }
   if constexpr (EPI == EPI_RESID) {
-    epilogue_tile_staged_t<BLOCK_N, EPI, true>(p, m_tile, n_tile, tmem_acc, ew, lane, stg);
+    epilogue_tile_staged_t<BLOCK_N, EPI, true>(p, m_tile, n_tile, acc_base, ew, lane, stg);
   } else if constexpr (EPI == EPI_GELU) {
-    epilogue_tile_staged_t<BLOCK_N, EPI, false>(p, m_tile, n_tile, tmem_acc, ew, lane, stg);
+    epilogue_tile_staged_t<BLOCK_N, EPI, false>(p, m_tile, n_tile, acc_base, ew, lane, stg);
   } else {
-    if (p.out_f32) epilogue_tile_staged_t<BLOCK_N, EPI, true>(p, m_tile, n_tile, tmem_acc, ew, lane, stg);
-    else epilogue_tile_staged_t<BLOCK_N, EPI, false>(p, m_tile, n_tile, tmem_acc, ew, lane, stg);
+    if (p.out_f32) epilogue_tile_staged_t<BLOCK_N, EPI, true>(p, m_tile, n_tile, acc_base, ew, lane, stg);
+    else epilogue_tile_staged_t<BLOCK_N, EPI, false>(p, m_tile, n_tile, acc_base, ew, lane, stg);
   }
 }
 

@@ -17,8 +17,6 @@
 // head (heads/top_down_doublemask_xyz_region_head.py:177-211: ConvTranspose2d, six 3x3 convs, 1x1 out
 // conv) and by ConvPnPNet (heads/conv_pnp_net.py:120-183: three 3x3 s2 convs and four Linear layers).
 #include <stdio.h>
-#include <stdlib.h>
-#include <string.h>
 #include "gemm_tc.h"
 #include "gemm_epilogue.cuh"
 #include "wgmma.cuh"
@@ -98,10 +96,6 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) gemm_tc_kernel(const __grid_co
 
   const int total_tiles = p.m_tiles * p.n_tiles;
   const int k_iters = p.num_taps * p.k_chunks;
-  // optional cycle accounting of CTA 0 (GDRN_GEMM_TRACE, api_core.cu): who waits for whom
-  const bool tr = (p.trace != nullptr) && blockIdx.x == 0;
-  long long tr_acc0 = 0, tr_acc1 = 0, tr_epi = 0;
-  const long long tr_start = tr ? clock64() : 0;
 
   // REG: the consumers keep their accumulators live through the epilogue, so they take the registers the producer
   // warpgroup does not use (setmaxnreg is per warpgroup: warps 1..3 and lanes 1..31 of warp 0 lower theirs too)
@@ -112,8 +106,8 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) gemm_tc_kernel(const __grid_co
       int stage = 0;
       uint32_t phase = 0;
       for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
-        const int n_tile = p.n_major ? tile / p.m_tiles : tile % p.n_tiles;
-        const int m_tile = p.n_major ? tile % p.m_tiles : tile / p.n_tiles;
+        const int n_tile = tile % p.n_tiles;
+        const int m_tile = tile / p.n_tiles;
         int x0 = 0, y0 = 0, b0 = 0;
         if (p.a_rank != 2) {
           int tx = m_tile % p.tiles_x;
@@ -133,7 +127,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) gemm_tc_kernel(const __grid_co
         for (int tap = 0; tap < p.num_taps; ++tap) {
           const GemmTap tp = p.taps[tap];
           for (int kc = 0; kc < p.k_chunks; ++kc) {
-            { const long long t0 = tr ? clock64() : 0; ptx::mbar_wait_nocall(empty_bar(stage), phase ^ 1); if (tr) tr_acc0 += clock64() - t0; }
+            ptx::mbar_wait_nocall(empty_bar(stage), phase ^ 1);
             const uint32_t sa = ring_base + stage * C::STAGE_BYTES;
             const uint32_t sb = sa + C::A_BYTES;
             ptx::mbar_arrive_expect_tx(full_bar(stage), C::STAGE_BYTES);
@@ -158,7 +152,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) gemm_tc_kernel(const __grid_co
               if (pk >= p.k_chunks) {
                 pk -= p.k_chunks;
                 const int nt = tile + gridDim.x;
-                const int nm = p.n_major ? nt % p.m_tiles : nt / p.n_tiles;
+                const int nm = nt / p.n_tiles;
                 pm = (nt < total_tiles && nm != m_tile) ? nm : -1;
               }
               if (pm >= 0 && pk < p.k_chunks && p.num_taps == 1) ptx::tma_prefetch_2d(&p.tmap_a, pk * C::BLOCK_K, pm * BLOCK_M);
@@ -167,7 +161,6 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) gemm_tc_kernel(const __grid_co
           }
         }
       }
-      if (tr) { p.trace[0] = tr_acc0; p.trace[6] = clock64() - tr_start; p.trace[7] = (total_tiles - 1 - (int)blockIdx.x) / (int)gridDim.x + 1; }
     }
   } else {
     if constexpr (REG) ptx::setmaxnreg_inc<232>();
@@ -175,13 +168,12 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) gemm_tc_kernel(const __grid_co
     const int ew = warp - 4;
     const int wg = ew >> 2;             // rows [64 wg, 64 wg + 64) of the tile
     const int wl = ew & 3;              // warp inside the warpgroup
-    const bool tr_me = tr && ew == 0 && lane == 0;
     int stage = 0;
     uint32_t phase = 0;
     uint32_t sbuf = 0;  // REG, EPI_GELU: chunks this warp has TMA-stored (picks the half of its staging slot)
     for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
-      const int n_tile = p.n_major ? tile / p.m_tiles : tile % p.n_tiles;
-      const int m_tile = p.n_major ? tile % p.m_tiles : tile / p.n_tiles;
+      const int n_tile = tile % p.n_tiles;
+      const int m_tile = tile / p.n_tiles;
       float acc[BLOCK_N / 2];
 #pragma unroll
       for (int i = 0; i < BLOCK_N / 2; ++i) acc[i] = 0.f;
@@ -207,14 +199,14 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) gemm_tc_kernel(const __grid_co
             ptx::Wgmma<BLOCK_N>::mma(acc, ad, bd, accumulate);
             ptx::Wgmma<BLOCK_N>::mma(acc, ad + 2u, bd + 2u, 1u);
           };
-          { const long long t0 = tr_me ? clock64() : 0; ptx::mbar_wait_nocall(full_bar(s0), ph0); if (tr_me) tr_acc0 += clock64() - t0; }
+          ptx::mbar_wait_nocall(full_bar(s0), ph0);
           ptx::wgmma_fence();
           mma32(a0 + C::A_TILE_BYTES, b0, k != 0 ? 1u : 0u);                  // lo*hi, k [0, 32)
           ptx::wgmma_commit();
           // the previous k-step's last group has retired: release its second stage
           ptx::wgmma_wait<1>();
           if (prev_stage >= 0 && wl == 0 && lane == 0) ptx::mbar_arrive(empty_bar(prev_stage));
-          { const long long t0 = tr_me ? clock64() : 0; ptx::mbar_wait_nocall(full_bar(s1), ph1); if (tr_me) tr_acc0 += clock64() - t0; }
+          ptx::mbar_wait_nocall(full_bar(s1), ph1);
           ptx::wgmma_fence();
           mma32(a1 + C::A_TILE_BYTES, b1, 1u);                                // lo*hi, k [32, 64)
           mma32(a0, b0 + C::B_TILE_BYTES, 1u);                                // hi*lo, k [0, 32)
@@ -230,7 +222,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) gemm_tc_kernel(const __grid_co
         }
       } else {
         for (int k = 0; k < k_iters; ++k) {
-          { const long long t0 = tr_me ? clock64() : 0; ptx::mbar_wait_nocall(full_bar(stage), phase); if (tr_me) tr_acc0 += clock64() - t0; }
+          ptx::mbar_wait_nocall(full_bar(stage), phase);
           const uint32_t sa = ring_base + stage * C::STAGE_BYTES + wg * (C::A_TILE_BYTES / 2);
           const uint32_t sb = ring_base + stage * C::STAGE_BYTES + C::A_BYTES;
           ptx::wgmma_fence();
@@ -260,10 +252,8 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) gemm_tc_kernel(const __grid_co
       ptx::wgmma_wait<0>();
       if (prev_stage >= 0 && wl == 0 && lane == 0) ptx::mbar_arrive(empty_bar(prev_stage));
       if constexpr (REG) {
-        const long long t0 = tr_me ? clock64() : 0;
         epilogue_regs<BLOCK_N, EPI>(p, m_tile, n_tile, wg * 64 + wl * 16, lane, acc, xres, stage_base + ew * EPI_STAGE_BYTES,
                                     sbuf);
-        if (tr_me) tr_epi += clock64() - t0;
         continue;
       }
 
@@ -282,7 +272,6 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) gemm_tc_kernel(const __grid_co
         }
         __syncwarp();
       }
-      long long t0 = tr_me ? clock64() : 0;
       // the previous tile's epilogue has finished reading the accumulator tile
       ptx::named_bar_sync(BAR_ACC, CONSUMER_THREADS);
       {
@@ -295,7 +284,6 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) gemm_tc_kernel(const __grid_co
         }
       }
       ptx::named_bar_sync(BAR_ACC, CONSUMER_THREADS);
-      if (tr_me) { const long long t1 = clock64(); tr_acc1 += t1 - t0; }
       if constexpr (kStaged) {
         epilogue_tile_staged<BLOCK_N, EPI>(p, m_tile, n_tile, 0u, ew, lane, stage_base + ew * EPI_STAGE_BYTES);
       } else if (ew < 4) {
@@ -303,7 +291,6 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) gemm_tc_kernel(const __grid_co
         epilogue_tile<BLOCK_N, EPI>(p, m_tile, n_tile, acc_row, lane, stage_base + ew * EPI_STAGE_BYTES);
       }
     }
-    if (tr_me) { p.trace[1] = tr_acc0; p.trace[3] = tr_acc1; if (REG) p.trace[9] = tr_epi; }
     if (lane == 0) ptx::bulk_wait0();  // outstanding TMA stores (no-op when none were issued)
   }
 }
@@ -325,11 +312,6 @@ int launch_inst(const GemmPlan& plan, cudaStream_t stream) {
 
 int gemm_tc_launch(const GemmPlan& plan_in, int block_n, cudaStream_t stream) {
   GemmPlan plan = plan_in;
-  {  // experiment knob: GDRN_TILE_ORDER=0/1 forces the tile order of every multi-n-tile GEMM
-    static int order = -2;
-    if (order == -2) { const char* e = getenv("GDRN_TILE_ORDER"); order = e ? atoi(e) : -1; }
-    if (order >= 0) plan.n_major = order;
-  }
   GDRN_REQUIRE(plan.a_rank == 2 || plan.a_rank == 4 || plan.a_rank == 5, "gemm: bad a_rank");
   GDRN_REQUIRE(plan.a_ptr != nullptr && plan.b_ptr != nullptr && plan.a_k > 0, "gemm: plan without operands");
   plan.use_tma_store = 0;
@@ -340,12 +322,9 @@ int gemm_tc_launch(const GemmPlan& plan_in, int block_n, cudaStream_t stream) {
     plan.n_tiles = (plan.N + block_n - 1) / block_n;
   }
   // split-bf16 (x3): taps[] lists the hi operands.  64- / 128-wide tiles run the shared four-tile stage (X3 kernel); the
-  // other widths expand every tap to (A lo, W hi) + (A hi, W lo) + (A hi, W hi), small terms first.
-  static int x3_shared_on = -1;  // GDRN_X3_SHARED=0 forces the expanded tap list (A/B experiments)
-  if (x3_shared_on < 0) { const char* e = getenv("GDRN_X3_SHARED"); x3_shared_on = e ? atoi(e) : 1; }
-  const bool x3_shared = x3_shared_on && plan.split && !plan.x3_expanded && (block_n == 64 || block_n == 128) &&
-                         plan.epi != EPI_OUTCONV;
-  if (plan.split && !plan.x3_expanded && !x3_shared) {
+  // other widths (the 80-wide out-conv) expand every tap to (A lo, W hi) + (A hi, W lo) + (A hi, W hi), small terms first.
+  const bool x3_shared = plan.split && (block_n == 64 || block_n == 128) && plan.epi != EPI_OUTCONV;
+  if (plan.split && !x3_shared) {
     GDRN_REQUIRE(plan.num_taps >= 1 && 3 * plan.num_taps <= GEMM_MAX_TAPS, "gemm: bad num_taps (split)");
     const int n = plan.num_taps;
     for (int t = n - 1; t >= 0; --t) {
@@ -355,7 +334,6 @@ int gemm_tc_launch(const GemmPlan& plan_in, int block_n, cudaStream_t stream) {
       plan.taps[t] = al; plan.taps[n + t] = bl; plan.taps[2 * n + t] = h;
     }
     plan.num_taps = 3 * n;
-    plan.x3_expanded = 1;
   }
   // k-chunk width.  Split-bf16 convolutions (rank-4/5 pixel boxes, A re-read from L2 by every tap) run 32-wide chunks: the
   // deeper ring covers their L2 round trips.  Plain rank-2 rows keep 64-wide chunks: they stream A from HBM, where 128-byte
@@ -374,10 +352,10 @@ int gemm_tc_launch(const GemmPlan& plan_in, int block_n, cudaStream_t stream) {
     plan.k_chunks = (plan.a_k + bk - 1) / bk;
   }
   {
-    static int tma_epi = -1;  // GDRN_TMA_STORE=0 falls back to the gather-store epilogue (A/B experiments)
-    if (tma_epi < 0) { const char* e = getenv("GDRN_TMA_STORE"); tma_epi = e ? atoi(e) : 1; }
+    // bf16 rank-2 rows in 128-wide tiles leave through TMA stores when the output is aligned for them; an in-place
+    // residual becomes an L2 reduce-add (x is never read by the SM), an out-of-place one a read-modify-write
     const bool f32 = plan.epi == EPI_RESID || plan.epi == EPI_BIAS_LN || (plan.epi == EPI_STORE && plan.out_f32);
-    if (tma_epi && plan.a_rank == 2 && !plan.split && block_n >= 128 && plan.N % 64 == 0 &&
+    if (plan.a_rank == 2 && !plan.split && block_n >= 128 && plan.N % 64 == 0 &&
         (plan.epi == EPI_STORE || plan.epi == EPI_GELU || plan.epi == EPI_RESID || plan.epi == EPI_BIAS_LN) &&
         ((uintptr_t)plan.out % 16 == 0) && ((plan.ldo * (f32 ? 4 : 2)) % 16 == 0) &&
         (plan.epi != EPI_RESID || ((uintptr_t)plan.resid % 16 == 0))) {
@@ -387,19 +365,17 @@ int gemm_tc_launch(const GemmPlan& plan_in, int block_n, cudaStream_t stream) {
       int rc = make_tmap_store(&plan.tmap_out, plan.out, f32 ? 1 : 0, dims, str, box);
       if (rc != GDRN_OK) return rc;
       plan.use_tma_store = 1;
-      static int red = -1;  // GDRN_RESID_REDUCE=0: read-modify-write in the SM instead of the L2 reduce-add
-      if (red < 0) { const char* e = getenv("GDRN_RESID_REDUCE"); red = e ? atoi(e) : 1; }
-      plan.resid_reduce = (red && plan.epi == EPI_RESID && plan.resid == plan.out) ? 1 : 0;
+      plan.resid_reduce = (plan.epi == EPI_RESID && plan.resid == plan.out) ? 1 : 0;
     }
   }
   // Split-bf16 plain rows with an element-wise epilogue (the ConvNeXt MLPs and downsamples) run it straight from the wgmma
   // registers: without the accumulator tile the operand ring is one stage deeper (DESIGN §4.1).  The split GELU output
-  // [hi N | lo N] leaves through TMA stores of 16-row x 64-byte tiles; without the alignment those need, the GELU keeps the
-  // accumulator-tile path.
-  const bool gelu_tma = plan.N % 64 == 0 && ((uintptr_t)plan.out % 16 == 0) && ((plan.ldo * 2) % 16 == 0);
+  // [hi N | lo N] leaves through TMA stores of 16-row x 64-byte tiles, which need N % 64 == 0 and 16-byte aligned rows.
   const bool reg_epi = x3_shared && plan.a_rank == 2 &&
-                       (plan.epi == EPI_RESID || (plan.epi == EPI_STORE && plan.out_f32) || (plan.epi == EPI_GELU && gelu_tma));
+                       (plan.epi == EPI_RESID || (plan.epi == EPI_STORE && plan.out_f32) || plan.epi == EPI_GELU);
   if (reg_epi && plan.epi == EPI_GELU) {
+    GDRN_REQUIRE(plan.N % 64 == 0 && (uintptr_t)plan.out % 16 == 0 && (plan.ldo * 2) % 16 == 0,
+                 "gemm: the split-bf16 GELU output needs N % 64 == 0 and a 16-byte aligned out and row pitch");
     const uint64_t dims[2] = {(uint64_t)plan.ldo, (uint64_t)plan.M};
     const uint64_t str[1] = {(uint64_t)plan.ldo * 2};
     const uint32_t box[2] = {32u, 16u};
@@ -408,42 +384,36 @@ int gemm_tc_launch(const GemmPlan& plan_in, int block_n, cudaStream_t stream) {
     plan.use_tma_store = 1;
   }
   GDRN_REQUIRE(plan.num_taps >= 1 && plan.num_taps <= GEMM_MAX_TAPS, "gemm: bad num_taps");
+  if (x3_shared) {
 #define GDRN_GEMM_CASE_REG(BN, E) \
   if (reg_epi && block_n == BN && plan.epi == E) return launch_inst<BN, E, true, 64, true>(plan, stream);
-  GDRN_GEMM_CASE_REG(128, EPI_GELU)
-  GDRN_GEMM_CASE_REG(128, EPI_RESID)
-  GDRN_GEMM_CASE_REG(128, EPI_STORE)
-  GDRN_GEMM_CASE_REG(64, EPI_GELU)
-  GDRN_GEMM_CASE_REG(64, EPI_RESID)
-  GDRN_GEMM_CASE_REG(64, EPI_STORE)
+    GDRN_GEMM_CASE_REG(128, EPI_GELU)
+    GDRN_GEMM_CASE_REG(128, EPI_RESID)
+    GDRN_GEMM_CASE_REG(128, EPI_STORE)
+    GDRN_GEMM_CASE_REG(64, EPI_GELU)
+    GDRN_GEMM_CASE_REG(64, EPI_RESID)
+    GDRN_GEMM_CASE_REG(64, EPI_STORE)
 #undef GDRN_GEMM_CASE_REG
-#define GDRN_GEMM_CASE_X3(BN, E) \
-  if (x3_shared && block_n == BN && plan.epi == E)                                                          \
-    return bk == 32 ? launch_inst<BN, E, true, 32>(plan, stream) : launch_inst<BN, E, true, 64>(plan, stream);
-  GDRN_GEMM_CASE_X3(128, EPI_GELU)
-  GDRN_GEMM_CASE_X3(128, EPI_RESID)
-  GDRN_GEMM_CASE_X3(128, EPI_STORE)
-  GDRN_GEMM_CASE_X3(128, EPI_GNSTATS)
-  GDRN_GEMM_CASE_X3(128, EPI_BIAS_LN)
-  GDRN_GEMM_CASE_X3(64, EPI_GELU)
-  GDRN_GEMM_CASE_X3(64, EPI_RESID)
-  GDRN_GEMM_CASE_X3(64, EPI_STORE)
-  GDRN_GEMM_CASE_X3(64, EPI_GNSTATS)
-#undef GDRN_GEMM_CASE_X3
+    // the stem (rank-2 rows, LayerNorm epilogue) and the convolutions (32-wide chunks, GroupNorm sums)
+    if (bk == 64 && block_n == 128 && plan.epi == EPI_BIAS_LN) return launch_inst<128, EPI_BIAS_LN, true, 64>(plan, stream);
+    if (bk == 32 && block_n == 128 && plan.epi == EPI_GNSTATS) return launch_inst<128, EPI_GNSTATS, true, 32>(plan, stream);
+    if (bk == 32 && block_n == 64 && plan.epi == EPI_GNSTATS) return launch_inst<64, EPI_GNSTATS, true, 32>(plan, stream);
+  } else {
 #define GDRN_GEMM_CASE(BN, E) \
   if (block_n == BN && plan.epi == E) return launch_inst<BN, E>(plan, stream);
-  GDRN_GEMM_CASE(128, EPI_GELU)
-  GDRN_GEMM_CASE(128, EPI_RESID)
-  GDRN_GEMM_CASE(128, EPI_STORE)
-  GDRN_GEMM_CASE(128, EPI_GNSTATS)
-  GDRN_GEMM_CASE(128, EPI_BIAS_LN)
-  GDRN_GEMM_CASE(64, EPI_GELU)
-  GDRN_GEMM_CASE(64, EPI_RESID)
-  GDRN_GEMM_CASE(64, EPI_STORE)
-  GDRN_GEMM_CASE(64, EPI_GNSTATS)
-  GDRN_GEMM_CASE(16, EPI_STORE)
-  GDRN_GEMM_CASE(80, EPI_OUTCONV)
+    GDRN_GEMM_CASE(128, EPI_GELU)
+    GDRN_GEMM_CASE(128, EPI_RESID)
+    GDRN_GEMM_CASE(128, EPI_STORE)
+    GDRN_GEMM_CASE(128, EPI_GNSTATS)
+    GDRN_GEMM_CASE(128, EPI_BIAS_LN)
+    GDRN_GEMM_CASE(64, EPI_GELU)
+    GDRN_GEMM_CASE(64, EPI_RESID)
+    GDRN_GEMM_CASE(64, EPI_STORE)
+    GDRN_GEMM_CASE(64, EPI_GNSTATS)
+    GDRN_GEMM_CASE(16, EPI_STORE)
+    GDRN_GEMM_CASE(80, EPI_OUTCONV)
 #undef GDRN_GEMM_CASE
+  }
   gdrn_set_last_error(__FILE__, __LINE__, "gemm: unsupported (block_n, epilogue) combination");
   return GDRN_ERR_INVALID;
 }

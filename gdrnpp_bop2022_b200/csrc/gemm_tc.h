@@ -50,19 +50,18 @@ struct GemmPlan {
   const void* b_ptr;    // W base / rows / row length (elements)
   long long b_rows, b_ktot;
   // ---- problem ----
-  int m_tiles, n_tiles;
-  int n_major;          // tile order: 0 = consecutive CTAs share an A tile (m-major), 1 = they share a B tile (n-major)
+  int m_tiles, n_tiles;  // tile t is (m_tile, n_tile) = (t / n_tiles, t % n_tiles): consecutive CTAs share an A tile
   int M;                // valid rows (rank 2) ; rank 4/5: number of images B
   int N;                // valid output columns
   // ---- epilogue ----
   int epi;
   int out_f32;          // EPI_STORE / EPI_GNSTATS: 1 -> fp32 output, 0 -> bf16
   int gelu_mode;        // EPI_GELU: 0 = fp32 ex2/rcp form (1.2e-5 of erf), 1 = packed half2 tanh.approx, 2 = fp32 tanh.approx, 3 = erff
+                        // (bf16 plans; a split GELU is always the erf form, mode 3, whatever this field says)
   int split;            // split-bf16 (x3) mode: operands are [hi | lo] pairs (see x3_*), bf16 outputs are written as
                         // [hi | lo] pairs (row width 2N, lo = bf16(v - hi))
   int x3_a_lo;          // split: offset of the lo half in A's coordinate 0 (channels / K); taps[] list the hi operands only
   int x3_b_lo;          // split: offset of the lo half inside a row of W (elements)
-  int x3_expanded;      // set by gemm_tc_launch once taps[] has been expanded to the three products
   void* out;            // [rows, ldo]
   CUtensorMap tmap_out; // rank-2 outputs: store map (filled by gemm_tc_launch when use_tma_store)
   int use_tma_store;    // set by gemm_tc_launch
@@ -84,10 +83,6 @@ struct GemmPlan {
   const float* roi_extents;      // [B,3]
   const float* roi_coord_2d;     // [B,2,64,64] fp32 NCHW
   void* pnp_in;                  // bf16 [B*4096, 128]
-  // debug: CTA 0 writes [0] producer empty-wait, [1] consumer full-wait, [3] accumulator hand-over, [6] CTA cycles,
-  // [7] tiles of CTA 0, [8..10] epilogue warp 0 accumulator loads / compute / flush (clock64 cycles; the register
-  // epilogue has no hand-over and books its whole epilogue as compute)
-  long long* trace;
   float* map_mask; float* map_full; float* map_x; float* map_y; float* map_z; float* map_region;  // NCHW or null
 };
 

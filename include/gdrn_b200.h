@@ -167,15 +167,10 @@ int gdrn_gemm_bf16(const void* A, const void* W, const float* bias, const float*
 /* The same for the split-bf16 ("bf16x3") precision mode, exported for tests and roofline measurement:
  * A [M, 2K] and W [N, 2K] hold [hi K | lo K] rows (hi = bf16(v), lo = bf16(v - hi)); the kernel accumulates
  * A_lo*W_hi + A_hi*W_lo + A_hi*W_hi in fp32.  epi: 0 = store fp32 [M,N]; 1 = exact-erf GELU -> split bf16 [M, 2N];
- * 2 = resid + gamma*(.) -> fp32 [M,N] (in place allowed).  block_n in {64, 128, 256}. */
+ * 2 = resid + gamma*(.) -> fp32 [M,N] (in place allowed).  block_n in {64, 128, 256}; N % 64 == 0, K % 64 == 0.
+ * epi 1 needs a 16-byte aligned out (GDRN_ERR_INVALID otherwise); epi 0 and 2 need 8-byte aligned out and resid. */
 int gdrn_gemm_x3(const void* A, const void* W, const float* bias, const float* gamma, const float* resid, void* out,
                  int M, int N, int K, int epi, int block_n, void* stream);
-
-/* DEPRECATED: same as gdrn_gemm_x3 with epi 2 and out == resid, x [M,N] fp32 += gamma * (A @ W^T + bias); kept for
- * callers of the earlier k-split schedule, which is no longer implemented.  `flags` must still be flag_words ZEROED device
- * words; they are not used and stay zeroed.  Run-to-run deterministic. */
-int gdrn_gemm_x3_ksplit(const void* A, const void* W, const float* bias, const float* gamma, float* x, int M, int N, int K,
-                        int block_n, unsigned* flags, int flag_words, void* stream);
 
 /* Fused ConvNeXt MLP half-block of the split-bf16 mode (stage 0, C = 128), exported for tests and measurement:
  * x [M,C] fp32 += gamma * (W2 . gelu(W1 . a + b1) + b2) with a [M,2C], W1 [4C,2C], W2 [C,8C] in [hi | lo] bf16 rows; the

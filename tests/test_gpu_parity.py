@@ -169,9 +169,9 @@ def test_gemm_x3_vs_fp64(dev, lib, M, N, K, bn, epi):
     (20000, 256, 1024, 256),    # ragged M, odd tile count
     (16384, 128, 512, 128),     # BLOCK_N 128
 ])
-def test_gemm_x3_ksplit_residual(dev, lib, M, N, K, bn):
-    """The deprecated k-split entry (now the whole-tile in-place residual GEMM): same result as the fp64 reference and as
-    gdrn_gemm_x3, run-to-run bit-identical, flag words left at zero."""
+def test_gemm_x3_residual_in_place(dev, lib, M, N, K, bn):
+    """gdrn_gemm_x3 with epi 2 in place (x += gamma * (A @ W^T + bias), how the forward runs fc2) at the MLP shapes: within
+    the fp64 bar, canary rows untouched, run-to-run bit-identical."""
     L = _lib()
     g = torch.Generator().manual_seed(M + N + K)
     A = (torch.randn(M, K, generator=g) * 0.5).to(dev)
@@ -180,27 +180,38 @@ def test_gemm_x3_ksplit_residual(dev, lib, M, N, K, bn):
     x = torch.randn(M, N, generator=g).to(dev)
     ref = x.double() + gamma.double() * (A.double() @ W.double().t() + bias.double())
     A2, W2 = _split_bf16(A), _split_bf16(W)
-    flags = torch.zeros(8192, dtype=torch.int32, device=dev)
     outs = []
     for _ in range(3):
         out = torch.full((M + 64, N), 7.0, dtype=torch.float32, device=dev)
         out[:M] = x
-        L.check(lib.gdrn_gemm_x3_ksplit(L.ptr(A2), L.ptr(W2), L.ptr(bias), L.ptr(gamma), L.ptr(out), M, N, K, bn,
-                                        L.ptr(flags), flags.numel(), L.current_stream()), "gemm_x3_ksplit")
+        L.check(lib.gdrn_gemm_x3(L.ptr(A2), L.ptr(W2), L.ptr(bias), L.ptr(gamma), L.ptr(out), L.ptr(out), M, N, K, 2, bn,
+                                 L.current_stream()), "gemm_x3")
         torch.cuda.synchronize()
-        assert int(flags.abs().max().item()) == 0
         assert torch.equal(out[M:], torch.full((64, N), 7.0, device=dev))
         outs.append(out[:M].clone())
     assert torch.equal(outs[0], outs[1]) and torch.equal(outs[0], outs[2])
     err = (outs[0].double() - ref).abs().max().item()
     assert err < 4e-5 * max(1.0, ref.abs().max().item()), err
-    # whole-tile schedule (no flags): same sums up to the fp32 rounding of the partial adds
-    whole = torch.full((M + 64, N), 7.0, dtype=torch.float32, device=dev)
-    whole[:M] = x
-    L.check(lib.gdrn_gemm_x3(L.ptr(A2), L.ptr(W2), L.ptr(bias), L.ptr(gamma), L.ptr(whole), L.ptr(whole), M, N, K, 2, bn,
-                             L.current_stream()), "gemm_x3")
+
+
+@pytest.mark.gpu
+def test_gemm_x3_gelu_rejects_misaligned_out(dev, lib):
+    """The split GELU output leaves through TMA stores, which need a 16-byte aligned `out`: an 8-byte offset is refused on
+    the host (non-zero return, nothing launched) and the buffer stays as it was."""
+    L = _lib()
+    M, N, K = 256, 128, 64
+    g = torch.Generator().manual_seed(5)
+    A2 = _split_bf16(torch.randn(M, K, generator=g).to(dev))
+    W2 = _split_bf16((torch.randn(N, K, generator=g) / np.sqrt(K)).to(dev))
+    bias = torch.randn(N, generator=g).to(dev)
+    buf = torch.full((M * 2 * N + 8,), float("nan"), dtype=torch.bfloat16, device=dev)
+    out = buf[4:]                                         # 4 bf16 = 8 bytes past a 16-byte aligned base
+    assert buf.data_ptr() % 16 == 0 and out.data_ptr() % 16 == 8
+    rc = lib.gdrn_gemm_x3(L.ptr(A2), L.ptr(W2), L.ptr(bias), None, None, L.ptr(out), M, N, K, 1, 128, L.current_stream())
     torch.cuda.synchronize()
-    assert (whole[:M] - outs[0]).abs().max().item() < 2e-5 * max(1.0, ref.abs().max().item())
+    assert rc != 0
+    assert "16-byte aligned" in L.last_error()
+    assert torch.isnan(buf.float()).all()
 
 
 @pytest.mark.gpu
