@@ -31,6 +31,7 @@ _SIGNATURES = {
     "gdrn_last_error": (c_char_p, []),
     "gdrn_version": (c_int, []),
     "gdrn_launch_count": (ctypes.c_longlong, []),
+    "gdrn_gemm_kernels_launched": (ctypes.c_uint64, [c_int]),
     "gdrn_model_set_profiling": (c_int, [c_void_p, c_int]),
     "gdrn_model_get_profile": (c_int, [c_void_p, c_void_p, c_void_p]),
     "gdrn_model_create": (c_int, [POINTER(c_void_p), c_char_p, c_int, c_int]),
@@ -172,6 +173,26 @@ _SIGNATURES = {
 }
 
 EXPORTED_SYMBOLS = tuple(_SIGNATURES.keys())
+
+# Bit i of gdrn_gemm_kernels_launched() is kernel GEMM_KERNELS[i]: gemm_tc_launch's instantiations in the order of the
+# kGemmKernels table in csrc/gemm_tc.cu ("<bf16 | x3> <BLOCK_N> <epilogue> bk<k-chunk width>[ reg]", reg = the register
+# epilogue), then the two fused ConvNeXt MLP kernels of csrc/mlp_fused.cu.
+GEMM_KERNELS = (
+    "bf16 128 GELU bk64", "bf16 128 RESID bk64", "bf16 128 STORE bk64", "bf16 128 GNSTATS bk64", "bf16 128 BIAS_LN bk64",
+    "bf16 64 GELU bk64", "bf16 64 RESID bk64", "bf16 64 STORE bk64", "bf16 64 GNSTATS bk64", "bf16 16 STORE bk64",
+    "bf16 80 OUTCONV bk64",
+    "x3 128 GELU bk64 reg", "x3 128 RESID bk64 reg", "x3 128 STORE bk64 reg", "x3 64 GELU bk64 reg",
+    "x3 64 RESID bk64 reg", "x3 64 STORE bk64 reg",
+    "x3 128 BIAS_LN bk64", "x3 128 GNSTATS bk32", "x3 64 GNSTATS bk32",
+    "mlp_fused", "mlp_fused_x3",
+)
+
+
+def gemm_kernel_names(mask):
+    """The names (GEMM_KERNELS) of the bits set in a gdrn_gemm_kernels_launched() mask, in id order."""
+    if mask >> len(GEMM_KERNELS):
+        raise ValueError(f"gemm kernel mask {mask:#x} has bits beyond the {len(GEMM_KERNELS)} known kernels")
+    return [n for i, n in enumerate(GEMM_KERNELS) if mask >> i & 1]
 
 
 def lib():

@@ -19,6 +19,12 @@ static std::atomic<long long> g_launches{0};
 void gdrn_count_launch(int n) { g_launches.fetch_add(n, std::memory_order_relaxed); }
 extern "C" long long gdrn_launch_count(void) { return g_launches.load(std::memory_order_relaxed); }
 
+static std::atomic<uint64_t> g_gemm_kernels{0};
+void gdrn_record_gemm_kernel(int id) { g_gemm_kernels.fetch_or(1ull << id, std::memory_order_relaxed); }
+extern "C" uint64_t gdrn_gemm_kernels_launched(int reset) {
+  return reset ? g_gemm_kernels.exchange(0, std::memory_order_relaxed) : g_gemm_kernels.load(std::memory_order_relaxed);
+}
+
 extern "C" const char* gdrn_last_error(void) { return g_last_error; }
 extern "C" int gdrn_version(void) { return 100; }
 

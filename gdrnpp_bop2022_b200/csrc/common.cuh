@@ -30,6 +30,7 @@
 
 void gdrn_set_last_error(const char* file, int line, const char* msg);
 void gdrn_count_launch(int n);  // bumps the counter behind gdrn_launch_count()
+void gdrn_record_gemm_kernel(int id);  // sets bit id of the record behind gdrn_gemm_kernels_launched()
 
 // The dynamic-shared-memory opt-in and the SM count are PER DEVICE: cache them per device ordinal so that a process
 // that drives several GPUs (GdrnPredictor(device="cuda:1"), one engine per device) configures each of them.

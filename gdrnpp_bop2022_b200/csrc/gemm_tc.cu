@@ -295,9 +295,64 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) gemm_tc_kernel(const __grid_co
   }
 }
 
+// Every kernel gemm_tc_launch can launch, numbered for the launch record (gdrn_gemm_kernels_launched).  The order is the
+// ABI of that record: append, never reorder (the Python side names the bits from the same list, _lib.GEMM_KERNELS).
+struct GemmKernelKey {
+  int block_n, epi;
+  bool x3;
+  int bk;
+  bool reg;
+};
+constexpr GemmKernelKey kGemmKernels[] = {
+    // bf16
+    {128, EPI_GELU, false, 64, false},
+    {128, EPI_RESID, false, 64, false},
+    {128, EPI_STORE, false, 64, false},
+    {128, EPI_GNSTATS, false, 64, false},
+    {128, EPI_BIAS_LN, false, 64, false},
+    {64, EPI_GELU, false, 64, false},
+    {64, EPI_RESID, false, 64, false},
+    {64, EPI_STORE, false, 64, false},
+    {64, EPI_GNSTATS, false, 64, false},
+    {16, EPI_STORE, false, 64, false},
+    {80, EPI_OUTCONV, false, 64, false},
+    // split-bf16, register epilogue
+    {128, EPI_GELU, true, 64, true},
+    {128, EPI_RESID, true, 64, true},
+    {128, EPI_STORE, true, 64, true},
+    {64, EPI_GELU, true, 64, true},
+    {64, EPI_RESID, true, 64, true},
+    {64, EPI_STORE, true, 64, true},
+    // split-bf16 stem and convolutions
+    {128, EPI_BIAS_LN, true, 64, false},
+    {128, EPI_GNSTATS, true, 32, false},
+    {64, EPI_GNSTATS, true, 32, false},
+};
+static_assert(sizeof(kGemmKernels) / sizeof(kGemmKernels[0]) == GEMM_NUM_TC_KERNELS, "gemm: kGemmKernels size");
+
+constexpr bool same_kernel(const GemmKernelKey& a, const GemmKernelKey& b) {
+  return a.block_n == b.block_n && a.epi == b.epi && a.x3 == b.x3 && a.bk == b.bk && a.reg == b.reg;
+}
+constexpr bool gemm_kernels_unique() {
+  for (int i = 0; i < GEMM_NUM_TC_KERNELS; ++i)
+    for (int j = i + 1; j < GEMM_NUM_TC_KERNELS; ++j)
+      if (same_kernel(kGemmKernels[i], kGemmKernels[j])) return false;
+  return true;
+}
+static_assert(gemm_kernels_unique(), "gemm: an instantiation is listed twice in kGemmKernels");
+
+template <int BLOCK_N, int EPI, bool X3, int BK, bool REG>
+constexpr int gemm_kernel_id() {
+  for (int i = 0; i < GEMM_NUM_TC_KERNELS; ++i)
+    if (same_kernel(kGemmKernels[i], GemmKernelKey{BLOCK_N, EPI, X3, BK, REG})) return i;
+  return -1;
+}
+
 template <int BLOCK_N, int EPI, bool X3 = false, int BK = 64, bool REG = false>
 int launch_inst(const GemmPlan& plan, cudaStream_t stream) {
   using C = Cfg<BLOCK_N, X3, BK, REG>;
+  constexpr int kId = gemm_kernel_id<BLOCK_N, EPI, X3, BK, REG>();
+  static_assert(kId >= 0, "gemm: every instantiation needs an entry in kGemmKernels");
   auto kfn = gemm_tc_kernel<BLOCK_N, EPI, X3, BK, REG>;
   GDRN_OPT_IN_SMEM(kfn, C::SMEM_BYTES);
   int total = plan.m_tiles * plan.n_tiles;
@@ -305,6 +360,7 @@ int launch_inst(const GemmPlan& plan, cudaStream_t stream) {
   int grid = total < gdrn_num_sms() ? total : gdrn_num_sms();
   GDRN_CHECK_CUDA(gdrn_launch_dep(kfn, dim3(grid), dim3(NUM_THREADS), C::SMEM_BYTES, stream, plan));
   gdrn_count_launch(1);
+  gdrn_record_gemm_kernel(kId);
   return GDRN_OK;
 }
 

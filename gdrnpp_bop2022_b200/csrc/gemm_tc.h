@@ -89,6 +89,13 @@ struct GemmPlan {
 // block_n in {16, 64, 80, 128, 256} (256: run as 128-wide tiles)
 int gemm_tc_launch(const GemmPlan& plan, int block_n, cudaStream_t stream);
 
+// Ids of the launch record (gdrn_gemm_kernels_launched): gemm_tc_launch's instantiations take 0 .. GEMM_NUM_TC_KERNELS - 1
+// in the order of gemm_tc.cu's kGemmKernels table, the fused MLP kernels the two after them.
+constexpr int GEMM_NUM_TC_KERNELS = 20;
+constexpr int GEMM_KERNEL_ID_MLP_FUSED = GEMM_NUM_TC_KERNELS;
+constexpr int GEMM_KERNEL_ID_MLP_FUSED_X3 = GEMM_NUM_TC_KERNELS + 1;
+static_assert(GEMM_KERNEL_ID_MLP_FUSED_X3 < 64, "gemm: the launch record is one 64-bit mask");
+
 // Fused ConvNeXt MLP block (C = 128, mlp_fused.cu): x += gamma * (W2 . gelu(W1 . A + b1) + b2), hidden activation kept on
 // chip.  A bf16 [M, C]; W1 bf16 [4C, C]; W2 bf16 [C, 4C]; x fp32 [M, C] updated in place.
 // split-bf16 (parity mode) twin: A [M,2C], W1 [4C,2C], W2 [C,8C] hold [hi | lo] halves

@@ -254,6 +254,7 @@ int mlp_launch(const void* A, const void* W1, const float* b1, const void* W2, c
   const int grid = fp.m_tiles < gdrn_num_sms() ? fp.m_tiles : gdrn_num_sms();
   GDRN_CHECK_CUDA(gdrn_launch_dep(kfn, dim3(grid), dim3(NUM_THREADS), C::SMEM_BYTES, stream, fp));
   gdrn_count_launch(1);
+  gdrn_record_gemm_kernel(X3 ? GEMM_KERNEL_ID_MLP_FUSED_X3 : GEMM_KERNEL_ID_MLP_FUSED);
   return GDRN_OK;
 }
 

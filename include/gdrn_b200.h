@@ -27,6 +27,11 @@ const char* gdrn_last_error(void);
 int gdrn_version(void);
 /* number of CUDA kernels this library has launched in the calling process (monotonic) */
 long long gdrn_launch_count(void);
+/* Which implicit-GEMM kernels this library has launched in the calling process since the last reset: bit i is set once
+ * kernel i ran (i numbers the instantiations of the kGemmKernels table in gemm_tc.cu, then the two fused ConvNeXt MLP
+ * kernels; gdrnpp_bop2022_b200._lib.GEMM_KERNELS names them).  reset != 0 clears the record after reading it.
+ * Host-side bookkeeping only: no launch and no result depends on it. */
+uint64_t gdrn_gemm_kernels_launched(int reset);
 
 /* ---------------------------------------------------------------------------------------------
  * Dense path: GDRN_DoubleMask.forward (eval, do_loss=False)

@@ -99,9 +99,13 @@ def _gn_ratio_weights(sd, li):
     return sd
 
 
-@functools.lru_cache(maxsize=None)
-def _setup(mode, num_classes=21, gn_ratio_conv=None):
+def _setup(mode, num_classes=21, gn_ratio_conv=None, max_batch=64):
     """(model, fp64 reference state dict) of one precision mode; class-agnostic for num_classes == 1."""
+    return _setup_cached(mode, num_classes, gn_ratio_conv, max_batch)
+
+
+@functools.lru_cache(maxsize=None)
+def _setup_cached(mode, num_classes, gn_ratio_conv, max_batch):
     from gdrnpp_bop2022_b200.gdrn_model import GDRN_DoubleMask, default_cfg
 
     cfg = default_cfg(num_classes=21)
@@ -111,7 +115,7 @@ def _setup(mode, num_classes=21, gn_ratio_conv=None):
     sd = _state_dict(num_classes)
     if gn_ratio_conv is not None:
         sd = _gn_ratio_weights(sd, gn_ratio_conv)
-    model = GDRN_DoubleMask(cfg, max_batch=64, precision=mode)
+    model = GDRN_DoubleMask(cfg, max_batch=max_batch, precision=mode)
     assert model.head_classes == num_classes
     model.load_state_dict(sd)
     dev = torch.device("cuda:0")
@@ -173,7 +177,7 @@ def _gn_sum_errors(stats, raw, layer, B):
 
 # ------------------------------------------------------------------------------------------------ conv stages
 def head_stage_errors(stage, mode, B, x=None):
-    model, sd = _setup(mode)
+    model, sd = _setup(mode, max_batch=max(64, 1 << (B - 1).bit_length()))   # one engine per power of two above 64
     h = HEAD_IN_RES[stage]
     if x is None:
         x = _input((B, h, h, C3 if stage == "deconv" else 256), seed=10 * HEAD_STAGES.index(stage) + B)
