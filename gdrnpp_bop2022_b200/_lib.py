@@ -81,6 +81,7 @@ _SIGNATURES = {
     "rast_render_meshes_rgb": (c_int, [c_void_p] * 4 + [c_int] * 3 + [c_float, c_float] + [c_void_p] * 5),
     "rast_upload_mesh_tex": (c_int, [c_void_p, c_int, c_void_p, c_int] + [c_void_p] * 4 + [c_int, c_int]),
     "rast_render_scene": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_int, c_int, c_float, c_float] + [c_void_p] * 9),
+    "rast_render_scene_bg": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_int, c_int, c_float, c_float] + [c_void_p] * 10),
     "rast_scene_scratch_bytes": (c_size_t, [c_int, c_int, c_int]),
     "gdrn_pnp_ransac_maps": (c_int, [c_void_p] * 9 + [c_int] * 3 + [c_float, c_float, c_uint] + [c_void_p] * 4),
     "gdrn_pnp_ransac_points": (c_int, [c_void_p] * 4 + [c_int] * 3 + [c_float, c_uint] + [c_void_p] * 4),
@@ -152,6 +153,8 @@ _SIGNATURES = {
     "gdrn_xyz_crop_boxes": (c_int, [c_void_p] + [c_int] * 3 + [c_void_p, c_void_p]),
     "gdrn_xyz_crop_pack": (c_int, [c_void_p] * 6 + [c_int] * 3 + [c_void_p, c_void_p]),
     "gdrn_vis_poses_workspace_bytes": (c_size_t, [c_int] * 3),
+    "gdrn_vis_gray3": (c_int, [c_void_p] + [c_int] * 4 + [c_void_p] * 2),
+    "gdrn_vis_outlines": (c_int, [c_void_p] * 4 + [c_int] * 5 + [c_void_p] * 2),
     "gdrn_vis_poses": (c_int, [c_void_p] * 3 + [c_int] * 3 + [c_void_p] * 2 + [c_int] * 3 + [c_void_p] * 9 + [c_size_t,
                                                                                                          c_void_p]),
     "gdrn_train_composite": (c_int, [c_void_p, c_void_p] + [c_int] * 3 + [c_void_p] * 8 + [c_void_p]),

@@ -316,12 +316,15 @@ struct SceneLight {
 //   pc_obj = interp(x), normal = 0.5 interp(normalize(R n)) + 0.5, diff = max(dot(interp(normalize(R n)),
 //   normalize(light - interp(P))), 0);  textureless: colour (diff + 0.2) light;  textured: texture (diff light
 //   mat_diffuse + mat_ambient light) (the specular term is 0: with the identity view its view direction is
-//   normalize(0)); every channel clamped at 1.  seg = instance index + 1.  Background: every output 0.
+//   normalize(0)); every channel clamped at 1.  seg = instance index + 1.  Background: every output 0, except image
+//   when a background [H,W,3] u8 is given: there image = v / 255 in f32, channels in the given order (the full-viewport
+//   quad egl_renderer_v3's im2Texture draws before the models).
 __global__ void __launch_bounds__(256)
 rast_scene_resolve_kernel(const unsigned long long* __restrict__ zbuf, const MeshEntry* __restrict__ table,
                           const float* const* __restrict__ mesh_colors, const MeshTex* __restrict__ mesh_tex,
                           const int* __restrict__ mesh_ids, const unsigned* __restrict__ tri_off, int n,
                           const float* __restrict__ poses, const float* __restrict__ K, int H, int W, SceneLight lt,
+                          const uint8_t* __restrict__ background,
                           float* __restrict__ depth, float* __restrict__ pc_cam, float* __restrict__ pc_obj,
                           float* __restrict__ normal, float* __restrict__ image, float* __restrict__ seg) {
   const long long total = (long long)H * W;
@@ -336,7 +339,7 @@ rast_scene_resolve_kernel(const unsigned long long* __restrict__ zbuf, const Mes
         if (pc_cam) pc_cam[i * 3 + c] = 0.f;
         if (pc_obj) pc_obj[i * 3 + c] = 0.f;
         if (normal) normal[i * 3 + c] = 0.f;
-        if (image) image[i * 3 + c] = 0.f;
+        if (image) image[i * 3 + c] = background ? __fdiv_rn((float)background[i * 3 + c], 255.f) : 0.f;
       }
       if (seg) seg[i] = 0.f;
       continue;
@@ -799,12 +802,14 @@ extern "C" size_t rast_scene_scratch_bytes(int n_inst, int H, int W) {
   return (size_t)H * W * 8 + (((size_t)n_inst + 1) * 4 + 7) / 8 * 8;
 }
 
-extern "C" int rast_render_scene(const int* mesh_ids, const float* poses, int n_inst, const float* K, int H, int W,
-                                 float znear, float zfar, const float* light, float* depth, float* pc_cam, float* pc_obj,
-                                 float* normal, float* image, float* seg, void* scratch, void* stream) {
-  GDRN_REQUIRE(mesh_ids && poses && K && light && depth && scratch, "rast_render_scene: null argument");
-  GDRN_REQUIRE(n_inst > 0 && H > 0 && W > 0, "rast_render_scene: empty input");
-  GDRN_REQUIRE(g_meshes.count > 0, "rast_render_scene: no mesh uploaded (rast_upload_mesh)");
+extern "C" int rast_render_scene_bg(const int* mesh_ids, const float* poses, int n_inst, const float* K, int H, int W,
+                                    float znear, float zfar, const float* light, const uint8_t* background, float* depth,
+                                    float* pc_cam, float* pc_obj, float* normal, float* image, float* seg, void* scratch,
+                                    void* stream) {
+  GDRN_REQUIRE(K && light && depth && scratch && (n_inst == 0 || (mesh_ids && poses)), "rast_render_scene: null argument");
+  GDRN_REQUIRE(n_inst >= 0 && H > 0 && W > 0, "rast_render_scene: empty input");
+  GDRN_REQUIRE(n_inst > 0 || background, "rast_render_scene: no instance and no background");
+  GDRN_REQUIRE(n_inst == 0 || g_meshes.count > 0, "rast_render_scene: no mesh uploaded (rast_upload_mesh)");
   GDRN_REQUIRE(znear > 0.f && zfar > znear, "rast: need 0 < znear < zfar");
   SceneLight lt;
   for (int c = 0; c < 3; ++c) {
@@ -816,14 +821,24 @@ extern "C" int rast_render_scene(const int* mesh_ids, const float* poses, int n_
   unsigned* tri_off = (unsigned*)(zbuf + npx);
   int blocks = (int)((npx + 255) / 256 > 4096 ? 4096 : (npx + 255) / 256);
   rast_scene_clear_kernel<<<blocks, 256, 0, st>>>(zbuf, npx, g_meshes.dev_table, g_meshes.count, mesh_ids, n_inst, tri_off);
-  rast_scene_tri_kernel<<<dim3((g_meshes.max_faces + 255) / 256, n_inst < 65535 ? n_inst : 65535), 256, 0, st>>>(
-      g_meshes.dev_table, mesh_ids, g_meshes.count, n_inst, poses, K, H, W, znear, zfar, tri_off, zbuf);
+  if (n_inst > 0)
+    rast_scene_tri_kernel<<<dim3((g_meshes.max_faces + 255) / 256, n_inst < 65535 ? n_inst : 65535), 256, 0, st>>>(
+        g_meshes.dev_table, mesh_ids, g_meshes.count, n_inst, poses, K, H, W, znear, zfar, tri_off, zbuf);
   rast_scene_resolve_kernel<<<blocks, 256, 0, st>>>(zbuf, g_meshes.dev_table, g_meshes.dev_colors, g_meshes.dev_tex,
-                                                    mesh_ids, tri_off, n_inst, poses, K, H, W, lt, depth, pc_cam, pc_obj,
-                                                    normal, image, seg);
+                                                    mesh_ids, tri_off, n_inst, poses, K, H, W, lt, background, depth,
+                                                    pc_cam, pc_obj, normal, image, seg);
   GDRN_CHECK_CUDA(cudaGetLastError());
-  gdrn_count_launch(3);
+  gdrn_count_launch(n_inst > 0 ? 3 : 2);
   return GDRN_OK;
+}
+
+extern "C" int rast_render_scene(const int* mesh_ids, const float* poses, int n_inst, const float* K, int H, int W,
+                                 float znear, float zfar, const float* light, float* depth, float* pc_cam, float* pc_obj,
+                                 float* normal, float* image, float* seg, void* scratch, void* stream) {
+  GDRN_REQUIRE(mesh_ids && poses && K && light && depth && scratch, "rast_render_scene: null argument");
+  GDRN_REQUIRE(n_inst > 0 && H > 0 && W > 0, "rast_render_scene: empty input");
+  return rast_render_scene_bg(mesh_ids, poses, n_inst, K, H, W, znear, zfar, light, nullptr, depth, pc_cam, pc_obj,
+                              normal, image, seg, scratch, stream);
 }
 
 extern "C" int gdrn_depth_refine_step(const float* xyz, const float* mask, int mask_mode, const float* depth_sensor,

@@ -272,3 +272,77 @@ extern "C" int gdrn_vis_poses(const uint8_t* m_rgb, const float* m_depth, const 
   gdrn_count_launch(launches);
   return GDRN_OK;
 }
+
+// ---- pose outlines (the per-dataset vis_poses_full scripts) --------------------------------------------------------
+namespace {
+
+// mmcv.bgr2gray == cv2.cvtColor(BGR2GRAY) on u8: OpenCV 4's 15-bit fixed-point weights of R 0.299, G 0.587, B 0.114,
+// rounded (equal to cv2 on all 2^24 inputs; the older 14-bit weights 4899 / 9617 / 1868 differ on about 0.3 % of them).
+// rgb_order: the input's channels are R, G, B (else B, G, R); the output is the same either way.
+__global__ void vis_gray3_kernel(const uint8_t* __restrict__ img, long long npx, int rgb_order, uint8_t* __restrict__ out) {
+  const int ib = rgb_order ? 2 : 0, ir = 2 - ib;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < npx; i += (long long)gridDim.x * blockDim.x) {
+    const unsigned b = img[i * 3 + ib], g = img[i * 3 + 1], r = img[i * 3 + ir];
+    const uint8_t y = (uint8_t)((3735u * b + 19235u * g + 9798u * r + 16384u) >> 15);
+    out[i * 3] = y; out[i * 3 + 1] = y; out[i * 3 + 2] = y;
+  }
+}
+
+// get_edge(mask, bw) at (y, x) for the coverage plane c: set, with an unset neighbour bw away inside the image
+__device__ __forceinline__ bool edge_at(const float* __restrict__ c, int H, int W, int y, int x, int bw) {
+  if (c[(long long)y * W + x] == 0.f) return false;
+  return (y + bw < H && c[(long long)(y + bw) * W + x] == 0.f) || (y - bw >= 0 && c[(long long)(y - bw) * W + x] == 0.f) ||
+         (x + bw < W && c[(long long)y * W + x + bw] == 0.f) || (x - bw >= 0 && c[(long long)y * W + x - bw] == 0.f);
+}
+
+// grid (slices, N): one thread per pixel of image j; the estimate edges win over the GT edges, which win over the render
+__global__ void __launch_bounds__(VP_THREADS)
+vis_outlines_kernel(const float* __restrict__ shaded, const float* __restrict__ cover, const int* __restrict__ inst_off,
+                    const uint8_t* __restrict__ is_gt, int H, int W, int bw, uint8_t* __restrict__ out) {
+  const int j = blockIdx.y, k0 = inst_off[j], k1 = inst_off[j + 1];
+  const long long HW = (long long)H * W;
+  for (long long p = (long long)blockIdx.x * VP_THREADS + threadIdx.x; p < HW; p += (long long)gridDim.x * VP_THREADS) {
+    const int y = (int)(p / W), x = (int)(p - (long long)y * W);
+    bool est = false, gt = false;
+    for (int k = k0; k < k1 && !est; ++k) {
+      const bool g = is_gt[k] != 0;
+      if (g && gt) continue;
+      if (edge_at(cover + (size_t)k * HW, H, W, y, x, bw)) (g ? gt : est) = true;
+    }
+    const size_t o = ((size_t)j * HW + p) * 3;
+    if (est) { out[o] = 0; out[o + 1] = 255; out[o + 2] = 0; continue; }
+    if (gt) { out[o] = 255; out[o + 1] = 0; out[o + 2] = 0; continue; }
+#pragma unroll
+    for (int c = 0; c < 3; ++c)   // image_tensor = bgr(shaded) * 255, then (image_tensor + 0.5).astype(uint8), all f32
+      out[o + c] = (uint8_t)__fadd_rn(__fmul_rn(shaded[o + 2 - c], 255.f), 0.5f);
+  }
+}
+
+}  // namespace
+
+extern "C" int gdrn_vis_gray3(const uint8_t* img, int N, int H, int W, int rgb_order, uint8_t* out, void* stream) {
+  GDRN_REQUIRE(img && out && N > 0 && H > 0 && W > 0, "vis_gray3: need img, out and N, H, W > 0");
+  const long long npx = (long long)N * H * W;
+  const int blocks = (int)min((npx + 255) / 256, 4096LL);
+  vis_gray3_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(img, npx, rgb_order, out);
+  GDRN_CHECK_CUDA(cudaGetLastError());
+  gdrn_count_launch(1);
+  return GDRN_OK;
+}
+
+extern "C" int gdrn_vis_outlines(const float* shaded, const float* cover, const int* inst_off, const uint8_t* is_gt, int N,
+                                 int n, int H, int W, int bw, uint8_t* out, void* stream) {
+  GDRN_REQUIRE(shaded && inst_off && out && N > 0 && n >= 0 && H > 0 && W > 0, "vis_outlines: need shaded, inst_off, "
+               "out and N, H, W > 0");
+  GDRN_REQUIRE(n == 0 || (cover && is_gt), "vis_outlines: instances need cover and is_gt");
+  GDRN_REQUIRE(bw > 0, "vis_outlines: bw must be > 0");
+  GDRN_REQUIRE((long long)H * W <= INT_MAX, "vis_outlines: image too large");
+  const long long HW = (long long)H * W;
+  const int slices = (int)min((HW + VP_THREADS * VP_PIX_PER_THREAD - 1) / (VP_THREADS * VP_PIX_PER_THREAD),
+                              (long long)VP_MAX_SLICES);
+  vis_outlines_kernel<<<dim3(slices, N), VP_THREADS, 0, (cudaStream_t)stream>>>(shaded, cover, inst_off, is_gt, H, W, bw,
+                                                                                out);
+  GDRN_CHECK_CUDA(cudaGetLastError());
+  gdrn_count_launch(1);
+  return GDRN_OK;
+}

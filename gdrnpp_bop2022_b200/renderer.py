@@ -344,14 +344,16 @@ EGL_MAT_AMBIENT = (0.05, 0.05, 0.05)
 
 @_lib.on_device(1)
 def render_scene(mesh_ids, poses, K, H, W, znear=0.25, zfar=6.0, light_pos=(0.0, 0.0, 0.0), light_color=(1.0, 1.0, 1.0),
-                 outputs=("pc_cam", "seg"), mat_diffuse=EGL_MAT_DIFFUSE, mat_ambient=EGL_MAT_AMBIENT):
+                 outputs=("pc_cam", "seg"), mat_diffuse=EGL_MAT_DIFFUSE, mat_ambient=EGL_MAT_AMBIENT, background=None):
     """The registered meshes `mesh_ids` [n] (int32 CUDA) at poses [n,3,4] rendered into ONE image with one z-buffer and
     one K [3,3] (rast_render_scene): the draw loop of egl_renderer_v3.py:998-1177 in one launch set, no sync.  A depth
     tie between instances goes to the earlier one.  -> dict with depth [H,W] and each requested output of
     "pc_cam" [H,W,3] (camera-space point), "pc_obj" [H,W,3] (model-space point), "normal" [H,W,3] (0.5 n + 0.5 of the
     interpolated camera-frame normal), "image" [H,W,3] (RGB in [0,1], shader_textureless_texture.frag) and "seg" [H,W]
     (instance index + 1); every output is 0 on background and rows run top to bottom.  The light is in the camera
-    frame (the EGL renderer's view matrix is the identity)."""
+    frame (the EGL renderer's view matrix is the identity).  background: optional [H,W,3] u8 CUDA tensor; where no
+    instance covers a pixel, "image" takes background / 255 (f32, channels as given).  It changes no other output
+    (rast_render_scene_bg)."""
     dev = poses.device
     poses = _f32c(poses).reshape(-1, 3, 4)
     n = poses.shape[0]
@@ -360,18 +362,24 @@ def render_scene(mesh_ids, poses, K, H, W, znear=0.25, zfar=6.0, light_pos=(0.0,
     unknown = set(outputs) - {"pc_cam", "pc_obj", "normal", "image", "seg"}
     if unknown:
         raise ValueError(f"render_scene: unknown outputs {sorted(unknown)}")
+    if background is not None:
+        if background.dtype != torch.uint8 or tuple(background.shape) != (H, W, 3) or background.device != dev:
+            raise ValueError(f"render_scene: background must be a [{H},{W},3] uint8 tensor on {dev}, got "
+                             f"{tuple(background.shape)} {background.dtype} on {background.device}")
+        background = background.contiguous()
     out = {"depth": torch.empty((H, W), dtype=torch.float32, device=dev)}
     for k in outputs:
         out[k] = torch.empty((H, W) if k == "seg" else (H, W, 3), dtype=torch.float32, device=dev)
-    if n == 0:
+    if n == 0 and (background is None or "image" not in outputs):
         return {k: v.zero_() for k, v in out.items()}
     light = (ctypes.c_float * 12)(*[float(x) for x in (*light_pos, *light_color, *mat_diffuse, *mat_ambient)])
     L = _lib.lib()
     scratch = torch.empty((L.rast_scene_scratch_bytes(n, H, W) // 8,), dtype=torch.int64, device=dev)
     P = lambda k: _lib.ptr(out.get(k))
-    _lib.check(L.rast_render_scene(_lib.ptr(ids), _lib.ptr(poses), n, _lib.ptr(K), H, W, float(znear), float(zfar), light,
-                                   P("depth"), P("pc_cam"), P("pc_obj"), P("normal"), P("image"), P("seg"),
-                                   _lib.ptr(scratch), _lib.current_stream()), "rast_render_scene")
+    _lib.check(L.rast_render_scene_bg(_lib.ptr(ids), _lib.ptr(poses), n, _lib.ptr(K), H, W, float(znear), float(zfar),
+                                      light, _lib.ptr(background), P("depth"), P("pc_cam"), P("pc_obj"), P("normal"),
+                                      P("image"), P("seg"), _lib.ptr(scratch), _lib.current_stream()),
+               "rast_render_scene_bg")
     return out
 
 
@@ -386,7 +394,15 @@ class EGLRenderer:
     pc_cam; normal_tensor, which the reference does not flip, bottom to top.  image: BGR with to_bgr, times 255 with
     to_255 (alpha included), alpha 1; pc_obj and normal: alpha 1; everything 0 on background.  pc_cam_tensor[..., 3] is
     the coverage and seg_tensor[..., 0] the instance index + 1, its other channels left as they are.  The light
-    position and colour persist across calls, like set_light_pos / set_light_color."""
+    position and colour persist across calls, like set_light_pos / set_light_color.
+
+    render(background=): a uint8 [H,W,3] or [H,W] image (NumPy or tensor; 2-D is replicated to three channels, as PIL's
+    convert("RGB") does) shown where no instance covers a pixel, as the reference's im2Texture quad: there image_tensor
+    holds v / 255 per channel in the given order, then the same to_bgr swap and to_255 scaling as shaded pixels, alpha 1.
+    Covered pixels are unchanged.  It fills image_tensor only: depth, seg, pc_obj, pc_cam and normal are those of the
+    render without it.  Unlike the reference, which resamples a background of another size through its mip chain, a
+    size other than the render's raises ValueError; any dtype but uint8 raises NotImplementedError, as
+    PIL.Image.fromarray refuses those."""
 
     def __init__(self, model_paths, K=None, model_ids=None, texture_paths=None, model_colors=None, width=640, height=480,
                  gpu_id=None, render_marker=False, vertex_scale=1.0, znear=0.25, zfar=6.0, model_loadfn=None,
@@ -434,8 +450,10 @@ class EGLRenderer:
                pc_obj_tensor=None, pc_cam_tensor=None, phong=None, extents=None, gt_extents=None, background=None):
         """Fills the given [H,W,4] tensors (see the class) and returns depth [H,W].  `phong` is accepted and has no
         effect: shader_textureless_texture reads those weights only in its disabled aae_phong branch."""
-        for name, val in (("instance_colors", instance_colors), ("extents", extents), ("gt_extents", gt_extents),
-                          ("background", background)):
+        if background is not None and background.dtype not in (np.uint8, torch.uint8):
+            raise NotImplementedError(f"EGLRenderer.render: background of dtype {background.dtype} is not supported "
+                                      "(uint8 only)")
+        for name, val in (("instance_colors", instance_colors), ("extents", extents), ("gt_extents", gt_extents)):
             if val is not None:
                 raise NotImplementedError(f"EGLRenderer.render: {name} is not supported")
         if rot_type != "mat":
@@ -461,8 +479,17 @@ class EGLRenderer:
         ids = torch.tensor([self.models[o].mesh_id for o in obj_ids], dtype=torch.int32).to(self.device)
         outputs = [k for k, t in (("pc_cam", pc_cam_tensor), ("pc_obj", pc_obj_tensor), ("normal", normal_tensor),
                                   ("image", image_tensor), ("seg", seg_tensor)) if t is not None]
+        bg = None
+        if background is not None:
+            bg = torch.as_tensor(background)
+            if bg.ndim == 2:
+                bg = bg[:, :, None].expand(bg.shape[0], bg.shape[1], 3)
+            if tuple(bg.shape) != (H, W, 3):
+                raise ValueError(f"EGLRenderer.render: background must be [{H},{W},3] or [{H},{W}] (the render's size), "
+                                 f"got {tuple(np.shape(background))}")
+            bg = bg.to(self.device).contiguous()
         r = render_scene(ids, torch.from_numpy(P).to(self.device), torch.from_numpy(np.asarray(Kuse, np.float32)), H, W,
-                         self.znear, self.zfar, self.lightpos, self.lightcolor, outputs)
+                         self.znear, self.zfar, self.lightpos, self.lightcolor, outputs, background=bg)
         depth = r["depth"]
         if pc_cam_tensor is not None:
             pc_cam_tensor[..., :3] = r["pc_cam"]

@@ -325,6 +325,13 @@ int rast_upload_mesh_tex(const float* verts, int V, const int* faces, int F, con
 int rast_render_scene(const int* mesh_ids, const float* poses, int n_inst, const float* K, int H, int W, float znear,
                       float zfar, const float* light, float* depth, float* pc_cam, float* pc_obj, float* normal,
                       float* image, float* seg, void* scratch, void* stream);
+/* rast_render_scene_bg: rast_render_scene with an optional background [H,W,3] u8 (device; NULL: none).  Where no
+ *   instance covers a pixel, image takes v / 255 in f32 per channel, in the background's channel order; every other
+ *   output, and image on covered pixels, equals the render without a background.  n_inst may be 0 when a background is
+ *   given (mesh_ids and poses may then be NULL).  rast_render_scene(...) is rast_render_scene_bg(..., NULL, ...). */
+int rast_render_scene_bg(const int* mesh_ids, const float* poses, int n_inst, const float* K, int H, int W, float znear,
+                         float zfar, const float* light, const uint8_t* background, float* depth, float* pc_cam,
+                         float* pc_obj, float* normal, float* image, float* seg, void* scratch, void* stream);
 size_t rast_scene_scratch_bytes(int n_inst, int H, int W);
 
 /* ---------------------------------------------------------------------------------------------
@@ -498,6 +505,22 @@ int yolox_postprocess_layout(int B, int A, size_t* offsets);
 int yolox_postprocess(const float* preds, int B, int A, int num_classes, const int* hw, const int* strides, int n_levels,
                       float conf_thre, float nms_thre, int class_agnostic, int max_out, float* dets, int* n_det,
                       void* workspace, size_t workspace_bytes, void* stream);
+
+/* ---------------------------------------------------------------------------------------------
+ * Pose outlines over a test image (csrc/vis_poses.cu), the per-dataset vis_poses_full scripts' pixel work for N images
+ * of one size H x W.  No allocation, no synchronisation, the caller's stream.
+ *   gdrn_vis_gray3: img [N,H,W,3] u8, B, G, R (or R, G, B with rgb_order = 1) -> out [N,H,W,3] u8, each channel
+ *     (3735 b + 19235 g + 9798 r + 16384) >> 15, which is cv2.cvtColor(COLOR_BGR2GRAY) bit for bit.
+ *   gdrn_vis_outlines: shaded [N,H,W,3] f32, the RGB image output of rast_render_scene_bg (background included), and
+ *     cover [n,H,W] f32 (covered where != 0, e.g. rast_render_meshes depth) of the n GT and estimate instances;
+ *     image j owns instances [inst_off[j], inst_off[j+1]) (inst_off [N+1] i32, device), is_gt [n] u8 (device) flags
+ *     the GT ones.  An instance's edge pixel is covered with an uncovered pixel exactly bw rows or columns away in one
+ *     of the four directions (a neighbour outside the image does not count).  -> out [N,H,W,3] u8 BGR: (0, 255, 0)
+ *     on any estimate edge, else (255, 0, 0) on any GT edge, else (u8)(shaded[2 - c] * 255 + 0.5) in f32 without
+ *     contraction (to_bgr, to_255, then + 0.5 truncated). */
+int gdrn_vis_gray3(const uint8_t* img, int N, int H, int W, int rgb_order, uint8_t* out, void* stream);
+int gdrn_vis_outlines(const float* shaded, const float* cover, const int* inst_off, const uint8_t* is_gt, int N, int n,
+                      int H, int W, int bw, uint8_t* out, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
  * YOLOX training loss (csrc/yolox_loss.cu) -- replaces YOLOXHead.get_losses (det/yolox/models/yolo_head.py:256-426):
